@@ -1,6 +1,6 @@
 """Benchmark of the Stable Audio denoising hot path (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--config {2,3,4,5}] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--config {2,3,4,5}] [--impl reference] [--dump-outputs DIR]
 
 Default workload = BASELINE.json configs[2] (--config 3, the configuration the metric is quoted on): Stable Audio
 Open 1.0 DiT (1.06 B parameters, random init), 47.55 s stereo 44.1 kHz = 1024 latent tokens, batch 4 per GPU with
@@ -14,6 +14,11 @@ batch 8 per GPU (16 rows); --config 5 = the SA-2.0 length (6144 latents + prepen
 --impl reference times the reference's CPU path (the oracle port of the same DiT forward) with every host thread it
 can use, on a bounded sample of the same workload: the WHOLE batch of the configuration in one call through d of the
 24 identical blocks, scaled by 24 / d.
+
+--dump-outputs DIR writes, after the timed steps, the latents the last timed step returned (rank 0) as
+DIR/latents.npy (float32 [batch, 64, latent_len]) and, after the timed decode, the audio the last timed decode call
+returned as DIR/audio.npy (float32 [1, 2, 2048 * latent_len], the batch's last item).  Weights, conditioning, initial noise and sampler noise are seeded,
+so the same arguments give the same inputs on every run and two builds can be compared output for output.
 """
 import argparse
 import ctypes
@@ -77,7 +82,7 @@ def config_dict(args, extra=None):
                      f"T5-shaped conditioning [{CONFIGS[args.config]['name']}]",
          "baseline_config": args.config,
          "global_batch": BATCH * args.gpus, "latent_tokens": LATENT_LEN, "context_tokens": CTX_LEN,
-         "parallelism": f"dp{args.gpus}", "l2_policy": "per-step working set (2.1 GB of 16-bit weights) exceeds the 126 MB L2"}
+         "parallelism": f"dp{args.gpus}", "l2_policy": "per-step working set (2.1 GB of 16-bit weights) exceeds the 50 MB L2"}
     if extra:
         c.update(extra)
     return c
@@ -323,8 +328,9 @@ def run_native(args):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     wall0 = time.time()
     e0.record()
+    last = None
     for _ in range(args.steps):
-        loop.step()
+        last = loop.step()
     e1.record()
     barrier()
     wall1 = time.time()
@@ -337,6 +343,10 @@ def run_native(args):
         elapsed_ms = float(tmax.item())
     ms_per_step = elapsed_ms / args.steps
     value = world * args.steps / (elapsed_ms / 1e3)
+    if args.dump_outputs and rank == 0 and last is not None:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "latents.npy"), last.detach().float().cpu().numpy())
 
     # ---------------- e2e: same steps through the public call with HOST buffers --------------
     x_host = torch.empty(BATCH, 64, LATENT_LEN, pin_memory=True).copy_(loop.x.cpu())
@@ -405,6 +415,9 @@ def run_native(args):
     d1.record()
     torch.cuda.synchronize()
     decode_ms = d0.elapsed_time(d1) / 3
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        np.save(os.path.join(args.dump_outputs, "audio.npy"), audio.detach().float().cpu().numpy())
     if dist:
         tmax = torch.tensor([decode_ms], device=device)
         td.all_reduce(tmax, op=td.ReduceOp.MAX)
@@ -453,7 +466,7 @@ def run_native(args):
     # skip stream in fp16 (2 B) with fp16 operands, 128- / 256-channel ResidualUnits fused into one launch.
     import decoder_bytes
     raw_bytes = 4 if os.environ.get("SATB_RAW") == "fp32" else 2
-    dec_flops, dec_bytes = decoder_bytes.totals(LATENT_LEN, raw_bytes)
+    dec_flops, dec_bytes = decoder_bytes.totals(LATENT_LEN, raw_bytes, fused=os.environ.get("SATB_RESUNIT") != "unfused")
     dec_ms_sample = decode_ms / BATCH
     gen_ms = GEN_STEPS * ms_per_step + decode_ms
     audio_sec_per_s = world * BATCH * AUDIO_SECONDS / (gen_ms / 1e3)
@@ -470,13 +483,13 @@ def run_native(args):
             peaks = json.load(f)
     except Exception:
         pass
-    peak_tf = peaks.get("bf16_tflops_sustained") or 1400.0
+    peak_tf = peaks.get("bf16_tflops_sustained") or 989.0
     peak_src = "measured (MEASURED_PEAKS.json bf16_tflops_sustained, kernel timed inside a long step)" \
-        if "bf16_tflops_sustained" in peaks else "fallback (B200_PROFILING.md sustained 1.4 PFLOP/s)"
+        if "bf16_tflops_sustained" in peaks else "H100 SXM data sheet, dense FP16/BF16 at 700 W (not reached in practice)"
     M = 2 * BATCH * (LATENT_LEN + 1)
     ff_in_flops = 2.0 * M * 12288 * 1536
     peak_burst = peaks.get("bf16_tflops")
-    hbm_peak = peaks.get("hbm_gbs") or 6650.0
+    hbm_peak = peaks.get("hbm_gbs") or 3350.0   # H100 SXM data sheet, HBM3
     survey_gb = decoder_bytes.SURVEY_PER_RESUNIT_FUSED_FP32_GB * LATENT_LEN / 1024.0
     ff_in_ms = ms8[0] / max(cnt8[0], 1)
     achieved = ff_in_flops / (ff_in_ms / 1e3) / 1e12 if ff_in_ms > 0 else None
@@ -492,15 +505,11 @@ def run_native(args):
         "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": io_bytes, "d2h_bytes_per_step": io_bytes},
         "gpu_launches": int(launches),
         "clocks": clocks,
-        "roofline": {"bound": "tensor", "kernel": f"gemm_tcgen05_2cta_kernel<EpiSwiglu, 256> (FF-in {M}x12288x1536)",
+        "roofline": {"bound": "tensor", "kernel": f"gemm_wgmma_kernel<EpiSwiglu, 256> (FF-in {M}x12288x1536)",
                      "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s",
                      "frac": (achieved / peak_tf) if achieved else None,
                      "frac_of_burst_peak": (achieved / peak_burst) if (achieved and peak_burst) else None,
-                     # dram__bytes_read.sum + dram__bytes_write.sum of one launch of this kernel from the
-                     # `ncu --set full` capture summarised in profiles/r01_ncu_ff_in_gemm.txt (63.2 + 62.6 MB;
-                     # algorithmic A + W + out = 163.7 MB, part of the 16-bit output stays in the 126 MB L2)
-                     "traffic": 125806592, "traffic_unit": "bytes per launch (ncu)", "peak_source": peak_src,
-                     "avg_launch_ms": ff_in_ms},
+                     "peak_source": peak_src, "avg_launch_ms": ff_in_ms},
         "cuda_graph": not args.no_graph,
         "step_tflops": step_tflops, "step_frac_of_peak": step_tflops / peak_tf,
         "step_frac_of_burst_peak": (step_tflops / peak_burst) if peak_burst else None,
@@ -524,8 +533,8 @@ def run_native(args):
                             "audio_sec_per_s_100step_fp16x3": (world * BATCH * AUDIO_SECONDS /
                                                                ((GEN_STEPS * ms_per_step + BATCH * dec_x3_ms) / 1e3))
                             if dec_x3_ms else None,
-                            "note": "5.16 TFLOP per 1024 latents: with the 16-bit streams of this round the decoder's "
-                                    "tensor time exceeds its HBM time, i.e. the bound is the tensor pipe"},
+                            "note": "5.16 TFLOP per 1024 latents (algorithmic); roofline_floor_ms is the larger of the "
+                                    "tensor and HBM lower bounds at the peaks above"},
     }
     if not args.no_cpu_baseline:
         line["cpu_baseline"] = cpu_baseline_leg()
@@ -564,6 +573,9 @@ def main():
     ap.add_argument("--no-cpu-baseline", dest="no_cpu_baseline", action="store_true")
     ap.add_argument("--no-graph", dest="no_graph", action="store_true", help="enqueue every kernel of a step instead of "
                     "replaying the captured CUDA graph of the denoiser call")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                    help="write the latents of the last timed step (DIR/latents.npy) and the audio of the last timed decode "
+                         "call (DIR/audio.npy)")
     args = ap.parse_args()
     set_config(args.config)
     if args.impl == "reference":

@@ -30,10 +30,6 @@ int satb_linear_f32out(const void* a16, const void* w16, float* c, int M, int N,
   s.L = M; s.batches = 1; s.N = N; s.K = K; s.n_taps = 1; s.tap_base = 0; s.tap_step = 0; s.b_tap_rows = N; s.stride = 1;
   EpiStore32::Params ep{c, N, nullptr};
   SATB_PROPAGATE(make_tmap_a(&ta, a16, K, M, 1, K, static_cast<int64_t>(M) * K));
-  if ((N % 256 == 0 || N > 256) && gemm_use_2cta() && M >= 1024) {
-    SATB_PROPAGATE(make_tmap_b(&tb, w16, K, N, K, 128));
-    return bf16 ? launch_gemm_2cta<EpiStore32, 256, true>(ta, tb, s, ep, st) : launch_gemm_2cta<EpiStore32, 256, false>(ta, tb, s, ep, st);
-  }
   if (N % 256 == 0 || N > 256) {
     SATB_PROPAGATE(make_tmap_b(&tb, w16, K, N, K, 256));
     return bf16 ? launch_gemm<EpiStore32, 256, true>(ta, tb, s, ep, st) : launch_gemm<EpiStore32, 256, false>(ta, tb, s, ep, st);
@@ -60,17 +56,6 @@ int satb_attention(const void* q16, const void* k16, const void* v16, void* o16,
   return launch_attention_tc(q16, k16, v16, o16, dq, dk, dk, dq, Nq * dq, Nk * dk, Nk * dk, Nq * dq, static_cast<int>(dq),
                              static_cast<int>(dk), static_cast<int>(dk), 0, 0, 0, B, H, Hkv, Nq, Nk, bf16 != 0,
                              static_cast<cudaStream_t>(stream));
-}
-
-int satb_debug_attention_occupancy(int dyn_smem, int carveout_pct) { return debug_attention_occupancy(dyn_smem, carveout_pct); }
-
-// Debug: same as satb_attention, plus a clock64 trace of one CTA into dbg[tiles * 12] (device memory).
-int satb_attention_trace(const void* q16, const void* k16, const void* v16, void* o16, int B, int H, int Hkv, int Nq,
-                         int Nk, int bf16, unsigned long long* dbg, void* stream) {
-  const int64_t dq = static_cast<int64_t>(H) * 64, dk = static_cast<int64_t>(Hkv) * 64;
-  return launch_attention_tc(q16, k16, v16, o16, dq, dk, dk, dq, Nq * dq, Nk * dk, Nk * dk, Nq * dq, static_cast<int>(dq),
-                             static_cast<int>(dk), static_cast<int>(dk), 0, 0, 0, B, H, Hkv, Nq, Nk, bf16 != 0,
-                             static_cast<cudaStream_t>(stream), dbg);
 }
 
 }  // extern "C"

@@ -1,868 +1,231 @@
-// tcgen05 attention forward, head dim 64, no mask, non-causal, optional GQA:
+// Tensor-core attention forward, head dim 64, no mask, non-causal, optional GQA:
 //   O = softmax(Q K^T / sqrt(64)) V      (reference models/transformer.py:496-536)
 //
-// Persistent kernel, two CTAs of 384 threads per SM (2 x 256 TMEM columns, 2 x 111 KB shared memory).  A work unit is
-// 128 query rows of one (batch item, head); CTA c processes units c, c + grid, ... without re-initialising anything.
-// Keys are processed in tiles of 128:
-//   warp 0 (one thread)  TMA producer: Q of the unit, K / V tiles (2-stage rings), the unit's leftover-key rows
-//   warp 1 (one thread)  S = Q K_j^T -> TMEM (tcgen05.mma, smem operands) as soon as S has been read out
-//   warp 3 (one thread)  O += P V_j (A = P from TMEM, B = V tile addressed MN-major)
-//   warps 4-11           softmax: warps w and w + 4 own the same 32 query rows (TMEM lane quadrant w % 4) and split the
-//                        128 key columns of a tile; per 16-column chunk: tcgen05.ld -> row max -> P = exp2(S c - m_ref)
-//                        -> packed 16-bit pairs back to TMEM, with the next chunk's load in flight; row sums in fp32.
-//   warp 2               TMEM allocator; afterwards the CUDA-core path for ragged query rows (below)
-// TMEM columns: S [0,128)  P [128,192)  O [192,256).
-// What bounds it (measured, profiles/README.md): per 128 x 128 tile the SFU needs 1024 cycles (16 ex2 / clk / SM) and
-// tcgen05.ld as many (64 B / clk / SM for the fp32 S tile); with eight softmax warps per CTA and two CTAs per SM a tile
-// takes ~1400 cycles of the SM.  Around the tiles: a unit of 8 key tiles pays ~2500 cycles for its boundary (last P V,
-// normalise, first-tile max), and 1536 units on 296 CTAs are 5.2 rounds of work in 6.
-// O stays in TMEM for the whole unit: the reference max m_ref only moves when a tile's row max exceeds it by more
-// than 2^8 (lazy rescale: exponentials stay <= 256, sums in fp32), so the O rescale (TMEM load-scale-store) and the
-// recomputation of that tile's P are rare.
-// The normalised output tile is staged in shared memory and leaves with one TMA store under the next unit (per-thread
-// 16-byte stores to 3 KB-strided rows kept the load/store unit busy for ~2700 cycles per unit).
-//
-// Ragged shapes (1025 = 8 * 128 + 1 tokens: the prepended conditioning token):
-//   * leftover KEYS (Nk % 128 <= kExtraMax) do not get a tile of their own - a whole pipeline step for one column -:
-//     their scores S_x = Q K_x^T come from one 16-column MMA chain into the first columns of the P region while it is
-//     idle between two units; every softmax thread keeps exp2(s_x - m_ref) in fp32 registers (part of the first
-//     tile's reference max, scaled along in a rescale) and adds p_x v_x to its O row in the epilogue;
-//   * leftover QUERY rows (Nq % 128 <= kRowPathMax) are computed by warp 2 on CUDA cores (one warp per row:
-//     eight lanes per key, online softmax over blocks of 512 keys), concurrently with the tensor-core pipeline -
-//     unless the batch is so small that a partial ninth query tile is cheaper (cost model in launch_attention_tc).
+// One CTA of four warps per 64 query rows of one (batch item, head); each warp owns 16 query rows.  Keys are
+// processed in tiles of 64, double-buffered in shared memory by cp.async (rows past the end are zero-filled, their
+// scores masked).  Per tile and warp: S = Q K^T with mma.sync m16n8k16 (Q fragments stay in registers for the whole
+// row block, K fragments by ldmatrix), online softmax in fp32 on the S fragments (exp2, row max / sum reduced over the
+// four lanes of a row), then O += P V with P repacked from the S fragments into 16-bit A fragments and V fragments
+// by ldmatrix.trans.  The normalised output goes through shared memory so that it leaves as 16-byte row segments.
 #include "common.cuh"
 #include "gemm.cuh"
 #include "kernels.h"
 #include "ptx.cuh"
 #include <cmath>
-#include <cstdlib>
 
 namespace satb {
 
 namespace {
 
-constexpr int kQ = 128;        // query rows per unit
-constexpr int kK = 128;        // keys per tile
-constexpr int kD = 64;         // head dim
-constexpr int kStagesKV = 2;
-constexpr int kQBytes = kQ * kD * 2;                         // 16 KB
-constexpr int kKVBytes = kK * kD * 2;                        // 16 KB
-constexpr int kRowChunk = 512;                               // keys per block of the CUDA-core row path
-constexpr int kRowBatch = 8;                                 // independent 16-byte loads in flight per lane (row path)
-constexpr int kRowPathMax = 2;                               // Nq % 128 <= this: those rows take the row path
-constexpr int kAttnThreads = 384;                            // 4 control warps + 8 softmax warps
-constexpr int kSoftmaxThreads = 256;
-constexpr int kAttnPolyDefault = 0;                          // see SATB_ATTN_POLY
-constexpr int kExtraMax = 2;                                 // Nk % 128 <= this: those keys are added in the epilogue
-constexpr int kXRows = 16;                                   // rows of the leftover-key K / V tiles (TMA box)
-constexpr int kXBytes = kXRows * kD * 2;                     // 2 KB
-constexpr int kOBytes = kQ * kD * 2;                         // 16 KB: output tile staged for the TMA store
-// Q, K / V rings, output staging, leftover-key boxes, row-path scratch, exchange slots, barriers, alignment slack:
-// 111.25 KB, two CTAs per SM
-constexpr int kAttnSmem = kQBytes + 2 * kStagesKV * kKVBytes + kOBytes + 4 * kXBytes + kRowChunk * 4 + 4 * 2 * kQ * 4 + 256 + 1024;
-constexpr int kTmemColsAttn = 256;
-constexpr uint32_t kColS = 0, kColP = 128, kColO = 192;
-constexpr float kRescaleThreshold = 8.0f;                    // log2 units
+constexpr int kQ = 64;          // query rows per CTA
+constexpr int kK = 64;          // keys per tile
+constexpr int kD = 64;          // head dim
+constexpr int kAttnThreads = 128;
+constexpr int kTileElems = 64 * kD;                       // one 64 x 64 16-bit tile: 8 KB
+constexpr int kAttnSmem = (1 + 2 * 2) * kTileElems * 2;   // Q, two K and two V buffers: 40 KB
 
-struct AttnTcArgs {
+struct AttnArgs {
+  const uint16_t *q, *k, *v;
   uint16_t* o;
-  int64_t ldo, o_bs;
-  int Nq, Nk, group, H, batch;
+  int64_t ldq, ldk, ldv, ldo, q_bs, k_bs, v_bs, o_bs;
   int q_col, k_col, v_col;   // column offsets (elements) of head 0 inside the q / k / v tensors
-  int n_tiles, n_extra;      // key tiles on the tensor cores; leftover keys (Nk - 128 n_tiles <= kExtraMax) added in the epilogue
-  int n_qt;                  // tensor-core query tiles per (item, head)
-  int n_units;               // batch * H * n_qt
-  int step_bh, step_qt;      // grid / n_qt, grid % n_qt: the (item-head, query tile) step between a CTA's consecutive units
-  int row0, n_rows;          // rows [row0, row0 + n_rows) of every (item, head) take the CUDA-core path
-  const uint16_t *q, *k, *v; // raw pointers for the row path
-  int64_t ldq, ldk, ldv, q_bs, k_bs, v_bs;
+  int Nq, Nk, group;
   float scale_log2;
-  unsigned long long* dbg;   // optional clock64 trace of CTA 0's first softmax warp (tests / profiles only)
 };
 
-// V tile as the MN-major B operand: rows = keys (K dim), 64 contiguous 16-bit d values (128 B, one swizzle atom)
-// per row; 8-row groups 1024 B apart.
-__device__ __forceinline__ uint64_t make_desc_mnmajor_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
+// Element offset of 16-byte chunk `c` (0..7) of row `r` in a 64 x 64 tile: chunks are XOR-swizzled with the row so
+// that the eight rows an ldmatrix phase reads fall into different banks.
+__device__ __forceinline__ int swz(int r, int c) { return r * kD + ((c ^ (r & 7)) << 3); }
 
-// (volatile: a run of these stays in program order.  Left free, the compiler hoists all sixteen exponentials of a chunk
-// above their consumers, which costs ~90 bytes of spills at the 80-register budget and 5 % of the kernel, measured.)
-__device__ __forceinline__ float ex2_approx(float x) {
-  float y;
-  asm volatile("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool valid) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
 }
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
-// Packed fp32x2 arithmetic (FFMA2 / FADD2 on sm_100): two elements per issue slot for the scale-and-shift and the
-// row-sum accumulation.
-__device__ __forceinline__ uint64_t pack2(float lo, float hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "r"(__float_as_uint(lo)), "r"(__float_as_uint(hi)));
-  return r;
-}
-__device__ __forceinline__ void unpack2(uint64_t v, float& lo, float& hi) {
-  uint32_t a, b;
-  asm("mov.b64 {%0, %1}, %2;" : "=r"(a), "=r"(b) : "l"(v));
-  lo = __uint_as_float(a);
-  hi = __uint_as_float(b);
-}
-__device__ __forceinline__ uint64_t ffma2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ uint64_t fadd2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-
-// 2^x for a pair on the FMA / ALU pipes instead of the SFU (x <= ~8; clamped at -126): round-to-nearest split
-// x = i + f, |f| <= 0.5 by the magic-number add, 2^f by its degree-4 Taylor polynomial (relative error < 4.2e-5, below
-// the 16-bit rounding P gets anyway), 2^i by an integer add into the exponent field.
-__device__ __forceinline__ void ex2_poly2(float x0, float x1, float& y0, float& y1) {
-  const float kMagic = 12582912.f;   // 1.5 * 2^23
-  x0 = fmaxf(x0, -126.f);
-  x1 = fmaxf(x1, -126.f);
-  const uint64_t x = pack2(x0, x1), mg = pack2(kMagic, kMagic), nmg = pack2(-kMagic, -kMagic);
-  const uint64_t t = fadd2(x, mg);                 // integer part in the low mantissa bits
-  uint64_t fi = fadd2(t, nmg);                     // float(i)
-  float f0, f1, i0, i1;
-  unpack2(fi, i0, i1);
-  const uint64_t f = fadd2(x, pack2(-i0, -i1));    // f = x - i
-  // Horner: ((((c4 f + c3) f + c2) f + c1) f + 1)
-  const float c1 = 0.6931471806f, c2 = 0.2402265070f, c3 = 0.0555041087f, c4 = 0.0096181291f;
-  uint64_t acc = ffma2(pack2(c4, c4), f, pack2(c3, c3));
-  acc = ffma2(acc, f, pack2(c2, c2));
-  acc = ffma2(acc, f, pack2(c1, c1));
-  acc = ffma2(acc, f, pack2(1.f, 1.f));
-  float t0, t1, p0, p1;
-  unpack2(t, t0, t1);
-  unpack2(acc, p0, p1);
-  (void)f0; (void)f1;
-  y0 = __uint_as_float(__float_as_uint(p0) + ((__float_as_uint(t0) - 0x4B400000u) << 23));
-  y1 = __uint_as_float(__float_as_uint(p1) + ((__float_as_uint(t1) - 0x4B400000u) << 23));
-}
-
-__device__ __forceinline__ float warp_max(float v) {
+// rows [r0, r0 + 64) of a [rows, ld] 16-bit matrix, columns [col, col + 64), into a swizzled tile; rows >= n_rows
+// are zero-filled
+__device__ __forceinline__ void load_tile(uint16_t* tile, const uint16_t* base, int64_t ld, int r0, int n_rows, int col) {
+  const uint32_t s = smem_u32(tile);
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
+  for (int i = 0; i < 4; ++i) {
+    const int idx = threadIdx.x + i * kAttnThreads;
+    const int r = idx >> 3, c = idx & 7;
+    const bool ok = r0 + r < n_rows;
+    const uint16_t* src = base + static_cast<int64_t>(ok ? r0 + r : 0) * ld + col + c * 8;
+    cp_async16(s + swz(r, c) * 2, src, ok);
+  }
 }
 
-// --------------------------------------------------------------------------------- CUDA-core row path
-// One warp computes one query row of one (item, head): softmax(q K^T / 8) V in fp32.  Eight lanes share a key
-// (lane l holds dims 8 (l % 8) .. +7 of q, of the K row and of the V row: one 16-byte load per lane and key),
-// so one warp instruction covers four keys and every load of the loop is independent of the previous ones.
+__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
+               : "r"(addr));
+}
+__device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
+               : "r"(addr));
+}
+
+// d (16 x 8 fp32) += a (16 x 16) * b (16 x 8)
 template <bool BF16>
-__device__ void attn_row_path(const AttnTcArgs& p, int b, int h, int row, float* prow, int lane) {
-  const int hk = h / p.group;
-  const int sub = lane & 7, grp = lane >> 3;            // dims 8 sub .. 8 sub + 7; key phase grp (0..3)
-  const uint16_t* qp = p.q + b * p.q_bs + static_cast<int64_t>(row) * p.ldq + p.q_col + h * kD + 8 * sub;
-  const uint16_t* kp = p.k + b * p.k_bs + p.k_col + hk * kD + 8 * sub;
-  const uint16_t* vp = p.v + b * p.v_bs + p.v_col + hk * kD + 8 * sub;
-  float qf[8];
-  {
-    const uint4 u = __ldcg(reinterpret_cast<const uint4*>(qp));
-    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const float2 f = Op16<BF16>::unpack(w[e]);
-      qf[2 * e] = f.x * p.scale_log2;
-      qf[2 * e + 1] = f.y * p.scale_log2;
-    }
-  }
-  float m_run = -INFINITY, l_run = 0.f;
-  float o[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) o[e] = 0.f;
-  for (int k0 = 0; k0 < p.Nk; k0 += kRowChunk) {
-    const int nk = min(kRowChunk, p.Nk - k0);
-    const int n4 = (nk + 3) >> 2;                       // groups of four keys
-    // ---- scores of this block -> prow[], running block max.  Loads are issued in explicit batches of kRowBatch
-    // independent 16-byte loads per lane (the compiler will not hoist a global load above the shared-memory store
-    // of the previous iteration, which would serialise one L2 round trip per group of four keys).
-    float mx = -INFINITY;
-    for (int i0 = 0; i0 < n4; i0 += kRowBatch) {
-      uint4 u[kRowBatch];
-#pragma unroll
-      for (int jj = 0; jj < kRowBatch; ++jj) {
-        const int key = 4 * (i0 + jj) + grp;
-        u[jj] = key < nk ? __ldcg(reinterpret_cast<const uint4*>(kp + static_cast<int64_t>(k0 + key) * p.ldk))
-                         : make_uint4(0u, 0u, 0u, 0u);
-      }
-#pragma unroll
-      for (int jj = 0; jj < kRowBatch; ++jj) {
-        const int key = 4 * (i0 + jj) + grp;
-        const uint32_t w[4] = {u[jj].x, u[jj].y, u[jj].z, u[jj].w};
-        float s = 0.f;
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float2 f = Op16<BF16>::unpack(w[e]);
-          s = fmaf(qf[2 * e], f.x, s);
-          s = fmaf(qf[2 * e + 1], f.y, s);
-        }
-        s += __shfl_xor_sync(0xffffffffu, s, 1);
-        s += __shfl_xor_sync(0xffffffffu, s, 2);
-        s += __shfl_xor_sync(0xffffffffu, s, 4);
-        if (key < nk) {
-          if (sub == 0) prow[key] = s;
-          mx = fmaxf(mx, s);
-        }
-      }
-    }
-    mx = warp_max(mx);
-    const float m_new = fmaxf(m_run, mx);
-    const float f = ex2_approx(m_run - m_new);          // 0 on the first block (m_run = -inf)
-    l_run *= f;
-#pragma unroll
-    for (int e = 0; e < 8; ++e) o[e] *= f;
-    m_run = m_new;
-    __syncwarp();
-    float ls = 0.f;
-    for (int i = lane; i < nk; i += 32) {
-      const float e = ex2_approx(prow[i] - m_new);
-      prow[i] = e;
-      ls += e;
-    }
-    l_run += warp_sum(ls);
-    __syncwarp();
-    // ---- O += P V: lane accumulates its 8 dims over the keys of its phase (same batching)
-    for (int i0 = 0; i0 < n4; i0 += kRowBatch) {
-      uint4 u[kRowBatch];
-#pragma unroll
-      for (int jj = 0; jj < kRowBatch; ++jj) {
-        const int key = 4 * (i0 + jj) + grp;
-        u[jj] = key < nk ? __ldcg(reinterpret_cast<const uint4*>(vp + static_cast<int64_t>(k0 + key) * p.ldv))
-                         : make_uint4(0u, 0u, 0u, 0u);
-      }
-#pragma unroll
-      for (int jj = 0; jj < kRowBatch; ++jj) {
-        const int key = 4 * (i0 + jj) + grp;
-        const float e = key < nk ? prow[key] : 0.f;
-        const uint32_t w[4] = {u[jj].x, u[jj].y, u[jj].z, u[jj].w};
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          const float2 vv = Op16<BF16>::unpack(w[c]);
-          o[2 * c] = fmaf(e, vv.x, o[2 * c]);
-          o[2 * c + 1] = fmaf(e, vv.y, o[2 * c + 1]);
-        }
-      }
-    }
-    __syncwarp();
-  }
-  // combine the four key phases (lanes l, l + 8, l + 16, l + 24 hold the same dims)
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    o[e] += __shfl_xor_sync(0xffffffffu, o[e], 8);
-    o[e] += __shfl_xor_sync(0xffffffffu, o[e], 16);
-  }
-  if (grp == 0) {
-    const float inv = 1.0f / l_run;
-    uint16_t* og = p.o + b * p.o_bs + static_cast<int64_t>(row) * p.ldo + static_cast<int64_t>(h) * kD + 8 * sub;
-    *reinterpret_cast<uint4*>(og) = make_uint4(Op16<BF16>::pack(o[0] * inv, o[1] * inv), Op16<BF16>::pack(o[2] * inv, o[3] * inv),
-                                                Op16<BF16>::pack(o[4] * inv, o[5] * inv), Op16<BF16>::pack(o[6] * inv, o[7] * inv));
-  }
-}
-
-// POLY: every fourth pair of exponentials of a full chunk goes through ex2_poly2 (FMA / ALU pipes) instead of the SFU
-template <bool BF16, bool POLY>
-__global__ void __launch_bounds__(kAttnThreads, 2)
-attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-               const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmKx,
-               const __grid_constant__ CUtensorMap tmVx, const __grid_constant__ CUtensorMap tmO, const AttnTcArgs p) {
-  extern __shared__ uint8_t smem_raw[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // (an offset added to the array keeps the shared address space visible to the compiler: LDS / STS, not generic LD / ST)
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* sQ = smem;                                   // [16 KB] (single: the last Q K^T of a unit is issued a whole
-                                                        // tile before the unit ends, which is the time the next Q has to arrive)
-  uint8_t* sK = smem + kQBytes;                         // [kStagesKV][16 KB]
-  uint8_t* sV = sK + kStagesKV * kKVBytes;
-  uint8_t* sO = sV + kStagesKV * kKVBytes;              // [16 KB] normalised output tile (128B-swizzled rows) for the TMA store
-  uint8_t* sX = sO + kOBytes;                           // [2 units][K | V][2 KB] leftover-key rows (16-row TMA boxes)
-  float* prow = reinterpret_cast<float*>(sX + 4 * kXBytes);            // [kRowChunk] row-path scratch
-  float* xch = prow + kRowChunk;                        // [4][2][128] exchange between the two column halves of a row:
-                                                        // slots 0 / 1 = tile parity, 2 = first-tile max, 3 = row sums
-  uint64_t* bars = reinterpret_cast<uint64_t*>(xch + 4 * 2 * kQ);
-  uint64_t* q_full = bars;                 // TMA -> MMA / softmax: Q of the unit has landed
-  uint64_t* q_empty = bars + 1;            // MMA -> TMA: every MMA reading Q has retired
-  uint64_t* k_full = bars + 2;             // [kStagesKV]
-  uint64_t* k_empty = k_full + kStagesKV;
-  uint64_t* v_full = k_empty + kStagesKV;
-  uint64_t* v_empty = v_full + kStagesKV;
-  uint64_t* s_full = v_empty + kStagesKV;  // MMA -> softmax: S holds Q K_j^T
-  uint64_t* s_free = s_full + 1;           // softmax -> MMA: S has been read (256 arrivals)
-  uint64_t* p_ready = s_free + 1;          // softmax -> MMA: P written (256 arrivals)
-  uint64_t* p_free = p_ready + 1;          // MMA -> softmax: P V_j retired (P reusable, O up to date)
-  uint64_t* o_done = p_free + 1;           // MMA -> softmax: last P V of the unit retired
-  uint64_t* o_free = o_done + 1;           // softmax -> MMA: O of the previous unit has been read (256 arrivals)
-  uint64_t* x_full = o_free + 1;           // [2] TMA -> softmax: leftover-key K / V rows of the unit have landed
-  uint64_t* x_empty = x_full + 2;          // [2] softmax -> TMA: they have been used (256 arrivals)
-  uint64_t* sx_full = x_empty + 2;         // MMA -> softmax: P[0,16) holds Q K_x^T of the unit's leftover keys
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sx_full + 1);
-
-  const int n_tiles = p.n_tiles;           // tensor-core key tiles; the n_extra leftover keys are added in the epilogue
-  const int n_extra = p.n_extra;
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmV);
-    mbar_init(q_full, 1);
-    mbar_init(q_empty, 1);
-    mbar_init(sx_full, 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&x_full[i], 1);
-      mbar_init(&x_empty[i], kSoftmaxThreads);
-    }
-    for (int i = 0; i < kStagesKV; ++i) {
-      mbar_init(&k_full[i], 1);
-      mbar_init(&k_empty[i], 1);
-      mbar_init(&v_full[i], 1);
-      mbar_init(&v_empty[i], 1);
-    }
-    mbar_init(s_full, 1);
-    mbar_init(s_free, kSoftmaxThreads);
-    mbar_init(p_ready, kSoftmaxThreads);
-    mbar_init(p_free, 1);
-    mbar_init(o_done, 1);
-    mbar_init(o_free, kSoftmaxThreads);
-    fence_mbar_init();
-    if (p.dbg) {   // per-CTA residency record: SM id, start time (ns)
-      uint32_t smid;
-      unsigned long long t;
-      asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-      p.dbg[192 + blockIdx.x * 4 + 0] = smid;
-      p.dbg[192 + blockIdx.x * 4 + 2] = t;
-    }
-  }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, kTmemColsAttn);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_launch_dependents();
-  pdl_wait();
-
-  // unit u -> (item b, head h, query tile qt); consecutive units share (b, h), i.e. their K / V tiles in L2
-  // The CTA walks units blockIdx, blockIdx + grid, ...: the two divisions are done once, every further unit is reached by
-  // adding the precomputed (grid / n_qt, grid % n_qt) step (the divisions cost ~400 cycles on the softmax warps' path).
-  struct Unit { int u, b, h, q0; };
-  auto unit_first = [&]() -> Unit {
-    Unit t;
-    t.u = blockIdx.x;
-    const int nq = max(p.n_qt, 1);
-    const int bh = t.u / nq;
-    t.q0 = (t.u - bh * nq) * kQ;
-    t.b = bh / p.H;
-    t.h = bh - t.b * p.H;
-    return t;
-  };
-  auto unit_next = [&](Unit& t) {
-    t.u += gridDim.x;
-    t.q0 += p.step_qt * kQ;
-    int dh = p.step_bh;
-    if (t.q0 >= p.n_qt * kQ) {
-      t.q0 -= p.n_qt * kQ;
-      ++dh;
-    }
-    t.h += dh;
-    while (t.h >= p.H) {
-      t.h -= p.H;
-      ++t.b;
-    }
-  };
-
-  if (warp == 0) {
-    if (elect_one()) {
-      // ---------------------------------------------------------------- TMA producer
-      int g = 0;   // global key-tile counter of this CTA
-      int i = 0;   // local unit counter
-      for (Unit t = unit_first(); t.u < p.n_units; unit_next(t), ++i) {
-        const int b = t.b, h = t.h, q0 = t.q0;
-        const int hk = h / p.group;
-        mbar_wait(q_empty, (i & 1) ^ 1);
-        mbar_expect_tx(q_full, kQBytes);
-        tma_load_4d(sQ, &tmQ, q_full, p.q_col + h * kD, 0, q0, b);
-        if (n_extra > 0) {               // the unit's leftover keys: 16-row boxes (rows past Nk are zero-filled)
-          const int xb = i & 1;
-          mbar_wait(&x_empty[xb], ((i >> 1) & 1) ^ 1);
-          mbar_expect_tx(&x_full[xb], 2 * kXBytes);
-          tma_load_4d(sX + xb * 2 * kXBytes, &tmKx, &x_full[xb], p.k_col + hk * kD, 0, n_tiles * kK, b);
-          tma_load_4d(sX + xb * 2 * kXBytes + kXBytes, &tmVx, &x_full[xb], p.v_col + hk * kD, 0, n_tiles * kK, b);
-        }
-        for (int j = 0; j < n_tiles; ++j, ++g) {
-          const int st = g % kStagesKV;
-          const uint32_t ph = ((g / kStagesKV) & 1) ^ 1;
-          mbar_wait(&k_empty[st], ph);
-          mbar_expect_tx(&k_full[st], kKVBytes);
-          tma_load_4d(sK + st * kKVBytes, &tmK, &k_full[st], p.k_col + hk * kD, 0, j * kK, b);
-          mbar_wait(&v_empty[st], ph);
-          mbar_expect_tx(&v_full[st], kKVBytes);
-          tma_load_4d(sV + st * kKVBytes, &tmV, &v_full[st], p.v_col + hk * kD, 0, j * kK, b);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      // ------------------------------------------------- MMA issuer 1: S = Q K_j^T
-      int g = 0, i = 0;
-      for (int u = blockIdx.x; u < p.n_units; u += gridDim.x, ++i) {
-        const uint32_t q_addr = smem_u32(sQ);
-        mbar_wait(q_full, i & 1);
-        tc_fence_after();
-        if (n_extra > 0) {
-          // S_x = Q K_x^T for the unit's leftover keys: one 16-column MMA chain into the first 16 columns of the P
-          // region, which is idle between the previous unit's last P V and this unit's first P store (rows past Nk of
-          // the 16-row box are zero-filled by the TMA; the softmax reads columns 0 .. n_extra - 1 only)
-          mbar_wait(&x_full[i & 1], (i >> 1) & 1);
-          if (i >= 1 && n_tiles > 0) mbar_wait(o_done, (i - 1) & 1);   // (one phase per unit: p_free's parity would alias)
-          tc_fence_after();
-          const uint32_t idesc = make_idesc_f16(kQ, kXRows, BF16);
-          const uint32_t kx_addr = smem_u32(sX + (i & 1) * 2 * kXBytes);
-#pragma unroll
-          for (int ks = 0; ks < kD / 16; ++ks)
-            umma_f16_ss(tmem_base + kColP, make_desc_kmajor_sw128(q_addr + ks * 32),
-                        make_desc_kmajor_sw128(kx_addr + ks * 32), idesc, ks != 0);
-          umma_commit(sx_full);
-        }
-        for (int j = 0; j < n_tiles; ++j, ++g) {
-          const int st = g % kStagesKV;
-          mbar_wait(&k_full[st], (g / kStagesKV) & 1);
-          if (g >= 1) mbar_spin(s_free, (g - 1) & 1);   // S of the previous tile has been read by every softmax thread
-          tc_fence_after();
-          const int nk = min(kK, p.Nk - j * kK);
-          const int n_mma = (nk + 15) & ~15;
-          const uint32_t idesc = make_idesc_f16(kQ, n_mma, BF16);
-          const uint32_t k_addr = smem_u32(sK + st * kKVBytes);
-#pragma unroll
-          for (int ks = 0; ks < kD / 16; ++ks)
-            umma_f16_ss(tmem_base + kColS, make_desc_kmajor_sw128(q_addr + ks * 32),
-                        make_desc_kmajor_sw128(k_addr + ks * 32), idesc, ks != 0);
-          umma_commit(&k_empty[st]);   // the K tile is free as soon as these MMAs retire
-          umma_commit(s_full);
-        }
-        umma_commit(q_empty);          // every MMA reading Q has retired (immediately, if there was none)
-      }
-    }
-  } else if (warp == 3) {
-    if (elect_one()) {
-      // ------------------------------------------------- MMA issuer 2: O += P V_j
-      constexpr uint32_t idesc_pv = make_idesc_f16(kQ, kD, BF16, /*b_mn_major=*/true);
-      int g = 0, i = 0;
-      for (int u = blockIdx.x; u < p.n_units; u += gridDim.x, ++i) {
-        for (int j = 0; j < n_tiles; ++j, ++g) {
-          const int st = g % kStagesKV;
-          mbar_wait(&v_full[st], (g / kStagesKV) & 1);
-          mbar_spin(p_ready, g & 1);
-          if (j == 0 && i >= 1) mbar_wait(o_free, (i - 1) & 1);   // the previous unit's O has been read out
-          tc_fence_after();
-          const int nk = min(kK, p.Nk - j * kK);
-          const int ksteps = (nk + 15) >> 4;
-          const uint32_t v_addr = smem_u32(sV + st * kKVBytes);
-          if (ksteps == kK / 16) {
-#pragma unroll
-            for (int ks = 0; ks < kK / 16; ++ks)
-              umma_f16_ts(tmem_base + kColO, tmem_base + kColP + ks * 8, make_desc_mnmajor_sw128(v_addr + ks * 2048),
-                          idesc_pv, (j | ks) != 0);
-          } else {
-            for (int ks = 0; ks < ksteps; ++ks)
-              umma_f16_ts(tmem_base + kColO, tmem_base + kColP + ks * 8, make_desc_mnmajor_sw128(v_addr + ks * 2048),
-                          idesc_pv, (j | ks) != 0);
-          }
-          umma_commit(p_free);
-          umma_commit(&v_empty[st]);
-          if (j == n_tiles - 1) umma_commit(o_done);
-        }
-      }
-    }
-  } else if (warp == 2) {
-    // ------------------------------------------------------- ragged query rows on CUDA cores
-    if (p.n_rows > 0) {
-      const int n_tasks = p.batch * p.H * p.n_rows;
-      for (int t = blockIdx.x; t < n_tasks; t += gridDim.x) {
-        const int bh = t / p.n_rows, r = t - bh * p.n_rows;
-        const int b = bh / p.H, h = bh - b * p.H;
-        attn_row_path<BF16>(p, b, h, p.row0 + r, prow, lane);
-      }
-    }
+__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  if constexpr (BF16) {
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+                 "{%0, %1, %2, %3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
   } else {
-    // ------------------------------------------------------- softmax + epilogue
-    // Eight warps: warp w may touch TMEM lanes 32 (w % 4) .. +31, so warps w and w + 4 share the 32 query rows of a
-    // quadrant and split the key columns of every tile (half 0: keys 0-63, half 1: keys 64-127).  Four warps per
-    // scheduler (two CTAs per SM) keep the SFU fed while others sit in TMEM / barrier latencies.
-    const int q = warp & 3;
-    const int half = (warp - 4) >> 2;
-    const int row = q * 32 + lane;
-    const uint32_t t_lane = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-    const uint32_t s_addr = t_lane + kColS, p_addr = t_lane + kColP, o_addr = t_lane + kColO;
-    const float sc = p.scale_log2;
-    const bool trace = p.dbg != nullptr && blockIdx.x == 0 && warp == 4 && lane == 0;
-    // exchange slot s: this thread writes xch[s][half][row] and reads xch[s][1 - half][row] after the pair barrier
-    auto xput = [&](int slot, float v) { xch[(slot * 2 + half) * kQ + row] = v; };
-    auto xget = [&](int slot) -> float { return xch[(slot * 2 + (half ^ 1)) * kQ + row]; };
-    auto pair_sync = [&]() { asm volatile("bar.sync %0, 64;" ::"r"(1 + q) : "memory"); };   // the two warps of a quadrant
-    auto softmax_sync = [&]() { asm volatile("bar.sync 5, 256;" ::: "memory"); };             // all eight softmax warps
-    int g = 0, i = 0;
-    for (Unit t = unit_first(); t.u < p.n_units; unit_next(t), ++i) {
-      const int b = t.b, h = t.h, q0 = t.q0;
-      float m_ref = -INFINITY, l = 0.f;
-      const uint8_t* xk = sX + (i & 1) * 2 * kXBytes;   // K rows of the unit's leftover keys; V rows follow at + kXBytes
-      // ---- leftover keys (Nk % 128 <= kExtraMax): their scores come from a 16-column MMA (P[0,16), see the MMA issuer);
-      // they count in the first tile's reference max, their exponentials p_x are kept in fp32 registers (scaled along
-      // in the rare rescale) and p_x V_x is added to the O row in the epilogue.
-      float s_x[kExtraMax], p_x[kExtraMax];
-#pragma unroll
-      for (int e = 0; e < kExtraMax; ++e) {
-        s_x[e] = -INFINITY;
-        p_x[e] = 0.f;
-      }
-      if (n_extra > 0) {
-        uint32_t sx[2];
-        mbar_spin(sx_full, i & 1);
-        tc_fence_after();
-        tmem_ld_32x2(p_addr, sx);
-        tmem_ld_wait();
-#pragma unroll
-        for (int e = 0; e < kExtraMax; ++e)
-          if (e < n_extra) s_x[e] = __uint_as_float(sx[e]);
-      }
-      if (trace && g < 16) p.dbg[g * 12 + 2] = clock64();
-      for (int j = 0; j < n_tiles; ++j, ++g) {
-        const int nk = min(kK, p.Nk - j * kK);
-        if (trace && g < 16) p.dbg[g * 12 + 0] = clock64();
-        mbar_spin(s_full, g & 1);
-        tc_fence_after();
-        if (trace && g < 16) p.dbg[g * 12 + 1] = clock64();
-        // This thread's 64 key columns of the tile, in four chunks of 16.  tcgen05.ld moves 64 B per clock and SM
-        // (a 128 x 128 fp32 S tile = 1024 clocks, as long as its 16 K exponentials take on the SFU), so the load of
-        // chunk c + 1 is in flight while chunk c is exponentiated: ra / rb alternate, one load outstanding at a time
-        // (tcgen05.wait::ld waits for all of a thread's loads).
-        const int cbase = 64 * half;
-        const int lim = nk - cbase;              // valid key columns among the 64 (<= 0: none)
-        const uint32_t sa = s_addr + cbase, pa = p_addr + cbase / 2;
-        uint32_t ra[16], rb[16];
-        auto max16 = [&](const uint32_t (&r)[16], float m) -> float {
-          float m0 = fmaxf(__uint_as_float(r[0]), __uint_as_float(r[1])), m1 = fmaxf(__uint_as_float(r[2]), __uint_as_float(r[3]));
-          float m2 = fmaxf(__uint_as_float(r[4]), __uint_as_float(r[5])), m3 = fmaxf(__uint_as_float(r[6]), __uint_as_float(r[7]));
-          m0 = fmaxf(m0, fmaxf(__uint_as_float(r[8]), __uint_as_float(r[9])));
-          m1 = fmaxf(m1, fmaxf(__uint_as_float(r[10]), __uint_as_float(r[11])));
-          m2 = fmaxf(m2, fmaxf(__uint_as_float(r[12]), __uint_as_float(r[13])));
-          m3 = fmaxf(m3, fmaxf(__uint_as_float(r[14]), __uint_as_float(r[15])));
-          return fmaxf(fmaxf(m, fmaxf(m0, m1)), fmaxf(m2, m3));
-        };
-        auto max16m = [&](const uint32_t (&r)[16], int n, float m) -> float {   // the first n (< 16 possible) columns
-#pragma unroll
-          for (int e = 0; e < 16; ++e)
-            if (e < n) m = fmaxf(m, __uint_as_float(r[e]));
-          return m;
-        };
-        // P chunk = exp2(S c - m_ref) of r[] -> TMEM columns [pcol, pcol + 8); adds to the packed fp32 row sum
-        auto exp16_store = [&](const uint32_t (&r)[16], uint32_t pcol, uint64_t& sum2) {
-          const uint64_t sc2 = pack2(sc, sc), nm2 = pack2(-m_ref, -m_ref);
-          uint32_t w[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            float t0, t1;
-            unpack2(ffma2(pack2(__uint_as_float(r[2 * e]), __uint_as_float(r[2 * e + 1])), sc2, nm2), t0, t1);
-            float p0, p1;
-            if (POLY && (e & 3) == 3) {
-              ex2_poly2(t0, t1, p0, p1);
-            } else {
-              p0 = ex2_approx(t0);
-              p1 = ex2_approx(t1);
-            }
-            sum2 = fadd2(sum2, pack2(p0, p1));
-            w[e] = Op16<BF16>::pack(p0, p1);
-          }
-          tmem_st_32x8(pcol, w);
-        };
-        auto exp16m_store = [&](const uint32_t (&r)[16], int n, uint32_t pcol) -> float {   // columns >= n give P = 0
-          uint32_t w[8];
-          float sm = 0.f;
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            const float s0 = 2 * e < n ? __uint_as_float(r[2 * e]) : -INFINITY;
-            const float s1 = 2 * e + 1 < n ? __uint_as_float(r[2 * e + 1]) : -INFINITY;
-            const float p0 = ex2_approx(fmaf(s0, sc, -m_ref));
-            const float p1 = ex2_approx(fmaf(s1, sc, -m_ref));
-            sm += p0 + p1;
-            w[e] = Op16<BF16>::pack(p0, p1);
-          }
-          tmem_st_32x8(pcol, w);
-          return sm;
-        };
-        if (j == 0) {
-          // first tile of the unit: the reference max = max over the whole first tile (both halves).  (Taking it from the
-          // first 16 columns only and leaving the rest to the lazy rescale was measured 13 % SLOWER: the rescale path then
-          // runs in about every third unit.)
-          float mx = -INFINITY;
-          if (lim >= 64) {
-            tmem_ld_32x16(sa, ra);
-            tmem_ld_wait16(ra);
-            tmem_ld_32x16(sa + 16, rb);
-            mx = max16(ra, mx);
-            tmem_ld_wait16(rb);
-            tmem_ld_32x16(sa + 32, ra);
-            mx = max16(rb, mx);
-            tmem_ld_wait16(ra);
-            tmem_ld_32x16(sa + 48, rb);
-            mx = max16(ra, mx);
-            tmem_ld_wait16(rb);
-            mx = max16(rb, mx);
-          } else {
-#pragma unroll 1
-            for (int c = 0; c < 4; ++c)
-              if (16 * c < lim) {
-                tmem_ld_32x16(sa + 16 * c, ra);
-                tmem_ld_wait16(ra);
-                mx = max16m(ra, lim - 16 * c, mx);
-              }
-          }
-#pragma unroll
-          for (int e = 0; e < kExtraMax; ++e) mx = fmaxf(mx, s_x[e]);
-          xput(2, mx);
-          pair_sync();                           // (also: both halves have read s_x before either stores P)
-          m_ref = fmaxf(mx, xget(2)) * sc;
-#pragma unroll
-          for (int e = 0; e < kExtraMax; ++e) {
-            if (e < n_extra) {
-              p_x[e] = ex2_approx(fmaf(s_x[e], sc, -m_ref));
-              if (half == 0) l += p_x[e];
-            }
-          }
-        }
-        // ---- hot path: chunks 0-2: exp2 -> P store while the next chunk loads; chunk 3: max only; exchange of the tile
-        // max between the halves; S is released (Q K_{j+1}^T runs under the exponentials of chunk 3); chunk 3: exp2 -> P
-        float mx_raw = -INFINITY, sum = 0.f;
-        uint64_t sum2 = pack2(0.f, 0.f);
-        bool waited = false;
-        auto wait_p_free = [&]() {
-          if (!waited && g >= 1) {
-            mbar_spin(p_free, (g - 1) & 1);      // P V of the previous tile retired: P may be overwritten, O is quiescent
-            tc_fence_after();
-          }
-          waited = true;
-        };
-        if (lim >= 64) {
-          tmem_ld_32x16(sa, ra);
-          tmem_ld_wait16(ra);
-          tmem_ld_32x16(sa + 16, rb);
-          mx_raw = max16(ra, mx_raw);
-          wait_p_free();
-          exp16_store(ra, pa, sum2);
-          tmem_ld_wait16(rb);
-          tmem_ld_32x16(sa + 32, ra);
-          mx_raw = max16(rb, mx_raw);
-          exp16_store(rb, pa + 8, sum2);
-          tmem_ld_wait16(ra);
-          tmem_ld_32x16(sa + 48, rb);
-          mx_raw = max16(ra, mx_raw);
-          exp16_store(ra, pa + 16, sum2);
-          tmem_ld_wait16(rb);
-          mx_raw = max16(rb, mx_raw);
-        } else if (lim > 0) {                    // partial last tile of a ragged key count: chunk by chunk, masked
-          wait_p_free();
-#pragma unroll 1
-          for (int c = 0; c < 3; ++c)
-            if (16 * c < lim) {
-              tmem_ld_32x16(sa + 16 * c, ra);
-              tmem_ld_wait16(ra);
-              mx_raw = max16m(ra, lim - 16 * c, mx_raw);
-              sum += exp16m_store(ra, lim - 16 * c, pa + 8 * c);
-            }
-          if (lim > 48) {
-            tmem_ld_32x16(sa + 48, rb);
-            tmem_ld_wait16(rb);
-            mx_raw = max16m(rb, lim - 48, mx_raw);
-          }
-        }
-        if (trace && g < 16) p.dbg[g * 12 + 3] = clock64();
-        // lazy rescale: only when the tile's row max (over BOTH halves) exceeds the reference max by more than 2^8
-        xput(g & 1, mx_raw);
-        pair_sync();
-        const float mx_tile = fmaxf(mx_raw, xget(g & 1));
-        const bool need = mx_tile * sc > m_ref + kRescaleThreshold;
-        if (!__any_sync(0xffffffffu, need)) {    // both warps of the quadrant see the same rows, i.e. decide alike
-          tc_fence_before();
-          // This thread holds its last chunk in registers.  (Releasing S one chunk earlier - two chunks held, so that
-          // Q K_{j+1}^T has 32 exponentials per thread to hide under instead of 16 - was measured 7 % slower: the second
-          // live buffer spills.)
-          mbar_arrive(s_free);
-          if (lim >= 64) exp16_store(rb, pa + 24, sum2);
-          else if (lim > 48) sum += exp16m_store(rb, lim - 48, pa + 24);
-        } else {
-          wait_p_free();
-          const float m_new = need ? mx_tile * sc : m_ref;
-          const float f = ex2_approx(m_ref - m_new);   // 1 for rows that keep their reference
-          m_ref = m_new;
-          l *= f;
-#pragma unroll
-          for (int e = 0; e < kExtraMax; ++e) p_x[e] *= f;
-          sum = 0.f;                             // P again with the new reference max: chunk 3 from registers ...
-          sum2 = pack2(0.f, 0.f);
-          if (lim > 48) sum += exp16m_store(rb, lim - 48, pa + 24);
-#pragma unroll 1
-          for (int c = 0; c < 3; ++c)            // ... chunks 0-2 from S, which has not been released yet
-            if (16 * c < lim) {
-              tmem_ld_32x16(sa + 16 * c, ra);
-              tmem_ld_wait16(ra);
-              sum += exp16m_store(ra, lim - 16 * c, pa + 8 * c);
-            }
-          tc_fence_before();
-          mbar_arrive(s_free);
-          if (j > 0) {                           // each half rescales its 32 columns of O
-#pragma unroll 1
-            for (int hh = 0; hh < 2; ++hh) {
-              tmem_ld_32x16(o_addr + half * 32 + hh * 16, ra);
-              tmem_ld_wait16(ra);
-              uint32_t w[16];
-#pragma unroll
-              for (int e = 0; e < 16; ++e) w[e] = __float_as_uint(__uint_as_float(ra[e]) * f);
-              tmem_st_32x16(o_addr + half * 32 + hh * 16, w);
-            }
-          }
-        }
-        {
-          float a0, a1;
-          unpack2(sum2, a0, a1);
-          sum += a0 + a1;
-        }
-        if (trace && g < 16) p.dbg[g * 12 + 4] = clock64();
-        l += sum;
-        wait_p_free();                           // (threads without valid keys in this tile have not waited yet)
-        tmem_st_wait();
-        tc_fence_before();
-        mbar_arrive(p_ready);
-        if (trace && g < 16) p.dbg[g * 12 + 11] = clock64();
-      }
-      // ---- epilogue of the unit: (O + leftover keys) / l -> global; each half stores 32 of the 64 columns, in two
-      // passes of 16 (the 80-register budget of a 384-thread CTA does not hold a 32-column row plus the extras)
-      const int gt = g - 1;                      // trace row of the unit's last tile
-      if (trace && gt >= 0 && gt < 16) p.dbg[gt * 12 + 5] = clock64();
-      if (n_extra > 0) {
-        if (n_tiles == 0) {
-          // no tensor-core tile at all (Nk <= kExtraMax): the leftover keys are the whole softmax
-          float mx = -INFINITY;
-#pragma unroll
-          for (int e = 0; e < kExtraMax; ++e) mx = fmaxf(mx, s_x[e]);
-          m_ref = mx * sc;
-#pragma unroll
-          for (int e = 0; e < kExtraMax; ++e) {
-            if (e < n_extra) {
-              p_x[e] = ex2_approx(fmaf(s_x[e], sc, -m_ref));
-              if (half == 0) l += p_x[e];
-            }
-          }
-        }
-        mbar_spin(&x_full[i & 1], (i >> 1) & 1);   // (landed long ago: makes the V_x rows visible to this thread)
-      }
-      xput(3, l);
-      pair_sync();
-      const float inv = 1.0f / (l + xget(3));
-      // (the staging tile is free once the previous unit's store has read it; this barrier sits in the shadow of the
-      // wait for the last P V below)
-      if (warp == 4 && lane == 0) tma_store_wait_read();
-      softmax_sync();
-      if (n_tiles > 0) {
-        mbar_spin(o_done, i & 1);
-        tc_fence_after();
-      }
-      if (trace && gt >= 0 && gt < 16) p.dbg[gt * 12 + 6] = clock64();
-      // The normalised tile goes to shared memory (rows of 128 B in the 128B-swizzle pattern of the tensor map) and
-      // leaves with ONE TMA store, asynchronously under the next unit: per-thread 16-byte stores to 3 KB-strided rows
-      // cost ~5000 cycles per unit in the load/store unit (32 lines per warp instruction).  The tensor map ends at row
-      // p.row0, so rows past Nq - or owned by the CUDA-core row path - are clipped by the TMA.
-      if (trace && gt >= 0 && gt < 16) p.dbg[gt * 12 + 9] = clock64();
-      const uint8_t* xv = xk + kXBytes;
-#pragma unroll 1
-      for (int sub = 0; sub < 2; ++sub) {
-        uint32_t ro[16];
-        if (n_tiles > 0) {
-          tmem_ld_32x16(o_addr + half * 32 + sub * 16, ro);
-          tmem_ld_wait();
-        } else {
-#pragma unroll
-          for (int e = 0; e < 16; ++e) ro[e] = 0u;
-        }
-        float ov[16];
-#pragma unroll
-        for (int e = 0; e < 16; ++e) ov[e] = __uint_as_float(ro[e]);
-        if (n_extra > 0) {
-#pragma unroll
-          for (int e = 0; e < kExtraMax; ++e) {
-            if (e < n_extra) {
-#pragma unroll
-              for (int c = 0; c < 2; ++c) {
-                const uint4 vv = *reinterpret_cast<const uint4*>(xv + e * 128 + (((half * 4 + sub * 2 + c) ^ e) << 4));
-                const uint32_t vw[4] = {vv.x, vv.y, vv.z, vv.w};
-#pragma unroll
-                for (int d = 0; d < 4; ++d) {
-                  const float2 f2 = Op16<BF16>::unpack(vw[d]);
-                  ov[c * 8 + 2 * d] = fmaf(p_x[e], f2.x, ov[c * 8 + 2 * d]);
-                  ov[c * 8 + 2 * d + 1] = fmaf(p_x[e], f2.y, ov[c * 8 + 2 * d + 1]);
-                }
-              }
-            }
-          }
-        }
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int chunk = half * 4 + sub * 2 + e;          // 16-byte chunk of the row's 128 bytes
-          *reinterpret_cast<uint4*>(sO + row * 128 + ((chunk ^ (row & 7)) << 4)) =
-              make_uint4(Op16<BF16>::pack(ov[8 * e] * inv, ov[8 * e + 1] * inv), Op16<BF16>::pack(ov[8 * e + 2] * inv, ov[8 * e + 3] * inv),
-                         Op16<BF16>::pack(ov[8 * e + 4] * inv, ov[8 * e + 5] * inv), Op16<BF16>::pack(ov[8 * e + 6] * inv, ov[8 * e + 7] * inv));
-        }
-      }
-      if (n_tiles > 0) {
-        tc_fence_before();
-        mbar_arrive(o_free);                     // O has been read: the next unit's first P V may overwrite it
-      }
-      if (n_extra > 0) mbar_arrive(&x_empty[i & 1]);   // this thread is done with the unit's leftover-key rows
-      fence_proxy_async_smem();                        // the staged tile becomes visible to the TMA
-      softmax_sync();
-      if (warp == 4 && lane == 0) {
-        tma_store_4d(&tmO, sO, h * kD, 0, q0, b);
-        tma_store_commit();
-      }
-      if (trace && gt >= 0 && gt < 16) p.dbg[gt * 12 + 10] = clock64();
-    }
-  }
-  if (warp == 4 && lane == 0) tma_store_wait_all();    // the last output tile has left shared memory and is written
-  tc_fence_before();
-  __syncthreads();
-  if (p.dbg && threadIdx.x == 0) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    p.dbg[192 + blockIdx.x * 4 + 3] = t;
-  }
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemColsAttn);
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+                 "{%0, %1, %2, %3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
   }
 }
 
-int make_tmap_rows(CUtensorMap* m, const void* ptr, int cols, int rows, int batches, int64_t ld, int64_t bs,
-                   int box_rows) {
-  // (cols, rows, batches) 16-bit, box (64, box_rows, 1): reuse the A-operand encoder (phase dim = 1)
-  return make_tmap_a(m, ptr, cols, rows, batches, ld, bs, 1, box_rows);
+template <bool BF16>
+__global__ void __launch_bounds__(kAttnThreads) attn_kernel(const AttnArgs p) {
+  extern __shared__ __align__(128) uint16_t smem_attn[];
+  uint16_t* sQ = smem_attn;
+  uint16_t* sK = sQ + kTileElems;        // [2][64 x 64]
+  uint16_t* sV = sK + 2 * kTileElems;    // [2][64 x 64]
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int q0 = blockIdx.x * kQ, h = blockIdx.y, b = blockIdx.z;
+  const int hk = h / p.group;
+  const uint16_t* qb = p.q + b * p.q_bs;
+  const uint16_t* kbase = p.k + b * p.k_bs;
+  const uint16_t* vbase = p.v + b * p.v_bs;
+  const int qc = p.q_col + h * kD, kc = p.k_col + hk * kD, vc = p.v_col + hk * kD;
+  const int n_tiles = (p.Nk + kK - 1) / kK;
+
+  pdl_launch_dependents();
+  pdl_wait();   // q / k / v are written by the previous kernels
+  load_tile(sQ, qb, p.ldq, q0, p.Nq, qc);
+  load_tile(sK, kbase, p.ldk, 0, p.Nk, kc);
+  load_tile(sV, vbase, p.ldv, 0, p.Nk, vc);
+  cp_async_commit();
+
+  uint32_t qf[4][4];   // Q fragments of this warp's 16 rows, four 16-wide slices of the head dim
+  float o[8][4];       // O: 16 rows x 64 columns as eight 8-column fragments
+  float m[2] = {-1e30f, -1e30f}, l[2] = {0.f, 0.f};   // rows lane / 4 and lane / 4 + 8 (scaled log2 units)
+#pragma unroll
+  for (int j = 0; j < 8; ++j) o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f;
+
+  for (int t = 0; t < n_tiles; ++t) {
+    const int buf = t & 1;
+    if (t + 1 < n_tiles) {   // next tile into the other buffer (freed by the barrier at the end of tile t - 1)
+      load_tile(sK + (buf ^ 1) * kTileElems, kbase, p.ldk, (t + 1) * kK, p.Nk, kc);
+      load_tile(sV + (buf ^ 1) * kTileElems, vbase, p.ldv, (t + 1) * kK, p.Nk, vc);
+      cp_async_commit();
+      cp_async_wait<1>();
+    } else {
+      cp_async_wait<0>();
+    }
+    __syncthreads();
+    if (t == 0) {
+      const uint32_t sq = smem_u32(sQ);
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        const int r = warp * 16 + (lane & 7) + 8 * ((lane >> 3) & 1), c = 2 * kk + (lane >> 4);
+        ldsm_x4(sq + swz(r, c) * 2, qf[kk][0], qf[kk][1], qf[kk][2], qf[kk][3]);
+      }
+    }
+    // S = Q K^T: 16 rows x 64 keys
+    float s[8][4];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
+    const uint32_t sk = smem_u32(sK + buf * kTileElems);
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+      for (int nb = 0; nb < 4; ++nb) {   // keys 16 nb .. 16 nb + 15
+        const int r = 16 * nb + (lane & 7) + 8 * (lane >> 4), c = 2 * kk + ((lane >> 3) & 1);
+        uint32_t b0, b1, b2, b3;
+        ldsm_x4(sk + swz(r, c) * 2, b0, b1, b2, b3);
+        mma16816<BF16>(s[2 * nb], qf[kk], b0, b1);
+        mma16816<BF16>(s[2 * nb + 1], qf[kk], b2, b3);
+      }
+    }
+    // online softmax
+    const int key0 = t * kK + 2 * (lane & 3);
+    float mx[2] = {m[0], m[1]};
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const bool ok = key0 + 8 * j + (e & 1) < p.Nk;
+        s[j][e] = ok ? s[j][e] * p.scale_log2 : -INFINITY;
+        mx[e >> 1] = fmaxf(mx[e >> 1], s[j][e]);
+      }
+    }
+    float alpha[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 1));
+      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 2));
+      alpha[i] = exp2f(m[i] - mx[i]);
+      m[i] = mx[i];
+      l[i] *= alpha[i];
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        s[j][e] = exp2f(s[j][e] - m[e >> 1]);
+        l[e >> 1] += s[j][e];
+        o[j][e] *= alpha[e >> 1];
+      }
+    }
+    // O += P V
+    const uint32_t sv = smem_u32(sV + buf * kTileElems);
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {   // keys 16 kk .. 16 kk + 15
+      uint32_t a[4];
+      a[0] = Op16<BF16>::pack(s[2 * kk][0], s[2 * kk][1]);
+      a[1] = Op16<BF16>::pack(s[2 * kk][2], s[2 * kk][3]);
+      a[2] = Op16<BF16>::pack(s[2 * kk + 1][0], s[2 * kk + 1][1]);
+      a[3] = Op16<BF16>::pack(s[2 * kk + 1][2], s[2 * kk + 1][3]);
+#pragma unroll
+      for (int db = 0; db < 4; ++db) {   // head-dim columns 16 db .. 16 db + 15
+        const int r = 16 * kk + (lane & 7) + 8 * ((lane >> 3) & 1), c = 2 * db + (lane >> 4);
+        uint32_t b0, b1, b2, b3;
+        ldsm_x4_t(sv + swz(r, c) * 2, b0, b1, b2, b3);
+        mma16816<BF16>(o[2 * db], a, b0, b1);
+        mma16816<BF16>(o[2 * db + 1], a, b2, b3);
+      }
+    }
+    __syncthreads();   // this buffer may be refilled
+  }
+
+  // normalise; stage the warp's 16 rows in its own rows of the Q tile, then 16-byte stores
+  float inv[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    l[i] += __shfl_xor_sync(0xffffffffu, l[i], 1);
+    l[i] += __shfl_xor_sync(0xffffffffu, l[i], 2);
+    inv[i] = 1.f / l[i];
+  }
+  const int rr = warp * 16 + (lane >> 2);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int col = 8 * j + 2 * (lane & 3);
+    *reinterpret_cast<uint32_t*>(sQ + swz(rr, col >> 3) + (col & 7)) = Op16<BF16>::pack(o[j][0] * inv[0], o[j][1] * inv[0]);
+    *reinterpret_cast<uint32_t*>(sQ + swz(rr + 8, col >> 3) + (col & 7)) =
+        Op16<BF16>::pack(o[j][2] * inv[1], o[j][3] * inv[1]);
+  }
+  __syncwarp();
+  uint16_t* ob = p.o + b * p.o_bs + h * kD;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int idx = lane + 32 * i;
+    const int r = warp * 16 + (idx >> 3), c = idx & 7;
+    if (q0 + r < p.Nq)
+      *reinterpret_cast<uint4*>(ob + static_cast<int64_t>(q0 + r) * p.ldo + c * 8) =
+          *reinterpret_cast<const uint4*>(sQ + swz(r, c));
+  }
 }
 
 }  // namespace
@@ -873,106 +236,40 @@ int make_tmap_rows(CUtensorMap* m, const void* ptr, int cols, int rows, int batc
 int launch_attention_tc(const void* q, const void* k, const void* v, void* o, int64_t ldq, int64_t ldk, int64_t ldv,
                         int64_t ldo, int64_t q_bs, int64_t k_bs, int64_t v_bs, int64_t o_bs, int q_cols, int k_cols,
                         int v_cols, int q_col, int k_col, int v_col, int batch, int H, int H_kv, int Nq, int Nk,
-                        bool bf16, cudaStream_t stream, unsigned long long* dbg) {
+                        bool bf16, cudaStream_t stream) {
   SATB_REQUIRE(H % H_kv == 0, "num_heads must be a multiple of kv heads");
   SATB_REQUIRE(Nk >= 1 && Nq >= 1, "empty attention problem");
-  SATB_REQUIRE(ldo % 8 == 0, "attention output stride must be 16B aligned");
-  SATB_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && q_col % 8 == 0 && k_col % 8 == 0 && v_col % 8 == 0,
+  SATB_REQUIRE(ldo % 8 == 0 && o_bs % 8 == 0 && (reinterpret_cast<uintptr_t>(o) & 15) == 0,
+               "attention output must be 16B aligned");
+  SATB_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && q_col % 8 == 0 && k_col % 8 == 0 && v_col % 8 == 0 &&
+                   q_bs % 8 == 0 && k_bs % 8 == 0 && v_bs % 8 == 0,
                "attention operand strides / column offsets must be 16B aligned");
-  CUtensorMap tq, tk, tv;
-  SATB_PROPAGATE(make_tmap_rows(&tq, q, q_cols, Nq, batch, ldq, q_bs, kQ));
-  SATB_PROPAGATE(make_tmap_rows(&tk, k, k_cols, Nk, batch, ldk, k_bs, kK));
-  SATB_PROPAGATE(make_tmap_rows(&tv, v, v_cols, Nk, batch, ldv, v_bs, kK));
-  CUtensorMap to;         // output tiles (TMA store), rows [0, row0): set below
-  CUtensorMap tkx, tvx;   // the leftover keys (rows 128 n_tiles ...) as 16-row boxes
-  SATB_PROPAGATE(make_tmap_rows(&tkx, k, k_cols, Nk, batch, ldk, k_bs, kXRows));
-  SATB_PROPAGATE(make_tmap_rows(&tvx, v, v_cols, Nk, batch, ldv, v_bs, kXRows));
-  AttnTcArgs a;
-  a.o = static_cast<uint16_t*>(o);
-  a.ldo = ldo; a.o_bs = o_bs;
-  a.Nq = Nq; a.Nk = Nk; a.group = H / H_kv; a.H = H; a.batch = batch;
-  a.q_col = q_col; a.k_col = k_col; a.v_col = v_col;
-  // keys: full 128-key tiles on the tensor cores; a remainder of <= kExtraMax keys in the epilogue, a larger one as one
-  // more (partial) tile
-  const int krem = Nk % kK;
-  const bool extra = krem != 0 && krem <= kExtraMax;
-  a.n_tiles = Nk / kK + ((krem != 0 && !extra) ? 1 : 0);
-  a.n_extra = extra ? krem : 0;
-  // query rows: full 128-row tiles on the tensor cores; a remainder of <= kRowPathMax rows either on CUDA cores (warp 2
-  // of the CTAs, concurrently) or as one more, partial, tensor-core tile.  One row task is a serial walk over all keys
-  // by a single warp (~110 cycles per key, measured: 65 us for 1025 keys), so it only pays when every CTA has enough
-  // tensor-core units to hide it behind - large batches; otherwise (B = 1, 2) the partial tile rides in the slack of
-  // the last wave for free.
-  const int rem = Nq % kQ;
-  const int slots_all = 2 * device_sm_count();
-  bool row_path = rem != 0 && rem <= kRowPathMax;
-  static int force_rows = -2;
-  if (force_rows == -2) {
-    const char* e = getenv("SATB_ATTN_ROWPATH");     // 0 / 1: force the partial tile / the CUDA-core rows (A-B switch)
-    force_rows = e ? (atoi(e) != 0) : -1;
-  }
-  if (row_path && force_rows == 0) row_path = false;
-  if (row_path && force_rows < 0) {
-    const double unit_cycles = a.n_tiles * 2900.0 + 4500.0, row_cycles = 100.0 * Nk;
-    const double units_per_cta = static_cast<double>(batch) * H * (Nq / kQ) / slots_all;
-    const double rows_per_cta = std::ceil(static_cast<double>(batch) * H * rem / slots_all);
-    if (units_per_cta * unit_cycles < rows_per_cta * row_cycles) row_path = false;
-  }
-  a.n_qt = Nq / kQ + ((rem != 0 && !row_path) ? 1 : 0);
-  a.n_units = batch * H * a.n_qt;
-  a.row0 = row_path ? Nq - rem : Nq;
-  a.n_rows = row_path ? rem : 0;
+  SATB_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(k) & 15) == 0 &&
+                   (reinterpret_cast<uintptr_t>(v) & 15) == 0,
+               "attention operands must be 16B aligned");
+  SATB_REQUIRE(q_col + H * kD <= q_cols && k_col + H_kv * kD <= k_cols && v_col + H_kv * kD <= v_cols,
+               "attention heads exceed the operand columns");
+  AttnArgs a;
   a.q = static_cast<const uint16_t*>(q); a.k = static_cast<const uint16_t*>(k); a.v = static_cast<const uint16_t*>(v);
-  a.ldq = ldq; a.ldk = ldk; a.ldv = ldv; a.q_bs = q_bs; a.k_bs = k_bs; a.v_bs = v_bs;
+  a.o = static_cast<uint16_t*>(o);
+  a.ldq = ldq; a.ldk = ldk; a.ldv = ldv; a.ldo = ldo;
+  a.q_bs = q_bs; a.k_bs = k_bs; a.v_bs = v_bs; a.o_bs = o_bs;
+  a.q_col = q_col; a.k_col = k_col; a.v_col = v_col;
+  a.Nq = Nq; a.Nk = Nk; a.group = H / H_kv;
   a.scale_log2 = (1.0f / sqrtf(64.0f)) * 1.4426950408889634f;
-  a.dbg = dbg;
-  SATB_REQUIRE(o_bs % 8 == 0 && (reinterpret_cast<uintptr_t>(o) & 15) == 0, "attention output must be 16B aligned");
-  SATB_PROPAGATE(make_tmap_rows(&to, o, H * kD, a.row0 > 0 ? a.row0 : 1, batch, ldo, o_bs, kQ));
-  const int row_tasks = batch * H * a.n_rows;
-  int grid = a.n_units > row_tasks ? a.n_units : row_tasks;
-  static int ctas_per_sm = -1;
-  if (ctas_per_sm < 0) {
-    const char* e = getenv("SATB_ATTN_CTAS_PER_SM");   // 1: one CTA per SM (A/B measurement of the SFU sharing)
-    ctas_per_sm = (e && atoi(e) == 1) ? 1 : 2;
-  }
-  const int slots = ctas_per_sm * device_sm_count();
-  if (grid > slots) grid = slots;
-  if (grid <= 0) return 0;
-  a.step_bh = a.n_qt > 0 ? grid / a.n_qt : 0;
-  a.step_qt = a.n_qt > 0 ? grid % a.n_qt : 0;
-  static int poly = -1;
-  if (poly < 0) {
-    const char* e = getenv("SATB_ATTN_POLY");        // 0 / 1: A-B of the FMA-pipe exponentials
-    poly = e ? (atoi(e) != 0) : kAttnPolyDefault;
-  }
-  auto prepare = [&](auto kern) -> int {
-    SATB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem));
-    // two CTAs per SM need 2 x 98 KB: ask for the largest shared-memory carveout
-    SATB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    return 0;
-  };
+  const dim3 grid(ceil_div(Nq, kQ), H, batch);
+  SATB_REQUIRE(grid.y <= 65535 && grid.z <= 65535, "attention grid too large");
   auto go = [&](auto kern, PerDeviceOnce& once) -> int {
-    if (once.first()) SATB_PROPAGATE(prepare(kern));
-    SATB_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kAttnThreads), kAttnSmem, stream, tq, tk, tv, tkx, tvx, to, a));
+    if (once.first()) SATB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem));
+    SATB_CHECK_CUDA(launch_pdl(kern, grid, dim3(kAttnThreads), kAttnSmem, stream, a));
     return 0;
   };
-  static PerDeviceOnce o00, o01, o10, o11;
-  if (bf16) SATB_PROPAGATE(poly ? go(attn_tc_kernel<true, true>, o11) : go(attn_tc_kernel<true, false>, o10));
-  else SATB_PROPAGATE(poly ? go(attn_tc_kernel<false, true>, o01) : go(attn_tc_kernel<false, false>, o00));
+  static PerDeviceOnce o16, ob16;
+  if (bf16) SATB_PROPAGATE(go(attn_kernel<true>, ob16));
+  else SATB_PROPAGATE(go(attn_kernel<false>, o16));
   count_launch();
   SATB_CHECK_CUDA(cudaGetLastError());
   return 0;
-}
-
-// Debug: resident CTAs per SM the runtime reports for the attention kernel with `dyn_smem` bytes of dynamic shared
-// memory and the given carveout preference (percent, -1 = leave unchanged); tests / profiling only.
-int debug_attention_occupancy(int dyn_smem, int carveout_pct) {
-  auto kern = attn_tc_kernel<false, false>;
-  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn_smem) != cudaSuccess) return -1;
-  if (carveout_pct >= 0) cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_pct);
-  int nb = -1;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kAttnThreads, dyn_smem) != cudaSuccess) return -2;
-  return nb;
 }
 
 }  // namespace satb

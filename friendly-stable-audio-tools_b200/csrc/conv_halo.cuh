@@ -1,221 +1,245 @@
-// k-tap (dilated) convolution with few output channels as a tcgen05 implicit GEMM that loads every
-// activation row ONCE per tile: the A operand of tap t is the same 128B-swizzled shared-memory tile,
-// read through a matrix descriptor whose start address is shifted by t * dilation rows (128 B each).
-// The swizzle is a function of the absolute smem address bits, which TMA (writer) and the tensor
-// core (reader) agree on, so a row-shifted start needs no re-layout.  The generic GEMM path reloads
-// the tile once per tap (7x the L2 -> SM traffic), which is what bounds the thin layers.
+// k-tap (dilated) convolutions that load every activation row ONCE per tile, as a wgmma implicit GEMM.
 //
-//   out[b, n, l] = bias[n] + sum_{t, k} A[b, l + (t - taps/2) * dil, k] * W[t * cout + n, k]     (N <= 32)
+//   conv[b, l, n] = sum_{t, k} A[b, l + (t - taps/2) * dil, k] * W[t * N + n, k]
 //
-// Used for the decoder's final convolution (128 -> 2 channels, k = 7; models/autoencoders.py:190).
-// One persistent CTA per SM: warp 0 TMA producer, warp 1 MMA issuer, warp 2 TMEM allocator,
-// warps 4-7 epilogue.  All tap weights stay resident in shared memory.
+// TMA brings the 128 + (taps - 1) * dil activation rows of a 64-channel k-block into one 128B-swizzled smem slot, and
+// tap t reads it through a matrix descriptor shifted by t * dil rows (make_desc_kmajor_sw128); only the tap
+// weights stream through the ring.  The generic GEMM reloads the A tile once per tap (7x the L2 -> SM traffic).
+//
+// FUSE = false: the decoder's final convolution (128 -> 2 channels, k = 7, models/autoencoders.py:190); the epilogue
+// (EpiStoreNCL) ignores the columns >= N of the 64-wide tile.
+// FUSE = true: a whole Oobleck ResidualUnit (models/autoencoders.py:45-68), y = x + conv1x1(snake2(conv7(snake1(x)))):
+// the conv7 accumulator never leaves the SM - bias + snake2 + 16-bit rounding, written to smem in the swizzled K-major
+// layout, feeds a second wgmma chain with the 1x1 weights (streamed through the same ring), whose accumulator goes to
+// EpiConv (+ bias + skip, raw stream, the consumer's Snake).  N = channels = 128 or 256.
+//
+// Same warp roles as gemm_wgmma_kernel: warpgroup 0 one TMA producer thread, warpgroups 1, 2 MMA + epilogue on 64 rows
+// each; one persistent CTA per SM over 128-position tiles.
 #pragma once
 #include "gemm.cuh"
 
 namespace satb {
 
-struct ConvHaloShape {
+struct HaloShape {
   int L;         // positions per batch item
   int batches;
-  int K;         // input channels (multiple of 64, <= 256)
+  int K;         // input channels (multiple of 64)
   int n_taps;    // odd
-  int dil;
-  int cout;      // real output channels (<= 32); B tile rows beyond them are ignored
+  int dil;       // (n_taps - 1) * dil <= kHaloMax
+  int N;         // output channels (rows of W per tap)
 };
 
-struct ConvHaloCfg {
-  static constexpr int kBN = 32;
-  static constexpr int kThreads = 256;
-  static constexpr int kBTile = kBN * kBlockK * 2;            // 4 KB per (tap, k-block)
-  static constexpr int kSmemBudget = 200 * 1024;
-  __host__ __device__ static int halo_rows(const ConvHaloShape& s) { return kBlockM + (s.n_taps - 1) * s.dil; }
-  __host__ __device__ static int slot_bytes(const ConvHaloShape& s) { return (halo_rows(s) * 128 + 1023) & ~1023; }
-  __host__ __device__ static int b_bytes(const ConvHaloShape& s) { return s.n_taps * (s.K / kBlockK) * kBTile; }
-  __host__ __device__ static int stages(const ConvHaloShape& s) {
-    int n = (kSmemBudget - b_bytes(s) - 1024) / slot_bytes(s);
-    return n > 8 ? 8 : n;
-  }
+struct ResUnitPre {      // FUSE: the inner conv7 -> snake2 step
+  const float* bias7;    // [N] or null
+  const float* sn2_a;    // e^alpha of snake2
+  const float* sn2_ib;   // 1/(e^beta + 1e-9) of snake2
 };
 
-// Measured on B200: the plain SW128 descriptor (matrix base offset field = 0) is what works for a
-// start address on any 128-byte row of the pattern; setting base offset = (addr >> 7) & 7 gives wrong results.
+constexpr int kHaloMax = 54;   // halo rows beyond the tile: 6 taps x dilation 9
 
-template <class Epi, bool BF16>
-__global__ void __launch_bounds__(ConvHaloCfg::kThreads, 1)
-conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const ConvHaloShape s,
-                 const typename Epi::Params ep) {
-  using Cfg = ConvHaloCfg;
+template <int BN, int kCols, int kEpiStage, bool FUSE>
+struct HaloCfg {
+  static constexpr int kSlotA = ((kBlockM + kHaloMax) * 128 + 1023) / 1024 * 1024;   // 24 KB halo slot
+  static constexpr int kStagesA = 2;
+  static constexpr int kStageB = BN * kBlockK * 2;
+  static constexpr int kA2 = FUSE ? kBlockM * BN * 2 : 0;                // snake2(conv7) tile, BN / 64 swizzled atoms
+  static constexpr int kAccStage = 2 * 64 * (kCols + 4) * 4;             // per MMA warpgroup (gemm_tile_epilogue)
+  static constexpr int kShared = kA2 > 2 * kAccStage ? kA2 : 2 * kAccStage;   // the A2 tile and the accumulator
+                                                                          // staging take turns in one region
+  static constexpr int kFixed = 1024 + kStagesA * kSlotA + kShared + 256 + kEpiWarps * kEpiStage;
+  static constexpr int kStagesB = (kSmemBudget - kFixed) / kStageB > 8 ? 8 : (kSmemBudget - kFixed) / kStageB;
+  static constexpr int kSmemBytes = kFixed + kStagesB * kStageB;
+  static_assert(kStagesB >= 2, "shared memory too small for a two-stage weight ring");
+};
+
+template <class Epi, int BN, bool BF16, bool FUSE>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+conv_halo_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                       const __grid_constant__ CUtensorMap tmB1, const HaloShape s, const ResUnitPre pre,
+                       const typename Epi::Params ep) {
+  using Cfg = HaloCfg<BN, Epi::kCols, Epi::kStageBytes, FUSE>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int n_stages = Cfg::stages(s);
-  const int slot = Cfg::slot_bytes(s);
-  const int kbs = s.K / kBlockK;
-  uint8_t* b_res = smem + n_stages * slot;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(b_res + Cfg::b_bytes(s));
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + 8;
-  uint64_t* tfull_bar = bars + 16;
-  uint64_t* tempty_bar = bars + 18;
-  uint64_t* b_full = bars + 20;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 21);
+  uint8_t* slot_a = smem;
+  uint8_t* shared = slot_a + Cfg::kStagesA * Cfg::kSlotA;
+  uint8_t* ring_b = shared + Cfg::kShared;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(ring_b + Cfg::kStagesB * Cfg::kStageB);
+  uint64_t* full_a = bars;
+  uint64_t* empty_a = bars + Cfg::kStagesA;
+  uint64_t* full_b = bars + 2 * Cfg::kStagesA;
+  uint64_t* empty_b = full_b + Cfg::kStagesB;
+  uint8_t* epi_smem = reinterpret_cast<uint8_t*>(bars) + 256;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
   const int m_tiles = (s.L + kBlockM - 1) / kBlockM;
   const int total_tiles = m_tiles * s.batches;
+  const int n_kb = s.K / kBlockK;
+  const int halo_rows = kBlockM + (s.n_taps - 1) * s.dil;
+  const int halo0 = -(s.n_taps / 2) * s.dil;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    for (int i = 0; i < 8; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
+    for (int i = 0; i < Cfg::kStagesA; ++i) {
+      mbar_init(&full_a[i], 1);
+      mbar_init(&empty_a[i], 2);
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 4);
+    for (int i = 0; i < Cfg::kStagesB; ++i) {
+      mbar_init(&full_b[i], 1);
+      mbar_init(&empty_b[i], 2);
     }
-    mbar_init(b_full, 1);
     fence_mbar_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, 2 * Cfg::kBN);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_launch_dependents();
-  if (warp != 0) pdl_wait();
 
-  if (warp == 0) {
-    if (elect_one()) {
-      // ---------------------------------------------------------------- TMA producer
-      // the tap weights are static: their loads start before the programmatic-dependency wait
-      mbar_expect_tx(b_full, Cfg::b_bytes(s));
-      for (int t = 0; t < s.n_taps; ++t)
-        for (int kb = 0; kb < kbs; ++kb)
-          tma_load_2d(b_res + (t * kbs + kb) * Cfg::kBTile, &tmB, b_full, kb * kBlockK, t * s.cout);
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one()) {
+      // ------------------------------------------------------------ TMA producer
       pdl_wait();
-      int stage = 0;
-      uint32_t phase = 0;
-      const int tx = Cfg::halo_rows(s) * 128;
-      const int lead = (s.n_taps / 2) * s.dil;
+      int ia = 0, ib = 0;
+      uint32_t pa = 0, pb = 0;
+      auto load_b = [&](const CUtensorMap* m, int k0, int row) {
+        mbar_wait(&empty_b[ib], pb ^ 1);
+        mbar_expect_tx(&full_b[ib], Cfg::kStageB);
+        tma_load_2d(ring_b + ib * Cfg::kStageB, m, &full_b[ib], k0, row);
+        if (++ib == Cfg::kStagesB) {
+          ib = 0;
+          pb ^= 1;
+        }
+      };
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const int batch = tile / m_tiles;
         const int m0 = (tile - batch * m_tiles) * kBlockM;
-        for (int kb = 0; kb < kbs; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          mbar_expect_tx(&full_bar[stage], tx);
-          tma_load_4d(smem + stage * slot, &tmA, &full_bar[stage], kb * kBlockK, 0, m0 - lead, batch);
-          if (++stage == n_stages) {
-            stage = 0;
-            phase ^= 1;
+        for (int kb = 0; kb < n_kb; ++kb) {
+          mbar_wait(&empty_a[ia], pa ^ 1);
+          mbar_expect_tx(&full_a[ia], halo_rows * 128);
+          tma_load_4d(slot_a + ia * Cfg::kSlotA, &tmA, &full_a[ia], kb * kBlockK, 0, m0 + halo0, batch);
+          if (++ia == Cfg::kStagesA) {
+            ia = 0;
+            pa ^= 1;
           }
+          for (int tap = 0; tap < s.n_taps; ++tap) load_b(&tmB, kb * kBlockK, tap * s.N);
         }
+        if constexpr (FUSE)
+          for (int kb = 0; kb < BN / kBlockK; ++kb) load_b(&tmB1, kb * kBlockK, 0);
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      // ---------------------------------------------------------------- MMA issuer
-      constexpr uint32_t idesc = make_idesc_f16(kBlockM, Cfg::kBN, BF16);
-      const uint32_t b_addr0 = smem_u32(b_res);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      mbar_wait(b_full, 0);
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * Cfg::kBN;
-        for (int kb = 0; kb < kbs; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + stage * slot);
-          for (int t = 0; t < s.n_taps; ++t) {
-            const uint32_t a_tap = a_addr + t * s.dil * 128;
-            const uint32_t b_tap = b_addr0 + (t * kbs + kb) * Cfg::kBTile;
+  } else {
+    setmaxnreg_inc<232>();
+    pdl_wait();
+    // ------------------------------------------------------------ MMA + epilogue warpgroups
+    const int cw = wg - 1;
+    const uint32_t tid = threadIdx.x & 127;
+    float acc[BN / 2];
+    int ia = 0, ib = 0;
+    uint32_t pa = 0, pb = 0;
+    // one wgmma group per weight stage; a stage is released once the next group is issued and the previous retired
+    auto mma_stage = [&](uint32_t a_addr, bool first) {
+      mbar_wait(&full_b[ib], pb);
+      const uint32_t b_addr = smem_u32(ring_b + ib * Cfg::kStageB);
+      wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-              const uint64_t da = make_desc_kmajor_sw128(a_tap + k * kUmmaK * 2);
-              const uint64_t db = make_desc_kmajor_sw128(b_tap + k * kUmmaK * 2);
-              umma_f16_ss(d_tmem, da, db, idesc, (kb | t | k) != 0 ? 1u : 0u);
-            }
-          }
-          umma_commit(&empty_bar[stage]);
-          if (++stage == n_stages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(&tfull_bar[acc]);
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
+      for (int k = 0; k < kBlockK / kWgmmaK; ++k) {
+        const uint32_t a = a_addr + k * kWgmmaK * 2;
+        wgmma_ss<BN, BF16>(acc, make_desc_kmajor_sw128(a),
+                           make_desc_kmajor_sw128(b_addr + k * kWgmmaK * 2), (!first || k != 0) ? 1u : 0u);
       }
-    }
-  } else if (warp >= 4) {
-    // ------------------------------------------------------------------ epilogue
-    const int q = warp & 3;
-    int acc = 0;
-    uint32_t acc_phase = 0;
+      wgmma_commit();
+    };
+    auto retire = [&](int& prev) {   // after mma_stage: retire the previous group and free its stage
+      wgmma_wait<1>(acc);
+      if (prev >= 0 && tid == 0) mbar_arrive(&empty_b[prev]);
+      prev = ib;
+      if (++ib == Cfg::kStagesB) {
+        ib = 0;
+        pb ^= 1;
+      }
+    };
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int batch = tile / m_tiles;
       const int m0 = (tile - batch * m_tiles) * kBlockM;
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      EpiCtx c;
-      c.l = m0 + q * 32 + lane;
-      c.batch = batch;
-      c.row = batch * s.L + c.l;
-      c.valid = c.l < s.L;
-      c.l0 = m0 + q * 32;
-      c.L = s.L;
-      c.lane = lane;
-      c.stage = nullptr;
-      c.col0 = 0;
-      uint32_t r[32];
-      tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * Cfg::kBN, r);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-      Epi::apply(ep, c, r);
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
+      // conv (k taps) over the halo slots
+      for (int kb = 0; kb < n_kb; ++kb) {
+        mbar_wait(&full_a[ia], pa);
+        const uint32_t a_base = smem_u32(slot_a + ia * Cfg::kSlotA) + cw * 64 * 128;
+        int prev = -1;
+        for (int tap = 0; tap < s.n_taps; ++tap) {
+          mma_stage(a_base + tap * s.dil * 128, kb == 0 && tap == 0);
+          retire(prev);
+        }
+        wgmma_wait<0>(acc);
+        if (tid == 0) {
+          mbar_arrive(&empty_b[prev]);
+          mbar_arrive(&empty_a[ia]);
+        }
+        if (++ia == Cfg::kStagesA) {
+          ia = 0;
+          pa ^= 1;
+        }
       }
+      if constexpr (FUSE) {
+        named_bar_sync(3, 256);   // both warpgroups have read the previous tile's accumulator staging (same region)
+        // acc -> + bias7 -> snake2 -> 16-bit -> rows [64 cw, 64 cw + 64) of the A2 tile (K-major, 128B-swizzled atoms)
+        const int fr = 64 * cw + 16 * (warp & 3) + (lane >> 2), fc = 2 * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int col = 8 * j + fc;
+          const float b0 = pre.bias7 ? __ldg(pre.bias7 + col) : 0.f, b1 = pre.bias7 ? __ldg(pre.bias7 + col + 1) : 0.f;
+          const float a0 = __ldg(pre.sn2_a + col), a1 = __ldg(pre.sn2_a + col + 1);
+          const float i0 = __ldg(pre.sn2_ib + col), i1 = __ldg(pre.sn2_ib + col + 1);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int r = fr + 8 * h;
+            const uint32_t v = Op16<BF16>::pack(snake_fast(acc[4 * j + 2 * h] + b0, a0, i0),
+                                                snake_fast(acc[4 * j + 2 * h + 1] + b1, a1, i1));
+            const int chunk = (col & 63) >> 3;
+            *reinterpret_cast<uint32_t*>(shared + (col >> 6) * (kBlockM * 128) + r * 128 + ((chunk ^ (r & 7)) << 4) +
+                                         (col & 7) * 2) = v;
+          }
+        }
+        fence_proxy_async_smem();   // generic-proxy stores -> visible to the tensor core's reads
+        named_bar_sync(1 + cw, 128);
+        // 1x1 convolution: K = BN channels, A2 rows of this warpgroup, weights through the ring
+        int prev = -1;
+        const uint32_t a2 = smem_u32(shared) + cw * 64 * 128;
+        for (int kb = 0; kb < BN / kBlockK; ++kb) {
+          mma_stage(a2 + kb * kBlockM * 128, kb == 0);
+          retire(prev);
+        }
+        wgmma_wait<0>(acc);
+        if (tid == 0) mbar_arrive(&empty_b[prev]);
+        named_bar_sync(3, 256);   // both warpgroups' second chains have read A2: the region becomes the staging
+      }
+      float* epi_st = Epi::kStageBytes > 0
+                          ? reinterpret_cast<float*>(epi_smem + (warp - 4) * Epi::kStageBytes)
+                          : nullptr;
+      gemm_tile_epilogue<Epi, BN>(acc, reinterpret_cast<float*>(shared + cw * Cfg::kAccStage), epi_st, ep, s.L, s.N,
+                                  m0, 0, 0, batch, cw, warp, lane);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 2 * Cfg::kBN);
   }
 }
 
-template <class Epi, bool BF16>
-int launch_conv_halo(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvHaloShape& s, const typename Epi::Params& ep,
-                     cudaStream_t stream) {
-  using Cfg = ConvHaloCfg;
-  static_assert(Epi::kCols == 32 && Epi::kStageBytes == 0, "conv_halo epilogue: one 32-column chunk, no staging");
-  auto kern = conv_halo_kernel<Epi, BF16>;
-  const int smem = Cfg::stages(s) * Cfg::slot_bytes(s) + Cfg::b_bytes(s) + 256 + 1024;
-  SATB_REQUIRE(s.K % kBlockK == 0 && s.cout <= Cfg::kBN && Cfg::halo_rows(s) <= 256 && Cfg::stages(s) >= 2,
-               "conv_halo: unsupported shape");
-  SATB_REQUIRE(smem <= Cfg::kSmemBudget + 4096, "conv_halo: shared-memory request too large");
-  static PerDeviceOnce attr;   // once per device, to the largest size any shape may ask for
-  if (attr.first()) SATB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBudget + 4096));
+template <class Epi, int BN, bool BF16, bool FUSE>
+int launch_conv_halo(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap* tmB1, const HaloShape& s,
+                     const ResUnitPre& pre, const typename Epi::Params& ep, cudaStream_t stream) {
+  using Cfg = HaloCfg<BN, Epi::kCols, Epi::kStageBytes, FUSE>;
+  SATB_REQUIRE(s.K % kBlockK == 0 && s.n_taps % 2 == 1 && (s.n_taps - 1) * s.dil <= kHaloMax && s.N <= BN,
+               "halo convolution: unsupported shape");
+  SATB_REQUIRE(!FUSE || (tmB1 != nullptr && s.N == BN && s.K == BN && pre.sn2_a && pre.sn2_ib),
+               "fused ResidualUnit: needs the 1x1 weights, channels = tile width, and snake2");
+  auto kern = conv_halo_wgmma_kernel<Epi, BN, BF16, FUSE>;
+  static PerDeviceOnce attr;
+  if (attr.first()) SATB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
   const int total = ceil_div(s.L, kBlockM) * s.batches;
   if (total <= 0) return 0;
   int grid = device_sm_count();
   if (grid > total) grid = total;
-  SATB_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(Cfg::kThreads), smem, stream, tmA, tmB, s, ep));
+  SATB_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tmA, tmB, tmB1 ? *tmB1 : tmB,
+                             s, pre, ep));
   count_launch();
   return 0;
 }

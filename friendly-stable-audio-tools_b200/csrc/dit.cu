@@ -80,18 +80,6 @@ static int linear(TmapCache& tc, const void* A, int64_t lda, int M, int K, const
   GemmShape s;
   s.L = M; s.batches = 1; s.N = N; s.K = K; s.n_taps = 1; s.tap_base = 0; s.tap_step = 0; s.b_tap_rows = N; s.stride = 1;
   s.b_static = 1;   // W is a weight matrix prepared at finalize time
-  if constexpr (BN == 256 || BN == 128) {
-    // CTA-pair kernel (256 x BN tiles, half of B per CTA).  Also for BN = 128: a single CTA streaming
-    // 128 x 128 x 16 MMAs needs 128 B/clk of shared-memory operand reads, the SM's limit; the pair needs 96.
-    // (Choosing single CTAs where they save a round of the persistent grid -- QKV: 594 pair tiles = 8.03 -> 9
-    // rounds vs 1170 single tiles = 7.9 -> 8 -- was measured ~3 % slower: the pair's lower smem traffic wins.
-    // 192-wide pair tiles -- 792 tiles = 10.7 -> 11 rounds of 3/4 the work = 8.25 -- measured 6 % slower as well,
-    // 2.66 vs 2.50 ms per step: A is re-read a third more often.)
-    if (gemm_use_2cta() && M >= 1024) {
-      SATB_PROPAGATE(tc.get_b(W, K, N, K, BN / 2, &tb));
-      return launch_gemm_2cta<Epi, BN, BF16>(*ta, *tb, s, ep, stream);
-    }
-  }
   SATB_PROPAGATE(tc.get_b(W, K, N, K, BN, &tb));
   return launch_gemm<Epi, BN, BF16>(*ta, *tb, s, ep, stream);
 }

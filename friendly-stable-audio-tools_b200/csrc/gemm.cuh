@@ -1,4 +1,4 @@
-// tcgen05 / TMA / TMEM GEMM for sm_100a with fused epilogues.
+// wgmma / TMA GEMM for sm_90a with fused epilogues.
 //
 //   C[row, n] = sum_{tap, k} A[batch, l + tap_base + tap*tap_step, k] * B[tap*b_tap_rows + n, k]
 //
@@ -6,16 +6,13 @@
 // 4-D TMA tensor map (position = row*stride + phase; out-of-range rows are zero-filled
 // by TMA, which is how convolution padding and the ragged M tail are handled); B is the
 // K-major weight matrix [taps * N, K].  A plain Linear layer is n_taps = 1,
-// batches = 1.  Accumulation is fp32 in TMEM.
+// batches = 1.  Accumulation is fp32 in registers.
 //
-// Structure (one persistent CTA per SM, 384 threads):
-//   warp 0    TMA producer      global -> 128B-swizzled smem ring (mbarrier full/empty)
-//   warp 1    MMA issuer        one thread issues tcgen05.mma 128xBNx16, commits to mbarriers
-//   warp 2    TMEM allocator    2 x BN fp32 columns (double-buffered accumulator)
-//   warps 4-11 epilogue         two warps per TMEM lane quadrant (interleaved column chunks):
-//                               tcgen05.ld 32 lanes x 32 columns -> registers -> fused op -> global,
-//                               software-pipelined (the load of chunk c+1 overlaps the math of c)
-// The accumulator is double-buffered so the epilogue of tile i overlaps the MMAs of tile i+1.
+// Structure (one persistent CTA per SM, 384 threads, 128 x BN tiles):
+//   warpgroup 0      TMA producer      one thread: global -> 128B-swizzled smem ring (mbarrier full/empty)
+//   warpgroups 1, 2  MMA + epilogue    64 rows each: wgmma 64xBNx16 from the smem ring into registers, then the
+//                                      fused epilogue (accumulator -> smem -> one row per thread -> fused op -> global)
+// The producer runs ahead into the next tile's k-blocks while the epilogue of the current one runs.
 #pragma once
 #include <type_traits>
 
@@ -50,21 +47,23 @@ struct GemmShape {
 
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;   // 64 x 16-bit = 128 B = one swizzle atom row
-constexpr int kUmmaK = 16;
-constexpr int kGemmThreads = 384;   // 4 control warps + 8 epilogue warps
-constexpr int kSmemBudget = 220 * 1024;
+constexpr int kWgmmaK = 16;
+constexpr int kGemmThreads = 384;   // producer warpgroup + 2 MMA / epilogue warpgroups
+constexpr int kSmemBudget = 227 * 1024;   // the most shared memory a block may use on sm_90
 
 constexpr int kEpiWarps = 8;
-template <int BN, int kEpiStage = 0>   // kEpiStage: bytes of epilogue staging smem per epilogue warp
+template <int BN, int kCols, int kEpiStage = 0>   // kEpiStage: bytes of epilogue staging smem per epilogue warp
 struct GemmCfg {
   static constexpr int kStageA = kBlockM * kBlockK * 2;
   static constexpr int kStageB = BN * kBlockK * 2;
   static constexpr int kStage = kStageA + kStageB;
-  static constexpr int kAvail = kSmemBudget - 1024 - kEpiWarps * kEpiStage;
-  static constexpr int kStages = kAvail / kStage > 8 ? 8 : kAvail / kStage;
-  static constexpr int kTmemCols = 2 * BN < 32 ? 32 : 2 * BN;
-  static constexpr int kSmemBytes = kStages * kStage + 1024 /*align slack*/ + 256 /*barriers*/ + kEpiWarps * kEpiStage;
+  static constexpr int kAccLd = kCols + 4;              // fp32 row pitch of the accumulator staging tile
+  static constexpr int kAccStage = 2 * 64 * kAccLd * 4;  // per MMA warpgroup: two column chunks of its 64 rows
+  static constexpr int kFixed = 1024 /*align slack*/ + 256 /*barriers*/ + 2 * kAccStage + kEpiWarps * kEpiStage;
+  static constexpr int kStages = (kSmemBudget - kFixed) / kStage > 8 ? 8 : (kSmemBudget - kFixed) / kStage;
+  static constexpr int kSmemBytes = kStages * kStage + kFixed;
   static_assert(BN == 64 || BN == 128 || BN == 256, "BN must be 64/128/256");
+  static_assert(kStages >= 2, "shared memory too small for a two-stage ring");
 };
 
 struct EpiCtx {
@@ -107,22 +106,86 @@ struct EpiTile {
   }
 };
 
+// Epilogue of one 128 x BN tile, run by MMA warpgroup cw (rows [64 cw, 64 cw + 64)) on its accumulator fragment.
+// The accumulator goes through shared memory (acc_st: 2 x 64 x (kCols + 4) fp32 per warpgroup) two column chunks at a
+// time, so that every epilogue thread receives kCols consecutive columns of ONE row (thread = row, as the epilogues
+// expect).  epi_st: the epilogue's own per-warp staging (Epi::kStageBytes), or null.
+template <class Epi, int BN>
+__device__ __forceinline__ void gemm_tile_epilogue(const float (&acc)[BN / 2], float* acc_st, float* epi_st,
+                                                   const typename Epi::Params& ep, int L, int N, int m0, int n0, int nt,
+                                                   int batch, int cw, int warp, int lane) {
+  const int wq = warp & 3;           // warp within the warpgroup
+  const int half = wq >> 1;          // warps 0, 1 take the even column chunks, warps 2, 3 the odd ones
+  const int rsub = (wq & 1) * 32;    // rows [rsub, rsub + 32) of the warpgroup's 64
+  const int fr = 16 * wq + (lane >> 2);   // accumulator fragment rows fr, fr + 8
+  const int fc = 2 * (lane & 3);          // and columns 8 j + fc, + 1
+  constexpr int kChunks = BN / Epi::kCols;
+  constexpr int kLd = Epi::kCols + 4;
+  EpiCtx c;
+  c.l0 = m0 + 64 * cw + rsub;
+  c.l = c.l0 + lane;
+  c.batch = batch;
+  c.row = batch * L + c.l;
+  c.valid = c.l < L;
+  c.L = L;
+  c.lane = lane;
+  c.n_tile = nt;
+  c.half = half;
+  c.stage = epi_st;
+  int n_valid = (N - n0 + Epi::kCols - 1) / Epi::kCols;   // chunks that hold real columns (warp-uniform)
+  if (n_valid > kChunks) n_valid = kChunks;
+  typename EpiTile<Epi>::State est;
+  EpiTile<Epi>::begin(ep, c, est);
+#pragma unroll
+  for (int cp = 0; cp < (kChunks + 1) / 2; ++cp) {
+    named_bar_sync(1 + cw, 128);   // the previous chunk pair has been read out
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int ch = 2 * cp + hh;
+      if (ch < kChunks) {
+        float* dst = acc_st + hh * 64 * kLd;
+#pragma unroll
+        for (int j = 0; j < Epi::kCols / 8; ++j) {
+          const int ai = (ch * (Epi::kCols / 8) + j) * 4;
+          *reinterpret_cast<float2*>(dst + fr * kLd + 8 * j + fc) = make_float2(acc[ai], acc[ai + 1]);
+          *reinterpret_cast<float2*>(dst + (fr + 8) * kLd + 8 * j + fc) = make_float2(acc[ai + 2], acc[ai + 3]);
+        }
+      }
+    }
+    named_bar_sync(1 + cw, 128);
+    const int ci = 2 * cp + half;
+    if (ci < n_valid) {
+      uint32_t r[Epi::kCols];
+      const float4* src = reinterpret_cast<const float4*>(acc_st + half * 64 * kLd + (rsub + lane) * kLd);
+#pragma unroll
+      for (int j = 0; j < Epi::kCols / 4; ++j) {
+        const float4 v = src[j];
+        r[4 * j] = __float_as_uint(v.x);
+        r[4 * j + 1] = __float_as_uint(v.y);
+        r[4 * j + 2] = __float_as_uint(v.z);
+        r[4 * j + 3] = __float_as_uint(v.w);
+      }
+      c.col0 = n0 + ci * Epi::kCols;
+      EpiTile<Epi>::apply(ep, c, r, est);
+    }
+  }
+  EpiTile<Epi>::end(ep, c, est);
+}
 template <class Epi, int BN, bool BF16>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                    const __grid_constant__ CUtensorMap tmA2, const GemmShape s, const typename Epi::Params ep) {
-  using Cfg = GemmCfg<BN, Epi::kStageBytes>;
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                  const __grid_constant__ CUtensorMap tmA2, const GemmShape s, const typename Epi::Params ep) {
+  using Cfg = GemmCfg<BN, Epi::kCols, Epi::kStageBytes>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStage);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + Cfg::kStages;
-  uint64_t* tfull_bar = bars + 2 * Cfg::kStages;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
+  uint8_t* epi_smem = smem + Cfg::kStages * Cfg::kStage + 256;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
 
   const int m_tiles = (s.L + kBlockM - 1) / kBlockM;
   const int n_tiles = (s.N + BN - 1) / BN;
@@ -137,31 +200,19 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     tma_prefetch_desc(&tmB);
     for (int i = 0; i < Cfg::kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 8);
+      mbar_init(&empty_bar[i], 2);   // one arrival per MMA warpgroup
     }
     fence_mbar_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, Cfg::kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_launch_dependents();   // the next kernel may be scheduled as SMs drain
   // Everything above overlapped the previous kernel's tail.  The B operand (weights) never depends on the
   // previous kernel, so the producer thread also starts the B loads of its first stages before it waits for
-  // the dependency; every other thread waits here.
-  const bool is_producer_warp = warp == 0;
-  if (!is_producer_warp) pdl_wait();
+  // the dependency; the MMA warpgroups wait right away.
 
-  if (warp == 0) {
-    if (elect_one()) {
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one()) {
       // ------------------------------------------------------------ TMA producer
       int pre = 0;
       if (s.b_static && static_cast<int>(blockIdx.x) < total_tiles) {
@@ -212,351 +263,50 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         }
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      // -------------------------------------------------------------- MMA issuer
-      constexpr uint32_t idesc = make_idesc_f16(kBlockM, BN, BF16);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + stage * Cfg::kStage);
-          const uint32_t b_addr = a_addr + Cfg::kStageA;
-#pragma unroll
-          for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-            const uint64_t da = make_desc_kmajor_sw128(a_addr + k * kUmmaK * 2);
-            const uint64_t db = make_desc_kmajor_sw128(b_addr + k * kUmmaK * 2);
-            umma_f16_ss(d_tmem, da, db, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);
-          if (++stage == Cfg::kStages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(&tfull_bar[acc]);
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
-      }
-    }
-  } else if (warp >= 4) {
-    // ------------------------------------------------------------------ epilogue
-    const int q = warp & 3;            // TMEM lane quadrant == warp % 4
-    const int half = (warp - 4) >> 2;  // two warps per quadrant take alternate column chunks
-    constexpr int kChunks = BN / Epi::kCols;
-    int acc = 0;
-    uint32_t acc_phase = 0;
+  } else {
+    setmaxnreg_inc<232>();
+    pdl_wait();
+    // ------------------------------------------------------------ MMA + epilogue warpgroups
+    const int cw = wg - 1;             // rows [64 cw, 64 cw + 64) of the tile
+    float* acc_st = reinterpret_cast<float*>(epi_smem + cw * Cfg::kAccStage);
+    float* epi_st = Epi::kStageBytes > 0
+                        ? reinterpret_cast<float*>(epi_smem + 2 * Cfg::kAccStage + (warp - 4) * Epi::kStageBytes)
+                        : nullptr;
+    float acc[BN / 2];
+    int stage = 0;
+    uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int nt = tile / tiles_per_n;
       const int rem = tile - nt * tiles_per_n;
       const int batch = rem / m_tiles;
       const int m0 = (rem - batch * m_tiles) * kBlockM;
       const int n0 = nt * BN;
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      EpiCtx c;
-      c.l = m0 + q * 32 + lane;
-      c.batch = batch;
-      c.row = batch * s.L + c.l;
-      c.valid = c.l < s.L;
-      c.l0 = m0 + q * 32;
-      c.L = s.L;
-      c.lane = lane;
-      c.n_tile = nt;
-      c.half = half;
-      c.stage = Epi::kStageBytes > 0
-                    ? reinterpret_cast<float*>(smem + Cfg::kStages * Cfg::kStage + 256 + (warp - 4) * Epi::kStageBytes)
-                    : nullptr;
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * BN;
-      int n_valid = (s.N - n0 + Epi::kCols - 1) / Epi::kCols;   // chunks that hold real columns (warp-uniform)
-      if (n_valid > kChunks) n_valid = kChunks;
-      uint32_t r0[Epi::kCols], r1[Epi::kCols];
-      auto load_chunk = [&](int ci, uint32_t (&dst)[Epi::kCols]) {
+      // mainloop: one wgmma group per k-block; the smem slot of k-block kb - 1 is released once group kb is issued
+      // and group kb - 1 has retired
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t a_addr = smem_u32(smem + stage * Cfg::kStage) + cw * 64 * kBlockK * 2;
+        const uint32_t b_addr = smem_u32(smem + stage * Cfg::kStage) + Cfg::kStageA;
+        wgmma_fence();
 #pragma unroll
-        for (int j = 0; j < Epi::kCols / 32; ++j) {
-          uint32_t(&rj)[32] = *reinterpret_cast<uint32_t(*)[32]>(&dst[j * 32]);
-          tmem_ld_32x32(t_row + ci * Epi::kCols + j * 32, rj);
-        }
-      };
-      typename EpiTile<Epi>::State est;
-      EpiTile<Epi>::begin(ep, c, est);
-      if (half < n_valid) {
-        load_chunk(half, r0);
-        tmem_ld_wait();
-      }
-#pragma unroll 1
-      for (int ci = half; ci < n_valid; ci += 4) {
-        const bool has1 = ci + 2 < n_valid;
-        if (has1) load_chunk(ci + 2, r1);
-        c.col0 = n0 + ci * Epi::kCols;
-        EpiTile<Epi>::apply(ep, c, r0, est);
-        tmem_ld_wait();
-        if (has1) {
-          if (ci + 4 < n_valid) load_chunk(ci + 4, r0);
-          c.col0 = n0 + (ci + 2) * Epi::kCols;
-          EpiTile<Epi>::apply(ep, c, r1, est);
-          tmem_ld_wait();
+        for (int k = 0; k < kBlockK / kWgmmaK; ++k)
+          wgmma_ss<BN, BF16>(acc, make_desc_kmajor_sw128(a_addr + k * kWgmmaK * 2),
+                             make_desc_kmajor_sw128(b_addr + k * kWgmmaK * 2), (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>(acc);
+        if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == Cfg::kStages) {
+          stage = 0;
+          phase ^= 1;
         }
       }
-      EpiTile<Epi>::end(ep, c, est);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::kTmemCols);
-  }
-}
+      wgmma_wait<0>(acc);
+      if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
 
-// ---------------------------------------------------------------- CTA-pair variant
-// Same pipeline with two CTAs (one cluster, one TPC) cooperating on a 256 x BN tile through
-// tcgen05.mma.cta_group::2: each CTA loads its own 128 A rows and HALF of the B tile, so the
-// shared-memory traffic per MMA cycle drops from 96 to 64 B/clk per SM and the ring holds 6 stages.
-// CTA 0 issues the MMAs for the pair; the smem-slot and accumulator barriers are signalled in
-// both CTAs by multicast commits; CTA 1's epilogue warps release the accumulator on CTA 0's barrier.
-template <int BN, int kEpiStage = 0>
-struct Gemm2Cfg {
-  static constexpr int kStageA = kBlockM * kBlockK * 2;
-  static constexpr int kStageB = (BN / 2) * kBlockK * 2;
-  static constexpr int kStage = kStageA + kStageB;
-  static constexpr int kAvail = kSmemBudget - 1024 - kEpiWarps * kEpiStage;
-  static constexpr int kStages = kAvail / kStage > 8 ? 8 : kAvail / kStage;
-  static constexpr int kTmemCols = 2 * BN;
-  static constexpr int kSmemBytes = kStages * kStage + 1024 + 256 + kEpiWarps * kEpiStage;
-  static_assert(BN == 256 || BN == 128, "BN must be 128/256");
-};
-
-template <class Epi, int BN, bool BF16>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kGemmThreads, 1)
-gemm_tcgen05_2cta_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                         const __grid_constant__ CUtensorMap tmA2, const GemmShape s, const typename Epi::Params ep) {
-  using Cfg = Gemm2Cfg<BN, Epi::kStageBytes>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStage);
-  uint64_t* full_bar = bars;                     // used in CTA 0 only (credited by both CTAs' TMA)
-  uint64_t* empty_bar = bars + Cfg::kStages;     // per CTA, multicast-committed
-  uint64_t* tfull_bar = bars + 2 * Cfg::kStages; // per CTA, multicast-committed
-  uint64_t* tempty_bar = tfull_bar + 2;          // CTA 0's is the one the MMA thread waits on (16 arrivals)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const int cluster_id = blockIdx.x >> 1, n_clusters = gridDim.x >> 1;
-
-  const int m_tiles = (s.L + 2 * kBlockM - 1) / (2 * kBlockM);   // 256-row pair tiles
-  const int n_tiles = (s.N + BN - 1) / BN;
-  const int tiles_per_n = m_tiles * s.batches;
-  const int total_tiles = tiles_per_n * n_tiles;
-  const int kb_per_tap = (s.K + kBlockK - 1) / kBlockK;
-  const int kb_per_part = kb_per_tap * s.n_taps;
-  const int num_kb = kb_per_part * s.n_parts;
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int i = 0; i < Cfg::kStages; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
+      gemm_tile_epilogue<Epi, BN>(acc, acc_st, epi_st, ep, s.L, s.N, m0, n0, nt, batch, cw, warp, lane);
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 16);
-    }
-    fence_mbar_init();
-  }
-  cluster_sync_all();   // both CTAs' barriers exist before any remote arrive / TMA credit
-  if (warp == 2) {
-    tmem_alloc_2sm(tmem_slot, Cfg::kTmemCols);
-    tmem_relinquish_2sm();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_launch_dependents();
-  if (warp != 0) pdl_wait();   // the producer warp first prefetches weights (see the single-CTA kernel)
-
-  if (warp == 0) {
-    if (elect_one()) {
-      // ------------------------------------------------------ TMA producer (both CTAs)
-      int pre = 0;
-      if (s.b_static && cluster_id < total_tiles) {
-        pre = num_kb < Cfg::kStages ? num_kb : Cfg::kStages;
-        const int n0 = (cluster_id / tiles_per_n) * BN + rank * (BN / 2);
-        for (int kb = 0; kb < pre; ++kb) {
-          const int pidx = kb / kb_per_part, kbp = kb - pidx * kb_per_part;
-          const int part = split_part(pidx, s.n_parts);
-          const int tap = kbp / kb_per_tap;
-          const int k0 = (kbp - tap * kb_per_tap) * kBlockK;
-          if (rank == 0) mbar_expect_tx(&full_bar[kb], 2 * Cfg::kStage);
-          tma_load_2d_2sm(smem + kb * Cfg::kStage + Cfg::kStageA, &tmB, &full_bar[kb], k0,
-                          tap * s.b_tap_rows + n0 + (part == 2 ? s.b_part_rows : 0));
-        }
-      }
-      pdl_wait();
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = cluster_id; tile < total_tiles; tile += n_clusters) {
-        const int nt = tile / tiles_per_n;
-        const int rem = tile - nt * tiles_per_n;
-        const int batch = rem / m_tiles;
-        const int m0 = (rem - batch * m_tiles) * 2 * kBlockM + rank * kBlockM;
-        const int n0 = nt * BN + rank * (BN / 2);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          const int pidx = kb / kb_per_part, kbp = kb - pidx * kb_per_part;
-          const int part = split_part(pidx, s.n_parts);
-          const int tap = kbp / kb_per_tap;
-          const int k0 = (kbp - tap * kb_per_tap) * kBlockK;
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * Cfg::kStage;
-          uint8_t* sb = sa + Cfg::kStageA;
-          const bool b_done = tile == cluster_id && kb < pre;
-          if (rank == 0 && !b_done) mbar_expect_tx(&full_bar[stage], 2 * Cfg::kStage);
-          const int u = s.tap_base + tap * s.tap_step;
-          int ph = 0, ro = u;
-          if (s.stride > 1) {
-            ro = (u >= 0) ? u / s.stride : -((-u + s.stride - 1) / s.stride);
-            ph = u - ro * s.stride;
-          }
-          tma_load_4d_2sm(sa, part == 1 ? &tmA2 : &tmA, &full_bar[stage], k0, ph, m0 + ro, batch);
-          if (!b_done)
-            tma_load_2d_2sm(sb, &tmB, &full_bar[stage], k0, tap * s.b_tap_rows + n0 + (part == 2 ? s.b_part_rows : 0));
-          if (++stage == Cfg::kStages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (rank == 0 && elect_one()) {
-      // ------------------------------------------------------ MMA issuer (CTA 0 for the pair)
-      constexpr uint32_t idesc = make_idesc_f16(2 * kBlockM, BN, BF16);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = cluster_id; tile < total_tiles; tile += n_clusters) {
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + stage * Cfg::kStage);
-          const uint32_t b_addr = a_addr + Cfg::kStageA;
-#pragma unroll
-          for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-            const uint64_t da = make_desc_kmajor_sw128(a_addr + k * kUmmaK * 2);
-            const uint64_t db = make_desc_kmajor_sw128(b_addr + k * kUmmaK * 2);
-            umma_f16_ss_2sm(d_tmem, da, db, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit_2sm(&empty_bar[stage]);
-          if (++stage == Cfg::kStages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit_2sm(&tfull_bar[acc]);
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
-      }
-    }
-  } else if (warp >= 4) {
-    // ------------------------------------------------------------------ epilogue (both CTAs)
-    const int q = warp & 3;
-    const int half = (warp - 4) >> 2;
-    constexpr int kChunks = BN / Epi::kCols;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = cluster_id; tile < total_tiles; tile += n_clusters) {
-      const int nt = tile / tiles_per_n;
-      const int rem = tile - nt * tiles_per_n;
-      const int batch = rem / m_tiles;
-      const int m0 = (rem - batch * m_tiles) * 2 * kBlockM + rank * kBlockM;
-      const int n0 = nt * BN;
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      EpiCtx c;
-      c.l = m0 + q * 32 + lane;
-      c.batch = batch;
-      c.row = batch * s.L + c.l;
-      c.valid = c.l < s.L;
-      c.l0 = m0 + q * 32;
-      c.L = s.L;
-      c.lane = lane;
-      c.n_tile = nt;
-      c.half = half;
-      c.stage = Epi::kStageBytes > 0
-                    ? reinterpret_cast<float*>(smem + Cfg::kStages * Cfg::kStage + 256 + (warp - 4) * Epi::kStageBytes)
-                    : nullptr;
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * BN;
-      int n_valid = (s.N - n0 + Epi::kCols - 1) / Epi::kCols;
-      if (n_valid > kChunks) n_valid = kChunks;
-      uint32_t r0[Epi::kCols], r1[Epi::kCols];
-      auto load_chunk = [&](int ci, uint32_t (&dst)[Epi::kCols]) {
-#pragma unroll
-        for (int j = 0; j < Epi::kCols / 32; ++j) {
-          uint32_t(&rj)[32] = *reinterpret_cast<uint32_t(*)[32]>(&dst[j * 32]);
-          tmem_ld_32x32(t_row + ci * Epi::kCols + j * 32, rj);
-        }
-      };
-      typename EpiTile<Epi>::State est;
-      EpiTile<Epi>::begin(ep, c, est);
-      if (half < n_valid) {
-        load_chunk(half, r0);
-        tmem_ld_wait();
-      }
-#pragma unroll 1
-      for (int ci = half; ci < n_valid; ci += 4) {
-        const bool has1 = ci + 2 < n_valid;
-        if (has1) load_chunk(ci + 2, r1);
-        c.col0 = n0 + ci * Epi::kCols;
-        EpiTile<Epi>::apply(ep, c, r0, est);
-        tmem_ld_wait();
-        if (has1) {
-          if (ci + 4 < n_valid) load_chunk(ci + 4, r0);
-          c.col0 = n0 + (ci + 2) * Epi::kCols;
-          EpiTile<Epi>::apply(ep, c, r1, est);
-          tmem_ld_wait();
-        }
-      }
-      EpiTile<Epi>::end(ep, c, est);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(&tempty_bar[acc], 0);   // the pair's accumulator lock lives in CTA 0
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
-    }
-  }
-  tc_fence_before();
-  cluster_sync_all();   // no CTA may free TMEM / exit while its peer can still signal it
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem_base, Cfg::kTmemCols);
   }
 }
 
@@ -1013,8 +763,7 @@ __device__ __forceinline__ float snake_fast(float v, float a, float ib) {
   return fmaf(ib, sn * sn, v);
 }
 
-// Packed fp32x2 arithmetic (Blackwell FADD2 / FMUL2 / FFMA2: one issue slot for two lanes' worth of
-// work) for the convolution epilogues, which are issue-bound rather than FMA-throughput-bound.
+// fp32 pairs in one 64-bit register (two lanes of a 4-element segment) for the convolution epilogues.
 __device__ __forceinline__ uint64_t f2_pack(float lo, float hi) {
   uint64_t d;
   asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "f"(lo), "f"(hi));
@@ -1024,19 +773,23 @@ __device__ __forceinline__ void f2_unpack(uint64_t v, float& lo, float& hi) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
 __device__ __forceinline__ uint64_t f2_add(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  f2_unpack(a, a0, a1);
+  f2_unpack(b, b0, b1);
+  return f2_pack(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 __device__ __forceinline__ uint64_t f2_mul(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  f2_unpack(a, a0, a1);
+  f2_unpack(b, b0, b1);
+  return f2_pack(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 __device__ __forceinline__ uint64_t f2_fma(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  float a0, a1, b0, b1, c0, c1;
+  f2_unpack(a, a0, a1);
+  f2_unpack(b, b0, b1);
+  f2_unpack(c, c0, c1);
+  return f2_pack(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 // snake_fast on two values at once: same operations and roundings as the scalar version.
 __device__ __forceinline__ uint64_t snake_fast2(uint64_t v, uint64_t a, uint64_t ib) {
@@ -1436,8 +1189,8 @@ int make_tmap_b(CUtensorMap* m, const void* ptr, int K, int rows, int64_t row_st
 template <class Epi, int BN, bool BF16>
 int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape& s, const typename Epi::Params& ep,
                 cudaStream_t stream, const CUtensorMap* tmA2 = nullptr) {
-  using Cfg = GemmCfg<BN, Epi::kStageBytes>;
-  auto kern = gemm_tcgen05_kernel<Epi, BN, BF16>;
+  using Cfg = GemmCfg<BN, Epi::kCols, Epi::kStageBytes>;
+  auto kern = gemm_wgmma_kernel<Epi, BN, BF16>;
   static PerDeviceOnce attr;
   if (attr.first()) SATB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
   const int m_tiles = ceil_div(s.L, kBlockM), n_tiles = ceil_div(s.N, BN);
@@ -1447,25 +1200,6 @@ int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape&
   if (grid > total) grid = total;
   SATB_REQUIRE(s.n_parts == 1 || tmA2 != nullptr, "split-operand GEMM needs the second A tensor map");
   SATB_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tmA, tmB, tmA2 ? *tmA2 : tmA, s, ep));
-  count_launch();
-  return 0;
-}
-
-template <class Epi, int BN, bool BF16>
-int launch_gemm_2cta(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape& s, const typename Epi::Params& ep,
-                     cudaStream_t stream, const CUtensorMap* tmA2 = nullptr) {
-  using Cfg = Gemm2Cfg<BN, Epi::kStageBytes>;
-  auto kern = gemm_tcgen05_2cta_kernel<Epi, BN, BF16>;
-  static PerDeviceOnce attr;
-  if (attr.first()) SATB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-  const int m_tiles = ceil_div(s.L, 2 * kBlockM), n_tiles = ceil_div(s.N, BN);
-  const int total = m_tiles * s.batches * n_tiles;
-  if (total <= 0) return 0;
-  int clusters = device_sm_count() / 2;
-  if (clusters > total) clusters = total;
-  SATB_REQUIRE(s.n_parts == 1 || tmA2 != nullptr, "split-operand GEMM needs the second A tensor map");
-  SATB_CHECK_CUDA(launch_pdl(kern, dim3(2 * clusters), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tmA, tmB,
-                             tmA2 ? *tmA2 : tmA, s, ep));
   count_launch();
   return 0;
 }

@@ -5,17 +5,15 @@
 
 namespace satb {
 
-// ---- attention_tc.cu (tcgen05)
+// ---- attention_tc.cu (tensor-core flash attention)
 int launch_attention_tc(const void* q, const void* k, const void* v, void* o, int64_t ldq, int64_t ldk, int64_t ldv,
                         int64_t ldo, int64_t q_bs, int64_t k_bs, int64_t v_bs, int64_t o_bs, int q_cols, int k_cols,
                         int v_cols, int q_col, int k_col, int v_col, int batch, int H, int H_kv, int Nq, int Nk,
-                        bool bf16, cudaStream_t stream, unsigned long long* dbg = nullptr);
-int debug_attention_occupancy(int dyn_smem, int carveout_pct);
+                        bool bf16, cudaStream_t stream);
 // debugging switches (environment variables; the defaults are the production path)
-bool conv_halo_enabled();     // SATB_CONV_HALO=off: generic 7-tap loads for the final conv (A/B debugging)
+bool conv_halo_enabled();     // SATB_CONV_HALO=off: generic per-tap loads for the final conv (A/B debugging)
+bool resunit_use_fused();      // SATB_RESUNIT=unfused runs the 128/256-channel ResidualUnits as two GEMM launches (A/B debugging)
 bool conv_epi_masked();        // SATB_CONV_EPI=general keeps the combined-epilogue GEMM kernels for the 16-bit convolutions (A/B debugging)
-bool resunit_use_fused();      // SATB_RESUNIT=unfused runs the 128-channel ResidualUnits as two GEMM launches (A/B debugging)
-bool gemm_use_2cta();          // SATB_GEMM=1cta disables the CTA-pair GEMM (A/B debugging)
 bool ln_fold_enabled();        // SATB_LN=fold: LayerNorm folded into the GEMM epilogues (A/B; measured slower, off by default)
 bool raw_stream_16bit();       // SATB_RAW=fp32 keeps the Oobleck skip stream in fp32 (A/B debugging)
 

@@ -1,10 +1,10 @@
-// Oobleck VAE encoder / decoder (reference models/autoencoders.py:45-194) on the tcgen05
+// Oobleck VAE encoder / decoder (reference models/autoencoders.py:45-194) on the wgmma
 // implicit-GEMM convolution of gemm.cuh.
 //
 // Data layout: activations are channels-last [B, L, C].  Every tensor-core convolution
 // reads a 16-bit, already Snake-activated copy of its input (written by the producer's
 // epilogue with the consumer's alpha/beta) and, where a ResidualUnit skip needs it, an fp32
-// copy of the raw value.  A dilated k=7 convolution is 7 shifted GEMMs accumulated in TMEM
+// copy of the raw value.  A dilated k=7 convolution is 7 shifted GEMMs accumulated in registers
 // (TMA zero-fills the padding); a transposed convolution (k = 2s, stride s) is a 2-tap GEMM
 // over N = s*Cout columns; a strided convolution (k = 2s, stride s) is a 2s-tap GEMM whose
 // taps address the input as (phase, row) through a 4-D tensor map.  The encoder's first
@@ -21,7 +21,6 @@
 
 #include "../../include/satb200.h"
 #include "common.cuh"
-#include "resunit.cuh"
 #include "conv_halo.cuh"
 #include "kernels.h"
 
@@ -368,20 +367,9 @@ int run_conv_gemm(SatbOobleck* h, const ConvW& cw, const void* in16, int B, int 
   }
   auto get_b = [&](int box, const CUtensorMap** out) -> int { return get_tmap_b(h, cw, b_rows, box, out); };
   const CUtensorMap* tb;
-  // CTA pairs pay off where the mainloop is long (k7 / strided convolutions: >= 3 taps).  The 1x1 convolutions and
-  // the transposed convolutions (2 taps) are epilogue-bound, and there the per-tile hand-offs between the two CTAs
-  // cost more than the halved B traffic saves: single CTAs measured 495 vs 578 us (stride 2, 128 channels), 159 vs
-  // 185 us (stride 4, 512 -> 256), 33 vs 40 and 88 vs 107 us (1x1 + skip at 1024 / 512 channels).
-  const bool pair = gemm_use_2cta() && s.L >= 512 && s.n_taps >= 3;
-  if (s.N >= 256 && pair) {
-    SATB_PROPAGATE(get_b(128, &tb));   // CTA pair: each CTA loads half of the 256-wide B tile
-    return launch_gemm_2cta<Epi, 256, BF16>(ta, *tb, s, ep, st, ta2);
-  } else if (s.N >= 256) {
+  if (s.N >= 256) {
     SATB_PROPAGATE(get_b(256, &tb));
     return launch_gemm<Epi, 256, BF16>(ta, *tb, s, ep, st, ta2);
-  } else if (s.N == 128 && pair) {
-    SATB_PROPAGATE(get_b(64, &tb));    // CTA pair on 256 x 128 tiles: halves the B traffic of the 128-channel layers
-    return launch_gemm_2cta<Epi, 128, BF16>(ta, *tb, s, ep, st, ta2);
   } else if (s.N > 64) {
     SATB_PROPAGATE(get_b(128, &tb));
     return launch_gemm<Epi, 128, BF16>(ta, *tb, s, ep, st, ta2);
@@ -402,30 +390,23 @@ int residual_unit(SatbOobleck* h, const std::string& pfx, int C, int B, int L, i
   typedef EpiConv<BF16> E;
   typename E::Params e1{c1.bias, raw, keep_raw ? raw : nullptr, sA, next_snake ? next_snake->a : nullptr,
                         next_snake ? next_snake->ib : nullptr, C, L, 1, 0, h->split3 ? static_cast<char*>(sA) + h->lo_off : nullptr, h->raw16};
-  if (C == ResUnitCfg::kC && c7.k == ResUnitCfg::kTaps && dil <= ResUnitCfg::kMaxDil && L >= 512 && gemm_use_2cta() &&
-      resunit_use_fused() && !h->split3) {
+  if ((C == 128 || C == 256) && c7.k == 7 && 6 * dil <= kHaloMax && resunit_use_fused() && !h->split3) {
     // one kernel: conv7 -> snake2 -> conv1 -> + skip; reads sA (with a halo), so it must write elsewhere
     const CUtensorMap *ta, *tb7, *tb1;
-    SATB_PROPAGATE(get_tmap_a(h, sA, C, L, B, L, 1, &ta, ResUnitCfg::halo_rows(dil)));   // one halo box per k-block
-    SATB_PROPAGATE(get_tmap_b(h, c7, c7.k * C, 64, &tb7));
-    SATB_PROPAGATE(get_tmap_b(h, c1, C, 64, &tb1));
+    SATB_PROPAGATE(get_tmap_a(h, sA, C, L, B, L, 1, &ta, kBlockM + 6 * dil));   // one halo box per k-block
+    SATB_PROPAGATE(get_tmap_b(h, c7, c7.k * C, C, &tb7));
+    SATB_PROPAGATE(get_tmap_b(h, c1, C, C, &tb1));
     e1.s16_out = sT;
-    ResUnitParams<BF16> rp{c7.bias, s2.a, s2.ib, e1};
-    ResUnitShape rs{L, B, dil};
-    SATB_PROPAGATE(launch_resunit<BF16>(*ta, *tb7, *tb1, rs, rp, st));
-    std::swap(sA, sT);
-    return 0;
-  }
-  if (C == ResUnit256Cfg::kC && c7.k == ResUnit256Cfg::kTaps && dil <= ResUnit256Cfg::kMaxDil && L >= 512 &&
-      gemm_use_2cta() && resunit_use_fused() && !h->split3) {
-    const CUtensorMap *ta, *tb7, *tb1;
-    SATB_PROPAGATE(get_tmap_a(h, sA, C, L, B, L, 1, &ta, ResUnit256Cfg::halo_rows(dil)));
-    SATB_PROPAGATE(get_tmap_b(h, c7, c7.k * C, 128, &tb7));
-    SATB_PROPAGATE(get_tmap_b(h, c1, C, 128, &tb1));
-    e1.s16_out = sT;
-    ResUnitParams<BF16> rp{c7.bias, s2.a, s2.ib, e1};
-    ResUnitShape rs{L, B, dil};
-    SATB_PROPAGATE(launch_resunit256<BF16>(*ta, *tb7, *tb1, rs, rp, st));
+    const HaloShape hs{L, B, C, 7, dil, C};
+    const ResUnitPre pre{c7.bias, s2.a, s2.ib};
+    if (E::fast_flags(e1) && conv_epi_masked()) {
+      typedef EpiConv<BF16, true> EM;
+      SATB_PROPAGATE(C == 128 ? (launch_conv_halo<EM, 128, BF16, true>(*ta, *tb7, tb1, hs, pre, e1, st))
+                              : (launch_conv_halo<EM, 256, BF16, true>(*ta, *tb7, tb1, hs, pre, e1, st)));
+    } else {
+      SATB_PROPAGATE(C == 128 ? (launch_conv_halo<E, 128, BF16, true>(*ta, *tb7, tb1, hs, pre, e1, st))
+                              : (launch_conv_halo<E, 256, BF16, true>(*ta, *tb7, tb1, hs, pre, e1, st)));
+    }
     std::swap(sA, sT);
     return 0;
   }
@@ -506,14 +487,14 @@ int decode_impl(SatbOobleck* h, const float* z, float* audio, int B, int L, cuda
   {
     const ConvW& cf = h->convs.at("layers." + std::to_string(n + 2) + ".");
     EpiStoreNCL::Params ep{audio, nullptr, cf.cout, static_cast<int>(Lc), c.final_tanh};
-    ConvHaloShape hs{static_cast<int>(Lc), B, cf.cin, cf.k, 1, cf.cout};
-    if (conv_halo_enabled() && !h->split3 && cf.cout <= ConvHaloCfg::kBN && cf.cin % kBlockK == 0 && cf.cin <= 256 &&
-        ConvHaloCfg::halo_rows(hs) <= 256) {
+    if (conv_halo_enabled() && !h->split3 && cf.cout <= 64 && cf.cin % kBlockK == 0 && cf.k % 2 == 1 &&
+        cf.k - 1 <= kHaloMax) {
       // every activation row is fetched once per tile instead of once per tap (see conv_halo.cuh)
       const CUtensorMap *ta, *tb;
-      SATB_PROPAGATE(get_tmap_a(h, sA, cf.cin, static_cast<int>(Lc), B, static_cast<int>(Lc), 1, &ta, ConvHaloCfg::halo_rows(hs)));
-      SATB_PROPAGATE(get_tmap_b(h, cf, cf.k * cf.cout, ConvHaloCfg::kBN, &tb));
-      SATB_PROPAGATE((launch_conv_halo<EpiStoreNCL, BF16>(*ta, *tb, hs, ep, st)));
+      SATB_PROPAGATE(get_tmap_a(h, sA, cf.cin, static_cast<int>(Lc), B, static_cast<int>(Lc), 1, &ta, kBlockM + cf.k - 1));
+      SATB_PROPAGATE(get_tmap_b(h, cf, cf.k * cf.cout, 64, &tb));
+      const HaloShape hs{static_cast<int>(Lc), B, cf.cin, cf.k, 1, cf.cout};
+      SATB_PROPAGATE((launch_conv_halo<EpiStoreNCL, 64, BF16, false>(*ta, *tb, nullptr, hs, ResUnitPre{}, ep, st)));
     } else {
       SATB_PROPAGATE((run_conv_gemm<EpiStoreNCL, BF16>(h, cf, sA, B, static_cast<int>(Lc), 0, 1, 1, ep, st)));
     }

@@ -16,20 +16,10 @@ unsigned long long g_launch_count = 0;
 void set_last_error(const std::string& msg) { g_last_error = msg; }
 const char* get_last_error() { return g_last_error.c_str(); }
 
-bool gemm_use_2cta() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SATB_GEMM");
-    v = (e && std::string(e) == "1cta") ? 0 : 1;
-  }
-  return v == 1;
-}
-
 bool ln_fold_enabled() {
-  // Opt-in (SATB_LN=fold).  Measured on B200, SA-Open B=4: the fold removes the 1.0 ms / step of LayerNorm kernels but
-  // the heavier epilogues cost more than that (residual GEMMs +0.3 .. +0.4 ms each class, QKV +0.35 ms: they read h,
-  // write h + x16 + partial sums, and load the per-column vector c) - a net loss of ~0.4 ms / step, so the LayerNorm
-  // kernels stay the default (profiles/README.md).
+  // Opt-in (SATB_LN=fold): the fold removes the LayerNorm kernels but makes the residual and QKV epilogues heavier
+  // (they read h, write h + x16 + partial sums, and load the per-column vector c), so the LayerNorm kernels stay the
+  // default (DESIGN.md section 4).
   static int v = -1;
   if (v < 0) {
     const char* e = getenv("SATB_LN");
@@ -56,20 +46,20 @@ bool conv_halo_enabled() {
   return v == 1;
 }
 
-bool conv_epi_masked() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SATB_CONV_EPI");    // "general": the combined fast + general epilogue kernels (A/B debugging)
-    v = (e && std::string(e) == "general") ? 0 : 1;
-  }
-  return v == 1;
-}
-
 bool resunit_use_fused() {
   static int v = -1;
   if (v < 0) {
     const char* e = getenv("SATB_RESUNIT");
     v = (e && std::string(e) == "unfused") ? 0 : 1;
+  }
+  return v == 1;
+}
+
+bool conv_epi_masked() {
+  static int v = -1;
+  if (v < 0) {
+    const char* e = getenv("SATB_CONV_EPI");    // "general": the combined fast + general epilogue kernels (A/B debugging)
+    v = (e && std::string(e) == "general") ? 0 : 1;
   }
   return v == 1;
 }
@@ -81,7 +71,7 @@ int device_sm_count() {
   if (dev < 0 || dev >= 64) dev = 0;
   if (cached[dev] == 0) {
     cudaDeviceGetAttribute(&cached[dev], cudaDevAttrMultiProcessorCount, dev);
-    if (cached[dev] <= 0) cached[dev] = 148;
+    if (cached[dev] <= 0) cached[dev] = 132;
   }
   return cached[dev];
 }

@@ -61,8 +61,6 @@ SIGNATURES = {
     "satb_layernorm": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _VP]),
     "satb_linear_f32out": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _VP]),
     "satb_attention": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP]),
-    "satb_debug_attention_occupancy": (_I, [_I, _I]),
-    "satb_attention_trace": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP, _VP]),
     "satb_oobleck_create": (_I, [ctypes.POINTER(SatbOobleckConfig), ctypes.POINTER(_VP)]),
     "satb_oobleck_destroy": (None, [_VP]),
     "satb_oobleck_load_weight": (_I, [_VP, ctypes.c_char_p, _VP, _LL, _VP]),

@@ -1,4 +1,4 @@
-"""Model package of the B200-native drop-in: only the factory functions are re-exported here."""
+"""Model package of the H100-native drop-in: only the factory functions are re-exported here."""
 from . import factory as _factory
 
 create_model_from_config = _factory.create_model_from_config

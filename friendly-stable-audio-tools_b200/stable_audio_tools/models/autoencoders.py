@@ -7,7 +7,7 @@ weight-norm ``weight_g`` / ``weight_v`` pairs), ``AudioAutoencoder`` (:234-645: 
 decode with ``iterate_batch`` micro-batching, chunked ``encode_audio`` / ``decode_audio`` /
 ``reconstruct_audio`` with Bartlett cross-fades) and the config factories (:693-787).
 
-The encoder / decoder ``forward`` run in ``libsatb200.so`` (``satb_oobleck_*``): tcgen05
+The encoder / decoder ``forward`` run in ``libsatb200.so`` (``satb_oobleck_*``): wgmma
 implicit-GEMM convolutions with Snake fused into the producing epilogue.  The inner blocks
 are parameter containers.  The chunking / cross-fade orchestration is host-side tensor
 slicing on the device, exactly as in the reference.

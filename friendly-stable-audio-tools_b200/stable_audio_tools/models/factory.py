@@ -11,7 +11,7 @@ def create_model_from_config(model_config):
         from .diffusion import create_diffusion_cond_from_config
         return create_diffusion_cond_from_config(model_config)
     raise NotImplementedError(
-        f"model_type '{model_type}' is outside the B200-native hot path (supported: autoencoder, diffusion_cond)")
+        f"model_type '{model_type}' is outside the H100-native hot path (supported: autoencoder, diffusion_cond)")
 
 
 def create_model_from_config_path(model_config_path):

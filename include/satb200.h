@@ -1,5 +1,5 @@
 /*
- * satb200 - C ABI of the B200-native Stable Audio denoising hot path.
+ * satb200 - C ABI of the GPU-native (H100, sm_90a) Stable Audio denoising hot path.
  *
  * The reference (yukara-ikemiya/friendly-stable-audio-tools) is pure Python/PyTorch and has
  * no FFI of its own; the boundary it offers for this path is a Python object contract
@@ -127,14 +127,6 @@ int satb_sampler_update(const float* x, const float* v, const float* den_1, cons
  * out [B, Nq, H*64]; 16-bit, contiguous. */
 int satb_attention(const void* q16, const void* k16, const void* v16, void* o16, int B, int H, int Hkv, int Nq, int Nk,
                    int bf16, void* stream);
-
-/* Debug / profiling: resident CTAs per SM reported by the runtime for the attention kernel with the given dynamic
- * shared-memory size and carveout preference (percent, -1 = unchanged). */
-int satb_debug_attention_occupancy(int dyn_smem, int carveout_pct);
-/* satb_attention plus a clock64 trace (16 key tiles x 12 slots) of CTA 0's first softmax warp followed by one
- * (SM id, slot, start ns, end ns) record per CTA: dbg must hold 16 * 12 + 4 * gridDim entries (<= 1376). */
-int satb_attention_trace(const void* q16, const void* k16, const void* v16, void* o16, int B, int H, int Hkv, int Nq,
-                         int Nk, int bf16, unsigned long long* dbg, void* stream);
 
 /* ---- Oobleck VAE: replaces OobleckDecoder / OobleckEncoder.forward
  *      (models/autoencoders.py:119-194) behind AudioAutoencoder.encode/decode (:268-343) */

@@ -222,6 +222,217 @@ def gen_config1(ref, path):
     np.savez_compressed(path, model_cfg=json.dumps(cfg), enc_seed=31, dec_seed=32, noise_seed=34,
                         enc_wsum=weights_checksum(esd), dec_wsum=weights_checksum(dsd), audio=_np(audio), rec=_np(rec))
 
+# ---- reference_checks.npz: what tests/test_oracle_vs_reference.py compares the oracle and the drop-in modules with
+CHECK_DIT = dict(io_channels=64, embed_dim=128, depth=3, num_heads=2, cond_token_dim=64, global_cond_dim=128,
+                 transformer_type="continuous_transformer")
+CHECK_DIT_KW = (dict(cfg_scale=1.0), dict(cfg_scale=5.0), dict(cfg_scale=5.0, scale_phi=0.5))
+CHECK_MASK_ARGS = dict(cropfrom=10.0, pastefrom=20.0, pasteto=90.0, maskstart=25.0, maskend=80.0, softnessL=12.0,
+                       softnessR=7.0, marination=0.2)
+CHECK_META = [{"prompt": "warm analog pad with slow attack", "seconds_start": 0, "seconds_total": 30},
+              {"prompt": "drum loop 120 bpm", "seconds_start": 5, "seconds_total": 47}]
+CHECK_TOKENS = 8   # conditioning rows stored per item (the prompts above are <= 6 tokens; the rest is zero padding)
+
+
+def check_dit_case(gtype, seed):
+    """Config, weights and inputs of one DiT comparison case."""
+    cfg = dict(CHECK_DIT, project_cond_tokens=bool(seed), global_cond_type=gtype)
+    sd = do.make_dit_weights(cfg, seed=seed)
+    g = torch.Generator().manual_seed(seed)
+    x, t = torch.randn(3, 64, 33, generator=g), torch.rand(3, generator=g)
+    c, ge = torch.randn(3, 7, 64, generator=g), torch.randn(3, 128, generator=g)
+    return cfg, sd, (x, t, c, ge)
+
+
+def toy_denoiser():
+    """A linear toy denoiser with seeded weights and the seeded initial noise of the sampler comparisons."""
+    torch.manual_seed(0)
+    w = torch.randn(4, 4) * 0.3
+
+    def toy(x, t, **kw):
+        return torch.einsum("ij,bjl->bil", w, x) * (1 + t[:, None, None])
+    return toy
+
+
+class FakeTokenizer:
+    """Stands for AutoTokenizer.from_pretrained('t5-base') (no model files offline): whitespace 'tokens', padded."""
+
+    def __call__(self, texts, truncation=True, max_length=128, padding="max_length", return_tensors="pt"):
+        ids = torch.zeros(len(texts), max_length, dtype=torch.long)
+        mask = torch.zeros(len(texts), max_length, dtype=torch.long)
+        for i, t in enumerate(texts):
+            toks = [(sum(map(ord, w)) % 1000) + 1 for w in t.split()][:max_length]
+            ids[i, :len(toks)] = torch.tensor(toks)
+            mask[i, :len(toks)] = 1
+        return {"input_ids": ids, "attention_mask": mask}
+
+
+class FakeT5(torch.nn.Module):
+    def __init__(self, dim=768):
+        super().__init__()
+        g = torch.Generator().manual_seed(3)
+        self.emb = torch.nn.Parameter(torch.randn(1001, dim, generator=g))
+
+    def forward(self, input_ids=None, attention_mask=None):
+        return {"last_hidden_state": self.emb[input_ids]}
+
+
+class ChunkFakeEnc(torch.nn.Module):
+    """average-pool 'encoder' (ratio 4, 2 -> 3 channels) so the chunking logic runs on CPU"""
+
+    def forward(self, x):
+        p = torch.nn.functional.avg_pool1d(x, 4)
+        return torch.cat([p, p[:, :1] * 0.5 - 3.0], dim=1)
+
+
+class ChunkFakeDec(torch.nn.Module):
+    def forward(self, z):
+        return torch.repeat_interleave(z[:, :2] + z[:, 2:3] * 0.25, 4, dim=-1)
+
+
+def chunk_inputs():
+    """Seeded audio and latents of the chunked encode / decode / reconstruct comparison."""
+    torch.manual_seed(0)
+    return torch.randn(2, 2, 4 * 37), torch.randn(2, 3, 41)
+
+
+def chunked_calls(ae, a, z):
+    """encode / decode / reconstruct of an AudioAutoencoder (reference or drop-in) with the chunking parameters the
+    comparison uses."""
+    return (ae.encode_audio(a.clone(), chunked=True, chunk_size=8, overlap=2, max_batch_size=3),
+            ae.decode_audio(z.clone(), chunked=True, chunk_size=8, overlap=2, max_batch_size=2),
+            ae.reconstruct_audio(a.clone(), chunked=True, chunk_size=8, overlap=2, max_batch_size=4))
+
+
+def small_txt2audio(cfg):
+    """The shipped text-to-audio config cut to depth 2 and a 2-stage, 32-channel VAE."""
+    small = json.loads(json.dumps(cfg))
+    small["model"]["diffusion"]["config"]["depth"] = 2
+    for half in ("encoder", "decoder"):
+        c = small["model"]["pretransform"]["config"][half]["config"]
+        c["c_mults"], c["strides"], c["channels"] = [1, 2], [2, 4], 32
+    small["model"]["pretransform"]["config"]["downsampling_ratio"] = 8
+    return small
+
+
+def seeded_conditioner_params(sd, seed=7):
+    """Seeded replacements (same on every machine) for the conditioner entries of a state dict, in key order."""
+    g = torch.Generator().manual_seed(seed)
+    return {k: 0.1 * torch.randn(tuple(sd[k].shape), generator=g).to(sd[k].dtype)
+            for k in sorted(sd) if k.startswith("conditioner.") and sd[k].is_floating_point()}
+
+
+def _shapes(sd):
+    return {k: list(v.shape) for k, v in sd.items()}
+
+
+def gen_reference_checks(ref, path):
+    import functools
+    import transformers
+    out = {}
+    # DiT forward of the reference on fresh random cases
+    for gtype in ("prepend", "adaLN"):
+        for seed in (0, 1):
+            cfg, sd, (x, t, c, ge) = check_dit_case(gtype, seed)
+            m = ref.dit.DiffusionTransformer(**cfg).eval()
+            m.load_state_dict(sd, strict=True)
+            with torch.no_grad():
+                for i, kw in enumerate(CHECK_DIT_KW):
+                    out[f"dit_{gtype}_{seed}_{i}"] = _np(m(x, t, cross_attn_cond=c, global_embed=ge, **kw))
+    # state-dict keys and shapes of the reference modules
+    keys = {}
+    for gtype in ("prepend", "adaLN"):
+        cfg = dict(CHECK_DIT, depth=2, project_cond_tokens=False, global_cond_type=gtype)
+        keys[f"dit_{gtype}"] = _shapes(ref.dit.DiffusionTransformer(**cfg).state_dict())
+    keys["decoder"] = _shapes(ref.autoencoders.OobleckDecoder(**DEC_SMALL).state_dict())
+    keys["encoder"] = _shapes(ref.autoencoders.OobleckEncoder(**ENC_SMALL).state_dict())
+    # the shipped SA-2.0 VAE config through the reference factory
+    vae_path = os.path.join(ref_shims.REFERENCE_ROOT, "stable_audio_tools/configs/model_configs/autoencoders/stable_audio_2_0_vae.json")
+    vae_cfg = json.load(open(vae_path))
+    vae = ref.factory.create_model_from_config(json.loads(json.dumps(vae_cfg)))
+    keys["vae_2_0"] = _shapes(vae.state_dict())
+    out["vae_2_0_cfg"] = json.dumps(vae_cfg)
+    out["vae_2_0_ratio"] = vae.downsampling_ratio
+    # sample_k of the reference with injected noise
+    toy = toy_denoiser()
+    noise = torch.randn(2, 4, 16)
+    seq = [torch.randn(2, 4, 16) for _ in range(8)]
+    K = __import__("k_diffusion")
+    for st in ("dpmpp-2m-sde", "dpmpp-3m-sde"):
+        fn_name = "sample_dpmpp_2m_sde" if "2m" in st else "sample_dpmpp_3m_sde"
+        orig = getattr(K.sampling, fn_name)
+        it = iter(seq)
+        setattr(K.sampling, fn_name, functools.partial(orig, noise_sampler=lambda s, sn: next(it)))
+        try:
+            out[f"sample_k_{st}"] = _np(ref.sampling.sample_k(toy, noise.clone(), steps=8, sampler_type=st, sigma_min=0.3,
+                                                             sigma_max=50, device="cpu"))
+        finally:
+            setattr(K.sampling, fn_name, orig)
+    # NumberConditioner of the reference
+    with ref_shims.reference_modules(ref):
+        import importlib
+        ref_cond = importlib.import_module("stable_audio_tools.models.conditioners")
+        torch.manual_seed(0)
+        a = ref_cond.NumberConditioner(64, min_val=0, max_val=512)
+        xa, ma = a([0.0, 12.5, 600.0])
+    for k, v in a.state_dict().items():
+        out[f"numcond_sd.{k}"] = _np(v)
+    out["numcond_x"], out["numcond_m"] = _np(xa), _np(ma)
+    # inpainting sample_k and build_mask of the reference
+    L = 48
+    out["mask"] = _np(ref.generation.build_mask(L, CHECK_MASK_ARGS))
+    toy = toy_denoiser()
+    noise, init = torch.randn(2, 4, L), torch.randn(2, 4, L)
+    mask = ref.generation.build_mask(L, CHECK_MASK_ARGS)
+    for st in ("dpmpp-2m-sde", "dpmpp-3m-sde"):
+        for mi, m in enumerate((mask, None)):
+            with seeded_randn_like(5):
+                out[f"inpaint_{st}_{mi}"] = _np(ref.sampling.sample_k(toy, noise.clone(), init.clone(), m, steps=7,
+                                                                      sampler_type=st, sigma_min=0.3, sigma_max=20, device="cpu"))
+    # the shipped text-to-audio configs through the reference factory (T5 stubbed)
+    tok0, t50 = transformers.AutoTokenizer.from_pretrained, transformers.T5EncoderModel.from_pretrained
+    transformers.AutoTokenizer.from_pretrained = classmethod(lambda cls, *a, **k: FakeTokenizer())
+    transformers.T5EncoderModel.from_pretrained = classmethod(lambda cls, *a, **k: FakeT5())
+    try:
+        for name in ("stable_audio_open_1_0", "stable_audio_2_0"):
+            cfg = json.load(open(os.path.join(ref_shims.REFERENCE_ROOT, "stable_audio_tools/configs/model_configs/txt2audio",
+                                              name + ".json")))
+            for c in cfg["model"]["conditioning"]["configs"]:
+                if c["type"] == "clap_text":
+                    c["type"], c["config"] = "t5", {"t5_model_name": "t5-base", "max_length": 128}
+            out[f"{name}_cfg"] = json.dumps(cfg)
+            with torch.device("meta"):
+                with ref_shims.reference_modules(ref):
+                    theirs = ref.factory.create_model_from_config(json.loads(json.dumps(cfg)))
+            keys[name] = _shapes(theirs.state_dict())
+            out[f"{name}_attrs"] = json.dumps({"min_input_length": theirs.min_input_length, "io_channels": theirs.io_channels,
+                                               "cross_attn_cond_ids": theirs.cross_attn_cond_ids,
+                                               "global_cond_ids": theirs.global_cond_ids})
+            torch.manual_seed(0)
+            with ref_shims.reference_modules(ref):
+                theirs = ref.factory.create_model_from_config(small_txt2audio(cfg)).eval()
+            keys[name + "_small"] = _shapes(theirs.state_dict())
+            theirs.load_state_dict(seeded_conditioner_params(theirs.state_dict()), strict=False)
+            with torch.no_grad():
+                ct = theirs.conditioner(CHECK_META)
+            for k, (emb, msk) in ct.items():
+                out[f"{name}_ct.{k}"] = _np(emb.float()[:, :CHECK_TOKENS])
+                out[f"{name}_ctmask.{k}"] = _np(msk.float())
+            ci = theirs.get_conditioning_inputs(ct)
+            out[f"{name}_ci.cross_attn_cond"] = _np(torch.cat([ci["cross_attn_cond"][:, :CHECK_TOKENS],
+                                                               ci["cross_attn_cond"][:, -2:]], 1).float())
+            out[f"{name}_ci.cross_attn_mask"] = _np(ci["cross_attn_mask"].float())
+            out[f"{name}_ci.global_cond"] = _np(ci["global_cond"].float())
+    finally:
+        transformers.AutoTokenizer.from_pretrained, transformers.T5EncoderModel.from_pretrained = tok0, t50
+    # chunked encode / decode / reconstruct of the reference AudioAutoencoder around position-wise fakes
+    a, z = chunk_inputs()
+    theirs = ref.autoencoders.AudioAutoencoder(ChunkFakeEnc(), ChunkFakeDec(), latent_dim=3, downsampling_ratio=4,
+                                               sample_rate=16000, io_channels=2, bottleneck=None)
+    for name, t in zip(("enc", "dec", "rec"), chunked_calls(theirs, a, z)):
+        out[f"chunked_{name}"] = _np(t)
+    out["keys"] = json.dumps(keys)
+    np.savez_compressed(path, **out)
+
 
 def main():
     os.makedirs(GOLDEN_DIR, exist_ok=True)
@@ -235,6 +446,7 @@ def main():
     gen_snake(ref, os.path.join(GOLDEN_DIR, "snake_beta.npz"))
     gen_oobleck(ref, os.path.join(GOLDEN_DIR, "oobleck_small.npz"))
     gen_config1(ref, os.path.join(GOLDEN_DIR, "config1_mono16k.npz"))
+    gen_reference_checks(ref, os.path.join(GOLDEN_DIR, "reference_checks.npz"))
     for f in sorted(os.listdir(GOLDEN_DIR)):
         print(f, os.path.getsize(os.path.join(GOLDEN_DIR, f)))
 

@@ -1,4 +1,4 @@
-"""Timing / accuracy driver for the attention kernel (not a test): [SATB_ATTN_*=..] python tests/attn_time.py [N ...]
+"""Timing / accuracy driver for the attention kernel (not a test): python tests/attn_time.py [N ...]
 SA-Open self-attention shape (8 rows x 24 heads x N tokens), CUDA events, error vs torch fp32 softmax."""
 import os
 import sys

@@ -15,6 +15,6 @@ for s in (1.0, 7.0):
     y1 = m(x[2:3].contiguous(), t[2:3].contiguous(), cross_attn_cond=c[2:3].contiguous(), global_embed=ge[2:3].contiguous(), cfg_scale=s)
     d = (y4[2:3] - y1).float()
     per_pos = d.pow(2).sum(dim=1).sqrt()[0] / y1.float().pow(2).sum(dim=1).sqrt()[0]
-    print("cfg %.0f rel_l2 %.3e  per-position err: first %.2e median %.2e last %.2e max %.2e at %d  [%s]" % (
-        s, rel_l2(y4[2:3].cpu(), y1.cpu()), per_pos[0], per_pos.median(), per_pos[-1], per_pos.max(), int(per_pos.argmax()),
-        os.environ.get("SATB_ATTN_ROWPATH", "")), flush=True)
+    print("cfg %.0f rel_l2 %.3e  per-position err: first %.2e median %.2e last %.2e max %.2e at %d" % (
+        s, rel_l2(y4[2:3].cpu(), y1.cpu()), per_pos[0], per_pos.median(), per_pos[-1], per_pos.max(), int(per_pos.argmax())),
+          flush=True)

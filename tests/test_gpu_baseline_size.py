@@ -71,10 +71,8 @@ def test_sao_dit_all_24_blocks_cfg7_vs_oracle(t_val):
 def test_sao_dit_24_blocks_batch_rows_do_not_depend_on_batch_mates():
     """BASELINE configs[2] batch (4 prompts + CFG = 8 rows): the 4 prompts equal, BIT FOR BIT, the same prompts inside a
     batch of 5 (same arithmetic per row; tiles differ only in position), so the oracle comparison of a single prompt
-    above covers every row of the batch.  Batches of fewer than 3 prompts take another - equally valid - route for the
-    1025th query row (a partial tensor-core tile instead of the fp32 CUDA-core row: the launcher's cost model,
-    attention_tc.cu; SATB_ATTN_ROWPATH=0/1 pins either and then batch 4 vs 1 is bit-equal as well, measured with
-    tests/batch_vs_single_probe.py) and land within the operand-rounding floor of the batch result."""
+    above covers every row of the batch, and a single prompt lands within the operand-rounding floor of the batch
+    result."""
     from oracle import dit_oracle as do
     sd = do.make_dit_weights(SAO_DIT, seed=21)
     m = build_native_dit(SAO_DIT, sd)

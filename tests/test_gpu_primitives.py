@@ -62,7 +62,7 @@ def test_layernorm_vs_torch(rows, D):
                                    (129, 384, 200)])
 @pytest.mark.parametrize("bf16", [0, 1])
 def test_tcgen05_linear_vs_torch(M, N, K, bf16):
-    """tcgen05 GEMM (TMA + TMEM, fp32 accumulate) vs torch matmul on the same 16-bit operands."""
+    """wgmma GEMM (TMA ring, fp32 register accumulators) vs torch matmul on the same 16-bit operands."""
     nat = _native()
     torch.manual_seed(M + N + K)
     dt = torch.bfloat16 if bf16 else torch.float16
@@ -77,11 +77,11 @@ def test_tcgen05_linear_vs_torch(M, N, K, bf16):
 
 @pytest.mark.parametrize("B,H,Hkv,Nq,Nk", [(2, 4, 4, 1025, 1025), (1, 24, 12, 1025, 130), (2, 2, 1, 64, 1),
                                            (1, 3, 3, 65, 191), (1, 24, 24, 300, 300),
-                                           # 2 ragged query rows (CUDA-core row path) x 1 leftover key; only row-path rows;
-                                           # no tensor-core key tile at all (2 keys); many units per CTA
+                                           # ragged query and key tiles (130 / 257); fewer query rows than one tile;
+                                           # a key tile with only 2 keys; many CTAs per (item, head)
                                            (1, 2, 2, 130, 257), (1, 2, 1, 2, 130), (2, 4, 2, 128, 2), (3, 24, 24, 1024, 384),
-                                           # small batch at the SA-Open length: the 1025th query row rides as a partial
-                                           # tile (no row path), one leftover key, several units per CTA back to back
+                                           # small batch at the SA-Open length: the 1025th query row and the 1025th key
+                                           # each in a tile of their own
                                            (2, 24, 24, 1025, 1025)])
 def test_attention_vs_oracle(B, H, Hkv, Nq, Nk):
     """softmax(q k^T / 8) v vs the oracle's einsum path (models/transformer.py:510-536), fp16 operands."""
@@ -103,10 +103,9 @@ def test_attention_vs_oracle(B, H, Hkv, Nq, Nk):
 
 @pytest.mark.parametrize("Nk", [700, 641])
 def test_attention_lazy_rescale_path_monotone_scores(Nk):
-    """Scores that keep growing along the key axis force the reference max to move in (almost)
-    every 64-key tile: exercises the O rescale + P recomputation path of the tcgen05 kernel.  Nk = 641 = 5 x 128 + 1:
-    the leftover key (scores by a 16-column MMA, exponential kept in registers) is the row maximum of head 0 and is
-    carried through every rescale of head 1."""
+    """Scores that keep growing along the key axis force the running max to move in every 64-key tile: exercises
+    the O rescale of the online softmax.  Nk = 641 = 10 x 64 + 1: the last, one-key tile (the other 63 rows
+    zero-filled and masked) holds the row maximum of head 0 and rescales everything before it."""
     from oracle.dit_oracle import attention_core
     nat = _native()
     B, H, Nq = 1, 2, 200
