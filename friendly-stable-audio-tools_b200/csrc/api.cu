@@ -51,10 +51,15 @@ int satb_sampler_update(const float* x, const float* v, const float* den_1, cons
 
 int satb_attention(const void* q16, const void* k16, const void* v16, void* o16, int B, int H, int Hkv, int Nq, int Nk,
                    int bf16, void* stream) {
+  return satb_attention_hd(q16, k16, v16, o16, B, H, Hkv, Nq, Nk, 64, bf16, stream);
+}
+
+int satb_attention_hd(const void* q16, const void* k16, const void* v16, void* o16, int B, int H, int Hkv, int Nq,
+                      int Nk, int head_dim, int bf16, void* stream) {
   SATB_REQUIRE(q16 && k16 && v16 && o16, "null argument");
-  const int64_t dq = static_cast<int64_t>(H) * 64, dk = static_cast<int64_t>(Hkv) * 64;
+  const int64_t dq = static_cast<int64_t>(H) * head_dim, dk = static_cast<int64_t>(Hkv) * head_dim;
   return launch_attention_tc(q16, k16, v16, o16, dq, dk, dk, dq, Nq * dq, Nk * dk, Nk * dk, Nq * dq, static_cast<int>(dq),
-                             static_cast<int>(dk), static_cast<int>(dk), 0, 0, 0, B, H, Hkv, Nq, Nk, bf16 != 0,
+                             static_cast<int>(dk), static_cast<int>(dk), 0, 0, 0, B, H, Hkv, Nq, Nk, head_dim, bf16 != 0,
                              static_cast<cudaStream_t>(stream));
 }
 

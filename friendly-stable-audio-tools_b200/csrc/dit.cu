@@ -3,6 +3,7 @@
 // (device, model); all work is enqueued on the caller's stream; no allocation and no
 // synchronisation inside satb_dit_forward once the workspace has been reserved, so a
 // whole denoise step can be captured in a CUDA graph.
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <map>
@@ -132,6 +133,7 @@ struct SatbDit {
   uint16_t *w_in16 = nullptr, *w_out16 = nullptr;
   float* w_ssg = nullptr;   // [depth*6D, D] fp32 (adaLN)
   int* ff_perm = nullptr;   // SwiGLU row interleave
+  int* qkv_perm = nullptr;  // rotary pair layout of the q / k rows of to_qkv (null: identity, head dims 32 and 64)
   std::map<std::string, int> loaded;
   bool finalized = false;
   // conditioning state
@@ -170,6 +172,25 @@ static bool ends_with(const std::string& s, const std::string& suf) {
   return s.size() >= suf.size() && s.compare(s.size() - suf.size(), suf.size(), suf) == 0;
 }
 
+// Source row of every stored row of to_qkv [3D, D] (the layout EpiQkvRope rotates, gemm.cuh): inside each q and k head,
+// stored position 32 ci + i (i < 16) holds dim 16 ci + i and 32 ci + 16 + i holds its rotary partner 16 ci + i + nf,
+// for the first clamp(nf - 16 ci, 0, 16) pairs of 32-column chunk ci; the dims from 2 nf up fill the remaining
+// positions in order.  v rows are untouched.  Head dim 128 (nf 32): chunk 0 = [0..15 | 32..47], chunk 1 = [16..31 |
+// 48..63], chunks 2-3 = 64..127.  Head dim 96 (nf 24): [0..15 | 24..39], [16..23, 48..55 | 40..47, 56..63], 64..95.
+// Head dims 32 and 64 give the identity.
+static std::vector<int> qkv_head_perm(int D, int dh, int nf) {
+  std::vector<int> within(dh);
+  int next_pass = 2 * nf;
+  for (int s = 0; s < dh; ++s) {
+    const int ci = s / 32, w = s % 32, i = w % 16;
+    const int n_rot = std::min(std::max(nf - 16 * ci, 0), 16);
+    within[s] = i < n_rot ? 16 * ci + i + (w >= 16 ? nf : 0) : next_pass++;
+  }
+  std::vector<int> perm(3 * D);
+  for (int n = 0; n < 3 * D; ++n) perm[n] = n < 2 * D ? (n / dh) * dh + within[n % dh] : n;
+  return perm;
+}
+
 extern "C" {
 
 const char* satb_last_error(void) { return get_last_error(); }
@@ -181,8 +202,10 @@ int satb_abi_version(void) { return SATB_ABI_VERSION; }
 int satb_dit_create(const SatbDitConfig* cfg, SatbDit** out) {
   SATB_REQUIRE(cfg && out, "null argument");
   SATB_REQUIRE(cfg->embed_dim % 128 == 0, "embed_dim must be a multiple of 128");
-  SATB_REQUIRE(cfg->num_heads > 0 && cfg->embed_dim / cfg->num_heads == 64 && cfg->embed_dim % cfg->num_heads == 0,
-               "head dim must be 64");
+  SATB_REQUIRE(cfg->num_heads > 0 && cfg->embed_dim % cfg->num_heads == 0, "embed_dim must be a multiple of num_heads");
+  const int dh = cfg->num_heads > 0 ? cfg->embed_dim / cfg->num_heads : 0;
+  SATB_REQUIRE(dh == 32 || dh == 64 || dh == 96 || dh == 128, "head dim (embed_dim / num_heads) must be 32, 64, 96 or 128");
+  SATB_REQUIRE(!(cfg->qk_norm && dh != 64), "qk_norm is supported with head dim 64 only");
   SATB_REQUIRE(cfg->io_channels % 8 == 0 && cfg->io_channels % 32 == 0, "io_channels must be a multiple of 32");
   SATB_REQUIRE(cfg->patch_size == 1, "patch_size 1 only");
   SATB_REQUIRE(cfg->input_concat_dim >= 0 && cfg->input_concat_dim % 8 == 0, "input_concat_dim must be a multiple of 8");
@@ -211,9 +234,11 @@ int satb_dit_create(const SatbDitConfig* cfg, SatbDit** out) {
   d->qk_norm = cfg->qk_norm != 0;
   d->P = d->adaln ? 0 : 1;
   if (d->ct > 0) {
-    if (d->ce % 64 != 0 || d->H % (d->ce / 64) != 0) {
+    // cross-attention kv heads = cond embed dim / head dim (models/transformer.py:306-312)
+    if (d->ce % d->dh != 0 || d->H % (d->ce / d->dh) != 0) {
       delete d;
-      set_last_error("cond embed dim must be a multiple of 64 with kv heads dividing num_heads");
+      set_last_error("cond embed dim must be a multiple of the head dim (" + std::to_string(d->dh) +
+                     ") with kv heads dividing num_heads");
       return -1;
     }
   }
@@ -222,7 +247,6 @@ int satb_dit_create(const SatbDitConfig* cfg, SatbDit** out) {
     set_last_error("global embed dim must equal embed_dim");
     return -1;
   }
-  SATB_REQUIRE(d->nf == 16, "rotary dim must be 32 (head dim 64)");
   d->layers.resize(d->depth);
   *out = d;
   return 0;
@@ -288,7 +312,14 @@ int satb_dit_load_weight(SatbDit* d, const char* name_c, const float* src, long 
     if (k == "cross_attend_norm.beta") return copy_f32(&L.ca_b, D);
     if (k == "ff_norm.gamma") return copy_f32(&L.ff_g, D);
     if (k == "ff_norm.beta") return copy_f32(&L.ff_b, D);
-    if (k == "self_attn.to_qkv.weight") return cast16(&L.w_qkv, 3 * D, D, nullptr);
+    if (k == "self_attn.to_qkv.weight") {
+      if (!d->qkv_perm && d->dh != 32 && d->dh != 64) {
+        const std::vector<int> perm = qkv_head_perm(D, d->dh, d->nf);
+        SATB_PROPAGATE(d->alloc(&d->qkv_perm, perm.size()));
+        SATB_CHECK_CUDA(cudaMemcpy(d->qkv_perm, perm.data(), perm.size() * sizeof(int), cudaMemcpyHostToDevice));
+      }
+      return cast16(&L.w_qkv, 3 * D, D, d->qkv_perm);
+    }
     if (k == "self_attn.to_out.weight") return cast16(&L.w_o, D, D, nullptr);
     if (k == "cross_attn.to_q.weight") return cast16(&L.w_q, D, D, nullptr);
     if (k == "cross_attn.to_kv.weight") return cast16(&L.w_kv, 2 * d->ce, d->ce, nullptr);
@@ -655,11 +686,11 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
       } else {
         if (fused && i > 0) {
           typedef EpiQkvRope<BF16, true> E;
-          typename E::Params ep{qkv, 3 * D, 2 * D, N_seq, cos_tab, sin_tab, fold(S1, W.c_qkv, W.d_qkv)};
+          typename E::Params ep{qkv, 3 * D, 2 * D, N_seq, d->dh, d->nf, cos_tab, sin_tab, fold(S1, W.c_qkv, W.d_qkv)};
           SATB_PROPAGATE((linear<E, 256, BF16>(d->tmaps, a16, D, M, D, W.w_qkv, 3 * D, ep, st)));
         } else {
           typedef EpiQkvRope<BF16> E;
-          typename E::Params ep{qkv, 3 * D, 2 * D, N_seq, cos_tab, sin_tab, no_ln};
+          typename E::Params ep{qkv, 3 * D, 2 * D, N_seq, d->dh, d->nf, cos_tab, sin_tab, no_ln};
           SATB_PROPAGATE((linear<E, 256, BF16>(d->tmaps, a16, D, M, D, W.w_qkv, 3 * D, ep, st)));
         }
       }
@@ -669,7 +700,7 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
       const int64_t qs = static_cast<int64_t>(N_seq) * 3 * D;
       SATB_PROPAGATE(launch_attention_tc(qkv, qkv, qkv, att, 3 * D, 3 * D, 3 * D, D, qs, qs, qs,
                                          static_cast<int64_t>(N_seq) * D, 3 * D, 3 * D, 3 * D, 0, D, 2 * D, R, H, H,
-                                         N_seq, N_seq, BF16, st));
+                                         N_seq, N_seq, d->dh, BF16, st));
     }
     {
       ProfScope ps(d, PROF_ATTN_OUT, st);
@@ -686,7 +717,7 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
     // ---- cross-attention on the rows that have a non-null context
     if (Mc > 0) {
       ProfScope ps(d, PROF_CROSS, st);
-      const int Hkv = d->ce / 64;
+      const int Hkv = d->ce / d->dh;
       if (!fused) SATB_PROPAGATE(launch_layernorm(h, W.ca_g, W.ca_b, a16, Mc, D, nullptr, nullptr, 0, N_seq, 1, BF16, st));
       if (d->qk_norm) {
         typedef EpiHeadNorm16<BF16> E;
@@ -707,7 +738,7 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
       const int64_t kvs = static_cast<int64_t>(d->Mctx) * 2 * d->ce;
       SATB_PROPAGATE(launch_attention_tc(q16, kv, kv, att, D, 2 * d->ce, 2 * d->ce, D, static_cast<int64_t>(N_seq) * D,
                                          kvs, kvs, static_cast<int64_t>(N_seq) * D, D, 2 * d->ce, 2 * d->ce, 0, 0,
-                                         d->ce, d->Rc, H, Hkv, N_seq, d->Mctx, BF16, st));
+                                         d->ce, d->Rc, H, Hkv, N_seq, d->Mctx, d->dh, BF16, st));
       if (fused) {
         typedef EpiResidualLN<BF16> E;
         typename E::Params ep{h, D, nullptr, a16, W.ff_g, W.ff_g, S3, S3, Mc};

@@ -570,9 +570,14 @@ struct EpiResidualLN {
 };
 
 // Fused QKV projection epilogue: split is implicit (q | k | v are column ranges of
-// one [M, 3D] buffer); partial rotary on the first 32 dims of every 64-wide q and k
-// head (models/transformer.py:158-183,438-452): pairs (i, i+16), position = token
-// index within the sequence (prepend token = position 0).  fp32 math, then cast.
+// one [M, 3D] buffer); partial rotary of every q and k head (models/transformer.py:158-183,
+// 438-452), position = token index within the sequence (prepend token = position 0).  fp32
+// math, then cast.  A head of width head_dim has nf = max(head_dim / 2, 32) / 2 rotary pairs
+// (j, j + nf).  The q / k rows of to_qkv are permuted inside each head at load time (dit.cu,
+// qkv_head_perm) so that the pairs sit at positions (i, i + 16) of the head's 32-column chunks:
+// chunk ci = (col % head_dim) / 32 rotates its first clamp(nf - 16 ci, 0, 16) pairs with the
+// table columns 16 ci + i, and the rest of the head passes through.  q and k share the
+// permutation, so every q . k is unchanged.  Head dim 64: identity; chunk 0 rotates 16 pairs.
 template <bool BF16, bool LN = false>
 struct EpiQkvRope {
   static constexpr int kCols = 32;
@@ -582,8 +587,10 @@ struct EpiQkvRope {
     int ld;            // 3*D
     int rope_cols;     // 2*D : columns >= this (v) are never rotated
     int seq_len;       // tokens per item (position = row % seq_len)
-    const float* cos_tab;  // [seq_len, 16]
-    const float* sin_tab;  // [seq_len, 16]
+    int head_dim;      // 32, 64, 96 or 128
+    int nf;            // rotary frequencies per head (table row stride): 16, 16, 24, 32
+    const float* cos_tab;  // [seq_len, nf]
+    const float* sin_tab;  // [seq_len, nf]
     LnFold ln = LnFold{nullptr, nullptr, nullptr, 0.f, 0.f, 0};
   };
   __device__ static __forceinline__ void apply(const Params& p, const EpiCtx& c, const uint32_t (&r)[32]) {
@@ -596,13 +603,16 @@ struct EpiQkvRope {
 #pragma unroll
       for (int j = 0; j < 32; j += 4) ln_apply4(p.ln, lr, v[j], v[j + 1], v[j + 2], v[j + 3], c.col0 + j);
     }
-    // chunk of 32 columns aligned to 32: even chunks of a 64-wide head are the rotary dims
-    if (c.col0 < p.rope_cols && ((c.col0 >> 5) & 1) == 0 && p.cos_tab) {
+    // chunk of 32 columns aligned to 32 (head_dim is a multiple of 32): its rotary pairs (i, i + 16), i < n_rot
+    const int ci = (c.col0 % p.head_dim) >> 5;
+    const int n_rot = min(max(p.nf - 16 * ci, 0), 16);   // 16 or 8 (head dim 96, chunk 1) or 0
+    if (c.col0 < p.rope_cols && n_rot > 0 && p.cos_tab) {
       const int pos = c.row % p.seq_len;
-      const float4* ct = reinterpret_cast<const float4*>(p.cos_tab + pos * 16);
-      const float4* st = reinterpret_cast<const float4*>(p.sin_tab + pos * 16);
+      const float4* ct = reinterpret_cast<const float4*>(p.cos_tab + pos * p.nf + 16 * ci);
+      const float4* st = reinterpret_cast<const float4*>(p.sin_tab + pos * p.nf + 16 * ci);
 #pragma unroll
       for (int j4 = 0; j4 < 4; ++j4) {
+        if (4 * j4 >= n_rot) break;
         const float4 cs = __ldg(ct + j4), sn = __ldg(st + j4);
         const float cc[4] = {cs.x, cs.y, cs.z, cs.w}, ss[4] = {sn.x, sn.y, sn.z, sn.w};
 #pragma unroll

@@ -5,11 +5,11 @@
 
 namespace satb {
 
-// ---- attention_tc.cu (tensor-core flash attention)
+// ---- attention_tc.cu (tensor-core flash attention; head_dim 32, 64, 96 or 128)
 int launch_attention_tc(const void* q, const void* k, const void* v, void* o, int64_t ldq, int64_t ldk, int64_t ldv,
                         int64_t ldo, int64_t q_bs, int64_t k_bs, int64_t v_bs, int64_t o_bs, int q_cols, int k_cols,
                         int v_cols, int q_col, int k_col, int v_col, int batch, int H, int H_kv, int Nq, int Nk,
-                        bool bf16, cudaStream_t stream);
+                        int head_dim, bool bf16, cudaStream_t stream);
 // debugging switches (environment variables; the defaults are the production path)
 bool conv_halo_enabled();     // SATB_CONV_HALO=off: generic per-tap loads for the final conv (A/B debugging)
 bool resunit_use_fused();      // SATB_RESUNIT=unfused runs the 128/256-channel ResidualUnits as two GEMM launches (A/B debugging)

@@ -61,6 +61,7 @@ SIGNATURES = {
     "satb_layernorm": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _VP]),
     "satb_linear_f32out": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _VP]),
     "satb_attention": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP]),
+    "satb_attention_hd": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _VP]),
     "satb_oobleck_create": (_I, [ctypes.POINTER(SatbOobleckConfig), ctypes.POINTER(_VP)]),
     "satb_oobleck_destroy": (None, [_VP]),
     "satb_oobleck_load_weight": (_I, [_VP, ctypes.c_char_p, _VP, _LL, _VP]),

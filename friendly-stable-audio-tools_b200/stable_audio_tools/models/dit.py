@@ -22,7 +22,7 @@ from torch import nn
 
 from .. import _native
 from .blocks import FourierFeatures
-from .transformer import ContinuousTransformer
+from .transformer import SUPPORTED_HEAD_DIMS, ContinuousTransformer, check_head_dim
 
 
 class DiffusionTransformer(nn.Module):
@@ -50,6 +50,10 @@ class DiffusionTransformer(nn.Module):
             # (the reference itself mis-handles this pair: prepend_length is only set in "prepend" mode, dit.py:185-197,
             # so its output keeps the prepended positions - L + n_prepend columns, a shape no sampler can consume)
             raise NotImplementedError("prepend_cond with global_cond_type='adaLN' is not on the native hot path")
+        if num_heads < 1 or embed_dim % num_heads != 0:
+            raise NotImplementedError(f"embed_dim {embed_dim} is not a multiple of num_heads {num_heads}: the native "
+                                      f"path needs a head dim of {', '.join(map(str, SUPPORTED_HEAD_DIMS))}")
+        check_head_dim(embed_dim // num_heads, bool(kwargs.get("attn_kwargs", {}).get("qk_norm", False)))
         if patch_size < 1:
             raise ValueError("patch_size must be >= 1")
         if global_cond_type not in ("prepend", "adaLN"):

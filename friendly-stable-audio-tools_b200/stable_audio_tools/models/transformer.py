@@ -14,6 +14,19 @@ import torch
 from torch import nn
 
 
+# Attention head widths the native attention kernel and RoPE epilogue are built for (csrc/attention_tc.cu, gemm.cuh).
+SUPPORTED_HEAD_DIMS = (32, 64, 96, 128)
+
+
+def check_head_dim(dim_heads, qk_norm=False):
+    """Raises NotImplementedError for a head dim the native path does not run (before any CUDA call)."""
+    if dim_heads not in SUPPORTED_HEAD_DIMS:
+        raise NotImplementedError(f"attention head dim {dim_heads} is not on the native hot path "
+                                  f"(supported head dims: {', '.join(map(str, SUPPORTED_HEAD_DIMS))})")
+    if qk_norm and dim_heads != 64:
+        raise NotImplementedError(f"qk_norm is on the native hot path for head dim 64 only (got {dim_heads})")
+
+
 class _FusedModule(nn.Module):
     """A module whose math is part of a fused native kernel sequence."""
 
@@ -86,6 +99,7 @@ class Attention(_FusedModule):
         super().__init__()
         if causal or natten_kernel_size:
             raise NotImplementedError("causal / neighbourhood attention are outside the native hot path")
+        check_head_dim(dim_heads, qk_norm)
         self.dim, self.dim_heads = dim, dim_heads
         self.qk_norm = bool(qk_norm)      # cosine-similarity attention (reference transformer.py:433-436)
         dim_kv = dim_context if dim_context else dim

@@ -127,6 +127,11 @@ int satb_sampler_update(const float* x, const float* v, const float* den_1, cons
  * out [B, Nq, H*64]; 16-bit, contiguous. */
 int satb_attention(const void* q16, const void* k16, const void* v16, void* o16, int B, int H, int Hkv, int Nq, int Nk,
                    int bf16, void* stream);
+/* The same for any supported head dim d (32, 64, 96 or 128; transformer.py:290-352 takes dim_heads from the model):
+ * softmax(q k^T / sqrt(d)) v with q [B, Nq, H*d], k/v [B, Nk, Hkv*d], out [B, Nq, H*d]; 16-bit, contiguous.
+ * Head h uses kv head h / (H / Hkv).  head_dim 64 gives the bits of satb_attention. */
+int satb_attention_hd(const void* q16, const void* k16, const void* v16, void* o16, int B, int H, int Hkv, int Nq,
+                      int Nk, int head_dim, int bf16, void* stream);
 
 /* ---- Oobleck VAE: replaces OobleckDecoder / OobleckEncoder.forward
  *      (models/autoencoders.py:119-194) behind AudioAutoencoder.encode/decode (:268-343) */
