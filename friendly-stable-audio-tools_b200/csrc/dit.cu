@@ -72,15 +72,17 @@ struct TmapCache {
   }
 };
 
-// Flat Linear: C[M, N] = A[M, K] * W[N, K]^T with a fused epilogue.
+// Flat Linear: C[M, N] = A[M, K] * W[N, K]^T with a fused epilogue.  b_static = 1: W is a weight matrix prepared at
+// finalize time, so its first tiles may be fetched before the dependency wait (every product call); satb_gemm_probe
+// also runs 0.
 template <class Epi, int BN, bool BF16>
 static int linear(TmapCache& tc, const void* A, int64_t lda, int M, int K, const void* W, int N,
-                  const typename Epi::Params& ep, cudaStream_t stream) {
+                  const typename Epi::Params& ep, cudaStream_t stream, int b_static = 1) {
   const CUtensorMap *ta, *tb;
   SATB_PROPAGATE(tc.get_a(A, K, M, 1, lda, static_cast<int64_t>(M) * lda, &ta));
   GemmShape s;
   s.L = M; s.batches = 1; s.N = N; s.K = K; s.n_taps = 1; s.tap_base = 0; s.tap_step = 0; s.b_tap_rows = N; s.stride = 1;
-  s.b_static = 1;   // W is a weight matrix prepared at finalize time
+  s.b_static = b_static;
   SATB_PROPAGATE(tc.get_b(W, K, N, K, BN, &tb));
   return launch_gemm<Epi, BN, BF16>(*ta, *tb, s, ep, stream);
 }
@@ -841,6 +843,134 @@ int satb_dit_forward_debug(SatbDit* d, const float* x, const float* t, float* ou
   cudaStream_t st = static_cast<cudaStream_t>(stream_v);
   return d->bf16 ? dit_forward_impl<true>(d, x, t, out, B, L, cfg_scale, scale_phi, st, hidden)
                  : dit_forward_impl<false>(d, x, t, out, B, L, cfg_scale, scale_phi, st, hidden);
+}
+
+}  // extern "C"
+
+// ---- satb_gemm_probe: one fused-epilogue GEMM for the tests.  It lives in this file so that it launches the very
+// gemm_wgmma_kernel instances the forward and satb_dit_prepare_cond launch (another .cu file would compile its own
+// copies); it instantiates no kernel the forward does not.
+static bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
+
+template <class E, int BN, bool BF16>
+static int probe_run(const void* a, const void* w, int M, int N, int K, const typename E::Params& ep, int b_static,
+                     cudaStream_t st) {
+  SATB_REQUIRE(N % E::kCols == 0, ("gemm probe: N must be a multiple of " + std::to_string(E::kCols)).c_str());
+  TmapCache tc;
+  return linear<E, BN, BF16>(tc, a, K, M, K, w, N, ep, st, b_static);
+}
+
+template <bool BF16>
+static int gemm_probe(const void* a, const void* w, int M, int N, int K, const SatbGemmProbe& p, cudaStream_t st) {
+  const int bn = p.bn;
+  const LnFold ln{static_cast<const float2*>(p.ln_stats), p.ln_c, p.ln_d, p.ln_inv_dim, p.ln_eps, p.ln_n_slots};
+  const int out_elem = p.epi == SATB_EPI_STORE32 ? 4 : 2;
+  if (p.epi != SATB_EPI_RESIDUAL && p.epi != SATB_EPI_RESIDUAL_LN) {
+    SATB_REQUIRE(p.out && aligned16(p.out), "gemm probe: out must be a 16-byte aligned device pointer");
+    SATB_REQUIRE(p.ld >= (p.epi == SATB_EPI_SWIGLU ? N / 2 : N) && (p.ld * out_elem) % 16 == 0,
+                 "gemm probe: ld must cover the output row and keep rows 16-byte aligned");
+  } else {
+    SATB_REQUIRE(p.h && aligned16(p.h) && p.ld >= N && p.ld % 4 == 0, "gemm probe: h must be 16-byte aligned, ld >= N, ld % 4 == 0");
+  }
+  for (const void* q : std::initializer_list<const void*>{p.bias, p.gate, p.cos_tab, p.sin_tab, p.x16, p.gamma_lo,
+                                                          p.gamma_hi, p.stats_lo, p.stats_hi, p.ln_stats, p.ln_c, p.ln_d})
+    SATB_REQUIRE(aligned16(q), "gemm probe: every vector must be 16-byte aligned");
+  const bool has_ln = p.ln != 0;
+  if (has_ln) {
+    SATB_REQUIRE(p.epi == SATB_EPI_STORE16 || p.epi == SATB_EPI_QKV_ROPE || p.epi == SATB_EPI_SWIGLU,
+                 "gemm probe: the LayerNorm fold exists for store16, qkv_rope and swiglu only");
+    SATB_REQUIRE(p.ln_stats && p.ln_c && p.ln_n_slots >= 1 && p.ln_n_slots <= kLnSlots, "gemm probe: LayerNorm fold needs stats and c");
+  }
+  switch (p.epi) {
+    case SATB_EPI_STORE32: {
+      const EpiStore32::Params ep{static_cast<float*>(p.out), p.ld, p.bias};
+      if (bn == 64) return probe_run<EpiStore32, 64, BF16>(a, w, M, N, K, ep, p.b_static, st);
+      if (bn == 256) return probe_run<EpiStore32, 256, BF16>(a, w, M, N, K, ep, p.b_static, st);
+      break;
+    }
+    case SATB_EPI_STORE16: {
+      if (has_ln) {
+        typedef EpiStore16<BF16, true> E;
+        const typename E::Params ep{p.out, p.ld, p.bias, p.act, ln};
+        if (bn == 128) return probe_run<E, 128, BF16>(a, w, M, N, K, ep, p.b_static, st);
+        if (bn == 256) return probe_run<E, 256, BF16>(a, w, M, N, K, ep, p.b_static, st);
+      } else {
+        typedef EpiStore16<BF16> E;
+        const typename E::Params ep{p.out, p.ld, p.bias, p.act};
+        if (bn == 128) return probe_run<E, 128, BF16>(a, w, M, N, K, ep, p.b_static, st);
+        if (bn == 256) return probe_run<E, 256, BF16>(a, w, M, N, K, ep, p.b_static, st);
+      }
+      break;
+    }
+    case SATB_EPI_HEAD_NORM16: {
+      SATB_REQUIRE(!p.cos_tab || (p.sin_tab && p.seq_len >= 1), "gemm probe: rotary needs sin_tab and seq_len");
+      typedef EpiHeadNorm16<BF16> E;
+      const typename E::Params ep{p.out, p.ld, p.norm_cols, p.rope_cols, p.seq_len, p.cos_tab, p.sin_tab};
+      if (bn == 128) return probe_run<E, 128, BF16>(a, w, M, N, K, ep, p.b_static, st);
+      if (bn == 256) return probe_run<E, 256, BF16>(a, w, M, N, K, ep, p.b_static, st);
+      break;
+    }
+    case SATB_EPI_QKV_ROPE: {
+      SATB_REQUIRE(p.head_dim >= 32 && p.head_dim % 32 == 0 && p.nf % 4 == 0 && p.nf >= 4 && 2 * p.nf <= p.head_dim,
+                   "gemm probe: head_dim must be a multiple of 32 and nf a multiple of 4 with 2 nf <= head_dim");
+      SATB_REQUIRE(!p.cos_tab || (p.sin_tab && p.seq_len >= 1), "gemm probe: rotary needs sin_tab and seq_len");
+      if (bn == 256) {
+        if (has_ln) {
+          typedef EpiQkvRope<BF16, true> E;
+          const typename E::Params ep{p.out, p.ld, p.rope_cols, p.seq_len, p.head_dim, p.nf, p.cos_tab, p.sin_tab, ln};
+          return probe_run<E, 256, BF16>(a, w, M, N, K, ep, p.b_static, st);
+        }
+        typedef EpiQkvRope<BF16> E;
+        const typename E::Params ep{p.out, p.ld, p.rope_cols, p.seq_len, p.head_dim, p.nf, p.cos_tab, p.sin_tab};
+        return probe_run<E, 256, BF16>(a, w, M, N, K, ep, p.b_static, st);
+      }
+      break;
+    }
+    case SATB_EPI_SWIGLU: {
+      if (bn == 256) {
+        if (has_ln) {
+          typedef EpiSwiglu<BF16, true> E;
+          return probe_run<E, 256, BF16>(a, w, M, N, K, typename E::Params{p.out, p.ld, p.bias, ln}, p.b_static, st);
+        }
+        typedef EpiSwiglu<BF16> E;
+        return probe_run<E, 256, BF16>(a, w, M, N, K, typename E::Params{p.out, p.ld, p.bias}, p.b_static, st);
+      }
+      break;
+    }
+    case SATB_EPI_RESIDUAL: {
+      SATB_REQUIRE(!p.gate || (p.rows_per_item >= 1 && p.n_items >= 1 && p.gate_ld % 4 == 0),
+                   "gemm probe: the gate needs rows_per_item, n_items >= 1 and gate_ld % 4 == 0");
+      const EpiResidual::Params ep{p.h, p.ld, p.bias, p.gate, p.rows_per_item, p.gate_ld, p.n_items};
+      if (bn == 128) return probe_run<EpiResidual, 128, BF16>(a, w, M, N, K, ep, p.b_static, st);
+      if (bn == 256) return probe_run<EpiResidual, 256, BF16>(a, w, M, N, K, ep, p.b_static, st);
+      break;
+    }
+    case SATB_EPI_RESIDUAL_LN: {
+      SATB_REQUIRE(p.x16 && p.gamma_hi, "gemm probe: residual_ln needs x16 and gamma_hi");
+      typedef EpiResidualLN<BF16> E;
+      const typename E::Params ep{p.h, p.ld, p.bias, p.x16, p.gamma_lo, p.gamma_hi, static_cast<float2*>(p.stats_lo),
+                                  static_cast<float2*>(p.stats_hi), p.split};
+      if (bn == 256) return probe_run<E, 256, BF16>(a, w, M, N, K, ep, p.b_static, st);
+      break;
+    }
+    default:
+      break;
+  }
+  set_last_error("gemm probe: no such instance (epi " + std::to_string(p.epi) + ", BN " + std::to_string(bn) +
+                 ", ln " + std::to_string(p.ln) +
+                 "); the forward's instances are store32 BN 64/256, store16 (ln 0/1), head_norm16 and residual "
+                 "BN 128/256, qkv_rope (ln 0/1), swiglu (ln 0/1) and residual_ln BN 256");
+  return -1;
+}
+
+extern "C" {
+
+int satb_gemm_probe(const void* a16, const void* w16, int M, int N, int K, const SatbGemmProbe* p, void* stream) {
+  SATB_REQUIRE(a16 && w16 && p, "null argument");
+  SATB_REQUIRE(M >= 1 && N >= 32 && K >= 8 && K % 8 == 0, "gemm probe: need M >= 1, N >= 32 and K % 8 == 0");
+  SATB_REQUIRE(aligned16(a16) && aligned16(w16), "gemm probe: operands must be 16-byte aligned");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return p->bf16 ? gemm_probe<true>(a16, w16, M, N, K, *p, st) : gemm_probe<false>(a16, w16, M, N, K, *p, st);
 }
 
 }  // extern "C"
