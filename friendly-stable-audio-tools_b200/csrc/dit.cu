@@ -700,9 +700,11 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
     {
       ProfScope ps(d, PROF_ATTN_SELF, st);
       const int64_t qs = static_cast<int64_t>(N_seq) * 3 * D;
+      const CUtensorMap* tm = nullptr;   // q, k and v are column ranges of one buffer: one map
+      if (d->dh == 64) SATB_PROPAGATE(d->tmaps.get_a(qkv, 3 * D, N_seq, R, 3 * D, qs, &tm));
       SATB_PROPAGATE(launch_attention_tc(qkv, qkv, qkv, att, 3 * D, 3 * D, 3 * D, D, qs, qs, qs,
                                          static_cast<int64_t>(N_seq) * D, 3 * D, 3 * D, 3 * D, 0, D, 2 * D, R, H, H,
-                                         N_seq, N_seq, d->dh, BF16, st));
+                                         N_seq, N_seq, d->dh, BF16, st, tm, tm, tm));
     }
     {
       ProfScope ps(d, PROF_ATTN_OUT, st);
@@ -738,9 +740,14 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
       }
       const uint16_t* kv = d->ws_kv.as<uint16_t>() + static_cast<size_t>(i) * d->Rc * d->Mctx * 2 * d->ce;
       const int64_t kvs = static_cast<int64_t>(d->Mctx) * 2 * d->ce;
+      const CUtensorMap *tq = nullptr, *tkv = nullptr;   // k and v are column ranges of one buffer: one map
+      if (d->dh == 64) {
+        SATB_PROPAGATE(d->tmaps.get_a(q16, D, N_seq, d->Rc, D, static_cast<int64_t>(N_seq) * D, &tq));
+        SATB_PROPAGATE(d->tmaps.get_a(kv, 2 * d->ce, d->Mctx, d->Rc, 2 * d->ce, kvs, &tkv));
+      }
       SATB_PROPAGATE(launch_attention_tc(q16, kv, kv, att, D, 2 * d->ce, 2 * d->ce, D, static_cast<int64_t>(N_seq) * D,
                                          kvs, kvs, static_cast<int64_t>(N_seq) * D, D, 2 * d->ce, 2 * d->ce, 0, 0,
-                                         d->ce, d->Rc, H, Hkv, N_seq, d->Mctx, d->dh, BF16, st));
+                                         d->ce, d->Rc, H, Hkv, N_seq, d->Mctx, d->dh, BF16, st, tq, tkv, tkv));
       if (fused) {
         typedef EpiResidualLN<BF16> E;
         typename E::Params ep{h, D, nullptr, a16, W.ff_g, W.ff_g, S3, S3, Mc};

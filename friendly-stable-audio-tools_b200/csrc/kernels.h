@@ -1,15 +1,19 @@
 // Internal launch API between translation units (not part of the C ABI).
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 namespace satb {
 
 // ---- attention_tc.cu (tensor-core flash attention; head_dim 32, 64, 96 or 128)
+// Head dim 64 reads q / k / v through tensor maps: make_tmap_a(ptr, cols, rows per item, batch, ld, batch stride) with
+// the default box.  tmq / tmk / tmv may pass such maps cached by the caller; null ones are encoded here.
 int launch_attention_tc(const void* q, const void* k, const void* v, void* o, int64_t ldq, int64_t ldk, int64_t ldv,
                         int64_t ldo, int64_t q_bs, int64_t k_bs, int64_t v_bs, int64_t o_bs, int q_cols, int k_cols,
                         int v_cols, int q_col, int k_col, int v_col, int batch, int H, int H_kv, int Nq, int Nk,
-                        int head_dim, bool bf16, cudaStream_t stream);
+                        int head_dim, bool bf16, cudaStream_t stream, const CUtensorMap* tmq = nullptr,
+                        const CUtensorMap* tmk = nullptr, const CUtensorMap* tmv = nullptr);
 // debugging switches (environment variables; the defaults are the production path)
 bool conv_halo_enabled();     // SATB_CONV_HALO=off: generic per-tap loads for the final conv (A/B debugging)
 bool resunit_use_fused();      // SATB_RESUNIT=unfused runs the 128/256-channel ResidualUnits as two GEMM launches (A/B debugging)
