@@ -218,7 +218,7 @@ conv_halo_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
                           ? reinterpret_cast<float*>(epi_smem + (warp - 4) * Epi::kStageBytes)
                           : nullptr;
       gemm_tile_epilogue<Epi, BN>(acc, reinterpret_cast<float*>(shared + cw * Cfg::kAccStage), epi_st, ep, s.L, s.N,
-                                  m0, 0, 0, batch, cw, warp, lane);
+                                  m0, 0, batch, cw, warp, lane);
     }
   }
 }

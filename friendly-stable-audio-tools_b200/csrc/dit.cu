@@ -107,8 +107,6 @@ struct LayerW {
   uint16_t *w_qkv = nullptr, *w_o = nullptr, *w_q = nullptr, *w_kv = nullptr, *w_co = nullptr, *w_ff1 = nullptr,
            *w_ff2 = nullptr;
   float *b_ff1 = nullptr, *b_ff2 = nullptr;
-  // LayerNorm folded into the following GEMM (LnFold): c = W gamma, d = W beta per output column
-  float *c_qkv = nullptr, *d_qkv = nullptr, *c_q = nullptr, *d_q = nullptr, *c_ff1 = nullptr, *d_ff1 = nullptr;
 };
 
 }  // namespace satb
@@ -123,7 +121,6 @@ struct SatbDit {
   int Pp = 0;                 // prepend-conditioning tokens of the current conditioning
   DevBuf ws_prep;             // their embeddings [B, Pp, D] + scratch
   bool bf16, adaln, qk_norm = false;
-  bool ln_fused = false;   // prepend-mode blocks without qk_norm: no LayerNorm kernels (see dit_forward_impl)
   int P;  // prepended tokens: 1 (the global-conditioning token; 0 in adaLN mode) + Pp
   std::vector<LayerW> layers;
   std::vector<void*> owned;   // every cudaMalloc of weight storage
@@ -143,7 +140,7 @@ struct SatbDit {
   bool cfg_on = false, has_cross = false, has_global = false;
   // workspace
   TmapCache tmaps;
-  DevBuf ws_h, ws_a16, ws_qkv, ws_attn, ws_q16, ws_ff, ws_ain, ws_y, ws_small, ws_cond, ws_kv, ws_rope, ws_stats;
+  DevBuf ws_h, ws_a16, ws_qkv, ws_attn, ws_q16, ws_ff, ws_ain, ws_y, ws_small, ws_cond, ws_kv, ws_rope;
   int rope_len = 0;
   int res_R = 0, res_L = 0, res_P = -1;
   // optional per-category CUDA-event timing (bench.py roofline)
@@ -259,7 +256,7 @@ void satb_dit_destroy(SatbDit* d) {
   for (void* p : d->owned) cudaFree(p);
   d->ws_h.release(); d->ws_a16.release(); d->ws_qkv.release(); d->ws_attn.release(); d->ws_q16.release();
   d->ws_ff.release(); d->ws_ain.release(); d->ws_y.release(); d->ws_small.release(); d->ws_cond.release();
-  d->ws_kv.release(); d->ws_rope.release(); d->ws_stats.release(); d->ws_prep.release();
+  d->ws_kv.release(); d->ws_rope.release(); d->ws_prep.release();
   delete d;
 }
 
@@ -409,36 +406,6 @@ int satb_dit_finalize(SatbDit* d, void* stream_v) {
   cudaFree(tmp_in);
   cudaFree(tmp_out);
   SATB_PROPAGATE(rc);
-  // LayerNorm folded into the consumer GEMMs (opt-in with SATB_LN=fold, plain prepend-mode blocks only; measured slower
-  // than the LayerNorm kernels, see runtime.cu): per-column vectors c = W gamma, d = W beta of every LayerNorm -> Linear pair
-  d->ln_fused = !d->adaln && !d->qk_norm && ln_fold_enabled() && d->D == 6 * 256;
-  if (d->ln_fused) {
-    for (int i = 0; i < d->depth; ++i) {
-      LayerW& L = d->layers[i];
-      auto prep = [&](float** c, float** dd, const uint16_t* w, const float* g, const float* b, int rows) -> int {
-        // beta is a zero buffer in the reference's LayerNorm (transformer.py:200-206): then d = W beta = 0 and the
-        // epilogues skip it (d pointer null)
-        bool has_beta = false;
-        if (b) {
-          std::vector<float> hb(D);
-          SATB_CHECK_CUDA(cudaMemcpy(hb.data(), b, D * sizeof(float), cudaMemcpyDeviceToHost));
-          for (float v : hb) has_beta = has_beta || v != 0.f;
-        }
-        if (!*c) SATB_PROPAGATE(d->alloc(c, rows));
-        float* scratch = nullptr;
-        if (has_beta && !*dd) SATB_PROPAGATE(d->alloc(dd, rows));
-        if (!has_beta) {
-          *dd = nullptr;
-          SATB_PROPAGATE(d->alloc(&scratch, rows));
-        }
-        return launch_ln_fold_vectors(w, g, has_beta ? b : nullptr, *c, has_beta ? *dd : scratch, rows, D, d->bf16, st);
-      };
-      SATB_PROPAGATE(prep(&L.c_qkv, &L.d_qkv, L.w_qkv, L.pre_g, L.pre_b, 3 * D));
-      if (d->ct > 0) SATB_PROPAGATE(prep(&L.c_q, &L.d_q, L.w_q, L.ca_g, L.ca_b, D));
-      SATB_PROPAGATE(prep(&L.c_ff1, &L.d_ff1, L.w_ff1, L.ff_g, L.ff_b, 2 * d->ffi));
-    }
-    SATB_CHECK_CUDA(cudaStreamSynchronize(st));
-  }
   d->tmaps.maps.clear();
   d->finalized = true;
   return 0;
@@ -481,7 +448,6 @@ int satb_dit_reserve(SatbDit* d, int R, int L) {
   SATB_PROPAGATE(d->ws_ff.ensure(M * d->ffi * 2));
   SATB_PROPAGATE(d->ws_ain.ensure(M * d->Cin * 2));
   SATB_PROPAGATE(d->ws_y.ensure(M * d->C * 4));
-  SATB_PROPAGATE(d->ws_stats.ensure(3 * M * kLnSlots * sizeof(float2)));
   SATB_PROPAGATE(ensure_rope(d, N_seq));
   d->tmaps.maps.clear();
   d->res_R = R;
@@ -658,24 +624,11 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
     SATB_PROPAGATE(launch_gate_sigmoid(sw.ssg, B, d->depth, D, st));
   }
 
-  // Plain prepend-mode blocks run WITHOUT LayerNorm kernels (d->ln_fused): every residual GEMM (self out-proj, cross
-  // out-proj, FF-out) writes h, the 16-bit x16 = h * gamma of the LayerNorm that follows and that row's partial
-  // (sum, sum of squares); the GEMM after the LayerNorm reads x16 and applies mean / rstd in its epilogue (LnFold,
-  // gemm.cuh).  Only the very first LayerNorm of the forward (block 0, whose input comes from project_in) is a kernel.
-  // 8 launches per block instead of 11.  adaLN / qk_norm models keep the LayerNorm kernels below.
-  const bool fused = d->ln_fused;
-  float2* S1 = d->ws_stats.as<float2>();                 // partial row sums in front of: the QKV projection
-  float2* S2 = S1 + static_cast<size_t>(M) * kLnSlots;   //   the cross-attention q projection (conditional rows)
-  float2* S3 = S2 + static_cast<size_t>(M) * kLnSlots;   //   the feed-forward input projection
-  auto fold = [&](const float2* st_, const float* c, const float* dd) {
-    return LnFold{st_, c, dd, 1.0f / static_cast<float>(D), 1e-5f, kLnSlots};
-  };
-  const LnFold no_ln{nullptr, nullptr, nullptr, 0.f, 0.f, 0};
   for (int i = 0; i < d->depth; ++i) {
     const LayerW& W = d->layers[i];
     const float* ssg_l = d->adaln ? sw.ssg + static_cast<size_t>(i) * 6 * D : nullptr;
     // ---- self-attention: LN -> QKV GEMM (+RoPE) -> attention -> out-proj (+residual)
-    if (!fused || i == 0) {
+    {
       ProfScope ps(d, PROF_LN, st);
       SATB_PROPAGATE(launch_layernorm(h, W.pre_g, W.pre_b, a16, M, D, ssg_l, ssg_l ? ssg_l + D : nullptr, ssg_ld, N_seq, B, BF16, st));
     }
@@ -686,15 +639,9 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
         typename E::Params ep{qkv, 3 * D, 2 * D, 2 * D, N_seq, cos_tab, sin_tab};
         SATB_PROPAGATE((linear<E, 256, BF16>(d->tmaps, a16, D, M, D, W.w_qkv, 3 * D, ep, st)));
       } else {
-        if (fused && i > 0) {
-          typedef EpiQkvRope<BF16, true> E;
-          typename E::Params ep{qkv, 3 * D, 2 * D, N_seq, d->dh, d->nf, cos_tab, sin_tab, fold(S1, W.c_qkv, W.d_qkv)};
-          SATB_PROPAGATE((linear<E, 256, BF16>(d->tmaps, a16, D, M, D, W.w_qkv, 3 * D, ep, st)));
-        } else {
-          typedef EpiQkvRope<BF16> E;
-          typename E::Params ep{qkv, 3 * D, 2 * D, N_seq, d->dh, d->nf, cos_tab, sin_tab, no_ln};
-          SATB_PROPAGATE((linear<E, 256, BF16>(d->tmaps, a16, D, M, D, W.w_qkv, 3 * D, ep, st)));
-        }
+        typedef EpiQkvRope<BF16> E;
+        typename E::Params ep{qkv, 3 * D, 2 * D, N_seq, d->dh, d->nf, cos_tab, sin_tab};
+        SATB_PROPAGATE((linear<E, 256, BF16>(d->tmaps, a16, D, M, D, W.w_qkv, 3 * D, ep, st)));
       }
     }
     {
@@ -708,35 +655,22 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
     }
     {
       ProfScope ps(d, PROF_ATTN_OUT, st);
-      if (fused) {
-        // rows < Mc go on to the cross-attention LayerNorm, the others straight to the feed-forward LayerNorm
-        typedef EpiResidualLN<BF16> E;
-        typename E::Params ep{h, D, nullptr, a16, W.ca_g, W.ff_g, S2, S3, Mc};
-        SATB_PROPAGATE((linear<E, 256, BF16>(d->tmaps, att, D, M, D, W.w_o, D, ep, st)));
-      } else {
-        EpiResidual::Params ep{h, D, nullptr, ssg_l ? ssg_l + 2 * D : nullptr, N_seq, static_cast<int>(ssg_ld), B};
-        SATB_PROPAGATE((linear_auto<EpiResidual, BF16>(d->tmaps, att, D, M, D, W.w_o, D, ep, st)));
-      }
+      EpiResidual::Params ep{h, D, nullptr, ssg_l ? ssg_l + 2 * D : nullptr, N_seq, static_cast<int>(ssg_ld), B};
+      SATB_PROPAGATE((linear_auto<EpiResidual, BF16>(d->tmaps, att, D, M, D, W.w_o, D, ep, st)));
     }
     // ---- cross-attention on the rows that have a non-null context
     if (Mc > 0) {
       ProfScope ps(d, PROF_CROSS, st);
       const int Hkv = d->ce / d->dh;
-      if (!fused) SATB_PROPAGATE(launch_layernorm(h, W.ca_g, W.ca_b, a16, Mc, D, nullptr, nullptr, 0, N_seq, 1, BF16, st));
+      SATB_PROPAGATE(launch_layernorm(h, W.ca_g, W.ca_b, a16, Mc, D, nullptr, nullptr, 0, N_seq, 1, BF16, st));
       if (d->qk_norm) {
         typedef EpiHeadNorm16<BF16> E;
         typename E::Params ep{q16, D, D, 0, N_seq, nullptr, nullptr};
         SATB_PROPAGATE((linear_auto<E, BF16>(d->tmaps, a16, D, Mc, D, W.w_q, D, ep, st)));
       } else {
-        if (fused) {
-          typedef EpiStore16<BF16, true> E;
-          typename E::Params ep{q16, D, nullptr, 0, fold(S2, W.c_q, W.d_q)};
-          SATB_PROPAGATE((linear_auto<E, BF16>(d->tmaps, a16, D, Mc, D, W.w_q, D, ep, st)));
-        } else {
-          typedef EpiStore16<BF16> E;
-          typename E::Params ep{q16, D, nullptr, 0, no_ln};
-          SATB_PROPAGATE((linear_auto<E, BF16>(d->tmaps, a16, D, Mc, D, W.w_q, D, ep, st)));
-        }
+        typedef EpiStore16<BF16> E;
+        typename E::Params ep{q16, D, nullptr, 0};
+        SATB_PROPAGATE((linear_auto<E, BF16>(d->tmaps, a16, D, Mc, D, W.w_q, D, ep, st)));
       }
       const uint16_t* kv = d->ws_kv.as<uint16_t>() + static_cast<size_t>(i) * d->Rc * d->Mctx * 2 * d->ce;
       const int64_t kvs = static_cast<int64_t>(d->Mctx) * 2 * d->ce;
@@ -748,51 +682,31 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
       SATB_PROPAGATE(launch_attention_tc(q16, kv, kv, att, D, 2 * d->ce, 2 * d->ce, D, static_cast<int64_t>(N_seq) * D,
                                          kvs, kvs, static_cast<int64_t>(N_seq) * D, D, 2 * d->ce, 2 * d->ce, 0, 0,
                                          d->ce, d->Rc, H, Hkv, N_seq, d->Mctx, d->dh, BF16, st, tq, tkv, tkv));
-      if (fused) {
-        typedef EpiResidualLN<BF16> E;
-        typename E::Params ep{h, D, nullptr, a16, W.ff_g, W.ff_g, S3, S3, Mc};
-        SATB_PROPAGATE((linear<E, 256, BF16>(d->tmaps, att, D, Mc, D, W.w_co, D, ep, st)));
-      } else {
-        EpiResidual::Params ep{h, D, nullptr, nullptr, N_seq, 0, 1};
-        SATB_PROPAGATE((linear_auto<EpiResidual, BF16>(d->tmaps, att, D, Mc, D, W.w_co, D, ep, st)));
-      }
+      EpiResidual::Params ep{h, D, nullptr, nullptr, N_seq, 0, 1};
+      SATB_PROPAGATE((linear_auto<EpiResidual, BF16>(d->tmaps, att, D, Mc, D, W.w_co, D, ep, st)));
     }
     // ---- feed-forward: LN -> GEMM (+bias, SwiGLU) -> GEMM (+bias, +residual)
-    if (!fused) {
+    {
       ProfScope ps(d, PROF_LN, st);
       SATB_PROPAGATE(launch_layernorm(h, W.ff_g, W.ff_b, a16, M, D, ssg_l ? ssg_l + 3 * D : nullptr,
                                       ssg_l ? ssg_l + 4 * D : nullptr, ssg_ld, N_seq, B, BF16, st));
     }
     {
       ProfScope ps(d, PROF_FF_IN, st);
-      if (fused) {
-        typedef EpiSwiglu<BF16, true> E;
-        typename E::Params ep{ff, d->ffi, W.b_ff1, fold(S3, W.c_ff1, W.d_ff1)};
-        SATB_PROPAGATE((linear<E, 256, BF16>(d->tmaps, a16, D, M, D, W.w_ff1, 2 * d->ffi, ep, st)));
-      } else {
-        typedef EpiSwiglu<BF16> E;
-        typename E::Params ep{ff, d->ffi, W.b_ff1, no_ln};
-        SATB_PROPAGATE((linear<E, 256, BF16>(d->tmaps, a16, D, M, D, W.w_ff1, 2 * d->ffi, ep, st)));
-      }
+      typedef EpiSwiglu<BF16> E;
+      typename E::Params ep{ff, d->ffi, W.b_ff1};
+      SATB_PROPAGATE((linear<E, 256, BF16>(d->tmaps, a16, D, M, D, W.w_ff1, 2 * d->ffi, ep, st)));
     }
     {
       ProfScope ps(d, PROF_FF_OUT, st);
-      if (fused) {
-        // prepares the next block's first LayerNorm; after the last block x16 is the plain 16-bit copy project_out reads
-        const bool last = i + 1 == d->depth;
-        typedef EpiResidualLN<BF16> E;
-        typename E::Params ep{h, D, W.b_ff2, a16, last ? nullptr : d->layers[i + 1].pre_g, nullptr, last ? nullptr : S1, nullptr, M};
-        SATB_PROPAGATE((linear<E, 256, BF16>(d->tmaps, ff, d->ffi, M, d->ffi, W.w_ff2, D, ep, st)));
-      } else {
-        EpiResidual::Params ep{h, D, W.b_ff2, ssg_l ? ssg_l + 5 * D : nullptr, N_seq, static_cast<int>(ssg_ld), B};
-        SATB_PROPAGATE((linear_auto<EpiResidual, BF16>(d->tmaps, ff, d->ffi, M, d->ffi, W.w_ff2, D, ep, st)));
-      }
+      EpiResidual::Params ep{h, D, W.b_ff2, ssg_l ? ssg_l + 5 * D : nullptr, N_seq, static_cast<int>(ssg_ld), B};
+      SATB_PROPAGATE((linear_auto<EpiResidual, BF16>(d->tmaps, ff, d->ffi, M, d->ffi, W.w_ff2, D, ep, st)));
     }
   }
   if (hidden_out)
     SATB_CHECK_CUDA(cudaMemcpyAsync(hidden_out, h, static_cast<size_t>(M) * D * 4, cudaMemcpyDeviceToDevice, st));
-  // project_out (with the 1x1 post-conv folded) needs 16-bit input: the last FF-out epilogue already wrote it, or cast
-  if (!fused || d->depth == 0) SATB_PROPAGATE(launch_cast_rows(h, a16, nullptr, M, D, D, D, BF16, st));
+  // project_out (with the 1x1 post-conv folded) reads a 16-bit copy of h
+  SATB_PROPAGATE(launch_cast_rows(h, a16, nullptr, M, D, D, D, BF16, st));
   SATB_PROPAGATE((linear<EpiStore32, 64, BF16>(d->tmaps, a16, D, M, D, d->w_out16, C, EpiStore32::Params{y, C, nullptr}, st)));
   SATB_PROPAGATE(launch_dit_post(y, out, B, C, L, N_seq, P, d->cfg_on ? 1 : 0, cfg_scale, scale_phi, st));
   return 0;
@@ -870,24 +784,16 @@ static int probe_run(const void* a, const void* w, int M, int N, int K, const ty
 template <bool BF16>
 static int gemm_probe(const void* a, const void* w, int M, int N, int K, const SatbGemmProbe& p, cudaStream_t st) {
   const int bn = p.bn;
-  const LnFold ln{static_cast<const float2*>(p.ln_stats), p.ln_c, p.ln_d, p.ln_inv_dim, p.ln_eps, p.ln_n_slots};
   const int out_elem = p.epi == SATB_EPI_STORE32 ? 4 : 2;
-  if (p.epi != SATB_EPI_RESIDUAL && p.epi != SATB_EPI_RESIDUAL_LN) {
+  if (p.epi != SATB_EPI_RESIDUAL) {
     SATB_REQUIRE(p.out && aligned16(p.out), "gemm probe: out must be a 16-byte aligned device pointer");
     SATB_REQUIRE(p.ld >= (p.epi == SATB_EPI_SWIGLU ? N / 2 : N) && (p.ld * out_elem) % 16 == 0,
                  "gemm probe: ld must cover the output row and keep rows 16-byte aligned");
   } else {
     SATB_REQUIRE(p.h && aligned16(p.h) && p.ld >= N && p.ld % 4 == 0, "gemm probe: h must be 16-byte aligned, ld >= N, ld % 4 == 0");
   }
-  for (const void* q : std::initializer_list<const void*>{p.bias, p.gate, p.cos_tab, p.sin_tab, p.x16, p.gamma_lo,
-                                                          p.gamma_hi, p.stats_lo, p.stats_hi, p.ln_stats, p.ln_c, p.ln_d})
+  for (const void* q : std::initializer_list<const void*>{p.bias, p.gate, p.cos_tab, p.sin_tab})
     SATB_REQUIRE(aligned16(q), "gemm probe: every vector must be 16-byte aligned");
-  const bool has_ln = p.ln != 0;
-  if (has_ln) {
-    SATB_REQUIRE(p.epi == SATB_EPI_STORE16 || p.epi == SATB_EPI_QKV_ROPE || p.epi == SATB_EPI_SWIGLU,
-                 "gemm probe: the LayerNorm fold exists for store16, qkv_rope and swiglu only");
-    SATB_REQUIRE(p.ln_stats && p.ln_c && p.ln_n_slots >= 1 && p.ln_n_slots <= kLnSlots, "gemm probe: LayerNorm fold needs stats and c");
-  }
   switch (p.epi) {
     case SATB_EPI_STORE32: {
       const EpiStore32::Params ep{static_cast<float*>(p.out), p.ld, p.bias};
@@ -896,17 +802,10 @@ static int gemm_probe(const void* a, const void* w, int M, int N, int K, const S
       break;
     }
     case SATB_EPI_STORE16: {
-      if (has_ln) {
-        typedef EpiStore16<BF16, true> E;
-        const typename E::Params ep{p.out, p.ld, p.bias, p.act, ln};
-        if (bn == 128) return probe_run<E, 128, BF16>(a, w, M, N, K, ep, p.b_static, st);
-        if (bn == 256) return probe_run<E, 256, BF16>(a, w, M, N, K, ep, p.b_static, st);
-      } else {
-        typedef EpiStore16<BF16> E;
-        const typename E::Params ep{p.out, p.ld, p.bias, p.act};
-        if (bn == 128) return probe_run<E, 128, BF16>(a, w, M, N, K, ep, p.b_static, st);
-        if (bn == 256) return probe_run<E, 256, BF16>(a, w, M, N, K, ep, p.b_static, st);
-      }
+      typedef EpiStore16<BF16> E;
+      const typename E::Params ep{p.out, p.ld, p.bias, p.act};
+      if (bn == 128) return probe_run<E, 128, BF16>(a, w, M, N, K, ep, p.b_static, st);
+      if (bn == 256) return probe_run<E, 256, BF16>(a, w, M, N, K, ep, p.b_static, st);
       break;
     }
     case SATB_EPI_HEAD_NORM16: {
@@ -922,11 +821,6 @@ static int gemm_probe(const void* a, const void* w, int M, int N, int K, const S
                    "gemm probe: head_dim must be a multiple of 32 and nf a multiple of 4 with 2 nf <= head_dim");
       SATB_REQUIRE(!p.cos_tab || (p.sin_tab && p.seq_len >= 1), "gemm probe: rotary needs sin_tab and seq_len");
       if (bn == 256) {
-        if (has_ln) {
-          typedef EpiQkvRope<BF16, true> E;
-          const typename E::Params ep{p.out, p.ld, p.rope_cols, p.seq_len, p.head_dim, p.nf, p.cos_tab, p.sin_tab, ln};
-          return probe_run<E, 256, BF16>(a, w, M, N, K, ep, p.b_static, st);
-        }
         typedef EpiQkvRope<BF16> E;
         const typename E::Params ep{p.out, p.ld, p.rope_cols, p.seq_len, p.head_dim, p.nf, p.cos_tab, p.sin_tab};
         return probe_run<E, 256, BF16>(a, w, M, N, K, ep, p.b_static, st);
@@ -935,10 +829,6 @@ static int gemm_probe(const void* a, const void* w, int M, int N, int K, const S
     }
     case SATB_EPI_SWIGLU: {
       if (bn == 256) {
-        if (has_ln) {
-          typedef EpiSwiglu<BF16, true> E;
-          return probe_run<E, 256, BF16>(a, w, M, N, K, typename E::Params{p.out, p.ld, p.bias, ln}, p.b_static, st);
-        }
         typedef EpiSwiglu<BF16> E;
         return probe_run<E, 256, BF16>(a, w, M, N, K, typename E::Params{p.out, p.ld, p.bias}, p.b_static, st);
       }
@@ -952,21 +842,12 @@ static int gemm_probe(const void* a, const void* w, int M, int N, int K, const S
       if (bn == 256) return probe_run<EpiResidual, 256, BF16>(a, w, M, N, K, ep, p.b_static, st);
       break;
     }
-    case SATB_EPI_RESIDUAL_LN: {
-      SATB_REQUIRE(p.x16 && p.gamma_hi, "gemm probe: residual_ln needs x16 and gamma_hi");
-      typedef EpiResidualLN<BF16> E;
-      const typename E::Params ep{p.h, p.ld, p.bias, p.x16, p.gamma_lo, p.gamma_hi, static_cast<float2*>(p.stats_lo),
-                                  static_cast<float2*>(p.stats_hi), p.split};
-      if (bn == 256) return probe_run<E, 256, BF16>(a, w, M, N, K, ep, p.b_static, st);
-      break;
-    }
     default:
       break;
   }
   set_last_error("gemm probe: no such instance (epi " + std::to_string(p.epi) + ", BN " + std::to_string(bn) +
-                 ", ln " + std::to_string(p.ln) +
-                 "); the forward's instances are store32 BN 64/256, store16 (ln 0/1), head_norm16 and residual "
-                 "BN 128/256, qkv_rope (ln 0/1), swiglu (ln 0/1) and residual_ln BN 256");
+                 "); the forward's instances are store32 BN 64/256, store16, head_norm16 and residual BN 128/256, "
+                 "qkv_rope and swiglu BN 256");
   return -1;
 }
 

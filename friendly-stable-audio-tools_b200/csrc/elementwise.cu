@@ -350,42 +350,7 @@ __global__ void gather_f32_kernel(const float* __restrict__ src, float* __restri
   if (i < n) dst[i] = src[perm ? perm[i] : i];
 }
 
-// c[n] = sum_k W16[n, k] gamma[k], d[n] = sum_k W16[n, k] beta[k]  (one warp per output row; see LnFold in gemm.cuh)
-template <bool BF16>
-__global__ void __launch_bounds__(256) ln_fold_vectors_kernel(const uint16_t* __restrict__ w, const float* __restrict__ gamma,
-                                                              const float* __restrict__ beta, float* __restrict__ c,
-                                                              float* __restrict__ d, int rows, int K) {
-  const int n = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (n >= rows) return;
-  const uint32_t* wr = reinterpret_cast<const uint32_t*>(w + static_cast<size_t>(n) * K);
-  float sc = 0.f, sd = 0.f;
-  for (int k2 = lane; k2 < (K >> 1); k2 += 32) {
-    const float2 wv = Op16<BF16>::unpack(wr[k2]);
-    sc = fmaf(wv.x, gamma[2 * k2], fmaf(wv.y, gamma[2 * k2 + 1], sc));
-    if (beta) sd = fmaf(wv.x, beta[2 * k2], fmaf(wv.y, beta[2 * k2 + 1], sd));
-  }
-  sc = warp_sum(sc);
-  sd = warp_sum(sd);
-  if (lane == 0) {
-    c[n] = sc;
-    d[n] = sd;
-  }
-}
-
 }  // namespace
-
-int launch_ln_fold_vectors(const void* w16, const float* gamma, const float* beta, float* c, float* d, int rows, int K,
-                           bool bf16, cudaStream_t stream) {
-  SATB_REQUIRE(K % 2 == 0, "ln fold: K must be even");
-  const int grid = ceil_div(rows, 8);
-  if (bf16)
-    ln_fold_vectors_kernel<true><<<grid, 256, 0, stream>>>(static_cast<const uint16_t*>(w16), gamma, beta, c, d, rows, K);
-  else
-    ln_fold_vectors_kernel<false><<<grid, 256, 0, stream>>>(static_cast<const uint16_t*>(w16), gamma, beta, c, d, rows, K);
-  count_launch();
-  SATB_CHECK_CUDA(cudaGetLastError());
-  return 0;
-}
 
 int launch_layernorm(const float* x, const float* gamma, const float* beta, void* out16, int rows, int D,
                      const float* scale, const float* shift, int64_t mod_stride, int rows_per_item, int n_items,

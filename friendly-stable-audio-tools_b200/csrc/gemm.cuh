@@ -14,8 +14,6 @@
 //                                      fused epilogue (accumulator -> smem -> one row per thread -> fused op -> global)
 // The producer runs ahead into the next tile's k-blocks while the epilogue of the current one runs.
 #pragma once
-#include <type_traits>
-
 #include "common.cuh"
 #include "ptx.cuh"
 
@@ -76,34 +74,6 @@ struct EpiCtx {
   int L;         // rows per batch item
   int lane;
   float* stage;  // per-warp staging smem (Epi::kStageBytes), or nullptr
-  int n_tile;    // index of the tile along N
-  int half;      // which of the two epilogue warps of the lane quadrant (they take alternate column chunks)
-};
-
-// Epilogues may carry per-thread state across the column chunks of one tile (e.g. the row sums that feed the next
-// LayerNorm): such an epilogue declares `State`, `tile_begin`, `apply(p, c, r, state)` and `tile_end`; all others keep
-// the plain `apply(p, c, r)`.
-template <class E, class = void>
-struct EpiHasState : std::false_type {};
-template <class E>
-struct EpiHasState<E, std::void_t<typename E::State>> : std::true_type {};
-struct EpiNoStateHolder {
-  struct State {};
-};
-template <class Epi>
-struct EpiTile {
-  using State = typename std::conditional<EpiHasState<Epi>::value, Epi, EpiNoStateHolder>::type::State;
-  template <int N>
-  __device__ static __forceinline__ void apply(const typename Epi::Params& p, const EpiCtx& c, const uint32_t (&r)[N], State& st) {
-    if constexpr (EpiHasState<Epi>::value) Epi::apply(p, c, r, st);
-    else Epi::apply(p, c, r);
-  }
-  __device__ static __forceinline__ void begin(const typename Epi::Params& p, const EpiCtx& c, State& st) {
-    if constexpr (EpiHasState<Epi>::value) Epi::tile_begin(p, c, st);
-  }
-  __device__ static __forceinline__ void end(const typename Epi::Params& p, const EpiCtx& c, State& st) {
-    if constexpr (EpiHasState<Epi>::value) Epi::tile_end(p, c, st);
-  }
 };
 
 // Epilogue of one 128 x BN tile, run by MMA warpgroup cw (rows [64 cw, 64 cw + 64)) on its accumulator fragment.
@@ -112,8 +82,8 @@ struct EpiTile {
 // expect).  epi_st: the epilogue's own per-warp staging (Epi::kStageBytes), or null.
 template <class Epi, int BN>
 __device__ __forceinline__ void gemm_tile_epilogue(const float (&acc)[BN / 2], float* acc_st, float* epi_st,
-                                                   const typename Epi::Params& ep, int L, int N, int m0, int n0, int nt,
-                                                   int batch, int cw, int warp, int lane) {
+                                                   const typename Epi::Params& ep, int L, int N, int m0, int n0, int batch,
+                                                   int cw, int warp, int lane) {
   const int wq = warp & 3;           // warp within the warpgroup
   const int half = wq >> 1;          // warps 0, 1 take the even column chunks, warps 2, 3 the odd ones
   const int rsub = (wq & 1) * 32;    // rows [rsub, rsub + 32) of the warpgroup's 64
@@ -129,13 +99,9 @@ __device__ __forceinline__ void gemm_tile_epilogue(const float (&acc)[BN / 2], f
   c.valid = c.l < L;
   c.L = L;
   c.lane = lane;
-  c.n_tile = nt;
-  c.half = half;
   c.stage = epi_st;
   int n_valid = (N - n0 + Epi::kCols - 1) / Epi::kCols;   // chunks that hold real columns (warp-uniform)
   if (n_valid > kChunks) n_valid = kChunks;
-  typename EpiTile<Epi>::State est;
-  EpiTile<Epi>::begin(ep, c, est);
 #pragma unroll
   for (int cp = 0; cp < (kChunks + 1) / 2; ++cp) {
     named_bar_sync(1 + cw, 128);   // the previous chunk pair has been read out
@@ -166,10 +132,9 @@ __device__ __forceinline__ void gemm_tile_epilogue(const float (&acc)[BN / 2], f
         r[4 * j + 3] = __float_as_uint(v.w);
       }
       c.col0 = n0 + ci * Epi::kCols;
-      EpiTile<Epi>::apply(ep, c, r, est);
+      Epi::apply(ep, c, r);
     }
   }
-  EpiTile<Epi>::end(ep, c, est);
 }
 template <class Epi, int BN, bool BF16>
 __global__ void __launch_bounds__(kGemmThreads, 1)
@@ -305,7 +270,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       wgmma_wait<0>(acc);
       if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
 
-      gemm_tile_epilogue<Epi, BN>(acc, acc_st, epi_st, ep, s.L, s.N, m0, n0, nt, batch, cw, warp, lane);
+      gemm_tile_epilogue<Epi, BN>(acc, acc_st, epi_st, ep, s.L, s.N, m0, n0, batch, cw, warp, lane);
     }
   }
 }
@@ -314,61 +279,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 // Every epilogue receives kCols consecutive fp32 accumulator columns of one row
 // (as raw bits in r[]) and writes them straight to global memory.
 
-// ---- LayerNorm folded into the consumer GEMM (prepend-mode DiT blocks) --------------------------------------------
-// The producer of the residual stream (EpiResidualLN below) stores x16 = 16-bit(h * gamma) next to h and accumulates the
-// row sums s1 = sum h, s2 = sum h^2.  With c[n] = sum_k gamma_k W[n,k] and d[n] = sum_k beta_k W[n,k] (prepared once),
-//   LayerNorm(h) W^T = rstd (h gamma) W^T - rstd mean c + d,   mean = s1 / D, rstd = rsqrt(s2 / D - mean^2 + eps)
-// (models/transformer.py:188-206 followed by the Linear), so the consumer GEMM reads x16 and its epilogue applies one
-// multiply-add per element: no LayerNorm pass over the residual stream, no extra kernel.
-constexpr int kLnSlots = 12;   // partial sums per row: 6 column tiles of 256 x 2 epilogue warps (D = 1536); fixed
-                               // slots summed in a fixed order keep the result bit-reproducible (no atomics)
-struct LnFold {
-  const float2* stats;   // [rows][n_slots] partial (s1, s2) of the residual row, or null: no LayerNorm in front
-  const float* c;        // [N]
-  const float* d;        // [N] or null (beta = 0)
-  float inv_dim;         // 1 / D
-  float eps;
-  int n_slots;
-};
-struct LnRow {
-  float rstd, mr;        // rstd, mean * rstd
-};
-__device__ __forceinline__ LnRow ln_row(const LnFold& f, int row) {
-  const float4* sp = reinterpret_cast<const float4*>(f.stats + static_cast<size_t>(row) * kLnSlots);
-  float s1 = 0.f, s2 = 0.f;
-#pragma unroll
-  for (int i = 0; i < kLnSlots / 2; ++i) {
-    if (2 * i < f.n_slots) {
-      const float4 v = __ldg(sp + i);
-      s1 += v.x + v.z;
-      s2 += v.y + v.w;
-    }
-  }
-  const float mean = s1 * f.inv_dim;
-  const float var = fmaxf(s2 * f.inv_dim - mean * mean, 0.f);
-  LnRow r;
-  r.rstd = rsqrtf(var + f.eps);
-  r.mr = mean * r.rstd;
-  return r;
-}
-// v[0..3] <- rstd * v - (mean rstd) * c[col..col+3] (+ d[col..col+3]); col % 4 == 0 (128-bit loads of c / d)
-__device__ __forceinline__ void ln_apply4(const LnFold& f, const LnRow& r, float& v0, float& v1, float& v2, float& v3, int col) {
-  const float4 cc = __ldg(reinterpret_cast<const float4*>(f.c + col));
-  v0 = fmaf(v0, r.rstd, -r.mr * cc.x);
-  v1 = fmaf(v1, r.rstd, -r.mr * cc.y);
-  v2 = fmaf(v2, r.rstd, -r.mr * cc.z);
-  v3 = fmaf(v3, r.rstd, -r.mr * cc.w);
-  if (f.d) {
-    const float4 dd = __ldg(reinterpret_cast<const float4*>(f.d + col));
-    v0 += dd.x; v1 += dd.y; v2 += dd.z; v3 += dd.w;
-  }
-}
-
 __device__ __forceinline__ float silu_f(float x) { return x / (1.0f + __expf(-x)); }
 
 // out16[row, col] = act(acc + bias)   (act: 0 none, 1 SiLU)
-template <bool BF16, bool LN = false>   // LN: a LayerNorm is folded into this GEMM (LnFold); separate instantiation so that
-struct EpiStore16 {                      // the plain epilogue carries none of its code or registers
+template <bool BF16>
+struct EpiStore16 {
   static constexpr int kCols = 32;
   static constexpr int kStageBytes = 0;
   struct Params {
@@ -376,18 +291,12 @@ struct EpiStore16 {                      // the plain epilogue carries none of i
     int ld;
     const float* bias;  // may be null
     int act;
-    LnFold ln = LnFold{nullptr, nullptr, nullptr, 0.f, 0.f, 0};
   };
   __device__ static __forceinline__ void apply(const Params& p, const EpiCtx& c, const uint32_t (&r)[32]) {
     if (!c.valid) return;
     float v[32];
 #pragma unroll
     for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-    if constexpr (LN) {
-      const LnRow lr = ln_row(p.ln, c.row);
-#pragma unroll
-      for (int j = 0; j < 32; j += 4) ln_apply4(p.ln, lr, v[j], v[j + 1], v[j + 2], v[j + 3], c.col0 + j);
-    }
     if (p.bias) {
 #pragma unroll
       for (int j = 0; j < 32; j += 4) {
@@ -476,99 +385,6 @@ struct EpiResidual {
   }
 };
 
-// Residual stream update that also prepares the NEXT LayerNorm (see LnFold): h = h + acc + bias is written back in
-// fp32 (plain load / store: every element belongs to exactly one lane of one tile), x16 = 16-bit(h * gamma) is what
-// the next GEMM reads, and the partial row sums of this tile go to a fixed slot of stats.  Rows below `split` are
-// followed by one LayerNorm (gamma_lo, stats_lo: the cross-attention norm of the conditional rows), the others by
-// another (gamma_hi, stats_hi: the feed-forward norm of rows without cross-attention).
-template <bool BF16>
-struct EpiResidualLN {
-  static constexpr int kCols = 32;
-  static constexpr int kStageBytes = 32 * 36 * 4;   // per-warp [32 rows][32 + 4 pad] fp32 transpose tile
-  struct Params {
-    float* h;
-    int ld;
-    const float* bias;       // may be null
-    void* x16;               // [rows, ld] 16-bit
-    const float* gamma_lo;   // may be null (= 1)
-    const float* gamma_hi;
-    float2* stats_lo;        // may be null (no LayerNorm follows: last block)
-    float2* stats_hi;
-    int split;               // rows < split: *_lo, else *_hi
-  };
-  // Warp-cooperative like EpiConv: the accumulator chunk (thread = row, 32 columns) goes through the per-warp smem
-  // tile so that every global access is a coalesced 128 B row segment (8 lanes x 16 B, 4 rows per instruction); the
-  // old h values are requested BEFORE the transpose so the loads are in flight meanwhile.  Lane = (row offset
-  // lane / 8 within groups of 4 rows, 4-column group lane % 8): it owns rows l0 + lane / 8 + 4 i, i < 8.
-  struct State {
-    float s1[8], s2[8];
-  };
-  __device__ static __forceinline__ void tile_begin(const Params&, const EpiCtx&, State& st) {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) st.s1[i] = st.s2[i] = 0.f;
-  }
-  __device__ static __forceinline__ void apply(const Params& p, const EpiCtx& c, const uint32_t (&r)[32], State& st) {
-    const int g = c.lane & 7, r0 = c.lane >> 3;
-    const int col = c.col0 + 4 * g;
-    float4 old[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int l = c.l0 + r0 + 4 * i;
-      old[i] = l < c.L ? *reinterpret_cast<const float4*>(p.h + (static_cast<size_t>(c.batch) * c.L + l) * p.ld + col)
-                       : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    float* stg = c.stage;
-    {
-      float4* mine = reinterpret_cast<float4*>(stg + c.lane * 36);
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-        mine[j] = make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]), __uint_as_float(r[4 * j + 2]),
-                              __uint_as_float(r[4 * j + 3]));
-    }
-    __syncwarp();
-    float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f), glo = make_float4(1.f, 1.f, 1.f, 1.f), ghi = glo;
-    if (p.bias) b4 = __ldg(reinterpret_cast<const float4*>(p.bias + col));
-    if (p.gamma_lo) glo = __ldg(reinterpret_cast<const float4*>(p.gamma_lo + col));
-    if (p.gamma_hi) ghi = __ldg(reinterpret_cast<const float4*>(p.gamma_hi + col));
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int l = c.l0 + r0 + 4 * i;
-      if (l < c.L) {
-        const size_t row = static_cast<size_t>(c.batch) * c.L + l;
-        const float4 a = *reinterpret_cast<const float4*>(stg + (r0 + 4 * i) * 36 + 4 * g);
-        float4 v;
-        v.x = a.x + b4.x + old[i].x; v.y = a.y + b4.y + old[i].y; v.z = a.z + b4.z + old[i].z; v.w = a.w + b4.w + old[i].w;
-        *reinterpret_cast<float4*>(p.h + row * p.ld + col) = v;
-        st.s1[i] += (v.x + v.y) + (v.z + v.w);
-        st.s2[i] = fmaf(v.x, v.x, fmaf(v.y, v.y, fmaf(v.z, v.z, fmaf(v.w, v.w, st.s2[i]))));
-        const float4 gg = static_cast<int>(row) < p.split ? glo : ghi;
-        *reinterpret_cast<uint2*>(static_cast<uint16_t*>(p.x16) + row * p.ld + col) =
-            make_uint2(Op16<BF16>::pack(v.x * gg.x, v.y * gg.y), Op16<BF16>::pack(v.z * gg.z, v.w * gg.w));
-      }
-    }
-    __syncwarp();
-  }
-  __device__ static __forceinline__ void tile_end(const Params& p, const EpiCtx& c, State& st) {
-    const int g = c.lane & 7, r0 = c.lane >> 3;
-    const int slot = c.n_tile * 2 + c.half;      // one writer per (row, slot): plain store, summed by ln_row in order
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      float a = st.s1[i], b = st.s2[i];
-#pragma unroll
-      for (int o = 1; o < 8; o <<= 1) {            // the 8 lanes of a row segment (same lane / 8)
-        a += __shfl_xor_sync(0xffffffffu, a, o);
-        b += __shfl_xor_sync(0xffffffffu, b, o);
-      }
-      const int l = c.l0 + r0 + 4 * i;
-      if (g == 0 && l < c.L && slot < kLnSlots) {
-        const size_t row = static_cast<size_t>(c.batch) * c.L + l;
-        float2* sp = static_cast<int>(row) < p.split ? p.stats_lo : p.stats_hi;
-        if (sp) sp[row * kLnSlots + slot] = make_float2(a, b);
-      }
-    }
-  }
-};
-
 // Fused QKV projection epilogue: split is implicit (q | k | v are column ranges of
 // one [M, 3D] buffer); partial rotary of every q and k head (models/transformer.py:158-183,
 // 438-452), position = token index within the sequence (prepend token = position 0).  fp32
@@ -578,7 +394,7 @@ struct EpiResidualLN {
 // chunk ci = (col % head_dim) / 32 rotates its first clamp(nf - 16 ci, 0, 16) pairs with the
 // table columns 16 ci + i, and the rest of the head passes through.  q and k share the
 // permutation, so every q . k is unchanged.  Head dim 64: identity; chunk 0 rotates 16 pairs.
-template <bool BF16, bool LN = false>
+template <bool BF16>
 struct EpiQkvRope {
   static constexpr int kCols = 32;
   static constexpr int kStageBytes = 0;
@@ -591,18 +407,12 @@ struct EpiQkvRope {
     int nf;            // rotary frequencies per head (table row stride): 16, 16, 24, 32
     const float* cos_tab;  // [seq_len, nf]
     const float* sin_tab;  // [seq_len, nf]
-    LnFold ln = LnFold{nullptr, nullptr, nullptr, 0.f, 0.f, 0};
   };
   __device__ static __forceinline__ void apply(const Params& p, const EpiCtx& c, const uint32_t (&r)[32]) {
     if (!c.valid) return;
     float v[32];
 #pragma unroll
     for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-    if constexpr (LN) {
-      const LnRow lr = ln_row(p.ln, c.row);
-#pragma unroll
-      for (int j = 0; j < 32; j += 4) ln_apply4(p.ln, lr, v[j], v[j + 1], v[j + 2], v[j + 3], c.col0 + j);
-    }
     // chunk of 32 columns aligned to 32 (head_dim is a multiple of 32): its rotary pairs (i, i + 16), i < n_rot
     const int ci = (c.col0 % p.head_dim) >> 5;
     const int n_rot = min(max(p.nf - 16 * ci, 0), 16);   // 16 or 8 (head dim 96, chunk 1) or 0
@@ -699,7 +509,7 @@ struct EpiHeadNorm16 {
 // half of the projection).  The weight rows are interleaved at load time so every
 // 64-column group holds 32 value columns followed by their 32 gate columns:
 //   out[row, g*32 + j] = (acc[g*64 + j] + b) * silu(acc[g*64 + 32 + j] + b')
-template <bool BF16, bool LN = false>
+template <bool BF16>
 struct EpiSwiglu {
   static constexpr int kCols = 64;
   static constexpr int kStageBytes = 0;
@@ -707,52 +517,23 @@ struct EpiSwiglu {
     void* out;
     int ld;             // inner dim (N/2)
     const float* bias;  // interleaved like the weight rows; may be null
-    LnFold ln = LnFold{nullptr, nullptr, nullptr, 0.f, 0.f, 0};
   };
   __device__ static __forceinline__ void apply(const Params& p, const EpiCtx& c, const uint32_t (&r)[64]) {
     if (!c.valid) return;
-    // four value columns and their four gate columns at a time, straight from the accumulator registers (a 64-float
+    // two value columns and their two gate columns at a time, straight from the accumulator registers (a 64-float
     // working copy next to the two 64-register chunk buffers of the epilogue loop spills)
     uint32_t o[16];
-    if constexpr (!LN) {
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        float a0 = __uint_as_float(r[2 * j]), a1 = __uint_as_float(r[2 * j + 1]);
-        float g0 = __uint_as_float(r[32 + 2 * j]), g1 = __uint_as_float(r[33 + 2 * j]);
-        if (p.bias) {
-          a0 += __ldg(p.bias + c.col0 + 2 * j);
-          a1 += __ldg(p.bias + c.col0 + 2 * j + 1);
-          g0 += __ldg(p.bias + c.col0 + 32 + 2 * j);
-          g1 += __ldg(p.bias + c.col0 + 33 + 2 * j);
-        }
-        o[j] = Op16<BF16>::pack(a0 * silu_f(g0), a1 * silu_f(g1));
-      }
-      uint4* dst0 =
-          reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.out) + static_cast<size_t>(c.row) * p.ld + (c.col0 >> 1));
-#pragma unroll
-      for (int j = 0; j < 4; ++j) dst0[j] = make_uint4(o[4 * j], o[4 * j + 1], o[4 * j + 2], o[4 * j + 3]);
-      return;
-    }
-    LnRow lr{1.f, 0.f};
-    if constexpr (LN) lr = ln_row(p.ln, c.row);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      float a0 = __uint_as_float(r[4 * j]), a1 = __uint_as_float(r[4 * j + 1]), a2 = __uint_as_float(r[4 * j + 2]),
-            a3 = __uint_as_float(r[4 * j + 3]);
-      float g0 = __uint_as_float(r[32 + 4 * j]), g1 = __uint_as_float(r[33 + 4 * j]), g2 = __uint_as_float(r[34 + 4 * j]),
-            g3 = __uint_as_float(r[35 + 4 * j]);
-      if constexpr (LN) {
-        ln_apply4(p.ln, lr, a0, a1, a2, a3, c.col0 + 4 * j);
-        ln_apply4(p.ln, lr, g0, g1, g2, g3, c.col0 + 32 + 4 * j);
-      }
+    for (int j = 0; j < 16; ++j) {
+      float a0 = __uint_as_float(r[2 * j]), a1 = __uint_as_float(r[2 * j + 1]);
+      float g0 = __uint_as_float(r[32 + 2 * j]), g1 = __uint_as_float(r[33 + 2 * j]);
       if (p.bias) {
-        const float4 ba = __ldg(reinterpret_cast<const float4*>(p.bias + c.col0 + 4 * j));
-        const float4 bg = __ldg(reinterpret_cast<const float4*>(p.bias + c.col0 + 32 + 4 * j));
-        a0 += ba.x; a1 += ba.y; a2 += ba.z; a3 += ba.w;
-        g0 += bg.x; g1 += bg.y; g2 += bg.z; g3 += bg.w;
+        a0 += __ldg(p.bias + c.col0 + 2 * j);
+        a1 += __ldg(p.bias + c.col0 + 2 * j + 1);
+        g0 += __ldg(p.bias + c.col0 + 32 + 2 * j);
+        g1 += __ldg(p.bias + c.col0 + 33 + 2 * j);
       }
-      o[2 * j] = Op16<BF16>::pack(a0 * silu_f(g0), a1 * silu_f(g1));
-      o[2 * j + 1] = Op16<BF16>::pack(a2 * silu_f(g2), a3 * silu_f(g3));
+      o[j] = Op16<BF16>::pack(a0 * silu_f(g0), a1 * silu_f(g1));
     }
     uint4* dst =
         reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.out) + static_cast<size_t>(c.row) * p.ld + (c.col0 >> 1));
@@ -831,10 +612,13 @@ struct EpiConvParams {
                         // 8 instead of 12 bytes per element and channel through a fused ResidualUnit (the sums
                         // are still formed in fp32; only the value carried to the next unit's skip is rounded)
 };
-// MASKED = true: the kernel carries ONLY the lean path (one index per chunk, per-segment validity as a bit mask, Snake and
-// 16-bit raw streams unconditional) - for launches whose Params satisfy fast_flags(); the host picks the instantiation
-// (oobleck.cu run_conv_gemm).  Compiled next to the general path in one kernel the lean path pays ~200 bytes of spills
-// in the persistent GEMM kernels (long-scoreboard stalls on the reloads, profiles/r02_ncu_convT_s2.txt).
+// MASKED = true: the kernel carries ONLY the lean path - for launches whose Params satisfy fast_flags(); the host picks
+// the instantiation (oobleck.cu run_conv_gemm).  The general path costs ~120 instructions per 4-element segment, ~55 %
+// of them index arithmetic, bounds tests and branches on the launch-uniform Params flags, and the 128-channel layers
+// are bound by exactly this epilogue.  The lean path computes one index per chunk (the 8 segments of a lane are
+// idx0 + i * stride), keeps per-segment validity as a bit mask and makes Snake and the 16-bit raw streams
+// unconditional.  Compiled next to the general path in one kernel it pays ~200 bytes of spills in the persistent GEMM
+// kernels (long-scoreboard stalls on the reloads, profiles/r02_ncu_convT_s2.txt).
 template <bool BF16, bool MASKED = false>
 struct EpiConv {
   static constexpr int kCols = 32;
@@ -870,91 +654,18 @@ struct EpiConv {
     *idx = (static_cast<size_t>(c.batch) * p.L_out + (ok ? lo : 0)) * p.cout + sg.co;
     return ok;
   }
-  // ---- fast path.  The general code below costs ~120 instructions per 4-element segment, of which ~55 % are index
-  // arithmetic, bounds tests and branches on the (launch-uniform) Params flags (ncu source page of the stride-2
-  // transposed convolution, profiles/r02_ncu_convT_s2.txt: 30 instructions per element; the 128-channel layers are
-  // bound by exactly this epilogue).  For a chunk whose 32 rows all exist - every chunk but the ragged ends of an item -
-  // the 8 segments of a lane are idx0 + i * stride, so one index, one bounds test and one branch per chunk do;
-  // the flags become template parameters.  Conditions: 16-bit raw streams (or none), a 16-bit output, no lo copy.
+  // ---- lean path (MASKED): the same arithmetic for every chunk, ragged ones included (mask bit i: segment i exists)
   struct Plan {
-    size_t idx0;      // element index of segment 0
-    int stride;       // elements between consecutive segments (4 rows)
-    bool fast;        // warp-uniform
-    int co;
-  };
-  __device__ static __forceinline__ Plan plan_of(const Params& p, const EpiCtx& c) {
-    const Seg sg = seg_of(p, c);
-    const int l_first = c.l0 + (c.lane >> 3), l_last = l_first + 28;
-    const int lo_first = l_first * p.up + sg.phase - p.pad, lo_last = l_last * p.up + sg.phase - p.pad;
-    const bool ok = l_last < c.L && lo_first >= 0 && lo_last < p.L_out;
-    // (Moving the general path out of line instead - __noinline__ - made the decode 40-90 % SLOWER: the call sites
-    // force the chunk registers through local memory.)
-    const bool flags = fast_flags(p);
-    Plan pl;
-    pl.fast = flags && __all_sync(0xffffffffu, ok);
-    pl.idx0 = (static_cast<size_t>(c.batch) * p.L_out + (ok ? lo_first : 0)) * p.cout + sg.co;
-    pl.stride = 4 * p.up * p.cout;
-    pl.co = sg.co;
-    return pl;
-  }
-  template <bool RESID, bool RAWOUT, bool SNAKE>
-  __device__ static __forceinline__ void finish_fast(const Params& p, const EpiCtx& c, const Plan& pl, const uint32_t (&r)[32],
-                                                     const float4 (&rs)[8]) {
-    const uint32_t st = smem_u32(c.stage);
-    const int g = c.lane & 7, r0 = c.lane >> 3;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) sts128(st + (c.lane * 36 + 4 * j) * 4, r[4 * j], r[4 * j + 1], r[4 * j + 2], r[4 * j + 3]);
-    __syncwarp();
-    ulonglong2 b2 = make_ulonglong2(0ull, 0ull), a2 = b2, ib2 = b2;   // (x,y) and (z,w) pairs; 0 bits = 0.f
-    if (p.bias) b2 = __ldg(reinterpret_cast<const ulonglong2*>(p.bias + pl.co));
-    if (SNAKE) {
-      a2 = __ldg(reinterpret_cast<const ulonglong2*>(p.sn_a + pl.co));
-      ib2 = __ldg(reinterpret_cast<const ulonglong2*>(p.sn_ib + pl.co));
-    }
-    uint16_t* raw_o = static_cast<uint16_t*>(p.raw_out) + pl.idx0;
-    uint16_t* s_o = static_cast<uint16_t*>(p.s16_out) + pl.idx0;
-    uint32_t ld_addr = st + (r0 * 36 + 4 * g) * 4;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const ulonglong2 acc = lds128_b64x2(ld_addr);   // (reading all eight segments back first was not faster)
-      ld_addr += 4 * 36 * 4;
-      uint64_t v01 = f2_add(acc.x, b2.x), v23 = f2_add(acc.y, b2.y);
-      if (RESID) {
-        const float2 lo = Op16<BF16>::unpack(__float_as_uint(rs[i].x)), hi = Op16<BF16>::unpack(__float_as_uint(rs[i].y));
-        v01 = f2_add(v01, f2_pack(lo.x, lo.y));
-        v23 = f2_add(v23, f2_pack(hi.x, hi.y));
-      }
-      if (RAWOUT) {
-        float y0, y1, y2, y3;
-        f2_unpack(v01, y0, y1);
-        f2_unpack(v23, y2, y3);
-        *reinterpret_cast<uint2*>(raw_o) = make_uint2(Op16<BF16>::pack(y0, y1), Op16<BF16>::pack(y2, y3));
-        raw_o += pl.stride;
-      }
-      if (SNAKE) {
-        v01 = snake_fast2(v01, a2.x, ib2.x);
-        v23 = snake_fast2(v23, a2.y, ib2.y);
-      }
-      float x0, x1, x2, x3;
-      f2_unpack(v01, x0, x1);
-      f2_unpack(v23, x2, x3);
-      *reinterpret_cast<uint2*>(s_o) = make_uint2(Op16<BF16>::pack(x0, x1), Op16<BF16>::pack(x2, x3));
-      s_o += pl.stride;
-    }
-    __syncwarp();
-  }
-  // ---- MASKED kernels: the same arithmetic for every chunk, ragged ones included (bit i of the mask = segment i exists)
-  struct MPlan {
     long long idx0;   // element index of segment 0 (may point before the buffer when that segment does not exist)
     int stride;
     uint32_t mask;
     int co;
   };
-  __device__ static __forceinline__ MPlan mplan_of(const Params& p, const EpiCtx& c) {
+  __device__ static __forceinline__ Plan chunk_plan(const Params& p, const EpiCtx& c) {
     const Seg sg = seg_of(p, c);
     const int l0 = c.l0 + (c.lane >> 3);
     const int lo0 = l0 * p.up + sg.phase - p.pad;
-    MPlan pl;
+    Plan pl;
     pl.mask = 0;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -968,7 +679,7 @@ struct EpiConv {
   }
   __device__ static __forceinline__ void prefetch_masked(const Params& p, const EpiCtx& c, float4 (&rs)[8]) {
     if (p.resid) {
-      const MPlan pl = mplan_of(p, c);
+      const Plan pl = chunk_plan(p, c);
       const uint16_t* rp = static_cast<const uint16_t*>(p.resid) + pl.idx0;
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
@@ -982,7 +693,7 @@ struct EpiConv {
   template <bool RESID, bool RAWOUT>
   __device__ static __forceinline__ void finish_masked_t(const Params& p, const EpiCtx& c, const uint32_t (&r)[32],
                                                          const float4 (&rs)[8]) {
-    const MPlan pl = mplan_of(p, c);
+    const Plan pl = chunk_plan(p, c);
     const uint32_t st = smem_u32(c.stage);
     const int g = c.lane & 7, r0 = c.lane >> 3;
 #pragma unroll
@@ -1027,7 +738,7 @@ struct EpiConv {
                                                        const float4 (&rs)[8]) {
     if (p.resid) {
       if (p.raw_out) finish_masked_t<true, true>(p, c, r, rs);
-      else finish_masked_t<true, false>(p, c, r, rs);
+      else finish_masked_t<true, false>(p, c, r, rs);    // last unit of a block: nobody reads its raw output
     } else {
       if (p.raw_out) finish_masked_t<false, true>(p, c, r, rs);
       else finish_masked_t<false, false>(p, c, r, rs);
@@ -1038,21 +749,6 @@ struct EpiConv {
     if constexpr (MASKED) {
       prefetch_masked(p, c, rs);
       return;
-    }
-    {
-      const Plan pl = plan_of(p, c);
-      if (pl.fast) {
-        if (p.resid) {
-          const uint16_t* rp = static_cast<const uint16_t*>(p.resid) + pl.idx0;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const uint2 u = *reinterpret_cast<const uint2*>(rp);     // the loaded BITS (converted in finish())
-            rp += pl.stride;
-            rs[i] = make_float4(__uint_as_float(u.x), __uint_as_float(u.y), 0.f, 0.f);
-          }
-        }
-        return;
-      }
     }
     const Seg sg = seg_of(p, c);
 #pragma unroll
@@ -1077,19 +773,6 @@ struct EpiConv {
     if constexpr (MASKED) {
       finish_masked(p, c, r, rs);
       return;
-    }
-    {
-      const Plan pl = plan_of(p, c);
-      if (pl.fast) {
-        if (p.resid) {
-          if (p.raw_out) finish_fast<true, true, true>(p, c, pl, r, rs);
-          else finish_fast<true, false, true>(p, c, pl, r, rs);    // last unit of a block: nobody reads its raw output
-        } else {
-          if (p.raw_out) finish_fast<false, true, true>(p, c, pl, r, rs);
-          else finish_fast<false, false, true>(p, c, pl, r, rs);
-        }
-        return;
-      }
     }
     float* st = c.stage;
     const int g = c.lane & 7, r0 = c.lane >> 3;

@@ -14,22 +14,12 @@ int launch_attention_tc(const void* q, const void* k, const void* v, void* o, in
                         int v_cols, int q_col, int k_col, int v_col, int batch, int H, int H_kv, int Nq, int Nk,
                         int head_dim, bool bf16, cudaStream_t stream, const CUtensorMap* tmq = nullptr,
                         const CUtensorMap* tmk = nullptr, const CUtensorMap* tmv = nullptr);
-// debugging switches (environment variables; the defaults are the production path)
-bool conv_halo_enabled();     // SATB_CONV_HALO=off: generic per-tap loads for the final conv (A/B debugging)
-bool resunit_use_fused();      // SATB_RESUNIT=unfused runs the 128/256-channel ResidualUnits as two GEMM launches (A/B debugging)
-bool conv_epi_masked();        // SATB_CONV_EPI=general keeps the combined-epilogue GEMM kernels for the 16-bit convolutions (A/B debugging)
-bool ln_fold_enabled();        // SATB_LN=fold: LayerNorm folded into the GEMM epilogues (A/B; measured slower, off by default)
-bool raw_stream_16bit();       // SATB_RAW=fp32 keeps the Oobleck skip stream in fp32 (A/B debugging)
 
 // ---- elementwise.cu
 // LayerNorm over the last dim (eps 1e-5), optional adaLN modulation y*(1+scale)+shift, 16-bit output.
 int launch_layernorm(const float* x, const float* gamma, const float* beta, void* out16, int rows, int D,
                      const float* scale, const float* shift, int64_t mod_stride, int rows_per_item, int n_items,
                      bool bf16, cudaStream_t stream);
-// c[n] = sum_k W16[n,k] gamma[k], d[n] = sum_k W16[n,k] beta[k] (beta may be null -> d = 0): the per-column vectors of a
-// LayerNorm folded into the GEMM that follows it (gemm.cuh: LnFold)
-int launch_ln_fold_vectors(const void* w16, const float* gamma, const float* beta, float* c, float* d, int rows, int K,
-                           bool bf16, cudaStream_t stream);
 // Fused VDenoiser scaling + multistep sampler update + noise (see elementwise.cu).
 int launch_sampler_update(const float* x, const float* v, const float* d1, const float* d2, const float* nz, float* den,
                           float* x_next, float* x_in, long long n, float c_skip, float c_out, float A, float B, float C,

@@ -15,6 +15,7 @@
 #include <algorithm>
 #include <cmath>
 #include <tuple>
+#include <type_traits>
 #include <map>
 #include <string>
 #include <vector>
@@ -334,7 +335,7 @@ int run_conv_gemm(SatbOobleck* h, const ConvW& cw, const void* in16, int B, int 
                   const typename Epi::Params& ep, cudaStream_t st) {
   // the default 16-bit decode / encode runs the lean-epilogue instantiation of the GEMM kernels (EpiConv<.., MASKED>)
   if constexpr (std::is_same<Epi, EpiConv<BF16, false>>::value) {
-    if (Epi::fast_flags(ep) && conv_epi_masked())
+    if (Epi::fast_flags(ep))
       return run_conv_gemm<EpiConv<BF16, true>, BF16>(h, cw, in16, B, L_in, kind, dil, factor, ep, st);
   }
   GemmShape s;
@@ -390,7 +391,7 @@ int residual_unit(SatbOobleck* h, const std::string& pfx, int C, int B, int L, i
   typedef EpiConv<BF16> E;
   typename E::Params e1{c1.bias, raw, keep_raw ? raw : nullptr, sA, next_snake ? next_snake->a : nullptr,
                         next_snake ? next_snake->ib : nullptr, C, L, 1, 0, h->split3 ? static_cast<char*>(sA) + h->lo_off : nullptr, h->raw16};
-  if ((C == 128 || C == 256) && c7.k == 7 && 6 * dil <= kHaloMax && resunit_use_fused() && !h->split3) {
+  if ((C == 128 || C == 256) && c7.k == 7 && 6 * dil <= kHaloMax && !h->split3) {
     // one kernel: conv7 -> snake2 -> conv1 -> + skip; reads sA (with a halo), so it must write elsewhere
     const CUtensorMap *ta, *tb7, *tb1;
     SATB_PROPAGATE(get_tmap_a(h, sA, C, L, B, L, 1, &ta, kBlockM + 6 * dil));   // one halo box per k-block
@@ -399,7 +400,7 @@ int residual_unit(SatbOobleck* h, const std::string& pfx, int C, int B, int L, i
     e1.s16_out = sT;
     const HaloShape hs{L, B, C, 7, dil, C};
     const ResUnitPre pre{c7.bias, s2.a, s2.ib};
-    if (E::fast_flags(e1) && conv_epi_masked()) {
+    if (E::fast_flags(e1)) {
       typedef EpiConv<BF16, true> EM;
       SATB_PROPAGATE(C == 128 ? (launch_conv_halo<EM, 128, BF16, true>(*ta, *tb7, tb1, hs, pre, e1, st))
                               : (launch_conv_halo<EM, 256, BF16, true>(*ta, *tb7, tb1, hs, pre, e1, st)));
@@ -487,8 +488,7 @@ int decode_impl(SatbOobleck* h, const float* z, float* audio, int B, int L, cuda
   {
     const ConvW& cf = h->convs.at("layers." + std::to_string(n + 2) + ".");
     EpiStoreNCL::Params ep{audio, nullptr, cf.cout, static_cast<int>(Lc), c.final_tanh};
-    if (conv_halo_enabled() && !h->split3 && cf.cout <= 64 && cf.cin % kBlockK == 0 && cf.k % 2 == 1 &&
-        cf.k - 1 <= kHaloMax) {
+    if (!h->split3 && cf.cout <= 64 && cf.cin % kBlockK == 0 && cf.k % 2 == 1 && cf.k - 1 <= kHaloMax) {
       // every activation row is fetched once per tile instead of once per tap (see conv_halo.cuh)
       const CUtensorMap *ta, *tb;
       SATB_PROPAGATE(get_tmap_a(h, sA, cf.cin, static_cast<int>(Lc), B, static_cast<int>(Lc), 1, &ta, kBlockM + cf.k - 1));
@@ -585,8 +585,8 @@ int satb_oobleck_create(const SatbOobleckConfig* cfg, SatbOobleck** out) {
   h->split3 = cfg->operand_dtype == 2;
   // fp16 operands: the un-activated skip stream is carried in fp16 as well (8 instead of 12 bytes per element and
   // channel through a fused ResidualUnit; measured +23 % on the fp16-operand error floor, tests/test_gpu_baseline_size).
-  // bf16 (8 mantissa bits) keeps the fp32 stream.  SATB_RAW=fp32 restores fp32 for A/B measurements.
-  h->raw16 = (!h->bf16 && !h->split3 && raw_stream_16bit()) ? 1 : 0;
+  // bf16 (8 mantissa bits) keeps the fp32 stream.
+  h->raw16 = (!h->bf16 && !h->split3) ? 1 : 0;
   h->chans.push_back(cfg->channels);
   for (int i = 0; i < cfg->n_stages; ++i) h->chans.push_back(cfg->c_mults[i] * cfg->channels);
   *out = h;

@@ -6,7 +6,6 @@
 #include "common.cuh"
 #include "gemm.cuh"
 #include "kernels.h"
-#include <cstdlib>
 
 namespace satb {
 
@@ -15,54 +14,6 @@ unsigned long long g_launch_count = 0;
 
 void set_last_error(const std::string& msg) { g_last_error = msg; }
 const char* get_last_error() { return g_last_error.c_str(); }
-
-bool ln_fold_enabled() {
-  // Opt-in (SATB_LN=fold): the fold removes the LayerNorm kernels but makes the residual and QKV epilogues heavier
-  // (they read h, write h + x16 + partial sums, and load the per-column vector c), so the LayerNorm kernels stay the
-  // default (DESIGN.md section 4).
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SATB_LN");
-    v = (e && std::string(e) == "fold") ? 1 : 0;
-  }
-  return v == 1;
-}
-
-bool raw_stream_16bit() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SATB_RAW");
-    v = (e && std::string(e) == "fp32") ? 0 : 1;
-  }
-  return v == 1;
-}
-
-bool conv_halo_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SATB_CONV_HALO");   // "off": generic per-tap loads (A/B debugging)
-    v = (e && std::string(e) == "off") ? 0 : 1;
-  }
-  return v == 1;
-}
-
-bool resunit_use_fused() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SATB_RESUNIT");
-    v = (e && std::string(e) == "unfused") ? 0 : 1;
-  }
-  return v == 1;
-}
-
-bool conv_epi_masked() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SATB_CONV_EPI");    // "general": the combined fast + general epilogue kernels (A/B debugging)
-    v = (e && std::string(e) == "general") ? 0 : 1;
-  }
-  return v == 1;
-}
 
 int device_sm_count() {
   static int cached[64] = {};

@@ -41,17 +41,15 @@ class SatbOobleckConfig(ctypes.Structure):
 _VP, _I, _LL, _F = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong, ctypes.c_float
 
 # satb_gemm_probe (tests only): epilogue kinds and the parameter block, in the order of include/satb200.h
-EPI_STORE32, EPI_STORE16, EPI_HEAD_NORM16, EPI_QKV_ROPE, EPI_SWIGLU, EPI_RESIDUAL, EPI_RESIDUAL_LN = range(7)
+EPI_STORE32, EPI_STORE16, EPI_HEAD_NORM16, EPI_QKV_ROPE, EPI_SWIGLU, EPI_RESIDUAL = range(6)
+EPI_RESIDUAL_LN = 6   # retired (the LayerNorm-fold residual epilogue): refused, and the number is not reused
 
 
 class SatbGemmProbe(ctypes.Structure):
     _fields_ = ([(n, _I) for n in ("epi", "bn", "bf16", "b_static")] + [("out", _VP), ("ld", _I), ("bias", _VP),
                 ("act", _I), ("h", _VP), ("gate", _VP)]
                 + [(n, _I) for n in ("rows_per_item", "gate_ld", "n_items", "rope_cols", "seq_len", "head_dim", "nf")]
-                + [("cos_tab", _VP), ("sin_tab", _VP), ("norm_cols", _I), ("x16", _VP), ("gamma_lo", _VP),
-                   ("gamma_hi", _VP), ("stats_lo", _VP), ("stats_hi", _VP), ("split", _I), ("ln", _I),
-                   ("ln_stats", _VP), ("ln_c", _VP), ("ln_d", _VP), ("ln_inv_dim", _F), ("ln_eps", _F),
-                   ("ln_n_slots", _I)])
+                + [("cos_tab", _VP), ("sin_tab", _VP), ("norm_cols", _I)])
 
 
 SIGNATURES = {

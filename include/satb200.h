@@ -116,42 +116,30 @@ int satb_layernorm(const float* x, const float* gamma, const float* beta, void* 
  * without bias (F.linear call sites transformer.py:422-430,548). */
 int satb_linear_f32out(const void* a16, const void* w16, float* c, int M, int N, int K, int bf16, void* stream);
 /* Test entry point (no product path calls it): C = A[M, K] * W[N, K]^T through ONE of the fused-epilogue GEMM
- * instances the DiT forward launches, chosen by `epi`, `bn`, `bf16` and `ln`.  The instances: store32 BN 64 / 256;
- * store16 (ln 0 / 1), head_norm16 and residual BN 128 / 256; qkv_rope (ln 0 / 1), swiglu (ln 0 / 1) and residual_ln
- * BN 256; anything else returns an error.  The remaining fields are the epilogue's parameters (csrc/gemm.cuh); all
- * pointers are device pointers, 16-byte aligned; fields an epilogue does not use are ignored. */
+ * instances the DiT forward launches, chosen by `epi`, `bn` and `bf16`.  The instances: store32 BN 64 / 256;
+ * store16, head_norm16 and residual BN 128 / 256; qkv_rope and swiglu BN 256; anything else returns an error.  The
+ * remaining fields are the epilogue's parameters (csrc/gemm.cuh); all pointers are device pointers, 16-byte aligned;
+ * fields an epilogue does not use are ignored. */
 #define SATB_EPI_STORE32 0      /* out fp32 = acc (+ bias) */
 #define SATB_EPI_STORE16 1      /* out 16-bit = act(acc (+ bias)) */
 #define SATB_EPI_HEAD_NORM16 2  /* 64-wide heads, L2-normalised below norm_cols, rotary (nf 16) below rope_cols */
 #define SATB_EPI_QKV_ROPE 3     /* partial rotary of every head below rope_cols */
 #define SATB_EPI_SWIGLU 4       /* out[:, N / 2] = value * silu(gate), 32 / 32 interleaved columns */
 #define SATB_EPI_RESIDUAL 5     /* h += (acc (+ bias)) (* gate) */
-#define SATB_EPI_RESIDUAL_LN 6  /* h += acc (+ bias); x16 = 16-bit(h * gamma); per-row partial sums */
+/* 6 was the LayerNorm-fold residual epilogue, since removed: it is refused, and the number is not reused. */
 typedef struct SatbGemmProbe {
   int epi, bn, bf16, b_static;      /* b_static 1: weight prefetch before the dependency wait, as the forward runs */
   void* out;                        /* store32 (fp32), store16, head_norm16, qkv_rope, swiglu (16-bit) */
-  int ld;                           /* row pitch in elements of out, or of h and x16 */
+  int ld;                           /* row pitch in elements of out, or of h */
   const float* bias;                /* [N] or NULL */
   int act;                          /* store16: 0 none, 1 SiLU */
-  float* h;                         /* residual, residual_ln: fp32 [M, ld] updated in place */
+  float* h;                         /* residual: fp32 [M, ld] updated in place */
   const float* gate;                /* residual: [*, gate_ld] or NULL; row item = (row / rows_per_item) % n_items */
   int rows_per_item, gate_ld, n_items;
   int rope_cols, seq_len, head_dim, nf;   /* rotary: position = row % seq_len; tables [seq_len, nf] */
   const float* cos_tab;
   const float* sin_tab;
   int norm_cols;                    /* head_norm16 */
-  void* x16;                        /* residual_ln: 16-bit [M, ld] */
-  const float* gamma_lo;            /* rows < split (NULL = 1) */
-  const float* gamma_hi;            /* rows >= split */
-  void* stats_lo;                   /* float2 [M, 12] or NULL */
-  void* stats_hi;
-  int split;
-  int ln;                           /* store16, qkv_rope, swiglu: 1 = the LayerNorm-fold instance */
-  const void* ln_stats;             /* float2 [M, 12] partial (sum, sum of squares) per row */
-  const float* ln_c;                /* [N] = W gamma */
-  const float* ln_d;                /* [N] = W beta, or NULL */
-  float ln_inv_dim, ln_eps;
-  int ln_n_slots;
 } SatbGemmProbe;
 int satb_gemm_probe(const void* a16, const void* w16, int M, int N, int K, const SatbGemmProbe* p, void* stream);
 /* One step of the v-objective k-diffusion samplers in a single pass over the latents (replaces the

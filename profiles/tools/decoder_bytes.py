@@ -4,7 +4,7 @@ profiles/tools/decoder_layer_table.py (per-layer table from an ncu launch list),
 
 Every tensor-core convolution reads a 16-bit Snake-activated copy of its input (2 B) and writes the 16-bit activated
 copy for its consumer (2 B); the un-activated skip stream of the ResidualUnits is `raw_bytes` wide (2 with fp16
-operands since round 2, 4 = fp32 with bf16 operands or SATB_RAW=fp32): written by the transposed convolution and by
+operands since round 2, 4 = fp32 with bf16 or fp16x3 operands): written by the transposed convolution and by
 the first two units of a stage, read by all three.  128- and 256-channel units are one fused launch (the conv7 ->
 conv1 intermediate never leaves the SM); 512- and 1024-channel units are two launches.
 """

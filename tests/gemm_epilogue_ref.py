@@ -13,7 +13,7 @@ Bound.  For one output element
   e_out                                half an ulp of the output type: 2^-11 fp16, 2^-8 bf16, 2^-24 fp32;
   e_epi * mag                          the fp32 arithmetic of the epilogue itself (mag: the size of its terms);
   tau                                  an absolute floor for fp16 subnormals.
-The rotary and LayerNorm steps are the oracle's own (oracle/dit_oracle.py).  The two load-time weight layouts of
+The rotary step is the oracle's own (oracle/dit_oracle.py).  The two load-time weight layouts of
 csrc/dit.cu are restated here from their comments (ff_perm, qkv_head_perm), so a test builds a weight in reference
 order and hands the kernel the stored (permuted) one.
 """
@@ -22,10 +22,9 @@ from dataclasses import dataclass
 
 import torch
 
-from oracle.dit_oracle import apply_rotary, layer_norm, rotary_freqs
+from oracle.dit_oracle import apply_rotary, rotary_freqs
 
 BLOCK_M, BLOCK_K = 128, 64
-LN_SLOTS = 12
 SILU_SLOPE_MAX = 1.0998           # max |silu'(x)| (at x ~ 2.4)
 E_EPI = 2.0 ** -21
 E_OUT = {"fp16": 2.0 ** -11, "bf16": 2.0 ** -8, "fp32": 2.0 ** -24}
@@ -205,37 +204,6 @@ def epi_residual(acc, S, h_old, bias=None, gate=None):
     y = h_old.double() + v * g
     return Expect(y, g.abs() * S, (acc.abs() + (bias.double().abs() if bias is not None else 0)) * g.abs()
                   + h_old.double().abs() + y.abs())
-
-
-def ln_slot_sums(h, n_tile_cols=256, kcols=32):
-    """Partial (sum, sum of squares) of every row in the 12 slots EpiResidualLN writes: slot n_tile * 2 + half holds the
-    32-column chunks ci = half, half + 2, ... of column tile n_tile.  float64, [M, 12, 2]."""
-    M, N = h.shape
-    h = h.double()
-    chunk = torch.arange(N, device=h.device) // kcols
-    slot = (torch.arange(N, device=h.device) // n_tile_cols) * 2 + chunk % 2
-    out = torch.zeros(M, LN_SLOTS, 2, dtype=torch.float64, device=h.device)
-    for s in range(min(LN_SLOTS, int(slot.max()) + 1)):
-        sel = slot == s
-        out[:, s, 0] = h[:, sel].sum(1)
-        out[:, s, 1] = (h[:, sel] ** 2).sum(1)
-    return out
-
-
-def check_slot_sums(got, h, slack=1.0):
-    """Ratio of |got - sum| to the fp32 summation bound (n terms: n * 2^-24 * sum |terms|) for every (row, slot,
-    component) of EpiResidualLN's stats.  got: [M, 12, 2]; h: the kernel's own h output."""
-    M, N = h.shape
-    ref = ln_slot_sums(h)
-    absref = ln_slot_sums(h.double().abs())
-    n = N // LN_SLOTS
-    bound = slack * n * 2.0 ** -24 * torch.stack([absref[..., 0], absref[..., 1]], -1) + 1e-30
-    return (got.double() - ref).abs() / bound
-
-
-def layer_norm_ref(h, gamma, beta=None):
-    """The oracle's LayerNorm (models/transformer.py:188-206) in float64."""
-    return layer_norm(h.double(), gamma.double(), None if beta is None else beta.double())
 
 
 # ---------------------------------------------------------------------------------------------------- checker

@@ -73,3 +73,11 @@ def test_no_cpu_fallback_in_the_product_path():
             if f.endswith((".py", ".cu", ".cuh", ".h")):
                 src = open(os.path.join(dirpath, f)).read()
                 assert not re.search(r"^\s*(from|import)\s+oracle\b", src, flags=re.M), f"{f} imports the oracle"
+
+
+def test_library_reads_no_environment_variables():
+    """Every launch route is chosen from the model config and the shape, never from a process-global switch."""
+    for d in (os.path.join(ROOT, "friendly-stable-audio-tools_b200", "csrc"), os.path.join(ROOT, "include")):
+        for f in sorted(os.listdir(d)):
+            if f.endswith((".cu", ".cuh", ".h")):
+                assert "getenv" not in open(os.path.join(d, f)).read(), f"{f} reads an environment variable"

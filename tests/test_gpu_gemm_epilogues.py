@@ -9,7 +9,6 @@ rows), a persistent grid of exactly `sms` and `sms + 1` tiles, N not a multiple 
 and K one k-block deeper than the shared-memory ring.  The last tests pin bit properties of the schedule.
 Each test prints its largest err/bound ratio ("[ratio] ...")."""
 import ctypes
-import math
 
 import pytest
 import torch
@@ -272,139 +271,6 @@ def test_residual(dt, bn, K, has_bias, has_gate):
         assert torch.equal(h[:M, :N], h0[:M, :N] + v), "h is not h_old + v in one fp32 add"
 
 
-# ------------------------------------------------------------------------------------------------- EpiResidualLN
-def _stats_buf(M):
-    s = torch.empty(M + GUARD_ROWS, R.LN_SLOTS, 2, device="cuda")
-    s.view(torch.int32).fill_(NAN_BITS[torch.float32])
-    return s
-
-
-@pytest.mark.parametrize("dt", DTS)
-@pytest.mark.parametrize("M,split,gamma_lo,stats", [(2050, 300, True, True), (1025, 1025, False, False),
-                                                    (8200, 4100, True, True), (129, 64, False, True)])
-def test_residual_ln(dt, M, split, gamma_lo, stats):
-    """h += acc + bias, x16 = 16-bit(h * gamma) with gamma from the correct side of `split` (mid-tile), and the
-    partial row sums: every slot n_tile * 2 + half of the rows on each side, nothing else.  gamma_lo null (= 1) and
-    null stats pointers (the last block) included."""
-    nat = _nat()
-    N = K = 1536
-    tdt = R.TORCH_DT[dt]
-    a, w, g = operands(dt, M, N, K, seed=M + split)
-    bias = torch.randn(N, device="cuda", generator=g) * 0.5
-    glo = (1 + 0.1 * torch.randn(N, device="cuda", generator=g)) if gamma_lo else None
-    ghi = 1 + 0.1 * torch.randn(N, device="cuda", generator=g)
-    h0 = torch.randn(M + GUARD_ROWS, N + GUARD_COLS, device="cuda", generator=g) * 2 + 0.3
-    h = guarded(M, N, torch.float32, h0)
-    x16 = guarded(M, N, tdt)
-    x_before = x16.clone()
-    s_lo, s_hi = (_stats_buf(M), _stats_buf(M)) if stats else (None, None)
-    probe(dt, nat.EPI_RESIDUAL_LN, 256, a, w, M, N, K, h=h, ld=h.shape[1], bias=bias, x16=x16, gamma_lo=glo,
-          gamma_hi=ghi, stats_lo=s_lo, stats_hi=s_hi, split=split)
-    assert_guard(h, h0, M, N, "residual_ln h")
-    assert_guard(x16, x_before, M, N, "residual_ln x16")
-    acc, S = R.accumulate(a, w)
-    report(f"residual_ln {dt} M{M} split{split}",
-           R.check(h[:M, :N], R.epi_residual(acc, S, h0[:M, :N], bias), K, "fp32", 256))
-    s32 = torch.empty(M, N, device="cuda")
-    probe(dt, nat.EPI_STORE32, 256, a, w, M, N, K, out=s32, ld=N, bias=bias)
-    hv = h[:M, :N]
-    assert torch.equal(hv, s32 + h0[:M, :N]), "h is not (acc + bias) + h_old"
-    rows = torch.arange(M, device="cuda")[:, None]
-    gam = torch.where(rows < split, glo if gamma_lo else torch.ones_like(ghi), ghi)
-    assert torch.equal(x16[:M, :N].view(torch.int16), (hv * gam).to(tdt).view(torch.int16)), "x16 != 16-bit(h * gamma)"
-    if stats:
-        for buf, sel in ((s_lo, slice(0, split)), (s_hi, slice(split, M))):
-            ratio = R.check_slot_sums(buf[sel], hv[sel])
-            print(f"[ratio] residual_ln stats {dt} M{M} split{split}: {float(ratio.max()) if ratio.numel() else 0:.3f}")
-            assert torch.isfinite(buf[sel]).all() and float(ratio.max() if ratio.numel() else 0) <= 1.0
-        assert torch.isnan(s_lo[split:]).all() and torch.isnan(s_hi[:split]).all(), "a stats row of the other side written"
-        assert torch.isnan(s_hi[M:]).all(), "a stats guard row written"
-
-
-# ------------------------------------------------------------------------------------------------- LayerNorm fold
-MEANS = [0.0, 1.0, 4.0, 16.0]      # row mean in units of the row's standard deviation (sigma = 1.5)
-
-
-def _ln_case(dt, kind, seed=0):
-    D, rows_per = 1536, 256
-    M = rows_per * len(MEANS)
-    g = torch.Generator(device="cuda").manual_seed(seed)
-    sigma = 1.5
-    mean = torch.tensor(MEANS, device="cuda").repeat_interleave(rows_per)[:, None] * sigma
-    h = (mean + sigma * torch.randn(M, D, device="cuda", generator=g)).float()
-    gamma = 1 + 0.1 * torch.randn(D, device="cuda", generator=g)
-    beta = 0.1 * torch.randn(D, device="cuda", generator=g)
-    return D, M, h, gamma, beta, g
-
-
-@pytest.mark.parametrize("dt", DTS)
-@pytest.mark.parametrize("kind", ["store16", "qkv_rope", "swiglu"])
-def test_ln_fold_consumers(dt, kind):
-    """The LayerNorm-fold instances (SATB_LN=fold): rstd (x16 W^T) - mean rstd c + d with x16 = 16-bit(h gamma),
-    c = W gamma, d = W beta and the 12-slot row sums, against the float64 LayerNorm -> Linear -> epilogue.  Gate per
-    group of rows: |mean| <= sigma within 2x the error of the plain path (LayerNorm kernel -> 16-bit -> the same GEMM
-    and epilogue), offset rows within 2x that times sqrt(1 + mean^2 / sigma^2) (the fold rounds h gamma before the
-    mean is taken out)."""
-    nat = _nat()
-    tdt = R.TORCH_DT[dt]
-    D, M, h, gamma, beta, g = _ln_case(dt, kind)
-    seq = 1025
-    if kind == "qkv_rope":
-        N, nf = 3 * D, 16
-        w_ref, w_st, perm = qkv_weight(D, 64, seed=5)
-        cos, sin, freqs = R.rope_tables(seq, nf)
-        extra = dict(rope_cols=2 * D, seq_len=seq, head_dim=64, nf=nf, cos_tab=cos.cuda(), sin_tab=sin.cuda())
-        epi, ld = nat.EPI_QKV_ROPE, N
-    elif kind == "swiglu":
-        N = 8 * D
-        w_ref, w_st, perm = swiglu_weight(D, 4 * D, seed=6, gate_std=2.0)
-        bias_ref = (torch.randn(N) * 0.1).cuda()
-        extra = dict(bias=bias_ref[perm.cuda()].contiguous())
-        epi, ld = nat.EPI_SWIGLU, N // 2
-    else:
-        N = D
-        w_ref = torch.randn(N, D, generator=torch.Generator().manual_seed(7)) * D ** -0.5
-        w_st, perm = w_ref, torch.arange(N)
-        extra = dict(act=0)
-        epi, ld = nat.EPI_STORE16, N
-    w_ref, w_st = w_ref.to(tdt).cuda(), w_st.to(tdt).cuda()
-    # fold inputs: x16, the slot sums (fp32), c and d from the stored 16-bit weight
-    x16 = (h * gamma).to(tdt)
-    stats = R.ln_slot_sums(h).float().contiguous()
-    c = (w_st.double() @ gamma.double()).float()
-    d = (w_st.double() @ beta.double()).float()
-    out_f = guarded(M, ld, tdt)
-    before = out_f.clone()
-    probe(dt, epi, 256, x16, w_st, M, N, D, out=out_f, ld=out_f.shape[1], ln=1, ln_stats=stats, ln_c=c, ln_d=d,
-          ln_inv_dim=1.0 / D, ln_eps=1e-5, ln_n_slots=R.LN_SLOTS, **extra)
-    assert_guard(out_f, before, M, ld, "ln fold")
-    # plain path on the same data
-    a16 = torch.empty(M, D, dtype=tdt, device="cuda")
-    nat.check(nat.lib().satb_layernorm(h.data_ptr(), gamma.data_ptr(), beta.data_ptr(), a16.data_ptr(), M, D,
-                                       int(dt == "bf16"), nat.stream_ptr()))
-    out_p = torch.empty(M, ld, dtype=tdt, device="cuda")
-    probe(dt, epi, 256, a16, w_st, M, N, D, out=out_p, ld=ld, **extra)
-    # float64 reference in reference column order, then the stored order of the kernel
-    ln = R.layer_norm_ref(h, gamma, beta)
-    acc = ln @ w_ref.double().T
-    if kind == "qkv_rope":
-        ref = R.epi_qkv_rope(acc, acc.abs(), R.row_freqs(freqs, M, seq).cuda(), 64, nf, 2 * D).ref[:, perm.cuda()]
-    elif kind == "swiglu":
-        ref = R.epi_swiglu(acc, acc.abs(), bias_ref).ref
-    else:
-        ref = acc
-    assert torch.isfinite(out_f[:M, :ld].float()).all()
-    rows = 256
-    for i, m in enumerate(MEANS):
-        sl = slice(i * rows, (i + 1) * rows)
-        rms = lambda o: float(((o[sl].double() - ref[sl]) ** 2).mean().sqrt())
-        ef, ep = rms(out_f[:M, :ld]), rms(out_p)
-        model = math.sqrt(1 + m * m)
-        print(f"[lnfold] {kind} {dt} mean {m:g} sigma: fold {ef:.3e} plain {ep:.3e} factor {ef / ep:.2f} "
-              f"(model {model:.2f})")
-        assert ef <= 2 * model * ep, (kind, dt, m, ef, ep)
-
-
 # ------------------------------------------------------------------------------------------------- schedule / bits
 def _schedule(M, N, bn, num_kb, stages, row_off=0):
     """(n tile, m tile of the rows starting at row_off) -> (CTA, ring position at the tile's start), as the persistent
@@ -436,20 +302,13 @@ def _prop_case(kind, dt, M, bn, K, seed):
     a = torch.randn(M, K, device="cuda", generator=g).to(tdt)
     w = (torch.randn(N, K, device="cuda", generator=g) * K ** -0.5).to(tdt)
     f, outs = {}, {}
-    if kind in ("residual", "residual_ln"):
+    if kind == "residual":
         h = torch.randn(M, N, device="cuda", generator=g)
         f.update(h=h, ld=N, bias=torch.randn(N, device="cuda", generator=g))
         outs["h"] = h
-        if kind == "residual":
-            # as many gate rows as items of 64 rows: an index without the % n_items wrap stays inside the buffer
-            f.update(gate=torch.rand(-(-M // 64), N, device="cuda", generator=g) + 0.2, rows_per_item=64, gate_ld=N,
-                     n_items=2)
-        else:
-            x16 = torch.zeros(M, N, dtype=tdt, device="cuda")
-            st = torch.zeros(M, R.LN_SLOTS, 2, device="cuda")
-            f.update(x16=x16, gamma_lo=torch.rand(N, device="cuda", generator=g) + 0.5,
-                     gamma_hi=torch.rand(N, device="cuda", generator=g) + 0.5, stats_lo=st, stats_hi=st, split=M // 2)
-            outs.update(x16=x16, stats=st)
+        # as many gate rows as items of 64 rows: an index without the % n_items wrap stays inside the buffer
+        f.update(gate=torch.rand(-(-M // 64), N, device="cuda", generator=g) + 0.2, rows_per_item=64, gate_ld=N,
+                 n_items=2)
     else:
         ld = N // 2 if kind == "swiglu" else N
         out = torch.zeros(M, ld, dtype=torch.float32 if kind == "store32" else tdt, device="cuda")
@@ -468,8 +327,7 @@ def _prop_case(kind, dt, M, bn, K, seed):
             else:
                 f.update(norm_cols=2 * N // 3)
     epi = {"store32": nat.EPI_STORE32, "store16": nat.EPI_STORE16, "head_norm16": nat.EPI_HEAD_NORM16,
-           "qkv_rope": nat.EPI_QKV_ROPE, "swiglu": nat.EPI_SWIGLU, "residual": nat.EPI_RESIDUAL,
-           "residual_ln": nat.EPI_RESIDUAL_LN}[kind]
+           "qkv_rope": nat.EPI_QKV_ROPE, "swiglu": nat.EPI_SWIGLU, "residual": nat.EPI_RESIDUAL}[kind]
     return dict(epi=epi, a=a, w=w, N=N, f=f, outs=outs, kc=kc)
 
 
@@ -483,8 +341,7 @@ def _run_prop(c, dt, M, bn, K, b_static=1):
 
 
 PROP_KINDS = [("store32", 256), ("store32", 64), ("store16", 128), ("store16", 256), ("head_norm16", 128),
-              ("head_norm16", 256), ("qkv_rope", 256), ("swiglu", 256), ("residual", 128), ("residual", 256),
-              ("residual_ln", 256)]
+              ("head_norm16", 256), ("qkv_rope", 256), ("swiglu", 256), ("residual", 128), ("residual", 256)]
 
 
 def _bits(d):
@@ -500,7 +357,7 @@ def test_schedule_bit_properties(dt, kind, bn):
     k-block more than the ring depth)."""
     M1 = 1025
     kc = 64 if kind in ("head_norm16", "swiglu") else 32
-    stages = R.gemm_stages(bn, kc, 32 * 36 * 4 if kind == "residual_ln" else 0)
+    stages = R.gemm_stages(bn, kc)
     P = 128 * (_sms() + 1)
     M2 = P + M1 + 77
     N = _prop_n(kind, bn)
@@ -526,12 +383,9 @@ def test_schedule_bit_properties(dt, kind, bn):
             cb["f"][key][P:P + M1] = c["f"][key]
     if "gate" in cb["f"]:
         cb["f"]["gate"][:c["f"]["gate"].shape[0]] = c["f"]["gate"]
-    for key in ("bias", "gamma_lo", "gamma_hi"):
-        if key in cb["f"]:
-            cb["f"][key] = c["f"][key]
+    if "bias" in cb["f"]:
+        cb["f"]["bias"] = c["f"]["bias"]
     cb["w"] = c["w"]
-    if kind == "residual_ln":
-        cb["f"]["split"] = P + c["f"]["split"]
     rb = _run_prop(cb, dt, M2, bn, K)
     for k in r1:
         assert torch.equal(_bits(r1)[k], _bits(rb)[k][P:P + M1]), f"{kind}: rows differ inside a larger M ({k})"
@@ -555,100 +409,9 @@ def test_probe_refuses_instances_the_forward_does_not_have():
     out = torch.zeros(128, 256, dtype=torch.float16, device="cuda")
     for epi, bn in ((nat.EPI_QKV_ROPE, 128), (nat.EPI_STORE16, 64), (nat.EPI_RESIDUAL_LN, 128), (nat.EPI_SWIGLU, 128)):
         with pytest.raises(nat.NativeError, match="instances"):
-            probe("fp16", epi, bn, a, w, 128, 256, 64, out=out, ld=256, head_dim=64, nf=16, h=out, x16=out,
-                  gamma_hi=out)
+            probe("fp16", epi, bn, a, w, 128, 256, 64, out=out, ld=256, head_dim=64, nf=16, h=out)
     with pytest.raises(nat.NativeError, match="multiple of 64"):
         probe("fp16", nat.EPI_SWIGLU, 256, a, w, 128, 96, 64, out=out, ld=256)
     with pytest.raises(nat.NativeError, match="K % 8"):
         probe("fp16", nat.EPI_STORE16, 256, a, w, 128, 256, 60, out=out, ld=256)
 
-
-# ------------------------------------------------------------------------------------------------- debugging switches
-# The switches are read once per process, hence one subprocess per setting.
-_LN_FOLD_RUN = r"""
-import sys
-sys.path[:0] = [{root!r}, {pkg!r}, {tests!r}]
-import torch
-from oracle import dit_oracle as do
-from helpers import SAO_DIT, build_native_dit, rel_l2
-cfg = dict(SAO_DIT, depth=2)
-sd = do.make_dit_weights(cfg, seed=31)
-g = torch.Generator().manual_seed(32)
-B = 2
-x, t = torch.randn(B, 64, 200, generator=g), torch.rand(B, generator=g)
-c, ge = torch.randn(B, 40, 768, generator=g), torch.randn(B, 1536, generator=g)
-c[:, 25:] = 0.0
-ref = do.dit_forward(sd, cfg, x, t, cross_attn_cond=c, global_embed=ge, cfg_scale=5.0)
-m = build_native_dit(cfg, sd)
-run = lambda: m(x.cuda(), t.cuda(), cross_attn_cond=c.cuda(), global_embed=ge.cuda(), cfg_scale=5.0).cpu()
-y = run()
-m.cuda_graph = True
-yg = run()
-torch.save(y, {out!r})
-print(rel_l2(y, ref), rel_l2(yg, ref), int(torch.equal(y, yg)))
-"""
-
-
-def test_ln_fold_switch_vs_oracle_and_default_path(tmp_path):
-    """SATB_LN=fold at SA-Open width (the only width it folds), depth 2, B = 2 with CFG and no negative prompt (the
-    cross-attention rows are a prefix of the rows): within the fp16 tolerance of the live oracle, eager and through a
-    CUDA graph (the same bits), and within the same tolerance of the default path."""
-    import os
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    res, outs = {}, {}
-    for tag, val in (("fold", "fold"), ("default", None)):
-        outs[tag] = str(tmp_path / f"{tag}.pt")
-        code = _LN_FOLD_RUN.format(root=root, pkg=os.path.join(root, "friendly-stable-audio-tools_b200"),
-                                   tests=os.path.join(root, "tests"), out=outs[tag])
-        env = {k: v for k, v in os.environ.items() if k != "SATB_LN"}
-        if val:
-            env["SATB_LN"] = val
-        p = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=env, timeout=900)
-        assert p.returncode == 0, p.stderr[-2000:]
-        e, eg, same = p.stdout.strip().splitlines()[-1].split()
-        res[tag] = (float(e), float(eg), int(same))
-    print("[switch] SATB_LN", res)
-    gate = 2e-3 * max(1.0, 5.0 / 1.5)
-    for tag, (e, eg, same) in res.items():
-        assert e < gate and eg < gate and same == 1, (tag, res)
-    yf, yd = torch.load(outs["fold"]), torch.load(outs["default"])
-    d = float((yf - yd).norm() / yd.norm())
-    print(f"[switch] SATB_LN=fold vs default rel-L2 {d:.3e}")
-    assert 0 < d < gate, d                        # the fold really ran, and agrees
-
-
-_DECODER_RUN = r"""
-import sys
-sys.path[:0] = [{root!r}, {pkg!r}]
-import torch
-from oracle import oobleck_oracle as oo
-from stable_audio_tools.models.autoencoders import OobleckDecoder
-dcfg = dict(out_channels=2, channels=128, c_mults=[1, 2], strides=[2, 4], latent_dim=16, use_snake=True, final_tanh=False)
-dsd = oo.make_oobleck_weights(oo.decoder_param_shapes(dcfg), seed=5, transposed=oo.decoder_transposed_prefixes(dcfg))
-dec = OobleckDecoder(**dcfg)
-dec.load_state_dict(dsd)
-z = torch.randn(2, 16, 150, generator=torch.Generator().manual_seed(4))
-a = dec.to("cuda:0").eval()(z.cuda()).cpu()
-r = oo.oobleck_decoder(z, dsd, dcfg)
-print(float((a - r).norm() / r.norm()))
-"""
-
-
-@pytest.mark.parametrize("switch", [("SATB_CONV_EPI", "general"), ("SATB_RAW", "fp32")])
-def test_decoder_debug_switches_vs_oracle(switch):
-    """The combined fast + general convolution epilogue and the fp32 skip stream: the small fused decoder within the
-    fp16 decoder tolerance of the oracle."""
-    import os
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    code = _DECODER_RUN.format(root=root, pkg=os.path.join(root, "friendly-stable-audio-tools_b200"))
-    env = {k: v for k, v in os.environ.items() if k not in ("SATB_CONV_EPI", "SATB_RAW")}
-    env[switch[0]] = switch[1]
-    p = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=env, timeout=600)
-    assert p.returncode == 0, p.stderr[-2000:]
-    err = float(p.stdout.strip().splitlines()[-1])
-    print(f"[switch] {switch[0]}={switch[1]} decoder rel-L2 {err:.3e}")
-    assert err < 4e-3, err

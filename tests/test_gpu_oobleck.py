@@ -231,38 +231,16 @@ def test_full_sao_decoder_split_operand_mode_reaches_70_db():
     assert esnr >= 68.0, esnr
 
 
-_FUSED_AB = r"""
-import os, sys
-sys.path[:0] = [{root!r}, {pkg!r}]
-import torch
-from oracle import oobleck_oracle as oo
-from stable_audio_tools.models.autoencoders import OobleckDecoder
-dcfg = dict(out_channels=2, channels=128, c_mults=[1, 2], strides=[2, 4], latent_dim=16, use_snake=True, final_tanh=False)
-dsd = oo.make_oobleck_weights(oo.decoder_param_shapes(dcfg), seed=5, transposed=oo.decoder_transposed_prefixes(dcfg))
-dec = OobleckDecoder(**dcfg)
-dec.load_state_dict(dsd)
-z = torch.randn(2, 16, 150, generator=torch.Generator().manual_seed(4))
-a = dec.to("cuda:0").eval()(z.cuda()).cpu()
-r = oo.oobleck_decoder(z, dsd, dcfg)
-print(float((a - r).norm() / r.norm()))
-"""
-
-
-def test_fused_residual_units_and_halo_conv_match_the_two_launch_path():
+def test_fused_residual_units_and_halo_conv_vs_oracle():
     """128- and 256-channel ResidualUnits as one kernel (conv7 -> snake2 -> conv1 -> skip) and the halo-tile final
-    convolution, against the oracle next to the two-launch / per-tap path (SATB_RESUNIT=unfused SATB_CONV_HALO=off,
-    read once per process, hence the subprocesses): both within the fp16 tolerance, the fused path no worse."""
-    import os
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    code = _FUSED_AB.format(root=root, pkg=os.path.join(root, "friendly-stable-audio-tools_b200"))
-    err = {}
-    for tag, extra in (("fused", {}), ("two_launch", {"SATB_RESUNIT": "unfused", "SATB_CONV_HALO": "off"})):
-        env = {k: v for k, v in os.environ.items() if k not in ("SATB_RESUNIT", "SATB_CONV_HALO")}
-        env.update(extra)
-        p = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=env, timeout=600)
-        assert p.returncode == 0, p.stderr[-2000:]
-        err[tag] = float(p.stdout.strip().splitlines()[-1])
-    assert err["two_launch"] < TOL["fp16"] and err["fused"] < TOL["fp16"], err
-    assert err["fused"] <= 1.1 * err["two_launch"], err
+    convolution: a small two-stage decoder that runs only these routes, within the fp16 tolerance of the oracle."""
+    from oracle import oobleck_oracle as oo
+    from stable_audio_tools.models.autoencoders import OobleckDecoder
+    dcfg = dict(out_channels=2, channels=128, c_mults=[1, 2], strides=[2, 4], latent_dim=16, use_snake=True,
+                final_tanh=False)
+    dsd = oo.make_oobleck_weights(oo.decoder_param_shapes(dcfg), seed=5, transposed=oo.decoder_transposed_prefixes(dcfg))
+    dec = OobleckDecoder(**dcfg)
+    dec.load_state_dict(dsd)
+    z = torch.randn(2, 16, 150, generator=torch.Generator().manual_seed(4))
+    err = rel_l2(dec.cuda().eval()(z.cuda()).cpu(), oo.oobleck_decoder(z, dsd, dcfg))
+    assert err < TOL["fp16"], err
