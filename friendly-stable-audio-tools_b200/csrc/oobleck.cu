@@ -196,6 +196,8 @@ struct SatbOobleck {
   int raw16 = 0;                   // 1: the raw skip stream is carried in the 16-bit operand type (fp16 mode), 0: fp32
   bool split3 = false;             // operand_dtype 2 ("fp16x3"): every product as (hi, hi) + (lo, hi) + (hi, lo), see GemmShape
   size_t lo_off = 0;               // bytes from a 16-bit activation buffer to its "lo" half (split3)
+  unsigned routes = 0;             // SATB_OOB_ROUTE_* bits of the kernels launched since the last reset (probe report)
+  bool wrote_raw = false;          // whether the last step wrote its raw output (probe report)
   std::vector<int> chans;          // c_mults[i] * channels, i = 0..n (c_mults prepended with 1)
   std::map<std::string, std::pair<float*, long long>> raw;   // state-dict entries (device fp32)
   std::vector<void*> owned;
@@ -338,6 +340,9 @@ int run_conv_gemm(SatbOobleck* h, const ConvW& cw, const void* in16, int B, int 
     if (Epi::fast_flags(ep))
       return run_conv_gemm<EpiConv<BF16, true>, BF16>(h, cw, in16, B, L_in, kind, dil, factor, ep, st);
   }
+  h->routes |= std::is_same<Epi, EpiStoreNCL>::value          ? SATB_OOB_ROUTE_GEMM_NCL
+               : std::is_same<Epi, EpiConv<BF16, true>>::value ? SATB_OOB_ROUTE_GEMM_LEAN
+                                                               : SATB_OOB_ROUTE_GEMM;
   GemmShape s;
   s.batches = B;
   s.b_static = 1;   // folded weight-norm weights, written at finalize time
@@ -400,6 +405,7 @@ int residual_unit(SatbOobleck* h, const std::string& pfx, int C, int B, int L, i
     e1.s16_out = sT;
     const HaloShape hs{L, B, C, 7, dil, C};
     const ResUnitPre pre{c7.bias, s2.a, s2.ib};
+    h->routes |= E::fast_flags(e1) ? SATB_OOB_ROUTE_FUSED_LEAN : SATB_OOB_ROUTE_FUSED;
     if (E::fast_flags(e1)) {
       typedef EpiConv<BF16, true> EM;
       SATB_PROPAGATE(C == 128 ? (launch_conv_halo<EM, 128, BF16, true>(*ta, *tb7, tb1, hs, pre, e1, st))
@@ -416,6 +422,137 @@ int residual_unit(SatbOobleck* h, const std::string& pfx, int C, int B, int L, i
   SATB_PROPAGATE((run_conv_gemm<E, BF16>(h, c7, sA, B, L, 0, dil, 1, e7, st)));
   SATB_PROPAGATE((run_conv_gemm<E, BF16>(h, c1, sT, B, L, 0, 1, 1, e1, st)));
   return 0;
+}
+
+void* lo_half(const SatbOobleck* h, void* p16) { return h->split3 ? static_cast<char*>(p16) + h->lo_off : nullptr; }
+
+// ---- the steps of a decode / encode.  decode_impl / encode_impl run them in order over the handle's workspaces;
+// satb_oobleck_probe runs one of them on caller-owned buffers.  Blocks b = 1 .. n, units j = 0 .. 2.
+
+// Decoder input: latents z NCL fp32 [B, latent_dim, L] -> channels-last 16-bit in tmp16 -> conv k7 latent -> chans[n],
+// whose epilogue applies block 1's leading Snake, into out16.
+template <bool BF16>
+int dec_input(SatbOobleck* h, const float* z, void* tmp16, void* out16, int B, int L, cudaStream_t st) {
+  const SatbOobleckConfig& c = h->cfg;
+  {
+    dim3 grid(ceil_div(L, 32), ceil_div(c.latent_dim, 32), B);
+    ncl_to_nlc16_kernel<BF16><<<grid, 256, 0, st>>>(z, static_cast<uint16_t*>(tmp16),
+                                                    static_cast<uint16_t*>(lo_half(h, tmp16)), c.latent_dim, L);
+    count_launch();
+  }
+  const ConvW& c0 = h->convs.at("layers.0.");
+  const SnakeW& sn = h->snakes.at("layers.1.layers.0.");
+  typename EpiConv<BF16>::Params ep{c0.bias, nullptr, nullptr, out16, sn.a, sn.ib, c0.cout, L, 1, 0, lo_half(h, out16), h->raw16};
+  h->wrote_raw = false;
+  return run_conv_gemm<EpiConv<BF16>, BF16>(h, c0, tmp16, B, L, 0, 1, 1, ep, st);
+}
+
+// Decoder block b: transposed conv of in16 [B, L_in, chans[n-b+1]] -> raw and snake(unit 0) into out16, both
+// [B, L_in * stride, chans[n-b]].
+template <bool BF16>
+int dec_upsample(SatbOobleck* h, int b, const void* in16, void* raw, void* out16, int B, int L_in, cudaStream_t st) {
+  const int n = h->cfg.n_stages, cout = h->chans[n - b], s = h->cfg.strides[n - b];
+  const std::string bp = "layers." + std::to_string(b) + ".";
+  const ConvW& ct = h->convs.at(bp + "layers.1.");
+  const SnakeW& s_ru0 = h->snakes.at(bp + "layers.2.layers.0.");
+  const int64_t Lo = static_cast<int64_t>(L_in) * s;
+  SATB_REQUIRE(Lo < (int64_t(1) << 31) && static_cast<int64_t>(B) * Lo * cout < (int64_t(1) << 40), "decoder: sequence too long");
+  typename EpiConv<BF16>::Params et{ct.bias, nullptr, raw, out16, s_ru0.a, s_ru0.ib, cout, static_cast<int>(Lo), s, (s + 1) / 2, lo_half(h, out16), h->raw16};
+  h->wrote_raw = true;
+  return run_conv_gemm<EpiConv<BF16>, BF16>(h, ct, in16, B, L_in, 1, 1, s, et, st);
+}
+
+// Decoder ResidualUnit j of block b over [B, L, chans[n-b]]; the Snake applied to its output is the next unit's, then
+// the next block's, then the final one.
+template <bool BF16>
+int dec_residual(SatbOobleck* h, int b, int j, int B, int L, void* raw, void*& sA, void*& sT, cudaStream_t st) {
+  static const int dils[3] = {1, 3, 9};
+  const int n = h->cfg.n_stages;
+  const std::string bp = "layers." + std::to_string(b) + ".";
+  const SnakeW* next;
+  if (j < 2)
+    next = &h->snakes.at(bp + "layers." + std::to_string(3 + j) + ".layers.0.");
+  else if (b < n)
+    next = &h->snakes.at("layers." + std::to_string(b + 1) + ".layers.0.");
+  else
+    next = &h->snakes.at("layers." + std::to_string(n + 1) + ".");
+  h->wrote_raw = j < 2;   // the last unit's raw output has no reader: the next step is a transposed or final conv
+  return residual_unit<BF16>(h, bp + "layers." + std::to_string(2 + j) + ".", h->chans[n - b], B, L, dils[j], raw, sA, sT,
+                             next, j < 2, st);
+}
+
+// Decoder final conv k7 chans[0] -> audio channels (no bias, optional tanh) of in16 [B, L, chans[0]] into audio NCL.
+// The 128 -> 2 contraction runs with the N tile mostly empty (8x wasted MMA work is still ~10x faster than the
+// shared-memory-bound CUDA-core version it replaces: 1.21 ms -> bandwidth-bound)
+template <bool BF16>
+int dec_output(SatbOobleck* h, const void* in16, float* audio, int B, int L, cudaStream_t st) {
+  const ConvW& cf = h->convs.at("layers." + std::to_string(h->cfg.n_stages + 2) + ".");
+  EpiStoreNCL::Params ep{audio, nullptr, cf.cout, L, h->cfg.final_tanh};
+  h->wrote_raw = false;
+  if (!h->split3 && cf.cout <= 64 && cf.cin % kBlockK == 0 && cf.k % 2 == 1 && cf.k - 1 <= kHaloMax) {
+    // every activation row is fetched once per tile instead of once per tap (see conv_halo.cuh)
+    const CUtensorMap *ta, *tb;
+    SATB_PROPAGATE(get_tmap_a(h, in16, cf.cin, L, B, L, 1, &ta, kBlockM + cf.k - 1));
+    SATB_PROPAGATE(get_tmap_b(h, cf, cf.k * cf.cout, 64, &tb));
+    const HaloShape hs{L, B, cf.cin, cf.k, 1, cf.cout};
+    h->routes |= SATB_OOB_ROUTE_HALO_NCL;
+    return launch_conv_halo<EpiStoreNCL, 64, BF16, false>(*ta, *tb, nullptr, hs, ResUnitPre{}, ep, st);
+  }
+  return run_conv_gemm<EpiStoreNCL, BF16>(h, cf, in16, B, L, 0, 1, 1, ep, st);
+}
+
+// Encoder input conv k7 audio NCL [B, in_channels, T] -> chans[0] on CUDA cores: raw, and block 1 / unit 0's Snake
+// into out16.
+template <bool BF16>
+int enc_input(SatbOobleck* h, const float* audio, void* raw, void* out16, int B, int64_t T, cudaStream_t st) {
+  const ConvW& c0 = h->convs.at("layers.0.");
+  const SnakeW& sn = h->snakes.at("layers.1.layers.0.layers.0.");
+  SATB_REQUIRE(c0.cin * c0.k <= 16, "encoder input conv: in_channels * kernel must be <= 16");
+  const size_t smem = static_cast<size_t>(c0.cin) * (64 + c0.k - 1) * 4;
+  dim3 grid(static_cast<unsigned>(ceil_div64(T, 64)), B);
+  conv_in_kernel<BF16><<<grid, 256, smem, st>>>(audio, c0.w32, c0.bias, sn.a, sn.ib, raw, static_cast<uint16_t*>(out16),
+                                                 static_cast<uint16_t*>(lo_half(h, out16)), c0.cin, c0.cout, T, c0.k,
+                                                 h->raw16);
+  count_launch();
+  h->routes |= SATB_OOB_ROUTE_CUDA_CORE;
+  h->wrote_raw = true;
+  return 0;
+}
+
+// Encoder ResidualUnit j of block b over [B, L, chans[b-1]]; the Snake applied to its output is the next unit's, then
+// the block's own before its strided conv.
+template <bool BF16>
+int enc_residual(SatbOobleck* h, int b, int j, int B, int L, void* raw, void*& sA, void*& sT, cudaStream_t st) {
+  static const int dils[3] = {1, 3, 9};
+  const std::string bp = "layers." + std::to_string(b) + ".";
+  const SnakeW* next = j < 2 ? &h->snakes.at(bp + "layers." + std::to_string(j + 1) + ".layers.0.")
+                             : &h->snakes.at(bp + "layers.3.");
+  h->wrote_raw = j < 2;   // the strided conv that follows the last unit has no skip
+  return residual_unit<BF16>(h, bp + "layers." + std::to_string(j) + ".", h->chans[b - 1], B, L, dils[j], raw, sA, sT,
+                             next, j < 2, st);
+}
+
+// Encoder block b: strided conv of in16 [B, L_in, chans[b-1]] (already Snake-activated) -> [B, L_in / s, chans[b]]:
+// raw (when a next block reads it as its first skip) and the next block's (or the final) Snake into out16.
+template <bool BF16>
+int enc_downsample(SatbOobleck* h, int b, const void* in16, void* raw, void* out16, int B, int L_in, cudaStream_t st) {
+  const int n = h->cfg.n_stages, s = h->cfg.strides[b - 1];
+  const ConvW& cs = h->convs.at("layers." + std::to_string(b) + ".layers.4.");
+  const int Lo = L_in / s;
+  const SnakeW* nx = b < n ? &h->snakes.at("layers." + std::to_string(b + 1) + ".layers.0.layers.0.")
+                           : &h->snakes.at("layers." + std::to_string(n + 1) + ".");
+  typename EpiConv<BF16>::Params ep{cs.bias, nullptr, b < n ? raw : nullptr, out16, nx->a, nx->ib, cs.cout, Lo, 1, 0, lo_half(h, out16), h->raw16};
+  h->wrote_raw = b < n;
+  return run_conv_gemm<EpiConv<BF16>, BF16>(h, cs, in16, B, L_in, 2, 1, s, ep, st);
+}
+
+// Encoder final conv k3 chans[n] -> latent_dim of in16 [B, L, chans[n]], NCL fp32 output
+template <bool BF16>
+int enc_output(SatbOobleck* h, const void* in16, float* latents, int B, int L, cudaStream_t st) {
+  const ConvW& cf = h->convs.at("layers." + std::to_string(h->cfg.n_stages + 2) + ".");
+  EpiStoreNCL::Params ep{latents, cf.bias, cf.cout, L, 0};
+  h->wrote_raw = false;
+  return run_conv_gemm<EpiStoreNCL, BF16>(h, cf, in16, B, L, 0, 1, 1, ep, st);
 }
 
 template <bool BF16>
@@ -439,66 +576,16 @@ int decode_impl(SatbOobleck* h, const float* z, float* audio, int B, int L, cuda
   void* raw = h->buf_raw;
   void* sA = h->buf_a;
   void* sB = h->buf_b;
-  typedef EpiConv<BF16> E;
-  // latent NCL fp32 -> channels-last 16-bit
-  {
-    dim3 grid(ceil_div(L, 32), ceil_div(c.latent_dim, 32), B);
-    ncl_to_nlc16_kernel<BF16><<<grid, 256, 0, st>>>(z, static_cast<uint16_t*>(sB),
-                                                    h->split3 ? reinterpret_cast<uint16_t*>(static_cast<char*>(sB) + h->lo_off) : nullptr,
-                                                    c.latent_dim, L);
-    count_launch();
-  }
-  // layers.0: conv k7 latent -> chans[n]; epilogue applies block 1's leading Snake
-  {
-    const ConvW& c0 = h->convs.at("layers.0.");
-    const SnakeW& sn = h->snakes.at("layers.1.layers.0.");
-    typename E::Params ep{c0.bias, nullptr, nullptr, sA, sn.a, sn.ib, c0.cout, L, 1, 0, h->split3 ? static_cast<char*>(sA) + h->lo_off : nullptr, h->raw16};
-    SATB_PROPAGATE((run_conv_gemm<E, BF16>(h, c0, sB, B, L, 0, 1, 1, ep, st)));
-  }
+  SATB_PROPAGATE(dec_input<BF16>(h, z, sB, sA, B, L, st));
   int64_t Lc = L;
   for (int b = 1; b <= n; ++b) {
-    const int cin = h->chans[n - b + 1], cout = h->chans[n - b], s = c.strides[n - b];
-    const std::string bp = "layers." + std::to_string(b) + ".";
-    const ConvW& ct = h->convs.at(bp + "layers.1.");
-    const SnakeW& s_ru0 = h->snakes.at(bp + "layers.2.layers.0.");
-    const int64_t Lo = Lc * s;
-    SATB_REQUIRE(Lo < (int64_t(1) << 31) && static_cast<int64_t>(B) * Lo * cout < (int64_t(1) << 40), "decoder: sequence too long");
     // transposed conv reads sA [B, Lc, cin], writes raw + snake(ru0) into sB
-    typename E::Params et{ct.bias, nullptr, raw, sB, s_ru0.a, s_ru0.ib, cout, static_cast<int>(Lo), s, (s + 1) / 2, h->split3 ? static_cast<char*>(sB) + h->lo_off : nullptr, h->raw16};
-    SATB_PROPAGATE((run_conv_gemm<E, BF16>(h, ct, sA, B, static_cast<int>(Lc), 1, 1, s, et, st)));
+    SATB_PROPAGATE(dec_upsample<BF16>(h, b, sA, raw, sB, B, static_cast<int>(Lc), st));
     std::swap(sA, sB);  // sA now holds the residual units' input
-    for (int j = 0; j < 3; ++j) {
-      static const int dils[3] = {1, 3, 9};
-      const SnakeW* next;
-      if (j < 2)
-        next = &h->snakes.at(bp + "layers." + std::to_string(3 + j) + ".layers.0.");
-      else if (b < n)
-        next = &h->snakes.at("layers." + std::to_string(b + 1) + ".layers.0.");
-      else
-        next = &h->snakes.at("layers." + std::to_string(n + 1) + ".");
-      SATB_PROPAGATE((residual_unit<BF16>(h, bp + "layers." + std::to_string(2 + j) + ".", cout, B, static_cast<int>(Lo),
-                                          dils[j], raw, sA, sB, next, j < 2, st)));
-    }
-    Lc = Lo;
-    (void)cin;
+    Lc *= c.strides[n - b];
+    for (int j = 0; j < 3; ++j) SATB_PROPAGATE(dec_residual<BF16>(h, b, j, B, static_cast<int>(Lc), raw, sA, sB, st));
   }
-  // final conv k7 chans[0] -> audio channels (no bias, optional tanh): the 128 -> 2 contraction runs as a
-  // 7-tap GEMM with the N tile mostly empty (8x wasted MMA work is still ~10x faster than the
-  // shared-memory-bound CUDA-core version it replaces: 1.21 ms -> bandwidth-bound)
-  {
-    const ConvW& cf = h->convs.at("layers." + std::to_string(n + 2) + ".");
-    EpiStoreNCL::Params ep{audio, nullptr, cf.cout, static_cast<int>(Lc), c.final_tanh};
-    if (!h->split3 && cf.cout <= 64 && cf.cin % kBlockK == 0 && cf.k % 2 == 1 && cf.k - 1 <= kHaloMax) {
-      // every activation row is fetched once per tile instead of once per tap (see conv_halo.cuh)
-      const CUtensorMap *ta, *tb;
-      SATB_PROPAGATE(get_tmap_a(h, sA, cf.cin, static_cast<int>(Lc), B, static_cast<int>(Lc), 1, &ta, kBlockM + cf.k - 1));
-      SATB_PROPAGATE(get_tmap_b(h, cf, cf.k * cf.cout, 64, &tb));
-      const HaloShape hs{static_cast<int>(Lc), B, cf.cin, cf.k, 1, cf.cout};
-      SATB_PROPAGATE((launch_conv_halo<EpiStoreNCL, 64, BF16, false>(*ta, *tb, nullptr, hs, ResUnitPre{}, ep, st)));
-    } else {
-      SATB_PROPAGATE((run_conv_gemm<EpiStoreNCL, BF16>(h, cf, sA, B, static_cast<int>(Lc), 0, 1, 1, ep, st)));
-    }
-  }
+  SATB_PROPAGATE(dec_output<BF16>(h, sA, audio, B, static_cast<int>(Lc), st));
   SATB_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -526,47 +613,44 @@ int encode_impl(SatbOobleck* h, const float* audio, float* latents, int B, int64
   void* raw = h->buf_raw;
   void* sA = h->buf_a;
   void* sB = h->buf_b;
-  typedef EpiConv<BF16> E;
-  // layers.0: conv k7 audio -> channels (CUDA cores), epilogue = block 1 / res unit 0 Snake
-  {
-    const ConvW& c0 = h->convs.at("layers.0.");
-    const SnakeW& sn = h->snakes.at("layers.1.layers.0.layers.0.");
-    SATB_REQUIRE(c0.cin * c0.k <= 16, "encoder input conv: in_channels * kernel must be <= 16");
-    const size_t smem = static_cast<size_t>(c0.cin) * (64 + c0.k - 1) * 4;
-    dim3 grid(static_cast<unsigned>(ceil_div64(T, 64)), B);
-    conv_in_kernel<BF16><<<grid, 256, smem, st>>>(audio, c0.w32, c0.bias, sn.a, sn.ib, raw, static_cast<uint16_t*>(sA),
-                                                   h->split3 ? reinterpret_cast<uint16_t*>(static_cast<char*>(sA) + h->lo_off) : nullptr,
-                                                   c0.cin, c0.cout, T, c0.k, h->raw16);
-    count_launch();
-  }
+  SATB_PROPAGATE(enc_input<BF16>(h, audio, raw, sA, B, T, st));
   int64_t Lc = T;
   for (int b = 1; b <= n; ++b) {
-    const int cin = h->chans[b - 1], s = c.strides[b - 1];
-    const std::string bp = "layers." + std::to_string(b) + ".";
-    for (int j = 0; j < 3; ++j) {
-      static const int dils[3] = {1, 3, 9};
-      const SnakeW* next = j < 2 ? &h->snakes.at(bp + "layers." + std::to_string(j + 1) + ".layers.0.")
-                                 : &h->snakes.at(bp + "layers.3.");
-      SATB_PROPAGATE((residual_unit<BF16>(h, bp + "layers." + std::to_string(j) + ".", cin, B, static_cast<int>(Lc), dils[j],
-                                          raw, sA, sB, next, j < 2, st)));
-    }
-    // strided conv reads sA [B, Lc, cin] (already Snake-activated) -> [B, Lc/s, cout]
-    const ConvW& cs = h->convs.at(bp + "layers.4.");
-    const int64_t Lo = Lc / s;
-    const SnakeW* nx = b < n ? &h->snakes.at("layers." + std::to_string(b + 1) + ".layers.0.layers.0.")
-                             : &h->snakes.at("layers." + std::to_string(n + 1) + ".");
-    typename E::Params ep{cs.bias, nullptr, b < n ? raw : nullptr, sB, nx->a, nx->ib, cs.cout, static_cast<int>(Lo), 1, 0, h->split3 ? static_cast<char*>(sB) + h->lo_off : nullptr, h->raw16};
-    SATB_PROPAGATE((run_conv_gemm<E, BF16>(h, cs, sA, B, static_cast<int>(Lc), 2, 1, s, ep, st)));
+    for (int j = 0; j < 3; ++j) SATB_PROPAGATE(enc_residual<BF16>(h, b, j, B, static_cast<int>(Lc), raw, sA, sB, st));
+    // strided conv reads sA [B, Lc, cin] -> [B, Lc/s, cout] in sB
+    SATB_PROPAGATE(enc_downsample<BF16>(h, b, sA, raw, sB, B, static_cast<int>(Lc), st));
     std::swap(sA, sB);
-    Lc = Lo;
+    Lc /= c.strides[b - 1];
   }
-  // final conv k3 chans[n] -> latent_dim, NCL fp32 output
-  {
-    const ConvW& cf = h->convs.at("layers." + std::to_string(n + 2) + ".");
-    EpiStoreNCL::Params ep{latents, cf.bias, cf.cout, static_cast<int>(Lc), 0};
-    SATB_PROPAGATE((run_conv_gemm<EpiStoreNCL, BF16>(h, cf, sA, B, static_cast<int>(Lc), 0, 1, 1, ep, st)));
-  }
+  SATB_PROPAGATE(enc_output<BF16>(h, sA, latents, B, static_cast<int>(Lc), st));
   return 0;
+}
+
+// One step on caller-owned buffers (satb_oobleck_probe).
+template <bool BF16>
+int probe_impl(SatbOobleck* h, SatbOobleckProbe* p, cudaStream_t st) {
+  const int b = p->block, j = p->unit, B = p->B, L = p->L;
+  if (p->step == SATB_OOB_DEC_RES || p->step == SATB_OOB_ENC_RES) {
+    const bool dec = p->step == SATB_OOB_DEC_RES;
+    const int C = h->chans[dec ? h->cfg.n_stages - b : b - 1];
+    if (p->raw_in != p->raw_out)
+      SATB_CHECK_CUDA(cudaMemcpyAsync(p->raw_out, p->raw_in, static_cast<size_t>(B) * L * C * (h->raw16 ? 2 : 4),
+                                      cudaMemcpyDeviceToDevice, st));
+    void* sA = p->in;
+    void* sT = p->scratch;
+    SATB_PROPAGATE(dec ? dec_residual<BF16>(h, b, j, B, L, p->raw_out, sA, sT, st)
+                       : enc_residual<BF16>(h, b, j, B, L, p->raw_out, sA, sT, st));
+    p->result_in_scratch = sA == p->scratch;
+    return 0;
+  }
+  switch (p->step) {
+    case SATB_OOB_DEC_IN: return dec_input<BF16>(h, static_cast<const float*>(p->in), p->scratch, p->out16, B, L, st);
+    case SATB_OOB_DEC_UP: return dec_upsample<BF16>(h, b, p->in, p->raw_out, p->out16, B, L, st);
+    case SATB_OOB_DEC_OUT: return dec_output<BF16>(h, p->in, p->out32, B, L, st);
+    case SATB_OOB_ENC_IN: return enc_input<BF16>(h, static_cast<const float*>(p->in), p->raw_out, p->out16, B, L, st);
+    case SATB_OOB_ENC_DOWN: return enc_downsample<BF16>(h, b, p->in, p->raw_out, p->out16, B, L, st);
+    default: return enc_output<BF16>(h, p->in, p->out32, B, L, st);
+  }
 }
 
 }  // namespace
@@ -579,6 +663,21 @@ int satb_oobleck_create(const SatbOobleckConfig* cfg, SatbOobleck** out) {
   SATB_REQUIRE(cfg->channels % 32 == 0, "channels must be a multiple of 32");
   SATB_REQUIRE(cfg->latent_dim % 8 == 0, "latent_dim must be a multiple of 8");
   SATB_REQUIRE(cfg->in_channels >= 1 && cfg->in_channels <= 2, "audio channels must be 1 or 2");
+  // A block's conv has kernel 2s, stride s, padding ceil(s/2) (models/autoencoders.py:75,86).  Its output length is
+  // L * s (decoder) and L / s (encoder) only for an even decoder stride and an encoder stride >= 2: an odd decoder
+  // stride gives L * s - 1, encoder stride 1 gives L + 1.
+  for (int i = 0; i < cfg->n_stages; ++i) {
+    const int s = cfg->strides[i];
+    if (cfg->is_decoder ? (s < 2 || s % 2 != 0) : s < 2) {
+      set_last_error(std::string(cfg->is_decoder ? "decoder" : "encoder") + ": stride " + std::to_string(s) +
+                     " is not supported: " +
+                     (cfg->is_decoder ? "strides must be even (a transposed conv with kernel 2s, padding ceil(s/2) "
+                                        "gives L * s positions only for even s)"
+                                      : "strides must be >= 2 (a conv with kernel 2s, padding ceil(s/2) gives L / s "
+                                        "positions only for s >= 2)"));
+      return -1;
+    }
+  }
   SatbOobleck* h = new SatbOobleck();
   h->cfg = *cfg;
   h->bf16 = cfg->operand_dtype == 1;
@@ -684,6 +783,79 @@ int satb_oobleck_encode(SatbOobleck* h, const float* audio, float* latents, int 
   SATB_REQUIRE(audio && latents && B >= 1 && T >= 1, "bad argument");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   return h->bf16 ? encode_impl<true>(h, audio, latents, B, T, st) : encode_impl<false>(h, audio, latents, B, T, st);
+}
+
+int satb_oobleck_probe(SatbOobleck* h, SatbOobleckProbe* p, void* stream) {
+  SATB_REQUIRE(h && h->finalized && p, "oobleck probe: needs a finalized handle and a parameter block");
+  const bool dec = h->cfg.is_decoder != 0;
+  const int n = h->cfg.n_stages;
+  const int step = p->step;
+  if (dec ? (step < SATB_OOB_DEC_IN || step > SATB_OOB_DEC_OUT) : (step < SATB_OOB_ENC_IN || step > SATB_OOB_ENC_OUT)) {
+    set_last_error(std::string("oobleck probe: unknown step ") + std::to_string(step) + " for " +
+                   (dec ? "a decoder; accepted: DEC_IN 0, DEC_UP 1, DEC_RES 2, DEC_OUT 3"
+                        : "an encoder; accepted: ENC_IN 4, ENC_RES 5, ENC_DOWN 6, ENC_OUT 7"));
+    return -1;
+  }
+  const bool res = step == SATB_OOB_DEC_RES || step == SATB_OOB_ENC_RES;
+  const bool blocked = res || step == SATB_OOB_DEC_UP || step == SATB_OOB_ENC_DOWN;
+  if ((blocked && (p->block < 1 || p->block > n)) || (res && (p->unit < 0 || p->unit > 2))) {
+    set_last_error("oobleck probe: block " + std::to_string(p->block) + " unit " + std::to_string(p->unit) +
+                   " out of range; accepted: block 1 .. " + std::to_string(n) + ", unit 0 .. 2 (ResidualUnit steps)");
+    return -1;
+  }
+  SATB_REQUIRE(p->B >= 1 && p->L >= 1, "oobleck probe: B and L must be >= 1");
+  SATB_REQUIRE(!h->split3 || (p->lo_off > 0 && p->lo_off % 16 == 0),
+               "oobleck probe: fp16x3 needs lo_off, a positive multiple of 16 bytes");
+  if (step == SATB_OOB_ENC_DOWN) {
+    const int s = h->cfg.strides[p->block - 1];
+    if (p->L % s != 0) {
+      set_last_error("oobleck probe: strided conv input length " + std::to_string(p->L) +
+                     " is not a multiple of the stride " + std::to_string(s));
+      return -1;
+    }
+  }
+  // the buffers each step uses (see include/satb200.h)
+  const bool raw_out = step == SATB_OOB_DEC_UP || step == SATB_OOB_ENC_IN || step == SATB_OOB_ENC_DOWN || res;
+  const bool out16 = step == SATB_OOB_DEC_IN || step == SATB_OOB_DEC_UP || step == SATB_OOB_ENC_IN || step == SATB_OOB_ENC_DOWN;
+  const bool out32 = step == SATB_OOB_DEC_OUT || step == SATB_OOB_ENC_OUT;
+  const bool scratch = step == SATB_OOB_DEC_IN || res;
+  const struct { const char* name; const void* ptr; bool used; } bufs[] = {
+      {"in", p->in, true}, {"raw_in", p->raw_in, res}, {"raw_out", p->raw_out, raw_out},
+      {"out16", p->out16, out16}, {"scratch", p->scratch, scratch}, {"out32", p->out32, out32}};
+  for (const auto& bf : bufs) {
+    if (bf.used && (bf.ptr == nullptr || reinterpret_cast<uintptr_t>(bf.ptr) % 16 != 0)) {
+      set_last_error(std::string("oobleck probe: ") + bf.name + " must be a non-null, 16-byte aligned device pointer");
+      return -1;
+    }
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  h->lo_off = h->split3 ? static_cast<size_t>(p->lo_off) : 0;
+  h->routes = 0;
+  p->result_in_scratch = 0;
+  const int rc = h->bf16 ? probe_impl<true>(h, p, st) : probe_impl<false>(h, p, st);
+  p->wrote_raw = h->wrote_raw ? 1 : 0;
+  p->routes = static_cast<int>(h->routes);
+  SATB_PROPAGATE(rc);
+  SATB_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int satb_oobleck_weights(SatbOobleck* h, const char* prefix, void* dst, long long* bytes, void* stream) {
+  SATB_REQUIRE(h && h->finalized && prefix && bytes, "oobleck weights: needs a finalized handle, a prefix and bytes");
+  auto it = h->convs.find(prefix);
+  if (it == h->convs.end()) {
+    set_last_error(std::string("oobleck weights: no conv ") + prefix);
+    return -1;
+  }
+  const ConvW& c = it->second;
+  const size_t total = static_cast<size_t>(c.cin) * c.cout * c.k;
+  const size_t n = c.small ? total * 4 : total * 2 * (h->split3 ? 2 : 1);
+  *bytes = static_cast<long long>(n);
+  if (dst) {
+    SATB_CHECK_CUDA(cudaMemcpyAsync(dst, c.small ? static_cast<const void*>(c.w32) : static_cast<const void*>(c.w16), n,
+                                    cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));
+  }
+  return 0;
 }
 
 }  // extern "C"

@@ -52,6 +52,17 @@ class SatbGemmProbe(ctypes.Structure):
                 + [("cos_tab", _VP), ("sin_tab", _VP), ("norm_cols", _I)])
 
 
+# satb_oobleck_probe / satb_oobleck_weights (tests only): steps, route bits and the parameter block of include/satb200.h
+OOB_DEC_IN, OOB_DEC_UP, OOB_DEC_RES, OOB_DEC_OUT, OOB_ENC_IN, OOB_ENC_RES, OOB_ENC_DOWN, OOB_ENC_OUT = range(8)
+OOB_ROUTES = {1: "gemm", 2: "gemm_lean", 4: "fused", 8: "fused_lean", 16: "halo_ncl", 32: "gemm_ncl", 64: "cuda_core"}
+
+
+class SatbOobleckProbe(ctypes.Structure):
+    _fields_ = ([(n, _I) for n in ("step", "block", "unit", "B", "L")]
+                + [(n, _VP) for n in ("in_", "raw_in", "raw_out", "out16", "scratch", "out32")]
+                + [("lo_off", _LL)] + [(n, _I) for n in ("result_in_scratch", "wrote_raw", "routes")])
+
+
 SIGNATURES = {
     "satb_last_error": (ctypes.c_char_p, []),
     "satb_abi_version": (_I, []),
@@ -82,6 +93,8 @@ SIGNATURES = {
     "satb_oobleck_finalize": (_I, [_VP, _VP]),
     "satb_oobleck_decode": (_I, [_VP, _VP, _VP, _I, _I, _VP]),
     "satb_oobleck_encode": (_I, [_VP, _VP, _VP, _I, _LL, _VP]),
+    "satb_oobleck_probe": (_I, [_VP, ctypes.POINTER(SatbOobleckProbe), _VP]),
+    "satb_oobleck_weights": (_I, [_VP, ctypes.c_char_p, _VP, ctypes.POINTER(_LL), _VP]),
 }
 
 

@@ -90,6 +90,19 @@ class DecoderBlock(_Container):
             ResidualUnit(out_channels, out_channels, 9, use_snake=use_snake))
 
 
+def _check_strides(strides, decoder):
+    """A block's conv has kernel 2s, stride s, padding ceil(s/2) (reference :75,86).  Its output has L * s (decoder) or
+    L / s (encoder) positions, which forward allocates, only for an even decoder stride and an encoder stride >= 2:
+    an odd decoder stride gives L * s - 1, encoder stride 1 gives L + 1."""
+    for s in strides:
+        if decoder and (s < 2 or s % 2):
+            raise NotImplementedError(f"OobleckDecoder: stride {s} is not supported: strides must be even (a transposed "
+                                      "conv with kernel 2s, padding ceil(s/2) gives L * s positions only for even s)")
+        if not decoder and s < 2:
+            raise NotImplementedError(f"OobleckEncoder: stride {s} is not supported: strides must be >= 2 (a conv with "
+                                      "kernel 2s, padding ceil(s/2) gives L / s positions only for s >= 2)")
+
+
 class _NativeOobleck(nn.Module):
     """Shared native-handle plumbing of OobleckEncoder / OobleckDecoder."""
 
@@ -162,6 +175,7 @@ class OobleckEncoder(_NativeOobleck):
         super().__init__()
         if not use_snake or antialias_activation:
             raise NotImplementedError("only use_snake=True without anti-aliasing is on the native hot path")
+        _check_strides(strides, decoder=False)
         self._init_native(in_channels, channels, latent_dim, c_mults, strides, False, operand_dtype)
         cm = [1] + list(c_mults)
         self.depth = len(cm)
@@ -198,6 +212,7 @@ class OobleckDecoder(_NativeOobleck):
         super().__init__()
         if not use_snake or antialias_activation:
             raise NotImplementedError("only use_snake=True without anti-aliasing is on the native hot path")
+        _check_strides(strides, decoder=True)
         self._init_native(out_channels, channels, latent_dim, c_mults, strides, final_tanh, operand_dtype)
         cm = [1] + list(c_mults)
         self.depth = len(cm)

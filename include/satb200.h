@@ -173,6 +173,58 @@ int satb_oobleck_decode(SatbOobleck* h, const float* z, float* audio, int B, int
  * (the deterministic mean|scale tensor; the VAE sampling stays in PyTorch, bottleneck.py:46-62). */
 int satb_oobleck_encode(SatbOobleck* h, const float* audio, float* latents, int B, long long T, void* stream);
 
+/* Test entry points (no product path calls them).
+ * satb_oobleck_probe runs ONE step of a finalized handle's decode or encode on caller-owned device buffers, through
+ * the same host function (and so the same kernel instances, route, next Snake and raw-stream choice) as the product
+ * loop.  Steps, with the buffers each one reads and writes ("16-bit": [B, L, C] channels-last in the operand type; in
+ * fp16x3 mode every 16-bit buffer has its lo half at byte offset lo_off; "raw": [B, L, C] fp16 in fp16 mode, fp32
+ * otherwise):
+ *   DEC_IN    in: fp32 NCL latents [B, latent_dim, L]; scratch: their 16-bit copy; out16
+ *   DEC_UP    block b: in (16-bit, L positions) -> raw_out, out16 (L * stride positions)
+ *   DEC_RES   unit (b, j): in (16-bit), raw_in -> raw_out (if wrote_raw), the result in `in` or `scratch`
+ *   DEC_OUT   in (16-bit) -> out32 (NCL fp32 audio)
+ *   ENC_IN    in: fp32 NCL audio [B, in_channels, L] -> raw_out, out16
+ *   ENC_RES   unit (b, j), as DEC_RES
+ *   ENC_DOWN  block b: in (16-bit, L positions, a multiple of the stride) -> raw_out (if wrote_raw), out16
+ *   ENC_OUT   in (16-bit) -> out32 (NCL fp32 pre-bottleneck)
+ * A ResidualUnit updates its raw stream in place: the probe first copies raw_in to raw_out (when they differ).  Its
+ * 16-bit result lands in `in` (two-launch route, which also uses scratch) or in `scratch` (fused route):
+ * result_in_scratch says which.  Blocks and units count as in the state dict: b = 1 .. n_stages, j = 0 .. 2.  Every
+ * pointer a step uses must be 16-byte aligned. */
+#define SATB_OOB_DEC_IN 0
+#define SATB_OOB_DEC_UP 1
+#define SATB_OOB_DEC_RES 2
+#define SATB_OOB_DEC_OUT 3
+#define SATB_OOB_ENC_IN 4
+#define SATB_OOB_ENC_RES 5
+#define SATB_OOB_ENC_DOWN 6
+#define SATB_OOB_ENC_OUT 7
+/* routes (bits of SatbOobleckProbe.routes): the kernels one step launched */
+#define SATB_OOB_ROUTE_GEMM 1           /* implicit-GEMM conv, general EpiConv epilogue */
+#define SATB_OOB_ROUTE_GEMM_LEAN 2      /* implicit-GEMM conv, lean EpiConv epilogue */
+#define SATB_OOB_ROUTE_FUSED 4          /* fused ResidualUnit (conv_halo, FUSE), general epilogue */
+#define SATB_OOB_ROUTE_FUSED_LEAN 8     /* fused ResidualUnit, lean epilogue */
+#define SATB_OOB_ROUTE_HALO_NCL 16      /* halo-tile conv with the NCL fp32 store */
+#define SATB_OOB_ROUTE_GEMM_NCL 32      /* implicit-GEMM conv with the NCL fp32 store */
+#define SATB_OOB_ROUTE_CUDA_CORE 64     /* encoder input conv on CUDA cores */
+typedef struct SatbOobleckProbe {
+  int step, block, unit, B, L;      /* L: input positions per item */
+  void* in;                         /* 16-bit input (overwritten by a two-launch ResidualUnit), or fp32 NCL */
+  const void* raw_in;
+  void* raw_out;
+  void* out16;
+  void* scratch;
+  float* out32;
+  long long lo_off;                 /* fp16x3 only */
+  /* set by the call */
+  int result_in_scratch, wrote_raw, routes;
+} SatbOobleckProbe;
+int satb_oobleck_probe(SatbOobleck* h, SatbOobleckProbe* p, void* stream);
+/* The stored weights of the finalized conv `prefix` ("layers.1.layers.1."): the 16-bit [tap][n][k] block (and, in
+ * fp16x3 mode, its lo block right after it), or the fp32 [cout][cin][k] weights of a CUDA-core conv.  *bytes gets
+ * the size; dst (device, may be NULL to ask for the size) receives the data. */
+int satb_oobleck_weights(SatbOobleck* h, const char* prefix, void* dst, long long* bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
