@@ -11,9 +11,12 @@
 // Structure (one persistent CTA per SM, 384 threads, 128 x BN tiles):
 //   warpgroup 0      TMA producer      one thread: global -> 128B-swizzled smem ring (mbarrier full/empty)
 //   warpgroups 1, 2  MMA + epilogue    64 rows each: wgmma 64xBNx16 from the smem ring into registers, then the
-//                                      fused epilogue (accumulator -> smem -> one row per thread -> fused op -> global)
+//                                      fused epilogue (accumulator -> smem -> one row per thread -> fused op -> global,
+//                                      or, for EpiSwiglu and EpiResidual, fused op on the fragment -> global)
 // The producer runs ahead into the next tile's k-blocks while the epilogue of the current one runs.
 #pragma once
+#include <type_traits>
+
 #include "common.cuh"
 #include "ptx.cuh"
 
@@ -50,19 +53,30 @@ constexpr int kGemmThreads = 384;   // producer warpgroup + 2 MMA / epilogue war
 constexpr int kSmemBudget = 227 * 1024;   // the most shared memory a block may use on sm_90
 
 constexpr int kEpiWarps = 8;
-template <int BN, int kCols, int kEpiStage = 0>   // kEpiStage: bytes of epilogue staging smem per epilogue warp
+// kCols: columns per accumulator staging chunk, 0 for an epilogue that works on the accumulator fragment (no staging).
+// kEpiStage: bytes of epilogue staging smem per epilogue warp.
+template <int BN, int kCols, int kEpiStage = 0>
 struct GemmCfg {
   static constexpr int kStageA = kBlockM * kBlockK * 2;
   static constexpr int kStageB = BN * kBlockK * 2;
   static constexpr int kStage = kStageA + kStageB;
   static constexpr int kAccLd = kCols + 4;              // fp32 row pitch of the accumulator staging tile
-  static constexpr int kAccStage = 2 * 64 * kAccLd * 4;  // per MMA warpgroup: two column chunks of its 64 rows
+  static constexpr int kAccStage = kCols ? 2 * 64 * kAccLd * 4 : 0;   // per MMA warpgroup: two column chunks of its 64 rows
   static constexpr int kFixed = 1024 /*align slack*/ + 256 /*barriers*/ + 2 * kAccStage + kEpiWarps * kEpiStage;
   static constexpr int kStages = (kSmemBudget - kFixed) / kStage > 8 ? 8 : (kSmemBudget - kFixed) / kStage;
   static constexpr int kSmemBytes = kStages * kStage + kFixed;
   static_assert(BN == 64 || BN == 128 || BN == 256, "BN must be 64/128/256");
   static_assert(kStages >= 2, "shared memory too small for a two-stage ring");
 };
+
+// An epilogue with `static constexpr bool kFragment = true` receives the MMA warpgroup's accumulator fragment itself
+// (Epi::apply_fragment) instead of row chunks staged through shared memory (Epi::apply).
+template <class Epi, class = void>
+struct EpiFragment : std::false_type {};
+template <class Epi>
+struct EpiFragment<Epi, std::void_t<decltype(Epi::kFragment)>> : std::bool_constant<Epi::kFragment> {};
+template <class Epi>
+constexpr int kStagedCols = EpiFragment<Epi>::value ? 0 : Epi::kCols;
 
 struct EpiCtx {
   int row;       // flattened output row = batch * L + l
@@ -140,7 +154,7 @@ template <class Epi, int BN, bool BF16>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmA2, const GemmShape s, const typename Epi::Params ep) {
-  using Cfg = GemmCfg<BN, Epi::kCols, Epi::kStageBytes>;
+  using Cfg = GemmCfg<BN, kStagedCols<Epi>, Epi::kStageBytes>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStage);
@@ -270,7 +284,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       wgmma_wait<0>(acc);
       if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
 
-      gemm_tile_epilogue<Epi, BN>(acc, acc_st, epi_st, ep, s.L, s.N, m0, n0, batch, cw, warp, lane);
+      if constexpr (EpiFragment<Epi>::value)
+        Epi::template apply_fragment<BN>(ep, acc, s.L, s.N, m0 + 64 * cw + 16 * (warp & 3) + (lane >> 2), n0, batch, lane);
+      else
+        gemm_tile_epilogue<Epi, BN>(acc, acc_st, epi_st, ep, s.L, s.N, m0, n0, batch, cw, warp, lane);
     }
   }
 }
@@ -347,9 +364,13 @@ struct EpiStore32 {
 
 // Residual stream update (models/transformer.py:692-700 and adaLN :670-689):
 //   h[row, col] += (acc + bias[col]) * gate[row / rows_per_item, col]
+// Runs on the accumulator fragment: each thread adds its column pairs (c, c + 1) of rows row0 and row0 + 8 with one
+// fire-and-forget fp32 vector reduction in L2 each, so every warp-wide reduction covers whole 32-byte sectors.  Every
+// element receives exactly one add per GEMM (no split-K), so the result is deterministic.
 struct EpiResidual {
   static constexpr int kCols = 32;
   static constexpr int kStageBytes = 0;
+  static constexpr bool kFragment = true;
   struct Params {
     float* h;
     int ld;
@@ -359,28 +380,36 @@ struct EpiResidual {
     int gate_ld;
     int n_items;        // item = (row / rows_per_item) % n_items (CFG halves share the conditioning)
   };
-  __device__ static __forceinline__ void apply(const Params& p, const EpiCtx& c, const uint32_t (&r)[32]) {
-    if (!c.valid) return;
-    float4* dst = reinterpret_cast<float4*>(p.h + static_cast<size_t>(c.row) * p.ld + c.col0);
-    const float4* g = p.gate ? reinterpret_cast<const float4*>(
-                                   p.gate + static_cast<size_t>((c.row / p.rows_per_item) % p.n_items) * p.gate_ld + c.col0)
-                             : nullptr;
+  template <int BN>
+  __device__ static __forceinline__ void apply_fragment(const Params& p, const float (&acc)[BN / 2], int L, int N,
+                                                        int row0, int n0, int batch, int lane) {
+    const int fc = 2 * (lane & 3);
+    const float* grow[2] = {nullptr, nullptr};
+    float* hrow[2];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      float4 v = make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]), __uint_as_float(r[4 * j + 2]),
-                             __uint_as_float(r[4 * j + 3]));
-      if (p.bias) {
-        const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + c.col0) + j);
-        v.x += b.x; v.y += b.y; v.z += b.z; v.w += b.w;
+    for (int rr = 0; rr < 2; ++rr) {
+      const int row = batch * L + row0 + 8 * rr;
+      hrow[rr] = p.h + static_cast<size_t>(row) * p.ld + n0 + fc;
+      if (p.gate) grow[rr] = p.gate + static_cast<size_t>((row / p.rows_per_item) % p.n_items) * p.gate_ld + n0 + fc;
+    }
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      if (n0 + 8 * j >= N) break;
+      float2 b = make_float2(0.f, 0.f);
+      if (p.bias) b = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + fc + 8 * j));
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        if (row0 + 8 * rr >= L) continue;
+        float2 v = make_float2(acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1]);
+        if (p.bias) {
+          v.x += b.x; v.y += b.y;
+        }
+        if (p.gate) {
+          const float2 gg = __ldg(reinterpret_cast<const float2*>(grow[rr] + 8 * j));
+          v.x *= gg.x; v.y *= gg.y;
+        }
+        asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(hrow[rr] + 8 * j), "f"(v.x), "f"(v.y) : "memory");
       }
-      if (g) {
-        const float4 gg = __ldg(g + j);
-        v.x *= gg.x; v.y *= gg.y; v.z *= gg.z; v.w *= gg.w;
-      }
-      // fire-and-forget fp32 vector reduction in L2: every element receives exactly one add
-      // per GEMM (no split-K), so the result is deterministic and no load stalls the epilogue
-      asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + j), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)
-                   : "memory");
     }
   }
 };
@@ -509,36 +538,54 @@ struct EpiHeadNorm16 {
 // half of the projection).  The weight rows are interleaved at load time so every
 // 64-column group holds 32 value columns followed by their 32 gate columns:
 //   out[row, g*32 + j] = (acc[g*64 + j] + b) * silu(acc[g*64 + 32 + j] + b')
+// Value column c and gate column c + 32 of a group sit in the same thread's accumulator fragment (8-column groups j
+// and j + 4), so the epilogue runs on the fragment: no staging through shared memory, no barrier, and each thread
+// stores its 16-bit pairs (c, c + 1) straight to global memory.
 template <bool BF16>
 struct EpiSwiglu {
   static constexpr int kCols = 64;
   static constexpr int kStageBytes = 0;
+  static constexpr bool kFragment = true;
   struct Params {
     void* out;
     int ld;             // inner dim (N/2)
     const float* bias;  // interleaved like the weight rows; may be null
   };
-  __device__ static __forceinline__ void apply(const Params& p, const EpiCtx& c, const uint32_t (&r)[64]) {
-    if (!c.valid) return;
-    // two value columns and their two gate columns at a time, straight from the accumulator registers (a 64-float
-    // working copy next to the two 64-register chunk buffers of the epilogue loop spills)
-    uint32_t o[16];
+  // acc: the wgmma fragment of 64 rows x BN columns (ptx.cuh wgmma_ss); row0: this thread's first fragment row (the
+  // second is row0 + 8), lane & 3 selects its column pair in every 8-column group.
+  template <int BN>
+  __device__ static __forceinline__ void apply_fragment(const Params& p, const float (&acc)[BN / 2], int L, int N,
+                                                        int row0, int n0, int batch, int lane) {
+    const int fc = 2 * (lane & 3);
 #pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      float a0 = __uint_as_float(r[2 * j]), a1 = __uint_as_float(r[2 * j + 1]);
-      float g0 = __uint_as_float(r[32 + 2 * j]), g1 = __uint_as_float(r[33 + 2 * j]);
-      if (p.bias) {
-        a0 += __ldg(p.bias + c.col0 + 2 * j);
-        a1 += __ldg(p.bias + c.col0 + 2 * j + 1);
-        g0 += __ldg(p.bias + c.col0 + 32 + 2 * j);
-        g1 += __ldg(p.bias + c.col0 + 33 + 2 * j);
+    for (int g = 0; g < BN / 64; ++g) {
+      const int col0 = n0 + 64 * g;
+      if (col0 >= N) break;
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const int c = 8 * jj + fc;   // value columns c, c + 1; gate columns c + 32, c + 33
+        float2 bv = make_float2(0.f, 0.f), bg = bv;
+        if (p.bias) {
+          bv = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + c));
+          bg = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + 32 + c));
+        }
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          const int l = row0 + 8 * rr;
+          if (l >= L) continue;
+          const int av = 4 * (8 * g + jj) + 2 * rr, ag = av + 16;
+          float a0 = acc[av], a1 = acc[av + 1], g0 = acc[ag], g1 = acc[ag + 1];
+          if (p.bias) {
+            a0 += bv.x;
+            a1 += bv.y;
+            g0 += bg.x;
+            g1 += bg.y;
+          }
+          uint16_t* dst = static_cast<uint16_t*>(p.out) + static_cast<size_t>(batch * L + l) * p.ld + (col0 >> 1) + c;
+          *reinterpret_cast<uint32_t*>(dst) = Op16<BF16>::pack(a0 * silu_f(g0), a1 * silu_f(g1));
+        }
       }
-      o[j] = Op16<BF16>::pack(a0 * silu_f(g0), a1 * silu_f(g1));
     }
-    uint4* dst =
-        reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.out) + static_cast<size_t>(c.row) * p.ld + (c.col0 >> 1));
-#pragma unroll
-    for (int j = 0; j < 4; ++j) dst[j] = make_uint4(o[4 * j], o[4 * j + 1], o[4 * j + 2], o[4 * j + 3]);
   }
 };
 
@@ -882,7 +929,7 @@ int make_tmap_b(CUtensorMap* m, const void* ptr, int K, int rows, int64_t row_st
 template <class Epi, int BN, bool BF16>
 int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape& s, const typename Epi::Params& ep,
                 cudaStream_t stream, const CUtensorMap* tmA2 = nullptr) {
-  using Cfg = GemmCfg<BN, Epi::kCols, Epi::kStageBytes>;
+  using Cfg = GemmCfg<BN, kStagedCols<Epi>, Epi::kStageBytes>;
   auto kern = gemm_wgmma_kernel<Epi, BN, BF16>;
   static PerDeviceOnce attr;
   if (attr.first()) SATB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
