@@ -21,6 +21,16 @@ int satb_layernorm(const float* x, const float* gamma, const float* beta, void* 
                           static_cast<cudaStream_t>(stream));
 }
 
+int satb_layernorm_fp8(const float* x, const float* gamma, const float* beta, const float* mod_scale,
+                       const float* mod_shift, long long mod_stride, int rows_per_item, int n_items, void* out8,
+                       float* row_scale, int rows, int D, void* stream) {
+  SATB_REQUIRE(x && gamma && out8 && row_scale, "null argument");
+  SATB_REQUIRE(!mod_scale || (mod_shift && rows_per_item >= 1 && n_items >= 1 && mod_stride % 4 == 0),
+               "adaLN modulation needs shift, rows_per_item >= 1, n_items >= 1 and mod_stride % 4 == 0");
+  return launch_layernorm_fp8(x, gamma, beta, out8, row_scale, rows, D, mod_scale, mod_shift, mod_stride,
+                              rows_per_item, n_items, static_cast<cudaStream_t>(stream));
+}
+
 int satb_linear_f32out(const void* a16, const void* w16, float* c, int M, int N, int K, int bf16, void* stream) {
   SATB_REQUIRE(a16 && w16 && c, "null argument");
   SATB_REQUIRE(M >= 1 && N >= 32 && N % 32 == 0 && K >= 8 && K % 8 == 0, "linear: need N % 32 == 0 and K % 8 == 0");

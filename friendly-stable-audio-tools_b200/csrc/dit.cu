@@ -45,26 +45,28 @@ struct DevBuf {
   }
 };
 
+// Tensor maps by (pointer, shape, strides, box rows, element bytes): one buffer may be read as 16-bit and as e4m3 rows.
 struct TmapCache {
-  typedef std::tuple<const void*, int, int, int, int64_t, int64_t, int> Key;
+  typedef std::tuple<const void*, int, int, int, int64_t, int64_t, int, int> Key;
   std::map<Key, CUtensorMap> maps;
-  int get_a(const void* ptr, int K, int L, int batches, int64_t rs, int64_t bs, const CUtensorMap** out) {
-    Key k(ptr, K, L, batches, rs, bs, -1);
+  int get_a(const void* ptr, int K, int L, int batches, int64_t rs, int64_t bs, const CUtensorMap** out,
+            int elem_bytes = 2) {
+    Key k(ptr, K, L, batches, rs, bs, -1, elem_bytes);
     auto it = maps.find(k);
     if (it == maps.end()) {
       CUtensorMap m;
-      SATB_PROPAGATE(make_tmap_a(&m, ptr, K, L, batches, rs, bs));
+      SATB_PROPAGATE(make_tmap_a(&m, ptr, K, L, batches, rs, bs, 1, kBlockM, elem_bytes));
       it = maps.emplace(k, m).first;
     }
     *out = &it->second;
     return 0;
   }
-  int get_b(const void* ptr, int K, int rows, int64_t rs, int box_rows, const CUtensorMap** out) {
-    Key k(ptr, K, rows, 0, rs, 0, box_rows);
+  int get_b(const void* ptr, int K, int rows, int64_t rs, int box_rows, const CUtensorMap** out, int elem_bytes = 2) {
+    Key k(ptr, K, rows, 0, rs, 0, box_rows, elem_bytes);
     auto it = maps.find(k);
     if (it == maps.end()) {
       CUtensorMap m;
-      SATB_PROPAGATE(make_tmap_b(&m, ptr, K, rows, rs, box_rows));
+      SATB_PROPAGATE(make_tmap_b(&m, ptr, K, rows, rs, box_rows, elem_bytes));
       it = maps.emplace(k, m).first;
     }
     *out = &it->second;
@@ -74,32 +76,33 @@ struct TmapCache {
 
 // Flat Linear: C[M, N] = A[M, K] * W[N, K]^T with a fused epilogue.  b_static = 1: W is a weight matrix prepared at
 // finalize time, so its first tiles may be fetched before the dependency wait (every product call); satb_gemm_probe
-// also runs 0.
-template <class Epi, int BN, bool BF16>
+// also runs 0.  FP8: A and W are e4m3 rows (lda in elements = bytes) with their row scales in sc.
+template <class Epi, int BN, bool BF16, bool FP8 = false>
 static int linear(TmapCache& tc, const void* A, int64_t lda, int M, int K, const void* W, int N,
-                  const typename Epi::Params& ep, cudaStream_t stream, int b_static = 1) {
+                  const typename Epi::Params& ep, cudaStream_t stream, int b_static = 1, const Fp8Scales& sc = Fp8Scales{}) {
+  const int eb = FP8 ? 1 : 2;
   const CUtensorMap *ta, *tb;
-  SATB_PROPAGATE(tc.get_a(A, K, M, 1, lda, static_cast<int64_t>(M) * lda, &ta));
+  SATB_PROPAGATE(tc.get_a(A, K, M, 1, lda, static_cast<int64_t>(M) * lda, &ta, eb));
   GemmShape s;
   s.L = M; s.batches = 1; s.N = N; s.K = K; s.n_taps = 1; s.tap_base = 0; s.tap_step = 0; s.b_tap_rows = N; s.stride = 1;
   s.b_static = b_static;
-  SATB_PROPAGATE(tc.get_b(W, K, N, K, BN, &tb));
-  return launch_gemm<Epi, BN, BF16>(*ta, *tb, s, ep, stream);
+  SATB_PROPAGATE(tc.get_b(W, K, N, K, BN, &tb, eb));
+  return launch_gemm<Epi, BN, BF16, FP8>(*ta, *tb, s, ep, stream, nullptr, sc);
 }
 
 // Picks the N tile (256 or 128) that wastes less of the last wave of the persistent grid; the
 // 128-wide tile streams as many smem bytes per MMA cycle as the tensor pipe can take, so it is
 // only preferred when it clearly wins on wave quantisation.
-template <class Epi, bool BF16>
+template <class Epi, bool BF16, bool FP8 = false>
 static int linear_auto(TmapCache& tc, const void* A, int64_t lda, int M, int K, const void* W, int N,
-                       const typename Epi::Params& ep, cudaStream_t stream) {
+                       const typename Epi::Params& ep, cudaStream_t stream, const Fp8Scales& sc = Fp8Scales{}) {
   const double sms = device_sm_count();
   auto eff = [&](int bn) {
     const double waves = static_cast<double>(ceil_div(M, kBlockM)) * ceil_div(N, bn) / sms;
     return waves / std::ceil(waves);
   };
-  if (N % 128 == 0 && eff(128) * 0.9 > eff(256)) return linear<Epi, 128, BF16>(tc, A, lda, M, K, W, N, ep, stream);
-  return linear<Epi, 256, BF16>(tc, A, lda, M, K, W, N, ep, stream);
+  if (N % 128 == 0 && eff(128) * 0.9 > eff(256)) return linear<Epi, 128, BF16, FP8>(tc, A, lda, M, K, W, N, ep, stream, 1, sc);
+  return linear<Epi, 256, BF16, FP8>(tc, A, lda, M, K, W, N, ep, stream, 1, sc);
 }
 
 struct LayerW {
@@ -107,6 +110,9 @@ struct LayerW {
   uint16_t *w_qkv = nullptr, *w_o = nullptr, *w_q = nullptr, *w_kv = nullptr, *w_co = nullptr, *w_ff1 = nullptr,
            *w_ff2 = nullptr;
   float *b_ff1 = nullptr, *b_ff2 = nullptr;
+  // FP8 mode: e4m3 copies of to_qkv, cross_attn.to_q and ff.0 (in place of their 16-bit ones) and their row scales
+  uint8_t *w8_qkv = nullptr, *w8_q = nullptr, *w8_ff1 = nullptr;
+  float *s_qkv = nullptr, *s_q = nullptr, *s_ff1 = nullptr;
 };
 
 }  // namespace satb
@@ -120,7 +126,7 @@ struct SatbDit {
   float *pe0_w = nullptr, *pe2_w = nullptr;   // to_prepend_embed (fp32, bias-free)
   int Pp = 0;                 // prepend-conditioning tokens of the current conditioning
   DevBuf ws_prep;             // their embeddings [B, Pp, D] + scratch
-  bool bf16, adaln, qk_norm = false;
+  bool bf16, fp8, adaln, qk_norm = false;   // fp8: e4m3 operands for the QKV, cross q and FF-in GEMMs (fp16 elsewhere)
   int P;  // prepended tokens: 1 (the global-conditioning token; 0 in adaLN mode) + Pp
   std::vector<LayerW> layers;
   std::vector<void*> owned;   // every cudaMalloc of weight storage
@@ -141,6 +147,7 @@ struct SatbDit {
   // workspace
   TmapCache tmaps;
   DevBuf ws_h, ws_a16, ws_qkv, ws_attn, ws_q16, ws_ff, ws_ain, ws_y, ws_small, ws_cond, ws_kv, ws_rope;
+  DevBuf ws_a8, ws_ascale;   // FP8 mode: e4m3 LayerNorm rows [M, D] and their scales [M]
   int rope_len = 0;
   int res_R = 0, res_L = 0, res_P = -1;
   // optional per-category CUDA-event timing (bench.py roofline)
@@ -211,6 +218,7 @@ int satb_dit_create(const SatbDitConfig* cfg, SatbDit** out) {
   SATB_REQUIRE(cfg->prepend_cond_dim >= 0 && cfg->prepend_cond_dim % 4 == 0, "prepend_cond_dim must be a multiple of 4");
   SATB_REQUIRE(!(cfg->prepend_cond_dim > 0 && cfg->global_cond_type == 1),
                "prepend conditioning is supported with global_cond_type \"prepend\" only");
+  SATB_REQUIRE(cfg->operand_dtype >= 0 && cfg->operand_dtype <= 2, "operand_dtype must be 0 (fp16), 1 (bf16) or 2 (fp8)");
   SatbDit* d = new SatbDit();
   d->cfg = *cfg;
   d->D = cfg->embed_dim;
@@ -229,6 +237,7 @@ int satb_dit_create(const SatbDitConfig* cfg, SatbDit** out) {
   const int rot = d->dh / 2 > 32 ? d->dh / 2 : 32;  // models/transformer.py:737
   d->nf = rot / 2;
   d->bf16 = cfg->operand_dtype == 1;
+  d->fp8 = cfg->operand_dtype == 2;
   d->adaln = cfg->global_cond_type == 1;
   d->qk_norm = cfg->qk_norm != 0;
   d->P = d->adaln ? 0 : 1;
@@ -256,7 +265,7 @@ void satb_dit_destroy(SatbDit* d) {
   for (void* p : d->owned) cudaFree(p);
   d->ws_h.release(); d->ws_a16.release(); d->ws_qkv.release(); d->ws_attn.release(); d->ws_q16.release();
   d->ws_ff.release(); d->ws_ain.release(); d->ws_y.release(); d->ws_small.release(); d->ws_cond.release();
-  d->ws_kv.release(); d->ws_rope.release(); d->ws_prep.release();
+  d->ws_kv.release(); d->ws_rope.release(); d->ws_prep.release(); d->ws_a8.release(); d->ws_ascale.release();
   delete d;
 }
 
@@ -278,6 +287,13 @@ int satb_dit_load_weight(SatbDit* d, const char* name_c, const float* src, long 
     SATB_REQUIRE(numel == static_cast<long long>(rows) * cols, ("bad size for " + name).c_str());
     if (!*dst) SATB_PROPAGATE(d->alloc(dst, static_cast<size_t>(rows) * cols));
     return launch_cast_rows(src, *dst, perm, rows, cols, cols, cols, d->bf16, st);
+  };
+  // FP8 mode: e4m3 rows with one power-of-two scale per stored row, taken after the row permutation
+  auto quant8 = [&](uint8_t** dst, float** scale, int rows, int cols, const int* perm) -> int {
+    SATB_REQUIRE(numel == static_cast<long long>(rows) * cols, ("bad size for " + name).c_str());
+    if (!*dst) SATB_PROPAGATE(d->alloc(dst, static_cast<size_t>(rows) * cols));
+    if (!*scale) SATB_PROPAGATE(d->alloc(scale, rows));
+    return launch_quant_rows_fp8(src, *dst, *scale, perm, rows, cols, st);
   };
   d->finalized = false;
   d->loaded[name] = 1;
@@ -317,10 +333,10 @@ int satb_dit_load_weight(SatbDit* d, const char* name_c, const float* src, long 
         SATB_PROPAGATE(d->alloc(&d->qkv_perm, perm.size()));
         SATB_CHECK_CUDA(cudaMemcpy(d->qkv_perm, perm.data(), perm.size() * sizeof(int), cudaMemcpyHostToDevice));
       }
-      return cast16(&L.w_qkv, 3 * D, D, d->qkv_perm);
+      return d->fp8 ? quant8(&L.w8_qkv, &L.s_qkv, 3 * D, D, d->qkv_perm) : cast16(&L.w_qkv, 3 * D, D, d->qkv_perm);
     }
     if (k == "self_attn.to_out.weight") return cast16(&L.w_o, D, D, nullptr);
-    if (k == "cross_attn.to_q.weight") return cast16(&L.w_q, D, D, nullptr);
+    if (k == "cross_attn.to_q.weight") return d->fp8 ? quant8(&L.w8_q, &L.s_q, D, D, nullptr) : cast16(&L.w_q, D, D, nullptr);
     if (k == "cross_attn.to_kv.weight") return cast16(&L.w_kv, 2 * d->ce, d->ce, nullptr);
     if (k == "cross_attn.to_out.weight") return cast16(&L.w_co, D, D, nullptr);
     if (k == "ff.ff.0.proj.weight" || k == "ff.ff.0.proj.bias") {
@@ -334,7 +350,8 @@ int satb_dit_load_weight(SatbDit* d, const char* name_c, const float* src, long 
         SATB_PROPAGATE(d->alloc(&d->ff_perm, perm.size()));
         SATB_CHECK_CUDA(cudaMemcpy(d->ff_perm, perm.data(), perm.size() * sizeof(int), cudaMemcpyHostToDevice));
       }
-      if (ends_with(k, "weight")) return cast16(&L.w_ff1, 2 * d->ffi, D, d->ff_perm);
+      if (ends_with(k, "weight"))
+        return d->fp8 ? quant8(&L.w8_ff1, &L.s_ff1, 2 * d->ffi, D, d->ff_perm) : cast16(&L.w_ff1, 2 * d->ffi, D, d->ff_perm);
       SATB_REQUIRE(numel == 2 * d->ffi, ("bad size for " + name).c_str());
       if (!L.b_ff1) SATB_PROPAGATE(d->alloc(&L.b_ff1, 2 * d->ffi));
       return launch_gather_f32(src, L.b_ff1, d->ff_perm, 2 * d->ffi, st);
@@ -368,8 +385,11 @@ int satb_dit_finalize(SatbDit* d, void* stream_v) {
   if (d->gd > 0) SATB_REQUIRE(d->ge0_w && d->ge2_w, "to_global_embed weights missing");
   for (int i = 0; i < d->depth; ++i) {
     const LayerW& L = d->layers[i];
-    SATB_REQUIRE(L.pre_g && L.ff_g && L.w_qkv && L.w_o && L.w_ff1 && L.w_ff2, "transformer layer weights missing");
-    if (d->ct > 0) SATB_REQUIRE(L.ca_g && L.w_q && L.w_kv && L.w_co, "cross-attention weights missing");
+    SATB_REQUIRE(L.pre_g && L.ff_g && (d->fp8 ? L.w8_qkv && L.w8_ff1 : L.w_qkv && L.w_ff1) && L.w_o && L.w_ff2,
+                 "transformer layer weights missing");
+    if (d->ct > 0)
+      SATB_REQUIRE(L.ca_g && (d->fp8 ? L.w8_q != nullptr : L.w_q != nullptr) && L.w_kv && L.w_co,
+                   "cross-attention weights missing");
   }
   if (d->adaln) SATB_REQUIRE(d->w_ssg, "adaLN to_scale_shift_gate weights missing");
   SATB_CHECK_CUDA(cudaStreamSynchronize(st));
@@ -448,6 +468,10 @@ int satb_dit_reserve(SatbDit* d, int R, int L) {
   SATB_PROPAGATE(d->ws_ff.ensure(M * d->ffi * 2));
   SATB_PROPAGATE(d->ws_ain.ensure(M * d->Cin * 2));
   SATB_PROPAGATE(d->ws_y.ensure(M * d->C * 4));
+  if (d->fp8) {
+    SATB_PROPAGATE(d->ws_a8.ensure(M * D));
+    SATB_PROPAGATE(d->ws_ascale.ensure(M * 4));
+  }
   SATB_PROPAGATE(ensure_rope(d, N_seq));
   d->tmaps.maps.clear();
   d->res_R = R;
@@ -586,7 +610,9 @@ struct ProfScope {
 };
 enum { PROF_FF_IN = 0, PROF_FF_OUT, PROF_QKV, PROF_ATTN_SELF, PROF_ATTN_OUT, PROF_CROSS, PROF_LN, PROF_OTHER, PROF_NCAT };
 
-template <bool BF16>
+// FP8 = true: the QKV, cross-attention q and FF-in GEMMs read e4m3 LayerNorm rows (a8, one scale per row in a_scale)
+// and the e4m3 weights; everything else runs as in fp16 mode (BF16 = false).
+template <bool BF16, bool FP8 = false>
 static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* out, int B, int L, float cfg_scale,
                             float scale_phi, cudaStream_t st, float* hidden_out) {
   const int D = d->D, C = d->C, H = d->H, P = d->P;
@@ -597,6 +623,15 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
   SmallWs sw = small_ws(d, 2 * d->B);
   float* h = d->ws_h.as<float>();
   uint16_t* a16 = d->ws_a16.as<uint16_t>();
+  uint8_t* a8 = d->ws_a8.as<uint8_t>();
+  float* a_scale = d->ws_ascale.as<float>();
+  // LayerNorm rows for one of the three FP8-capable GEMMs: e4m3 + row scales in FP8 mode, 16-bit otherwise
+  auto layernorm_in = [&](const float* g, const float* b, int rows, const float* mod_scale, const float* mod_shift,
+                          int64_t mod_ld, int n_items) -> int {
+    if (FP8) return launch_layernorm_fp8(h, g, b, a8, a_scale, rows, D, mod_scale, mod_shift, mod_ld, N_seq, n_items, st);
+    return launch_layernorm(h, g, b, a16, rows, D, mod_scale, mod_shift, mod_ld, N_seq, n_items, BF16, st);
+  };
+  const void* a_in = FP8 ? static_cast<const void*>(a8) : static_cast<const void*>(a16);
   uint16_t* qkv = d->ws_qkv.as<uint16_t>();
   uint16_t* att = d->ws_attn.as<uint16_t>();
   uint16_t* q16 = d->ws_q16.as<uint16_t>();
@@ -630,18 +665,22 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
     // ---- self-attention: LN -> QKV GEMM (+RoPE) -> attention -> out-proj (+residual)
     {
       ProfScope ps(d, PROF_LN, st);
-      SATB_PROPAGATE(launch_layernorm(h, W.pre_g, W.pre_b, a16, M, D, ssg_l, ssg_l ? ssg_l + D : nullptr, ssg_ld, N_seq, B, BF16, st));
+      SATB_PROPAGATE(layernorm_in(W.pre_g, W.pre_b, M, ssg_l, ssg_l ? ssg_l + D : nullptr, ssg_ld, B));
     }
     {
       ProfScope ps(d, PROF_QKV, st);
+      const void* w = FP8 ? static_cast<const void*>(W.w8_qkv) : static_cast<const void*>(W.w_qkv);
+      const Fp8Scales sc{a_scale, W.s_qkv};
       if (d->qk_norm) {
         typedef EpiHeadNorm16<BF16> E;   // q, k heads L2-normalised, then rotary
         typename E::Params ep{qkv, 3 * D, 2 * D, 2 * D, N_seq, cos_tab, sin_tab};
-        SATB_PROPAGATE((linear<E, 256, BF16>(d->tmaps, a16, D, M, D, W.w_qkv, 3 * D, ep, st)));
+        // FP8: BN 128 (the instance the cross q GEMM also runs; the BN 256 one spills a few registers)
+        constexpr int kBn = FP8 ? 128 : 256;
+        SATB_PROPAGATE((linear<E, kBn, BF16, FP8>(d->tmaps, a_in, D, M, D, w, 3 * D, ep, st, 1, sc)));
       } else {
         typedef EpiQkvRope<BF16> E;
         typename E::Params ep{qkv, 3 * D, 2 * D, N_seq, d->dh, d->nf, cos_tab, sin_tab};
-        SATB_PROPAGATE((linear<E, 256, BF16>(d->tmaps, a16, D, M, D, W.w_qkv, 3 * D, ep, st)));
+        SATB_PROPAGATE((linear<E, 256, BF16, FP8>(d->tmaps, a_in, D, M, D, w, 3 * D, ep, st, 1, sc)));
       }
     }
     {
@@ -662,15 +701,20 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
     if (Mc > 0) {
       ProfScope ps(d, PROF_CROSS, st);
       const int Hkv = d->ce / d->dh;
-      SATB_PROPAGATE(launch_layernorm(h, W.ca_g, W.ca_b, a16, Mc, D, nullptr, nullptr, 0, N_seq, 1, BF16, st));
+      SATB_PROPAGATE(layernorm_in(W.ca_g, W.ca_b, Mc, nullptr, nullptr, 0, 1));
+      const void* wq = FP8 ? static_cast<const void*>(W.w8_q) : static_cast<const void*>(W.w_q);
+      const Fp8Scales sc{a_scale, W.s_q};
       if (d->qk_norm) {
         typedef EpiHeadNorm16<BF16> E;
         typename E::Params ep{q16, D, D, 0, N_seq, nullptr, nullptr};
-        SATB_PROPAGATE((linear_auto<E, BF16>(d->tmaps, a16, D, Mc, D, W.w_q, D, ep, st)));
+        if (FP8)   // BN 128 only, as for the QKV GEMM above
+          SATB_PROPAGATE((linear<E, 128, BF16, FP8>(d->tmaps, a_in, D, Mc, D, wq, D, ep, st, 1, sc)));
+        else
+          SATB_PROPAGATE((linear_auto<E, BF16>(d->tmaps, a_in, D, Mc, D, wq, D, ep, st)));
       } else {
         typedef EpiStore16<BF16> E;
         typename E::Params ep{q16, D, nullptr, 0};
-        SATB_PROPAGATE((linear_auto<E, BF16>(d->tmaps, a16, D, Mc, D, W.w_q, D, ep, st)));
+        SATB_PROPAGATE((linear_auto<E, BF16, FP8>(d->tmaps, a_in, D, Mc, D, wq, D, ep, st, sc)));
       }
       const uint16_t* kv = d->ws_kv.as<uint16_t>() + static_cast<size_t>(i) * d->Rc * d->Mctx * 2 * d->ce;
       const int64_t kvs = static_cast<int64_t>(d->Mctx) * 2 * d->ce;
@@ -688,14 +732,16 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
     // ---- feed-forward: LN -> GEMM (+bias, SwiGLU) -> GEMM (+bias, +residual)
     {
       ProfScope ps(d, PROF_LN, st);
-      SATB_PROPAGATE(launch_layernorm(h, W.ff_g, W.ff_b, a16, M, D, ssg_l ? ssg_l + 3 * D : nullptr,
-                                      ssg_l ? ssg_l + 4 * D : nullptr, ssg_ld, N_seq, B, BF16, st));
+      SATB_PROPAGATE(layernorm_in(W.ff_g, W.ff_b, M, ssg_l ? ssg_l + 3 * D : nullptr, ssg_l ? ssg_l + 4 * D : nullptr,
+                                  ssg_ld, B));
     }
     {
       ProfScope ps(d, PROF_FF_IN, st);
       typedef EpiSwiglu<BF16> E;
       typename E::Params ep{ff, d->ffi, W.b_ff1};
-      SATB_PROPAGATE((linear<E, 256, BF16>(d->tmaps, a16, D, M, D, W.w_ff1, 2 * d->ffi, ep, st)));
+      const void* w = FP8 ? static_cast<const void*>(W.w8_ff1) : static_cast<const void*>(W.w_ff1);
+      SATB_PROPAGATE((linear<E, 256, BF16, FP8>(d->tmaps, a_in, D, M, D, w, 2 * d->ffi, ep, st, 1,
+                                                 Fp8Scales{a_scale, W.s_ff1})));
     }
     {
       ProfScope ps(d, PROF_FF_OUT, st);
@@ -712,6 +758,13 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
   return 0;
 }
 
+static int dit_forward_dispatch(SatbDit* d, const float* x, const float* t, float* out, int B, int L, float cfg_scale,
+                                float scale_phi, cudaStream_t st, float* hidden) {
+  if (d->fp8) return dit_forward_impl<false, true>(d, x, t, out, B, L, cfg_scale, scale_phi, st, hidden);
+  return d->bf16 ? dit_forward_impl<true>(d, x, t, out, B, L, cfg_scale, scale_phi, st, hidden)
+                 : dit_forward_impl<false>(d, x, t, out, B, L, cfg_scale, scale_phi, st, hidden);
+}
+
 extern "C" {
 
 // One denoiser call: x [B, C, L] fp32, t [B] fp32 -> out [B, C, L] fp32 (all device
@@ -724,8 +777,7 @@ int satb_dit_forward(SatbDit* d, const float* x, const float* t, float* out, int
   const int R = d->cfg_on ? 2 * B : B;
   if (R > d->res_R || L != d->res_L || d->P != d->res_P) SATB_PROPAGATE(satb_dit_reserve(d, R, L));
   cudaStream_t st = static_cast<cudaStream_t>(stream_v);
-  return d->bf16 ? dit_forward_impl<true>(d, x, t, out, B, L, cfg_scale, scale_phi, st, nullptr)
-                 : dit_forward_impl<false>(d, x, t, out, B, L, cfg_scale, scale_phi, st, nullptr);
+  return dit_forward_dispatch(d, x, t, out, B, L, cfg_scale, scale_phi, st, nullptr);
 }
 
 // Per-category kernel timing with CUDA events on the launching stream (bench.py roofline):
@@ -762,8 +814,7 @@ int satb_dit_forward_debug(SatbDit* d, const float* x, const float* t, float* ou
   const int R = d->cfg_on ? 2 * B : B;
   if (R > d->res_R || L != d->res_L || d->P != d->res_P) SATB_PROPAGATE(satb_dit_reserve(d, R, L));
   cudaStream_t st = static_cast<cudaStream_t>(stream_v);
-  return d->bf16 ? dit_forward_impl<true>(d, x, t, out, B, L, cfg_scale, scale_phi, st, hidden)
-                 : dit_forward_impl<false>(d, x, t, out, B, L, cfg_scale, scale_phi, st, hidden);
+  return dit_forward_dispatch(d, x, t, out, B, L, cfg_scale, scale_phi, st, hidden);
 }
 
 }  // extern "C"
@@ -773,17 +824,15 @@ int satb_dit_forward_debug(SatbDit* d, const float* x, const float* t, float* ou
 // copies); it instantiates no kernel the forward does not.
 static bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
 
-template <class E, int BN, bool BF16>
+template <class E, int BN, bool BF16, bool FP8 = false>
 static int probe_run(const void* a, const void* w, int M, int N, int K, const typename E::Params& ep, int b_static,
-                     cudaStream_t st) {
+                     cudaStream_t st, const Fp8Scales& sc = Fp8Scales{}) {
   SATB_REQUIRE(N % E::kCols == 0, ("gemm probe: N must be a multiple of " + std::to_string(E::kCols)).c_str());
   TmapCache tc;
-  return linear<E, BN, BF16>(tc, a, K, M, K, w, N, ep, st, b_static);
+  return linear<E, BN, BF16, FP8>(tc, a, K, M, K, w, N, ep, st, b_static, sc);
 }
 
-template <bool BF16>
-static int gemm_probe(const void* a, const void* w, int M, int N, int K, const SatbGemmProbe& p, cudaStream_t st) {
-  const int bn = p.bn;
+static int probe_check_outputs(const SatbGemmProbe& p, int N) {
   const int out_elem = p.epi == SATB_EPI_STORE32 ? 4 : 2;
   if (p.epi != SATB_EPI_RESIDUAL) {
     SATB_REQUIRE(p.out && aligned16(p.out), "gemm probe: out must be a 16-byte aligned device pointer");
@@ -794,6 +843,13 @@ static int gemm_probe(const void* a, const void* w, int M, int N, int K, const S
   }
   for (const void* q : std::initializer_list<const void*>{p.bias, p.gate, p.cos_tab, p.sin_tab})
     SATB_REQUIRE(aligned16(q), "gemm probe: every vector must be 16-byte aligned");
+  return 0;
+}
+
+template <bool BF16>
+static int gemm_probe(const void* a, const void* w, int M, int N, int K, const SatbGemmProbe& p, cudaStream_t st) {
+  const int bn = p.bn;
+  SATB_PROPAGATE(probe_check_outputs(p, N));
   switch (p.epi) {
     case SATB_EPI_STORE32: {
       const EpiStore32::Params ep{static_cast<float*>(p.out), p.ld, p.bias};
@@ -859,6 +915,58 @@ int satb_gemm_probe(const void* a16, const void* w16, int M, int N, int K, const
   SATB_REQUIRE(aligned16(a16) && aligned16(w16), "gemm probe: operands must be 16-byte aligned");
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   return p->bf16 ? gemm_probe<true>(a16, w16, M, N, K, *p, st) : gemm_probe<false>(a16, w16, M, N, K, *p, st);
+}
+
+// The FP8 instances of the forward: qkv_rope and swiglu BN 256, store16 BN 128 / 256, head_norm16 BN 128 (fp16 outputs).
+int satb_gemm_probe_fp8(const void* a8, const void* w8, const float* a_scale, const float* w_scale, int M, int N, int K,
+                        const SatbGemmProbe* p, void* stream) {
+  SATB_REQUIRE(a8 && w8 && a_scale && w_scale && p, "null argument");
+  SATB_REQUIRE(M >= 1 && N >= 32 && K >= 128 && K % 128 == 0, "gemm probe fp8: need M >= 1, N >= 32 and K % 128 == 0");
+  SATB_REQUIRE(aligned16(a8) && aligned16(w8) && aligned16(w_scale), "gemm probe fp8: operands must be 16-byte aligned");
+  SATB_REQUIRE(p->bf16 == 0, "gemm probe fp8: the FP8 instances store fp16");
+  SATB_PROPAGATE(probe_check_outputs(*p, N));
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const Fp8Scales sc{a_scale, w_scale};
+  const int bn = p->bn;
+  switch (p->epi) {
+    case SATB_EPI_STORE16: {
+      typedef EpiStore16<false> E;
+      const E::Params ep{p->out, p->ld, p->bias, p->act};
+      if (bn == 128) return probe_run<E, 128, false, true>(a8, w8, M, N, K, ep, p->b_static, st, sc);
+      if (bn == 256) return probe_run<E, 256, false, true>(a8, w8, M, N, K, ep, p->b_static, st, sc);
+      break;
+    }
+    case SATB_EPI_HEAD_NORM16: {
+      SATB_REQUIRE(!p->cos_tab || (p->sin_tab && p->seq_len >= 1), "gemm probe: rotary needs sin_tab and seq_len");
+      typedef EpiHeadNorm16<false> E;
+      const E::Params ep{p->out, p->ld, p->norm_cols, p->rope_cols, p->seq_len, p->cos_tab, p->sin_tab};
+      if (bn == 128) return probe_run<E, 128, false, true>(a8, w8, M, N, K, ep, p->b_static, st, sc);
+      break;
+    }
+    case SATB_EPI_QKV_ROPE: {
+      SATB_REQUIRE(p->head_dim >= 32 && p->head_dim % 32 == 0 && p->nf % 4 == 0 && p->nf >= 4 && 2 * p->nf <= p->head_dim,
+                   "gemm probe: head_dim must be a multiple of 32 and nf a multiple of 4 with 2 nf <= head_dim");
+      SATB_REQUIRE(!p->cos_tab || (p->sin_tab && p->seq_len >= 1), "gemm probe: rotary needs sin_tab and seq_len");
+      if (bn == 256) {
+        typedef EpiQkvRope<false> E;
+        const E::Params ep{p->out, p->ld, p->rope_cols, p->seq_len, p->head_dim, p->nf, p->cos_tab, p->sin_tab};
+        return probe_run<E, 256, false, true>(a8, w8, M, N, K, ep, p->b_static, st, sc);
+      }
+      break;
+    }
+    case SATB_EPI_SWIGLU: {
+      if (bn == 256) {
+        typedef EpiSwiglu<false> E;
+        return probe_run<E, 256, false, true>(a8, w8, M, N, K, E::Params{p->out, p->ld, p->bias}, p->b_static, st, sc);
+      }
+      break;
+    }
+    default:
+      break;
+  }
+  set_last_error("gemm probe fp8: no such instance (epi " + std::to_string(p->epi) + ", BN " + std::to_string(bn) +
+                 "); the forward's FP8 instances are qkv_rope and swiglu BN 256, store16 BN 128 / 256 and head_norm16 BN 128");
+  return -1;
 }
 
 }  // extern "C"

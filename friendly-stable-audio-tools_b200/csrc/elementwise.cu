@@ -1,6 +1,8 @@
 // Bandwidth-bound kernels of the DiT / Oobleck path: LayerNorm, SnakeBeta, layout
 // changes around the transformer, timestep features, tiny conditioning MLPs, CFG.
 // All fp32 math; 128-bit global accesses where the layout allows.
+#include <cuda_fp8.h>
+
 #include "common.cuh"
 #include "kernels.h"
 #include "ptx.cuh"
@@ -98,6 +100,137 @@ __global__ void __launch_bounds__(128, NV <= 8 ? 8 : (NV <= 12 ? 7 : 5)) layerno
       }
       o2[idx] = make_uint2(Op16<BF16>::pack(y.x, y.y), Op16<BF16>::pack(y.z, y.w));
     }
+  }
+}
+
+// ------------------------------------------------------- FP8 (e4m3) operands with power-of-two row scales
+// s = 2^e, e the smallest integer with amax <= 448 * 2^e (448: the largest finite e4m3), s = 1 for an all-zero row;
+// q = e4m3_rn(x * 2^-e).  With 448 = 1.75 * 2^8 and amax = m * 2^E, m in [1, 2): e = E - 8 if m <= 1.75, else E - 7.
+// e is kept >= -126 so that s and 2^-e are normal fp32 numbers (only rows with amax < 2^-117 are affected: their
+// values fall into the e4m3 subnormals).  Integer arithmetic on the bits: exact, whatever the fast-math flags.
+__device__ __forceinline__ int fp8_row_exp(float amax) {
+  if (!(amax > 0.f)) return 0;
+  const uint32_t b = __float_as_uint(amax);
+  const int E = static_cast<int>(b >> 23) - 127;
+  const int e = (b & 0x7FFFFFu) <= 0x600000u ? E - 8 : E - 7;
+  return e < -126 ? -126 : e;
+}
+__device__ __forceinline__ float pow2f(int e) { return __uint_as_float(static_cast<uint32_t>(e + 127) << 23); }
+// four values -> four e4m3 bytes (round to nearest even), the first value in the lowest byte
+__device__ __forceinline__ uint32_t e4m3x4(float a, float b, float c, float d) {
+  const uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(a, b), __NV_SATFINITE, __NV_E4M3);
+  const uint32_t hi = __nv_cvt_float2_to_fp8x2(make_float2(c, d), __NV_SATFINITE, __NV_E4M3);
+  return lo | (hi << 16);
+}
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+// layernorm_kernel with an e4m3 output: the same fp32 LayerNorm (and adaLN modulation) of the row held in registers,
+// then its absolute maximum, the row scale (written to row_scale[row]) and the e4m3 row.  A separate kernel, so that
+// the 16-bit one stays as it is.
+template <int NV>
+__global__ void __launch_bounds__(128, NV <= 8 ? 8 : (NV <= 12 ? 7 : 5)) layernorm_fp8_kernel(
+    const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
+    uint8_t* __restrict__ out, float* __restrict__ row_scale, int rows, int D, const float* __restrict__ scale,
+    const float* __restrict__ shift, int64_t mod_stride, int rows_per_item, int n_items) {
+  extern __shared__ float4 ln_gb[];   // [D / 4] gamma, then [D / 4] beta (if any)
+  const int row = blockIdx.x * 4 + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  const int nv = D >> 7;
+  pdl_launch_dependents();
+  for (int i = threadIdx.x; i < (D >> 2); i += blockDim.x) {
+    ln_gb[i] = __ldg(reinterpret_cast<const float4*>(gamma) + i);
+    if (beta) ln_gb[(D >> 2) + i] = __ldg(reinterpret_cast<const float4*>(beta) + i);
+  }
+  __syncthreads();
+  pdl_wait();
+  if (row >= rows) return;
+  const float4* xr = reinterpret_cast<const float4*>(x + static_cast<size_t>(row) * D);
+  float4 v[NV];
+  float sum = 0.f;
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    if (i < nv) {
+      v[i] = xr[lane + 32 * i];
+      sum += (v[i].x + v[i].y) + (v[i].z + v[i].w);
+    }
+  }
+  const float mean = warp_sum(sum) / static_cast<float>(D);
+  float sq = 0.f;
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    if (i < nv) {
+      const float a = v[i].x - mean, b = v[i].y - mean, c = v[i].z - mean, d = v[i].w - mean;
+      sq += (a * a + b * b) + (c * c + d * d);
+    }
+  }
+  const float rstd = rsqrtf(warp_sum(sq) / static_cast<float>(D) + 1e-5f);
+  const float4* b4 = beta ? ln_gb + (D >> 2) : nullptr;
+  const float4* sc4 = nullptr;
+  const float4* sh4 = nullptr;
+  if (scale) {
+    const int item = (row / rows_per_item) % n_items;
+    sc4 = reinterpret_cast<const float4*>(scale + item * mod_stride);
+    sh4 = reinterpret_cast<const float4*>(shift + item * mod_stride);
+  }
+  float amax = 0.f;
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    if (i < nv) {
+      const int idx = lane + 32 * i;
+      const float4 g = ln_gb[idx];
+      float4 y;
+      y.x = (v[i].x - mean) * rstd * g.x;
+      y.y = (v[i].y - mean) * rstd * g.y;
+      y.z = (v[i].z - mean) * rstd * g.z;
+      y.w = (v[i].w - mean) * rstd * g.w;
+      if (b4) {
+        const float4 b = b4[idx];
+        y.x += b.x; y.y += b.y; y.z += b.z; y.w += b.w;
+      }
+      if (sc4) {
+        const float4 s = __ldg(sc4 + idx), t = __ldg(sh4 + idx);
+        y.x = y.x * (1.f + s.x) + t.x;
+        y.y = y.y * (1.f + s.y) + t.y;
+        y.z = y.z * (1.f + s.z) + t.z;
+        y.w = y.w * (1.f + s.w) + t.w;
+      }
+      v[i] = y;
+      amax = fmaxf(amax, fmaxf(fmaxf(fabsf(y.x), fabsf(y.y)), fmaxf(fabsf(y.z), fabsf(y.w))));
+    }
+  }
+  const int e = fp8_row_exp(warp_max(amax));
+  const float inv = pow2f(-e);
+  if (lane == 0) row_scale[row] = pow2f(e);
+  uint32_t* o4 = reinterpret_cast<uint32_t*>(out + static_cast<size_t>(row) * D);
+#pragma unroll
+  for (int i = 0; i < NV; ++i)
+    if (i < nv) o4[lane + 32 * i] = e4m3x4(v[i].x * inv, v[i].y * inv, v[i].z * inv, v[i].w * inv);
+}
+
+// Weight rows -> e4m3 rows with their power-of-two scales (same rule), dst row r = src row perm[r]; one warp per row.
+__global__ void __launch_bounds__(128) quant_rows_fp8_kernel(const float* __restrict__ src, uint8_t* __restrict__ dst,
+                                                             float* __restrict__ row_scale, const int* __restrict__ perm,
+                                                             int rows, int cols) {
+  const int r = blockIdx.x * 4 + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (r >= rows) return;
+  const float4* s4 = reinterpret_cast<const float4*>(src + static_cast<size_t>(perm ? perm[r] : r) * cols);
+  float amax = 0.f;
+  for (int i = lane; i < cols / 4; i += 32) {
+    const float4 w = s4[i];
+    amax = fmaxf(amax, fmaxf(fmaxf(fabsf(w.x), fabsf(w.y)), fmaxf(fabsf(w.z), fabsf(w.w))));
+  }
+  const int e = fp8_row_exp(warp_max(amax));
+  const float inv = pow2f(-e);
+  if (lane == 0) row_scale[r] = pow2f(e);
+  uint32_t* d4 = reinterpret_cast<uint32_t*>(dst + static_cast<size_t>(r) * cols);
+  for (int i = lane; i < cols / 4; i += 32) {
+    const float4 w = s4[i];
+    d4[i] = e4m3x4(w.x * inv, w.y * inv, w.z * inv, w.w * inv);
   }
 }
 
@@ -374,6 +507,38 @@ int launch_layernorm(const float* x, const float* gamma, const float* beta, void
          : nv <= 12 ? go(layernorm_kernel<false, 12>) : go(layernorm_kernel<false, 16>);
   SATB_PROPAGATE(rc);
   count_launch();
+  return 0;
+}
+
+int launch_layernorm_fp8(const float* x, const float* gamma, const float* beta, void* out8, float* row_scale, int rows,
+                         int D, const float* scale, const float* shift, int64_t mod_stride, int rows_per_item,
+                         int n_items, cudaStream_t stream) {
+  SATB_REQUIRE(D % 128 == 0 && D <= kLnMaxVec * 128, "LayerNorm width must be a multiple of 128 and <= 2048");
+  if (rows <= 0) return 0;
+  const int grid = ceil_div(rows, 4);
+  const int items = n_items > 0 ? n_items : 1;
+  const int nv = D >> 7;
+  auto go = [&](auto kern) -> int {
+    SATB_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(128), static_cast<size_t>(D) * 8, stream, x, gamma, beta,
+                               static_cast<uint8_t*>(out8), row_scale, rows, D, scale, shift, mod_stride, rows_per_item,
+                               items));
+    return 0;
+  };
+  SATB_PROPAGATE(nv <= 4 ? go(layernorm_fp8_kernel<4>) : nv <= 8 ? go(layernorm_fp8_kernel<8>)
+                 : nv <= 12 ? go(layernorm_fp8_kernel<12>) : go(layernorm_fp8_kernel<16>));
+  count_launch();
+  return 0;
+}
+
+int launch_quant_rows_fp8(const float* src, void* dst, float* row_scale, const int* perm, int rows, int cols,
+                          cudaStream_t stream) {
+  SATB_REQUIRE(cols % 4 == 0 && (reinterpret_cast<uintptr_t>(src) & 15) == 0,
+               "FP8 row quantisation: cols must be a multiple of 4 and src 16-byte aligned");
+  if (rows <= 0) return 0;
+  quant_rows_fp8_kernel<<<ceil_div(rows, 4), 128, 0, stream>>>(src, static_cast<uint8_t*>(dst), row_scale, perm, rows,
+                                                                cols);
+  count_launch();
+  SATB_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
 

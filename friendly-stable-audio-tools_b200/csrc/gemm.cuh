@@ -150,10 +150,23 @@ __device__ __forceinline__ void gemm_tile_epilogue(const float (&acc)[BN / 2], f
     }
   }
 }
-template <class Epi, int BN, bool BF16>
+// FP8 operand mode (FP8 = true): A and B hold e4m3 bytes, one power-of-two scale per A row and per B row.  A k-block
+// is then 128 elements (the same 128 B per row, so the ring, its boxes and its barriers are unchanged) and takes four
+// m64nBNk32 e4m3 MMAs; the accumulator is dequantised, acc *= a_scale[row] * w_scale[col], before the epilogue runs
+// (exact: a product of powers of two).  K must be a multiple of 128.  Unused by the 16-bit instances.
+struct Fp8Scales {
+  const float* a = nullptr;   // [rows of A]
+  const float* w = nullptr;   // [rows of B] = [N]
+};
+constexpr int kBlockKFp8 = 128;   // 128 x 8-bit = 128 B
+
+template <class Epi, int BN, bool BF16, bool FP8 = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                  const __grid_constant__ CUtensorMap tmA2, const GemmShape s, const typename Epi::Params ep) {
+                  const __grid_constant__ CUtensorMap tmA2, const GemmShape s, const typename Epi::Params ep,
+                  const Fp8Scales sc) {
+  static_assert(!(FP8 && BF16), "the FP8 mode keeps fp16 as its 16-bit type");
+  constexpr int kKElems = FP8 ? kBlockKFp8 : kBlockK;   // elements of one k-block
   using Cfg = GemmCfg<BN, kStagedCols<Epi>, Epi::kStageBytes>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -170,7 +183,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int n_tiles = (s.N + BN - 1) / BN;
   const int tiles_per_n = m_tiles * s.batches;
   const int total_tiles = tiles_per_n * n_tiles;
-  const int kb_per_tap = (s.K + kBlockK - 1) / kBlockK;
+  const int kb_per_tap = (s.K + kKElems - 1) / kKElems;
   const int kb_per_part = kb_per_tap * s.n_taps;
   const int num_kb = kb_per_part * s.n_parts;
 
@@ -201,7 +214,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           const int pidx = kb / kb_per_part, kbp = kb - pidx * kb_per_part;
           const int part = split_part(pidx, s.n_parts);
           const int tap = kbp / kb_per_tap;
-          const int k0 = (kbp - tap * kb_per_tap) * kBlockK;
+          const int k0 = (kbp - tap * kb_per_tap) * kKElems;
           mbar_expect_tx(&full_bar[kb], Cfg::kStage);
           tma_load_2d(smem + kb * Cfg::kStage + Cfg::kStageA, &tmB, &full_bar[kb], k0,
                       tap * s.b_tap_rows + n0 + (part == 2 ? s.b_part_rows : 0));
@@ -220,7 +233,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           const int pidx = kb / kb_per_part, kbp = kb - pidx * kb_per_part;
           const int part = split_part(pidx, s.n_parts);
           const int tap = kbp / kb_per_tap;
-          const int k0 = (kbp - tap * kb_per_tap) * kBlockK;
+          const int k0 = (kbp - tap * kb_per_tap) * kKElems;
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * Cfg::kStage;
           uint8_t* sb = sa + Cfg::kStageA;
@@ -269,9 +282,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const uint32_t b_addr = smem_u32(smem + stage * Cfg::kStage) + Cfg::kStageA;
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < kBlockK / kWgmmaK; ++k)
-          wgmma_ss<BN, BF16>(acc, make_desc_kmajor_sw128(a_addr + k * kWgmmaK * 2),
-                             make_desc_kmajor_sw128(b_addr + k * kWgmmaK * 2), (kb | k) != 0 ? 1u : 0u);
+        for (int k = 0; k < kBlockK / kWgmmaK; ++k) {   // 4 x 32 B of every row: k16 (16-bit) or k32 (e4m3) steps
+          if constexpr (FP8)
+            wgmma_ss_e4m3<BN>(acc, make_desc_kmajor_sw128(a_addr + k * kWgmmaK * 2),
+                              make_desc_kmajor_sw128(b_addr + k * kWgmmaK * 2), (kb | k) != 0 ? 1u : 0u);
+          else
+            wgmma_ss<BN, BF16>(acc, make_desc_kmajor_sw128(a_addr + k * kWgmmaK * 2),
+                               make_desc_kmajor_sw128(b_addr + k * kWgmmaK * 2), (kb | k) != 0 ? 1u : 0u);
+        }
         wgmma_commit();
         wgmma_wait<1>(acc);
         if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
@@ -283,6 +301,23 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       }
       wgmma_wait<0>(acc);
       if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+      if constexpr (FP8) {
+        // dequantise the fragment (ptx.cuh wgmma_ss layout): rows r0, r0 + 8, column pairs 8 j + fc, + 1
+        const int r0 = m0 + 64 * cw + 16 * (warp & 3) + (lane >> 2);
+        const int fc = 2 * (lane & 3);
+        const float* sa_row = sc.a + static_cast<size_t>(batch) * s.L;
+        const float sa0 = r0 < s.L ? __ldg(sa_row + r0) : 0.f;
+        const float sa1 = r0 + 8 < s.L ? __ldg(sa_row + r0 + 8) : 0.f;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int col = n0 + 8 * j + fc;
+          const float2 sw = col < s.N ? __ldg(reinterpret_cast<const float2*>(sc.w + col)) : make_float2(0.f, 0.f);
+          acc[4 * j] *= sa0 * sw.x;
+          acc[4 * j + 1] *= sa0 * sw.y;
+          acc[4 * j + 2] *= sa1 * sw.x;
+          acc[4 * j + 3] *= sa1 * sw.y;
+        }
+      }
 
       if constexpr (EpiFragment<Epi>::value)
         Epi::template apply_fragment<BN>(ep, acc, s.L, s.N, m0 + 64 * cw + 16 * (warp & 3) + (lane >> 2), n0, batch, lane);
@@ -922,15 +957,20 @@ struct EpiStoreNCL {
 };
 
 // ------------------------------------------------------------------ host side
+// elem_bytes: 2 (16-bit operands) or 1 (e4m3); the box is 128 B of every row either way.
 int make_tmap_a(CUtensorMap* m, const void* ptr, int K, int L, int batches, int64_t row_stride_elems,
-                int64_t batch_stride_elems, int stride = 1, int box_rows = kBlockM);
-int make_tmap_b(CUtensorMap* m, const void* ptr, int K, int rows, int64_t row_stride_elems, int box_rows);
+                int64_t batch_stride_elems, int stride = 1, int box_rows = kBlockM, int elem_bytes = 2);
+int make_tmap_b(CUtensorMap* m, const void* ptr, int K, int rows, int64_t row_stride_elems, int box_rows,
+                int elem_bytes = 2);
 
-template <class Epi, int BN, bool BF16>
+template <class Epi, int BN, bool BF16, bool FP8 = false>
 int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape& s, const typename Epi::Params& ep,
-                cudaStream_t stream, const CUtensorMap* tmA2 = nullptr) {
+                cudaStream_t stream, const CUtensorMap* tmA2 = nullptr, const Fp8Scales& sc = Fp8Scales{}) {
   using Cfg = GemmCfg<BN, kStagedCols<Epi>, Epi::kStageBytes>;
-  auto kern = gemm_wgmma_kernel<Epi, BN, BF16>;
+  auto kern = gemm_wgmma_kernel<Epi, BN, BF16, FP8>;
+  if (FP8)
+    SATB_REQUIRE(s.K % kBlockKFp8 == 0 && s.n_taps == 1 && s.n_parts == 1 && s.stride == 1 && sc.a && sc.w,
+                 "FP8 GEMM: K must be a multiple of 128, one tap, one part, and both scale vectors given");
   static PerDeviceOnce attr;
   if (attr.first()) SATB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
   const int m_tiles = ceil_div(s.L, kBlockM), n_tiles = ceil_div(s.N, BN);
@@ -939,7 +979,8 @@ int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape&
   int grid = device_sm_count();
   if (grid > total) grid = total;
   SATB_REQUIRE(s.n_parts == 1 || tmA2 != nullptr, "split-operand GEMM needs the second A tensor map");
-  SATB_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tmA, tmB, tmA2 ? *tmA2 : tmA, s, ep));
+  SATB_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tmA, tmB, tmA2 ? *tmA2 : tmA, s, ep,
+                             sc));
   count_launch();
   return 0;
 }

@@ -20,6 +20,14 @@ int launch_attention_tc(const void* q, const void* k, const void* v, void* o, in
 int launch_layernorm(const float* x, const float* gamma, const float* beta, void* out16, int rows, int D,
                      const float* scale, const float* shift, int64_t mod_stride, int rows_per_item, int n_items,
                      bool bf16, cudaStream_t stream);
+// The same LayerNorm with an e4m3 output and one power-of-two scale per row (elementwise.cu, fp8_row_exp):
+// out8[row, :] = e4m3(y / row_scale[row]).
+int launch_layernorm_fp8(const float* x, const float* gamma, const float* beta, void* out8, float* row_scale, int rows,
+                         int D, const float* scale, const float* shift, int64_t mod_stride, int rows_per_item,
+                         int n_items, cudaStream_t stream);
+// Weight matrix -> e4m3 rows with power-of-two row scales: dst[r, :] = e4m3(src[perm ? perm[r] : r, :] / row_scale[r]).
+int launch_quant_rows_fp8(const float* src, void* dst, float* row_scale, const int* perm, int rows, int cols,
+                          cudaStream_t stream);
 // Fused VDenoiser scaling + multistep sampler update + noise (see elementwise.cu).
 int launch_sampler_update(const float* x, const float* v, const float* d1, const float* d2, const float* nz, float* den,
                           float* x_next, float* x_in, long long n, float c_skip, float c_out, float A, float B, float C,

@@ -44,23 +44,25 @@ static EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// A operand: 16-bit, dims (K, phase, rows, batches) with position = row*stride + phase
-// (stride 1 for everything but strided convolutions), box (64, 1, 128, 1), 128B swizzle,
+// A operand: 16-bit (elem_bytes 2) or e4m3 (elem_bytes 1), dims (K, phase, rows, batches) with position =
+// row*stride + phase (stride 1 for everything but strided convolutions), box (128 B of K, 1, 128, 1), 128B swizzle,
 // zero OOB fill.  L = number of rows (positions / stride).
 int make_tmap_a(CUtensorMap* m, const void* ptr, int K, int L, int batches, int64_t row_stride_elems,
-                int64_t batch_stride_elems, int stride, int box_rows) {
+                int64_t batch_stride_elems, int stride, int box_rows, int elem_bytes) {
   EncodeTiledFn fn = get_encode_fn();
   SATB_REQUIRE(fn != nullptr, "cuTensorMapEncodeTiled entry point unavailable");
   SATB_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & 15) == 0, "TMA base must be 16B aligned");
-  SATB_REQUIRE((row_stride_elems * 2) % 16 == 0 && (batch_stride_elems * 2) % 16 == 0, "TMA strides must be 16B multiples");
+  SATB_REQUIRE(elem_bytes == 1 || elem_bytes == 2, "TMA element size must be 1 or 2 bytes");
+  const int eb = elem_bytes;
+  SATB_REQUIRE((row_stride_elems * eb) % 16 == 0 && (batch_stride_elems * eb) % 16 == 0, "TMA strides must be 16B multiples");
   cuuint64_t dims[4] = {static_cast<cuuint64_t>(K), static_cast<cuuint64_t>(stride), static_cast<cuuint64_t>(L),
                         static_cast<cuuint64_t>(batches)};
-  cuuint64_t strides[3] = {static_cast<cuuint64_t>(row_stride_elems) * 2,
-                           static_cast<cuuint64_t>(row_stride_elems) * 2 * stride,
-                           static_cast<cuuint64_t>(batch_stride_elems) * 2};
-  cuuint32_t box[4] = {static_cast<cuuint32_t>(kBlockK), 1, static_cast<cuuint32_t>(box_rows), 1};
+  cuuint64_t strides[3] = {static_cast<cuuint64_t>(row_stride_elems) * eb,
+                           static_cast<cuuint64_t>(row_stride_elems) * eb * stride,
+                           static_cast<cuuint64_t>(batch_stride_elems) * eb};
+  cuuint32_t box[4] = {static_cast<cuuint32_t>(kBlockK * 2 / eb), 1, static_cast<cuuint32_t>(box_rows), 1};
   cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_UINT16, 4, const_cast<void*>(ptr), dims, strides, box, estr,
+  CUresult r = fn(m, eb == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_UINT16, 4, const_cast<void*>(ptr), dims, strides, box, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -72,17 +74,20 @@ int make_tmap_a(CUtensorMap* m, const void* ptr, int K, int L, int batches, int6
   return 0;
 }
 
-// B operand (weights): 16-bit, dims (K, rows), box (64, box_rows), 128B swizzle.
-int make_tmap_b(CUtensorMap* m, const void* ptr, int K, int rows, int64_t row_stride_elems, int box_rows) {
+// B operand (weights): 16-bit or e4m3 (elem_bytes 1), dims (K, rows), box (128 B of K, box_rows), 128B swizzle.
+int make_tmap_b(CUtensorMap* m, const void* ptr, int K, int rows, int64_t row_stride_elems, int box_rows,
+                int elem_bytes) {
   EncodeTiledFn fn = get_encode_fn();
   SATB_REQUIRE(fn != nullptr, "cuTensorMapEncodeTiled entry point unavailable");
   SATB_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & 15) == 0, "TMA base must be 16B aligned");
-  SATB_REQUIRE((row_stride_elems * 2) % 16 == 0, "TMA strides must be 16B multiples");
+  SATB_REQUIRE(elem_bytes == 1 || elem_bytes == 2, "TMA element size must be 1 or 2 bytes");
+  const int eb = elem_bytes;
+  SATB_REQUIRE((row_stride_elems * eb) % 16 == 0, "TMA strides must be 16B multiples");
   cuuint64_t dims[2] = {static_cast<cuuint64_t>(K), static_cast<cuuint64_t>(rows)};
-  cuuint64_t strides[1] = {static_cast<cuuint64_t>(row_stride_elems) * 2};
-  cuuint32_t box[2] = {static_cast<cuuint32_t>(kBlockK), static_cast<cuuint32_t>(box_rows)};
+  cuuint64_t strides[1] = {static_cast<cuuint64_t>(row_stride_elems) * eb};
+  cuuint32_t box[2] = {static_cast<cuuint32_t>(kBlockK * 2 / eb), static_cast<cuuint32_t>(box_rows)};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_UINT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+  CUresult r = fn(m, eb == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_UINT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {

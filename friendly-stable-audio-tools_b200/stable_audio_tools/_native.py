@@ -83,8 +83,10 @@ SIGNATURES = {
     "satb_snake_beta": (_I, [_VP, _VP, _VP, _VP, _I, _I, _LL, _I, _VP]),
     "satb_sampler_update": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _LL] + [_F] * 8 + [_VP]),
     "satb_layernorm": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _VP]),
+    "satb_layernorm_fp8": (_I, [_VP, _VP, _VP, _VP, _VP, _LL, _I, _I, _VP, _VP, _I, _I, _VP]),
     "satb_linear_f32out": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _VP]),
     "satb_gemm_probe": (_I, [_VP, _VP, _I, _I, _I, ctypes.POINTER(SatbGemmProbe), _VP]),
+    "satb_gemm_probe_fp8": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, ctypes.POINTER(SatbGemmProbe), _VP]),
     "satb_attention": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP]),
     "satb_attention_hd": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _VP]),
     "satb_oobleck_create": (_I, [ctypes.POINTER(SatbOobleckConfig), ctypes.POINTER(_VP)]),

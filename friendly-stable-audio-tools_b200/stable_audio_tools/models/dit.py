@@ -24,6 +24,12 @@ from .. import _native
 from .blocks import FourierFeatures
 from .transformer import SUPPORTED_HEAD_DIMS, ContinuousTransformer, check_head_dim
 
+# operand_dtype -> SatbDitConfig.operand_dtype.  "fp16" (default) and "bf16": 16-bit operands for every tensor-core
+# contraction.  "fp8": e4m3 operands with power-of-two row scales for the self-attention QKV, cross-attention q and
+# feed-forward input GEMMs (the three Linear layers fed by a LayerNorm), fp16 everywhere else; a precision choice with
+# its own tolerance (DESIGN.md section 5), not a second path to the fp16 result.
+OPERAND_DTYPES = {"fp16": 0, "bf16": 1, "fp8": 2}
+
 
 class DiffusionTransformer(nn.Module):
     def __init__(self,
@@ -58,6 +64,8 @@ class DiffusionTransformer(nn.Module):
             raise ValueError("patch_size must be >= 1")
         if global_cond_type not in ("prepend", "adaLN"):
             raise ValueError(f"unknown global_cond_type {global_cond_type}")
+        if operand_dtype not in OPERAND_DTYPES:
+            raise ValueError(f"operand_dtype must be one of {', '.join(OPERAND_DTYPES)}, got {operand_dtype!r}")
         self.patch_size = patch_size
         self.cond_token_dim = cond_token_dim
         self.input_concat_dim = input_concat_dim
@@ -134,20 +142,25 @@ class DiffusionTransformer(nn.Module):
             except Exception:
                 pass
 
+    def native_config(self):
+        """The SatbDitConfig this module creates its native handle with.
+
+        patch_size p > 1 (dit.py:206-207,221-222): tokens are groups of p positions with features (c p).  The native
+        model simply sees io_channels * p channels and L / p positions; forward() does the two rearranges, and the 1x1
+        pre/post convs (which act per position on the un-patched signal) are handed over as kron(W, I_p) so that the
+        native fold into project_in/out stays generic."""
+        return _native.SatbDitConfig(
+            io_channels=self.io_channels * self.patch_size, embed_dim=self.embed_dim, depth=self.depth, num_heads=self.num_heads,
+            cond_token_dim=self.cond_token_dim, global_cond_dim=self.global_cond_dim,
+            project_cond_tokens=int(self.project_cond_tokens), project_global_cond=int(self.project_global_cond),
+            global_cond_type=1 if self.global_cond_type == "adaLN" else 0, patch_size=1,
+            operand_dtype=OPERAND_DTYPES[self.operand_dtype], qk_norm=int(self.qk_norm),
+            input_concat_dim=self.input_concat_dim * self.patch_size, prepend_cond_dim=self.prepend_cond_dim)
+
     def _handle(self, device):
         lib = _native.lib()
         if self.__dict__["_h"] is None:
-            # patch_size p > 1 (dit.py:206-207,221-222): tokens are groups of p positions with features (c p).
-            # The native model simply sees io_channels * p channels and L / p positions; forward() does the
-            # two rearranges, and the 1x1 pre/post convs (which act per position on the un-patched signal)
-            # are handed over as kron(W, I_p) so that the native fold into project_in/out stays generic.
-            cfg = _native.SatbDitConfig(
-                io_channels=self.io_channels * self.patch_size, embed_dim=self.embed_dim, depth=self.depth, num_heads=self.num_heads,
-                cond_token_dim=self.cond_token_dim, global_cond_dim=self.global_cond_dim,
-                project_cond_tokens=int(self.project_cond_tokens), project_global_cond=int(self.project_global_cond),
-                global_cond_type=1 if self.global_cond_type == "adaLN" else 0, patch_size=1,
-                operand_dtype=1 if self.operand_dtype == "bf16" else 0, qk_norm=int(self.qk_norm),
-                input_concat_dim=self.input_concat_dim * self.patch_size, prepend_cond_dim=self.prepend_cond_dim)
+            cfg = self.native_config()
             h = ctypes.c_void_p()
             _native.check(lib.satb_dit_create(ctypes.byref(cfg), ctypes.byref(h)))
             self.__dict__["_h"] = h

@@ -38,7 +38,9 @@ typedef struct SatbDitConfig {
   int project_global_cond;  /* dit.py:65 */
   int global_cond_type;     /* 0 = "prepend", 1 = "adaLN" (dit.py:29,185-204) */
   int patch_size;           /* must be 1 */
-  int operand_dtype;        /* 0 = fp16 (the reference's autocast dtype), 1 = bf16 */
+  int operand_dtype;        /* 0 = fp16 (the reference's autocast dtype), 1 = bf16, 2 = fp8: e4m3 operands with
+                               power-of-two row scales for the self-attention QKV, cross-attention q and feed-forward
+                               input GEMMs, fp16 everywhere else; any other value is refused */
   int qk_norm;              /* 1 = L2-normalise q and k per head before RoPE / attention
                                (attn_kwargs.qk_norm, models/transformer.py:298,433-436) */
   int input_concat_dim;     /* extra input channels concatenated to x before the 1x1 pre-conv (dit.py:38,163-168); the
@@ -112,6 +114,13 @@ int satb_snake_beta(const float* x, const float* alpha, const float* beta, float
 /* LayerNorm.forward (models/transformer.py:188-206) with 16-bit output (fp16/bf16 bits). */
 int satb_layernorm(const float* x, const float* gamma, const float* beta, void* out16, int rows, int D, int bf16,
                    void* stream);
+/* Test entry point: the LayerNorm of the FP8 mode, out8 [rows, D] e4m3 and row_scale [rows] fp32 with
+ * out8[r, :] = e4m3_rn(y[r, :] / row_scale[r]), row_scale[r] = 2^e, e the smallest integer (>= -126) with
+ * max |y[r, :]| <= 448 * 2^e (1 for an all-zero row).  y = LayerNorm(x) (* (1 + mod_scale) + mod_shift when mod_scale is
+ * given: adaLN, item = (r / rows_per_item) % n_items, row stride mod_stride; else mod_* are ignored). */
+int satb_layernorm_fp8(const float* x, const float* gamma, const float* beta, const float* mod_scale,
+                       const float* mod_shift, long long mod_stride, int rows_per_item, int n_items, void* out8,
+                       float* row_scale, int rows, int D, void* stream);
 /* C[M, N] (fp32) = A[M, K] * W[N, K]^T, A and W 16-bit (fp16/bf16 bits) row-major: nn.Linear
  * without bias (F.linear call sites transformer.py:422-430,548). */
 int satb_linear_f32out(const void* a16, const void* w16, float* c, int M, int N, int K, int bf16, void* stream);
@@ -142,6 +151,12 @@ typedef struct SatbGemmProbe {
   int norm_cols;                    /* head_norm16 */
 } SatbGemmProbe;
 int satb_gemm_probe(const void* a16, const void* w16, int M, int N, int K, const SatbGemmProbe* p, void* stream);
+/* Test entry point: the same through ONE of the FP8-mode instances of the DiT forward: a8 [M, K] and w8 [N, K] e4m3
+ * with one fp32 scale per row (a_scale [M], w_scale [N]); C = (a_scale[m] w_scale[n] sum_k a8[m, k] w8[n, k]) through
+ * the epilogue.  Instances: qkv_rope and swiglu BN 256, store16 BN 128 / 256, head_norm16 BN 128; bf16 must be 0
+ * (fp16 outputs) and K a multiple of 128. */
+int satb_gemm_probe_fp8(const void* a8, const void* w8, const float* a_scale, const float* w_scale, int M, int N, int K,
+                        const SatbGemmProbe* p, void* stream);
 /* One step of the v-objective k-diffusion samplers in a single pass over the latents (replaces the
  * ~20 elementwise torch kernels of K.external.VDenoiser.forward + sample_dpmpp_{2m,3m}_sde's update,
  * reference call sites inference/sampling.py:159,225-228): with v = model(x * c_in, t),
