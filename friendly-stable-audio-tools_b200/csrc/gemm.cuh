@@ -11,8 +11,8 @@
 // Structure (one persistent CTA per SM, 384 threads, 128 x BN tiles):
 //   warpgroup 0      TMA producer      one thread: global -> 128B-swizzled smem ring (mbarrier full/empty)
 //   warpgroups 1, 2  MMA + epilogue    64 rows each: wgmma 64xBNx16 from the smem ring into registers, then the
-//                                      fused epilogue (accumulator -> smem -> one row per thread -> fused op -> global,
-//                                      or, for EpiSwiglu and EpiResidual, fused op on the fragment -> global)
+//                                      fused epilogue (the DiT linears: fused op on the fragment -> global; EpiHeadNorm16
+//                                      and the convolutions: accumulator -> smem -> one row per thread -> fused op -> global)
 // The producer runs ahead into the next tile's k-blocks while the epilogue of the current one runs.
 #pragma once
 #include <type_traits>
@@ -328,71 +328,106 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 }
 
 // ------------------------------------------------------------------ epilogues
-// Every epilogue receives kCols consecutive fp32 accumulator columns of one row
-// (as raw bits in r[]) and writes them straight to global memory.
+// A staged epilogue (Epi::apply) receives kCols consecutive fp32 accumulator columns of one row (as raw bits in r[]);
+// a fragment epilogue (Epi::apply_fragment<BN>) receives the wgmma fragment of its warpgroup's 64 rows x BN columns
+// (ptx.cuh wgmma_ss): row0 is the thread's first fragment row (the second is row0 + 8), and in every 8-column group j
+// it holds columns 8 j + 2 (lane & 3), + 1 at acc[4 j], acc[4 j + 1] (row0) and acc[4 j + 2], acc[4 j + 3] (row0 + 8).
+// Both write straight to global memory.  kCols of a fragment epilogue is the column multiple N must have.
 
 __device__ __forceinline__ float silu_f(float x) { return x / (1.0f + __expf(-x)); }
 
-// out16[row, col] = act(acc + bias)   (act: 0 none, 1 SiLU)
+// Stores one fragment row's 16-bit pairs of two neighbouring 8-column groups starting at column c0: w0 holds columns
+// c0 + fc, + 1 and w1 holds c0 + 8 + fc, + 1 (fc = 2 (lane & 3)).  The lanes with fc = 0 and 2, and those with fc = 4
+// and 6, swap one word, so that the even lane stores columns c0 + fc .. + 3 and the odd one c0 + 8 + fc - 2 .. + 3 as
+// 8 bytes each: the four lanes of a row write one whole 32-byte sector per store instead of four 4-byte pieces of two
+// sectors.  Every lane of the warp must take part (the swap is a warp shuffle); `ok` only gates the store.
+__device__ __forceinline__ void store16_group_pair(uint16_t* row, int c0, uint32_t w0, uint32_t w1, int lane, bool ok) {
+  const bool odd = lane & 1;
+  const uint32_t got = __shfl_xor_sync(0xffffffffu, odd ? w0 : w1, 1);
+  const int fc = 2 * (lane & 3);
+  if (ok) *reinterpret_cast<uint2*>(row + c0 + (odd ? 6 + fc : fc)) = odd ? make_uint2(got, w1) : make_uint2(w0, got);
+}
+
+// out16[row, col] = act(acc + bias)   (act: 0 none, 1 SiLU); stored by store16_group_pair, two 8-column groups at a
+// time (N is a multiple of 32, so a pair of groups is either wholly inside N or wholly past it).
 template <bool BF16>
 struct EpiStore16 {
   static constexpr int kCols = 32;
   static constexpr int kStageBytes = 0;
+  static constexpr bool kFragment = true;
   struct Params {
     void* out;
     int ld;
     const float* bias;  // may be null
     int act;
   };
-  __device__ static __forceinline__ void apply(const Params& p, const EpiCtx& c, const uint32_t (&r)[32]) {
-    if (!c.valid) return;
-    float v[32];
+  template <int BN>
+  __device__ static __forceinline__ void apply_fragment(const Params& p, const float (&acc)[BN / 2], int L, int N,
+                                                        int row0, int n0, int batch, int lane) {
+    const int fc = 2 * (lane & 3);
 #pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-    if (p.bias) {
+    for (int j = 0; j < BN / 8; j += 2) {
+      if (n0 + 8 * j >= N) break;
+      float2 b[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
+      if (p.bias) {
+        b[0] = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + 8 * j + fc));
+        b[1] = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + 8 * j + 8 + fc));
+      }
 #pragma unroll
-      for (int j = 0; j < 32; j += 4) {
-        const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + c.col0 + j));
-        v[j] += b.x; v[j + 1] += b.y; v[j + 2] += b.z; v[j + 3] += b.w;
+      for (int rr = 0; rr < 2; ++rr) {
+        const int l = row0 + 8 * rr;
+        uint32_t w[2];
+#pragma unroll
+        for (int g = 0; g < 2; ++g) {
+          float x0 = acc[4 * (j + g) + 2 * rr], x1 = acc[4 * (j + g) + 2 * rr + 1];
+          if (p.bias) {
+            x0 += b[g].x;
+            x1 += b[g].y;
+          }
+          if (p.act == 1) {
+            x0 = silu_f(x0);
+            x1 = silu_f(x1);
+          }
+          w[g] = Op16<BF16>::pack(x0, x1);
+        }
+        store16_group_pair(static_cast<uint16_t*>(p.out) + static_cast<size_t>(batch * L + l) * p.ld, n0 + 8 * j, w[0],
+                           w[1], lane, l < L);
       }
     }
-    uint32_t o[16];
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      float a = v[2 * j], b = v[2 * j + 1];
-      if (p.act == 1) {
-        a = silu_f(a);
-        b = silu_f(b);
-      }
-      o[j] = Op16<BF16>::pack(a, b);
-    }
-    uint4* dst = reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.out) + static_cast<size_t>(c.row) * p.ld + c.col0);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) dst[j] = make_uint4(o[4 * j], o[4 * j + 1], o[4 * j + 2], o[4 * j + 3]);
   }
 };
 
-// out32[row, col] = acc (+ bias)
+// out32[row, col] = acc (+ bias); each thread stores its fp32 pairs (c, c + 1).
 struct EpiStore32 {
   static constexpr int kCols = 32;
   static constexpr int kStageBytes = 0;
+  static constexpr bool kFragment = true;
   struct Params {
     float* out;
     int ld;
     const float* bias;
   };
-  __device__ static __forceinline__ void apply(const Params& p, const EpiCtx& c, const uint32_t (&r)[32]) {
-    if (!c.valid) return;
-    float4* dst = reinterpret_cast<float4*>(p.out + static_cast<size_t>(c.row) * p.ld + c.col0);
+  template <int BN>
+  __device__ static __forceinline__ void apply_fragment(const Params& p, const float (&acc)[BN / 2], int L, int N,
+                                                        int row0, int n0, int batch, int lane) {
+    const int fc = 2 * (lane & 3);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      float4 v = make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]), __uint_as_float(r[4 * j + 2]),
-                             __uint_as_float(r[4 * j + 3]));
-      if (p.bias) {
-        const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + c.col0) + j);
-        v.x += b.x; v.y += b.y; v.z += b.z; v.w += b.w;
+    for (int j = 0; j < BN / 8; ++j) {
+      if (n0 + 8 * j >= N) break;
+      const int col = n0 + 8 * j + fc;
+      float2 b = make_float2(0.f, 0.f);
+      if (p.bias) b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int l = row0 + 8 * rr;
+        if (l >= L) continue;
+        float2 v = make_float2(acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1]);
+        if (p.bias) {
+          v.x += b.x;
+          v.y += b.y;
+        }
+        *reinterpret_cast<float2*>(p.out + static_cast<size_t>(batch * L + l) * p.ld + col) = v;
       }
-      dst[j] = v;
     }
   }
 };
@@ -458,10 +493,15 @@ struct EpiResidual {
 // chunk ci = (col % head_dim) / 32 rotates its first clamp(nf - 16 ci, 0, 16) pairs with the
 // table columns 16 ci + i, and the rest of the head passes through.  q and k share the
 // permutation, so every q . k is unchanged.  Head dim 64: identity; chunk 0 rotates 16 pairs.
+// Runs on the accumulator fragment: pair (i, i + 16) of a chunk lies in the same thread, in fragment groups jj and
+// jj + 2 of the chunk (i = 8 jj + 2 (lane & 3) + e, jj < 2), so the thread rotates its own pairs of rows row0 and
+// row0 + 8 with the table entries of its own columns; the 16-bit results go straight to global memory through
+// store16_group_pair.
 template <bool BF16>
 struct EpiQkvRope {
   static constexpr int kCols = 32;
   static constexpr int kStageBytes = 0;
+  static constexpr bool kFragment = true;
   struct Params {
     void* out;
     int ld;            // 3*D
@@ -472,37 +512,69 @@ struct EpiQkvRope {
     const float* cos_tab;  // [seq_len, nf]
     const float* sin_tab;  // [seq_len, nf]
   };
-  __device__ static __forceinline__ void apply(const Params& p, const EpiCtx& c, const uint32_t (&r)[32]) {
-    if (!c.valid) return;
-    float v[32];
+  // t*cos + rotate_half(t)*sin with rotate_half = [-b, a]: a' = a c - b s, b' = b c + a s.  The contraction is spelled
+  // out (b s and b c rounded, then one fused multiply-add with a) so the bits do not depend on how the compiler would
+  // contract the plain expressions; this is the contraction the expressions a * c - b * s and b * c + a * s compile to.
+  __device__ static __forceinline__ void rotate(float& a, float& b, float c, float s) {
+    const float ra = __fmaf_rn(a, c, -__fmul_rn(b, s));
+    const float rb = __fmaf_rn(a, s, __fmul_rn(b, c));
+    a = ra;
+    b = rb;
+  }
+  template <int BN>
+  __device__ static __forceinline__ void apply_fragment(const Params& p, const float (&acc)[BN / 2], int L, int N,
+                                                        int row0, int n0, int batch, int lane) {
+    const int fc = 2 * (lane & 3);
+    // Only chunks 0 and 1 of a head rotate (nf <= 32), and every rotating chunk with the same ci uses the same table
+    // entries: (cos, sin) of columns 16 ci + 8 jj + fc, + 1 at the positions of rows row0 and row0 + 8.  They are
+    // loaded once, up front, so that the loads are in flight together instead of one round trip per group.
+    float2 tc[2][2][2], ts[2][2][2];   // [ci][jj][rr]
+    const bool tile_rot = n0 < p.rope_cols && p.cos_tab;
 #pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-    // chunk of 32 columns aligned to 32 (head_dim is a multiple of 32): its rotary pairs (i, i + 16), i < n_rot
-    const int ci = (c.col0 % p.head_dim) >> 5;
-    const int n_rot = min(max(p.nf - 16 * ci, 0), 16);   // 16 or 8 (head dim 96, chunk 1) or 0
-    if (c.col0 < p.rope_cols && n_rot > 0 && p.cos_tab) {
-      const int pos = c.row % p.seq_len;
-      const float4* ct = reinterpret_cast<const float4*>(p.cos_tab + pos * p.nf + 16 * ci);
-      const float4* st = reinterpret_cast<const float4*>(p.sin_tab + pos * p.nf + 16 * ci);
+    for (int rr = 0; rr < 2; ++rr) {
+      const int pos = (batch * L + row0 + 8 * rr) % p.seq_len;   // a row past L still has a position in the table
 #pragma unroll
-      for (int j4 = 0; j4 < 4; ++j4) {
-        if (4 * j4 >= n_rot) break;
-        const float4 cs = __ldg(ct + j4), sn = __ldg(st + j4);
-        const float cc[4] = {cs.x, cs.y, cs.z, cs.w}, ss[4] = {sn.x, sn.y, sn.z, sn.w};
+      for (int ci = 0; ci < 2; ++ci) {
 #pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const int j = j4 * 4 + u;
-          const float a = v[j], b = v[j + 16];
-          v[j] = a * cc[u] - b * ss[u];       // t*cos + rotate_half(t)*sin, rotate_half = [-b, a]
-          v[j + 16] = b * cc[u] + a * ss[u];
+        for (int jj = 0; jj < 2; ++jj) {
+          tc[ci][jj][rr] = ts[ci][jj][rr] = make_float2(0.f, 0.f);
+          if (tile_rot && 8 * jj + fc < p.nf - 16 * ci) {
+            const int t = pos * p.nf + 16 * ci + 8 * jj + fc;
+            tc[ci][jj][rr] = __ldg(reinterpret_cast<const float2*>(p.cos_tab + t));
+            ts[ci][jj][rr] = __ldg(reinterpret_cast<const float2*>(p.sin_tab + t));
+          }
         }
       }
     }
-    uint4* dst = reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.out) + static_cast<size_t>(c.row) * p.ld + c.col0);
 #pragma unroll
-    for (int j = 0; j < 4; ++j)
-      dst[j] = make_uint4(Op16<BF16>::pack(v[8 * j], v[8 * j + 1]), Op16<BF16>::pack(v[8 * j + 2], v[8 * j + 3]),
-                          Op16<BF16>::pack(v[8 * j + 4], v[8 * j + 5]), Op16<BF16>::pack(v[8 * j + 6], v[8 * j + 7]));
+    for (int ch = 0; ch < BN / 32; ++ch) {
+      const int col0 = n0 + 32 * ch;
+      if (col0 >= N) break;
+      // chunk of 32 columns aligned to 32 (head_dim is a multiple of 32): its rotary pairs (i, i + 16), i < n_rot
+      const int ci = (col0 % p.head_dim) >> 5;
+      const int n_rot = col0 < p.rope_cols && p.cos_tab ? min(max(p.nf - 16 * ci, 0), 16) : 0;   // 16, 8 or 0
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int l = row0 + 8 * rr;
+        uint32_t w[4];                              // 16-bit pairs of groups 0..3 of the chunk, this row
+#pragma unroll
+        for (int jj = 0; jj < 2; ++jj) {
+          const int i = 8 * jj + fc;               // pair index of this thread's first column in the group
+          const int ia = 4 * (4 * ch + jj) + 2 * rr, ib = ia + 8;   // groups jj and jj + 2 of the chunk
+          float a0 = acc[ia], a1 = acc[ia + 1], b0 = acc[ib], b1 = acc[ib + 1];
+          if (i < n_rot) {                         // n_rot is even, so pair i + 1 is rotated with pair i; ci is 0 or 1
+            const float2 cs = ci ? tc[1][jj][rr] : tc[0][jj][rr], sn = ci ? ts[1][jj][rr] : ts[0][jj][rr];
+            rotate(a0, b0, cs.x, sn.x);
+            rotate(a1, b1, cs.y, sn.y);
+          }
+          w[jj] = Op16<BF16>::pack(a0, a1);
+          w[jj + 2] = Op16<BF16>::pack(b0, b1);
+        }
+        uint16_t* row = static_cast<uint16_t*>(p.out) + static_cast<size_t>(batch * L + l) * p.ld;
+        store16_group_pair(row, col0, w[0], w[1], lane, l < L);
+        store16_group_pair(row, col0 + 16, w[2], w[3], lane, l < L);
+      }
+    }
   }
 };
 
@@ -574,8 +646,8 @@ struct EpiHeadNorm16 {
 // 64-column group holds 32 value columns followed by their 32 gate columns:
 //   out[row, g*32 + j] = (acc[g*64 + j] + b) * silu(acc[g*64 + 32 + j] + b')
 // Value column c and gate column c + 32 of a group sit in the same thread's accumulator fragment (8-column groups j
-// and j + 4), so the epilogue runs on the fragment: no staging through shared memory, no barrier, and each thread
-// stores its 16-bit pairs (c, c + 1) straight to global memory.
+// and j + 4), so the epilogue runs on the fragment: no staging through shared memory, no barrier, and the 16-bit
+// results go straight to global memory through store16_group_pair, two 8-column output groups at a time.
 template <bool BF16>
 struct EpiSwiglu {
   static constexpr int kCols = 64;
@@ -597,27 +669,34 @@ struct EpiSwiglu {
       const int col0 = n0 + 64 * g;
       if (col0 >= N) break;
 #pragma unroll
-      for (int jj = 0; jj < 4; ++jj) {
-        const int c = 8 * jj + fc;   // value columns c, c + 1; gate columns c + 32, c + 33
-        float2 bv = make_float2(0.f, 0.f), bg = bv;
+      for (int jp = 0; jp < 4; jp += 2) {   // output groups jp, jp + 1 of this 32-column output chunk
+        float2 bv[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)}, bg[2] = {bv[0], bv[0]};
         if (p.bias) {
-          bv = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + c));
-          bg = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + 32 + c));
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int c = 8 * (jp + h) + fc;   // value columns c, c + 1; gate columns c + 32, c + 33
+            bv[h] = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + c));
+            bg[h] = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + 32 + c));
+          }
         }
 #pragma unroll
         for (int rr = 0; rr < 2; ++rr) {
           const int l = row0 + 8 * rr;
-          if (l >= L) continue;
-          const int av = 4 * (8 * g + jj) + 2 * rr, ag = av + 16;
-          float a0 = acc[av], a1 = acc[av + 1], g0 = acc[ag], g1 = acc[ag + 1];
-          if (p.bias) {
-            a0 += bv.x;
-            a1 += bv.y;
-            g0 += bg.x;
-            g1 += bg.y;
+          uint32_t w[2];
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int av = 4 * (8 * g + jp + h) + 2 * rr, ag = av + 16;
+            float a0 = acc[av], a1 = acc[av + 1], g0 = acc[ag], g1 = acc[ag + 1];
+            if (p.bias) {
+              a0 += bv[h].x;
+              a1 += bv[h].y;
+              g0 += bg[h].x;
+              g1 += bg[h].y;
+            }
+            w[h] = Op16<BF16>::pack(a0 * silu_f(g0), a1 * silu_f(g1));
           }
-          uint16_t* dst = static_cast<uint16_t*>(p.out) + static_cast<size_t>(batch * L + l) * p.ld + (col0 >> 1) + c;
-          *reinterpret_cast<uint32_t*>(dst) = Op16<BF16>::pack(a0 * silu_f(g0), a1 * silu_f(g1));
+          store16_group_pair(static_cast<uint16_t*>(p.out) + static_cast<size_t>(batch * L + l) * p.ld,
+                             (col0 >> 1) + 8 * jp, w[0], w[1], lane, l < L);
         }
       }
     }
