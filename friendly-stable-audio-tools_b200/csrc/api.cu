@@ -73,4 +73,17 @@ int satb_attention_hd(const void* q16, const void* k16, const void* v16, void* o
                              static_cast<cudaStream_t>(stream));
 }
 
+int satb_attention_probe(const SatbAttentionProbe* p, void* stream) {
+  SATB_REQUIRE(p && p->q && p->k && p->v && p->o, "null argument");
+  SATB_REQUIRE(p->B >= 1, "attention needs at least one batch item");
+  SATB_REQUIRE(p->q_col >= 0 && p->k_col >= 0 && p->v_col >= 0 && p->ldq >= 0 && p->ldk >= 0 && p->ldv >= 0 &&
+                   p->ldo >= 0 && p->q_bs >= 0 && p->k_bs >= 0 && p->v_bs >= 0 && p->o_bs >= 0,
+               "attention column offsets and strides must not be negative");
+  SATB_REQUIRE(p->q_cols <= p->ldq && p->k_cols <= p->ldk && p->v_cols <= p->ldv,
+               "attention operand columns exceed the row pitch");
+  return launch_attention_tc(p->q, p->k, p->v, p->o, p->ldq, p->ldk, p->ldv, p->ldo, p->q_bs, p->k_bs, p->v_bs, p->o_bs,
+                             p->q_cols, p->k_cols, p->v_cols, p->q_col, p->k_col, p->v_col, p->B, p->H, p->Hkv, p->Nq,
+                             p->Nk, p->head_dim, p->bf16 != 0, static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

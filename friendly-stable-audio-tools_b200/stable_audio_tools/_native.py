@@ -52,6 +52,14 @@ class SatbGemmProbe(ctypes.Structure):
                 + [("cos_tab", _VP), ("sin_tab", _VP), ("norm_cols", _I)])
 
 
+# satb_attention_probe (tests only): the parameter block of include/satb200.h
+class SatbAttentionProbe(ctypes.Structure):
+    _fields_ = ([(n, _I) for n in ("B", "H", "Hkv", "Nq", "Nk", "head_dim", "bf16")]
+                + [(n, _VP) for n in ("q", "k", "v", "o")]
+                + [(n, _LL) for n in ("ldq", "ldk", "ldv", "ldo", "q_bs", "k_bs", "v_bs", "o_bs")]
+                + [(n, _I) for n in ("q_cols", "k_cols", "v_cols", "q_col", "k_col", "v_col")])
+
+
 # satb_oobleck_probe / satb_oobleck_weights (tests only): steps, route bits and the parameter block of include/satb200.h
 OOB_DEC_IN, OOB_DEC_UP, OOB_DEC_RES, OOB_DEC_OUT, OOB_ENC_IN, OOB_ENC_RES, OOB_ENC_DOWN, OOB_ENC_OUT = range(8)
 OOB_ROUTES = {1: "gemm", 2: "gemm_lean", 4: "fused", 8: "fused_lean", 16: "halo_ncl", 32: "gemm_ncl", 64: "cuda_core"}
@@ -89,6 +97,7 @@ SIGNATURES = {
     "satb_gemm_probe_fp8": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, ctypes.POINTER(SatbGemmProbe), _VP]),
     "satb_attention": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP]),
     "satb_attention_hd": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _VP]),
+    "satb_attention_probe": (_I, [ctypes.POINTER(SatbAttentionProbe), _VP]),
     "satb_oobleck_create": (_I, [ctypes.POINTER(SatbOobleckConfig), ctypes.POINTER(_VP)]),
     "satb_oobleck_destroy": (None, [_VP]),
     "satb_oobleck_load_weight": (_I, [_VP, ctypes.c_char_p, _VP, _LL, _VP]),

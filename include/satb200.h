@@ -174,6 +174,25 @@ int satb_attention(const void* q16, const void* k16, const void* v16, void* o16,
  * Head h uses kv head h / (H / Hkv).  head_dim 64 gives the bits of satb_attention. */
 int satb_attention_hd(const void* q16, const void* k16, const void* v16, void* o16, int B, int H, int Hkv, int Nq,
                       int Nk, int head_dim, int bf16, void* stream);
+/* Test entry point (no product path calls it): the same attention on strided operands, through the launch the DiT
+ * forward makes (the fused [rows, N, 3 H d] QKV buffer of self-attention, the [rows, Mctx, 2 Hkv d] KV buffer of
+ * cross-attention).  q / k / v / o are 16-bit [B, rows, ld*] with batch strides *_bs (elements); head h of q starts
+ * at column q_col + h d, kv head h / (H / Hkv) of k and v at k_col + (h / (H / Hkv)) d, v_col + ...; o's head h at
+ * column h d.  q_cols / k_cols / v_cols are the widths (from column 0) the operand holds: head dim 64 reads it through
+ * a tensor map that spans exactly these columns and Nq / Nk rows per item.  Pointers, strides and column offsets
+ * must be multiples of 16 bytes; strides and column offsets must not be negative. */
+typedef struct SatbAttentionProbe {
+  int B, H, Hkv, Nq, Nk, head_dim, bf16;
+  const void* q;
+  const void* k;
+  const void* v;
+  void* o;
+  long long ldq, ldk, ldv, ldo;
+  long long q_bs, k_bs, v_bs, o_bs;
+  int q_cols, k_cols, v_cols;
+  int q_col, k_col, v_col;
+} SatbAttentionProbe;
+int satb_attention_probe(const SatbAttentionProbe* p, void* stream);
 
 /* ---- Oobleck VAE: replaces OobleckDecoder / OobleckEncoder.forward
  *      (models/autoencoders.py:119-194) behind AudioAutoencoder.encode/decode (:268-343) */

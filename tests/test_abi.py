@@ -52,6 +52,35 @@ def test_create_validates_config_and_reports_errors():
     assert rc != 0 and b"channels" in lib.satb_last_error()
 
 
+def test_attention_probe_refuses_bad_layouts():
+    """satb_attention_probe validates before any CUDA call: fake 16-byte-aligned addresses, never dereferenced."""
+    from stable_audio_tools import _native
+    lib = _native.lib()
+    fake = 1 << 20
+
+    def probe(**kw):
+        # the fused QKV layout of the forward: 2 items x 33 rows x 3 x 4 heads of 64
+        p = dict(B=2, H=4, Hkv=4, Nq=33, Nk=33, head_dim=64, bf16=0, q=fake, k=fake, v=fake, o=fake + 4096,
+                 ldq=768, ldk=768, ldv=768, ldo=256, q_bs=33 * 768, k_bs=33 * 768, v_bs=33 * 768, o_bs=33 * 256,
+                 q_cols=768, k_cols=768, v_cols=768, q_col=0, k_col=256, v_col=512)
+        p.update(kw)
+        return lib.satb_attention_probe(ctypes.byref(_native.SatbAttentionProbe(**p)), None)
+
+    bad = [(dict(head_dim=48), b"head dim"), (dict(Hkv=3), b"multiple of kv heads"),
+           (dict(Nq=0), b"empty"), (dict(Nk=0), b"empty"),
+           (dict(k_col=260), b"16B aligned"), (dict(v_col=516), b"16B aligned"), (dict(q_col=4), b"16B aligned"),
+           (dict(ldk=772, ldq=772, ldv=772), b"16B aligned"), (dict(k_bs=33 * 768 + 4), b"16B aligned"),
+           (dict(ldo=260), b"16B aligned"), (dict(v_col=520), b"exceed"), (dict(q_cols=248), b"exceed"),
+           (dict(k_cols=500), b"exceed"), (dict(q=fake + 8), b"16B aligned"),
+           (dict(q_cols=800), b"row pitch"), (dict(B=0), b"batch item"), (dict(o=None), b"null"),
+           (dict(q_col=-8), b"negative"), (dict(k_col=-256), b"negative"), (dict(ldv=-768), b"negative"),
+           (dict(o_bs=-33 * 256), b"negative")]
+    for kw, msg in bad:
+        rc = probe(**kw)
+        err = lib.satb_last_error()
+        assert rc != 0 and msg in err, f"{kw}: rc {rc}, {err}"
+
+
 def test_no_cpu_fallback_in_the_product_path():
     """CPU tensors are rejected by the drop-in modules; nothing under the package imports oracle/."""
     import torch
