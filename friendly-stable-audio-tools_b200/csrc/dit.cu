@@ -113,6 +113,13 @@ struct LayerW {
   // FP8 mode: e4m3 copies of to_qkv, cross_attn.to_q and ff.0 (in place of their 16-bit ones) and their row scales
   uint8_t *w8_qkv = nullptr, *w8_q = nullptr, *w8_ff1 = nullptr;
   float *s_qkv = nullptr, *s_q = nullptr, *s_ff1 = nullptr;
+  // conformer branch (satb_dit_set_conformer): in_norm, glu.proj folded with pointwise_conv (16-bit, SwiGLU row
+  // interleave, bias interleaved alike), depthwise_conv [D][17] fp32, mid_norm, pointwise_conv_2 (16-bit)
+  float *cf_in_g = nullptr, *cf_in_b = nullptr, *cf_b1 = nullptr, *cf_dw = nullptr, *cf_mid_g = nullptr,
+        *cf_mid_b = nullptr;
+  uint16_t *cf_w1 = nullptr, *cf_w2 = nullptr;
+  // fp32 copies of pointwise_conv [D, D] and glu.proj [2D, D] until both are loaded and folded into cf_w1 (then freed)
+  float *cf_pw_src = nullptr, *cf_glu_src = nullptr;
 };
 
 }  // namespace satb
@@ -127,6 +134,8 @@ struct SatbDit {
   int Pp = 0;                 // prepend-conditioning tokens of the current conditioning
   DevBuf ws_prep;             // their embeddings [B, Pp, D] + scratch
   bool bf16, fp8, adaln, qk_norm = false;   // fp8: e4m3 operands for the QKV, cross q and FF-in GEMMs (fp16 elsewhere)
+  bool conformer = false;     // every block runs the conformer branch (satb_dit_set_conformer)
+  int* cf_perm = nullptr;     // SwiGLU row interleave of the folded [2D, D] conformer GLU weight
   int P;  // prepended tokens: 1 (the global-conditioning token; 0 in adaLN mode) + Pp
   std::vector<LayerW> layers;
   std::vector<void*> owned;   // every cudaMalloc of weight storage
@@ -197,6 +206,39 @@ static std::vector<int> qkv_head_perm(int D, int dh, int nf) {
   return perm;
 }
 
+// Row interleave of a [2 n, K] GLU projection for EpiSwiglu: every 64-row group = 32 value rows, then their 32 gate rows.
+static std::vector<int> swiglu_perm(int n) {
+  std::vector<int> perm(2 * n);
+  for (int r = 0; r < 2 * n; ++r) {
+    const int g = r / 64, w = r % 64;
+    perm[r] = w < 32 ? g * 32 + w : n + g * 32 + (w - 32);
+  }
+  return perm;
+}
+
+// Conformer: W = W_glu W_pw ([2D, D], transformer.py:579-581: pointwise_conv then glu.proj, no nonlinearity between)
+// with fp64 accumulation, rounded to fp32 and then to the 16-bit operand type in the SwiGLU row interleave; the fp32
+// sources are freed.  Runs once both are loaded.
+static int fold_conformer_glu(SatbDit* d, LayerW& L, cudaStream_t st) {
+  const int D = d->D;
+  float* fused = nullptr;
+  SATB_CHECK_CUDA(cudaMalloc(&fused, static_cast<size_t>(2) * D * D * sizeof(float)));
+  if (!L.cf_w1) {
+    const int rc = d->alloc(&L.cf_w1, static_cast<size_t>(2) * D * D);
+    if (rc) { cudaFree(fused); return rc; }
+  }
+  int rc = launch_matmul_f64(L.cf_glu_src, L.cf_pw_src, fused, 2 * D, D, D, st);
+  if (rc == 0) rc = launch_cast_rows(fused, L.cf_w1, d->cf_perm, 2 * D, D, D, D, d->bf16, st);
+  const cudaError_t e = cudaStreamSynchronize(st);
+  cudaFree(fused);
+  cudaFree(L.cf_pw_src);
+  cudaFree(L.cf_glu_src);
+  L.cf_pw_src = L.cf_glu_src = nullptr;
+  SATB_PROPAGATE(rc);
+  SATB_CHECK_CUDA(e);
+  return 0;
+}
+
 extern "C" {
 
 const char* satb_last_error(void) { return get_last_error(); }
@@ -260,9 +302,22 @@ int satb_dit_create(const SatbDitConfig* cfg, SatbDit** out) {
   return 0;
 }
 
+// Conformer blocks (transformer.py:557-591,645): call before the first satb_dit_load_weight.
+int satb_dit_set_conformer(SatbDit* d, int enable) {
+  SATB_REQUIRE(d, "null handle");
+  SATB_REQUIRE(d->loaded.empty(), "satb_dit_set_conformer must be called before the first weight is loaded");
+  SATB_REQUIRE(!enable || d->D <= kConformerMaxDim, "conformer blocks are supported up to embed_dim 1536");
+  d->conformer = enable != 0;
+  return 0;
+}
+
 void satb_dit_destroy(SatbDit* d) {
   if (!d) return;
   for (void* p : d->owned) cudaFree(p);
+  for (LayerW& L : d->layers) {
+    if (L.cf_pw_src) cudaFree(L.cf_pw_src);
+    if (L.cf_glu_src) cudaFree(L.cf_glu_src);
+  }
   d->ws_h.release(); d->ws_a16.release(); d->ws_qkv.release(); d->ws_attn.release(); d->ws_q16.release();
   d->ws_ff.release(); d->ws_ain.release(); d->ws_y.release(); d->ws_small.release(); d->ws_cond.release();
   d->ws_kv.release(); d->ws_rope.release(); d->ws_prep.release(); d->ws_a8.release(); d->ws_ascale.release();
@@ -342,11 +397,7 @@ int satb_dit_load_weight(SatbDit* d, const char* name_c, const float* src, long 
     if (k == "ff.ff.0.proj.weight" || k == "ff.ff.0.proj.bias") {
       if (!d->ff_perm) {
         // interleave so that every 64-row group = 32 value rows then their 32 gate rows
-        std::vector<int> perm(2 * d->ffi);
-        for (int n = 0; n < 2 * d->ffi; ++n) {
-          const int g = n / 64, w = n % 64;
-          perm[n] = w < 32 ? g * 32 + w : d->ffi + g * 32 + (w - 32);
-        }
+        const std::vector<int> perm = swiglu_perm(d->ffi);
         SATB_PROPAGATE(d->alloc(&d->ff_perm, perm.size()));
         SATB_CHECK_CUDA(cudaMemcpy(d->ff_perm, perm.data(), perm.size() * sizeof(int), cudaMemcpyHostToDevice));
       }
@@ -365,6 +416,36 @@ int satb_dit_load_weight(SatbDit* d, const char* name_c, const float* src, long 
                                       cudaMemcpyDeviceToDevice, st));
       return 0;
     }
+    const std::string cp = "conformer.";
+    if (d->conformer && k.compare(0, cp.size(), cp) == 0) {   // transformer.py:557-574
+      const std::string c = k.substr(cp.size());
+      if (!d->cf_perm) {
+        const std::vector<int> perm = swiglu_perm(D);
+        SATB_PROPAGATE(d->alloc(&d->cf_perm, perm.size()));
+        SATB_CHECK_CUDA(cudaMemcpy(d->cf_perm, perm.data(), perm.size() * sizeof(int), cudaMemcpyHostToDevice));
+      }
+      if (c == "in_norm.gamma") return copy_f32(&L.cf_in_g, D);
+      if (c == "in_norm.beta") return copy_f32(&L.cf_in_b, D);
+      if (c == "mid_norm.gamma") return copy_f32(&L.cf_mid_g, D);
+      if (c == "mid_norm.beta") return copy_f32(&L.cf_mid_b, D);
+      if (c == "depthwise_conv.weight") return copy_f32(&L.cf_dw, 17LL * D);   // [D, 1, 17]
+      if (c == "pointwise_conv_2.weight") return cast16(&L.cf_w2, D, D, nullptr);   // [D, D, 1]
+      if (c == "glu.proj.bias") {
+        SATB_REQUIRE(numel == 2LL * D, ("bad size for " + name).c_str());
+        if (!L.cf_b1) SATB_PROPAGATE(d->alloc(&L.cf_b1, 2 * D));
+        return launch_gather_f32(src, L.cf_b1, d->cf_perm, 2 * D, st);
+      }
+      if (c == "pointwise_conv.weight" || c == "glu.proj.weight") {
+        const bool pw = c == "pointwise_conv.weight";
+        float** dst = pw ? &L.cf_pw_src : &L.cf_glu_src;
+        const long long n = (pw ? 1LL : 2LL) * D * D;
+        SATB_REQUIRE(numel == n, ("bad size for " + name).c_str());
+        if (!*dst) SATB_CHECK_CUDA(cudaMalloc(dst, n * sizeof(float)));
+        SATB_CHECK_CUDA(cudaMemcpyAsync(*dst, src, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        if (L.cf_pw_src && L.cf_glu_src) return fold_conformer_glu(d, L, st);
+        return 0;
+      }
+    }
   }
   d->loaded.erase(name);
   set_last_error("unknown DiT weight key: " + name);
@@ -378,6 +459,19 @@ int satb_dit_finalize(SatbDit* d, void* stream_v) {
   SATB_REQUIRE(d, "null handle");
   cudaStream_t st = static_cast<cudaStream_t>(stream_v);
   const int D = d->D, C = d->C;
+  if (d->conformer) {
+    for (int i = 0; i < d->depth; ++i) {
+      const LayerW& L = d->layers[i];
+      // cf_w1 is the fold of pointwise_conv and glu.proj; a source still pending means its partner is missing
+      if (!(L.cf_in_g && L.cf_in_b && L.cf_w1 && !L.cf_pw_src && !L.cf_glu_src && L.cf_b1 && L.cf_dw && L.cf_mid_g &&
+            L.cf_mid_b && L.cf_w2)) {
+        set_last_error("conformer weights missing in layer " + std::to_string(i) + ": every block needs conformer." +
+                       "{in_norm.gamma, in_norm.beta, pointwise_conv.weight, glu.proj.weight, glu.proj.bias, "
+                       "depthwise_conv.weight, mid_norm.gamma, mid_norm.beta, pointwise_conv_2.weight}");
+        return -1;
+      }
+    }
+  }
   SATB_REQUIRE(d->ts_w && d->te0_w && d->te0_b && d->te2_w && d->te2_b, "timestep embedding weights missing");
   SATB_REQUIRE(d->pin_w && d->pout_w && d->pre_w && d->post_w, "project_in/out or pre/post conv weights missing");
   SATB_REQUIRE(d->inv_freq, "rotary inv_freq missing");
@@ -608,7 +702,7 @@ struct ProfScope {
     if (a) { cudaEventRecord(b, st); d->prof_recs.push_back({cat, a, b}); }
   }
 };
-enum { PROF_FF_IN = 0, PROF_FF_OUT, PROF_QKV, PROF_ATTN_SELF, PROF_ATTN_OUT, PROF_CROSS, PROF_LN, PROF_OTHER, PROF_NCAT };
+enum { PROF_FF_IN = 0, PROF_FF_OUT, PROF_QKV, PROF_ATTN_SELF, PROF_ATTN_OUT, PROF_CROSS, PROF_LN, PROF_CONFORMER, PROF_NCAT };
 
 // FP8 = true: the QKV, cross-attention q and FF-in GEMMs read e4m3 LayerNorm rows (a8, one scale per row in a_scale)
 // and the e4m3 weights; everything else runs as in fp16 mode (BF16 = false).
@@ -729,6 +823,21 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
       EpiResidual::Params ep{h, D, nullptr, nullptr, N_seq, 0, 1};
       SATB_PROPAGATE((linear_auto<EpiResidual, BF16>(d->tmaps, att, D, Mc, D, W.w_co, D, ep, st)));
     }
+    // ---- conformer branch (transformer.py:576-591, added at :680-681 / :697-698 with no modulation or gate):
+    // in_norm -> one GEMM for pointwise_conv + glu.proj (+bias, SwiGLU) -> depthwise conv + mid_norm + SiLU ->
+    // pointwise_conv_2 (+residual).  16-bit operands in every mode (fp16 in the FP8 mode).  Its two [M, D] 16-bit
+    // intermediates live in ws_ff, which is idle between cross-attention and the feed-forward.
+    if (d->conformer) {
+      ProfScope ps(d, PROF_CONFORMER, st);
+      uint16_t* glu = ff;
+      uint16_t* cv = ff + static_cast<size_t>(M) * D;
+      SATB_PROPAGATE(launch_layernorm(h, W.cf_in_g, W.cf_in_b, a16, M, D, nullptr, nullptr, 0, N_seq, 1, BF16, st));
+      typedef EpiSwiglu<BF16> E;
+      SATB_PROPAGATE((linear<E, 256, BF16>(d->tmaps, a16, D, M, D, W.cf_w1, 2 * D, typename E::Params{glu, D, W.cf_b1}, st)));
+      SATB_PROPAGATE(launch_conformer_dwconv(glu, W.cf_dw, W.cf_mid_g, W.cf_mid_b, cv, R, N_seq, D, BF16, st));
+      EpiResidual::Params ep{h, D, nullptr, nullptr, N_seq, 0, 1};
+      SATB_PROPAGATE((linear_auto<EpiResidual, BF16>(d->tmaps, cv, D, M, D, W.cf_w2, D, ep, st)));
+    }
     // ---- feed-forward: LN -> GEMM (+bias, SwiGLU) -> GEMM (+bias, +residual)
     {
       ProfScope ps(d, PROF_LN, st);
@@ -782,7 +891,7 @@ int satb_dit_forward(SatbDit* d, const float* x, const float* t, float* out, int
 
 // Per-category kernel timing with CUDA events on the launching stream (bench.py roofline):
 // categories 0 ff_in GEMM, 1 ff_out GEMM, 2 qkv GEMM, 3 self-attention core, 4 attn out GEMM,
-// 5 cross-attention (LN + q GEMM + core + out GEMM), 6 LayerNorm.
+// 5 cross-attention (LN + q GEMM + core + out GEMM), 6 LayerNorm, 7 conformer branch (all four of its launches).
 int satb_dit_profile(SatbDit* d, int enable) {
   SATB_REQUIRE(d, "null handle");
   d->prof_on = enable != 0;

@@ -56,4 +56,13 @@ int launch_cast_rows(const float* src, void* dst, const int* perm, int rows, int
 int launch_gather_f32(const float* src, float* dst, const int* perm, int n, cudaStream_t stream);
 int launch_zero(void* p, size_t bytes, cudaStream_t stream);
 
+// ---- conformer.cu
+// out16 = silu(LayerNorm(depthwise_conv17(g16))) per item of n_seq rows (zero padding at each item's ends, eps 1e-5):
+// g16, out16 [items * n_seq, D] 16-bit; w fp32 [D][17]; gamma, beta [D] (beta may be null).  D <= kConformerMaxDim.
+constexpr int kConformerMaxDim = 1536;
+int launch_conformer_dwconv(const void* g16, const float* w, const float* gamma, const float* beta, void* out16,
+                            int items, int n_seq, int D, bool bf16, cudaStream_t stream);
+// C[M, N] = A[M, K] B[K, N], fp32 in and out, fp64 accumulation (weight folding).
+int launch_matmul_f64(const float* A, const float* B, float* C, int M, int N, int K, cudaStream_t stream);
+
 }  // namespace satb

@@ -79,6 +79,7 @@ SIGNATURES = {
     "satb_add_launch_count": (None, [ctypes.c_ulonglong]),
     "satb_dit_create": (_I, [ctypes.POINTER(SatbDitConfig), ctypes.POINTER(_VP)]),
     "satb_dit_destroy": (None, [_VP]),
+    "satb_dit_set_conformer": (_I, [_VP, _I]),
     "satb_dit_load_weight": (_I, [_VP, ctypes.c_char_p, _VP, _LL, _VP]),
     "satb_dit_finalize": (_I, [_VP, _VP]),
     "satb_dit_reserve": (_I, [_VP, _I, _I]),
@@ -98,6 +99,7 @@ SIGNATURES = {
     "satb_attention": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP]),
     "satb_attention_hd": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _VP]),
     "satb_attention_probe": (_I, [ctypes.POINTER(SatbAttentionProbe), _VP]),
+    "satb_conformer_dwconv": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _VP]),
     "satb_oobleck_create": (_I, [ctypes.POINTER(SatbOobleckConfig), ctypes.POINTER(_VP)]),
     "satb_oobleck_destroy": (None, [_VP]),
     "satb_oobleck_load_weight": (_I, [_VP, ctypes.c_char_p, _VP, _LL, _VP]),

@@ -10,7 +10,9 @@ and parameter names, ``forward`` signature and CFG semantics); the arithmetic ru
 * one ``forward`` = one ``satb_dit_forward`` call: batched CFG rows (cond first, uncond
   second, dit.py:270-320), 24 blocks, CFG combine / rescale (dit.py:338-347);
 * rows whose context is all-zero (the uncond half without a negative prompt) skip
-  cross-attention: the branch is bias-free, so its output is exactly 0 (SURVEY.md H5).
+  cross-attention: the branch is bias-free, so its output is exactly 0 (SURVEY.md H5);
+* ``conformer=True`` models run the conformer branch of every block natively
+  (``satb_dit_set_conformer``, csrc/conformer.cu), with 16-bit GEMM operands in every ``operand_dtype``.
 
 There is no eager / CPU fallback: tensors must live on a CUDA device.
 """
@@ -26,8 +28,9 @@ from .transformer import SUPPORTED_HEAD_DIMS, ContinuousTransformer, check_head_
 
 # operand_dtype -> SatbDitConfig.operand_dtype.  "fp16" (default) and "bf16": 16-bit operands for every tensor-core
 # contraction.  "fp8": e4m3 operands with power-of-two row scales for the self-attention QKV, cross-attention q and
-# feed-forward input GEMMs (the three Linear layers fed by a LayerNorm), fp16 everywhere else; a precision choice with
-# its own tolerance (DESIGN.md section 5), not a second path to the fp16 result.
+# feed-forward input GEMMs (the three Linear layers fed by a LayerNorm), fp16 everywhere else - the GEMMs of the
+# conformer branch included; a precision choice with its own tolerance (DESIGN.md section 5), not a second path to the
+# fp16 result.
 OPERAND_DTYPES = {"fp16": 0, "bf16": 1, "fp8": 2}
 
 
@@ -81,6 +84,8 @@ class DiffusionTransformer(nn.Module):
         self.global_cond_type = global_cond_type
         self.operand_dtype = operand_dtype
         self.qk_norm = bool(kwargs.get("attn_kwargs", {}).get("qk_norm", False))
+        # conformer=True (ContinuousTransformer kwarg): every block adds the conformer branch (satb_dit_set_conformer)
+        self.conformer = bool(kwargs.get("conformer", False))
 
         feat_dim = 256
         self.timestep_features = FourierFeatures(1, feat_dim)
@@ -163,6 +168,12 @@ class DiffusionTransformer(nn.Module):
             cfg = self.native_config()
             h = ctypes.c_void_p()
             _native.check(lib.satb_dit_create(ctypes.byref(cfg), ctypes.byref(h)))
+            if self.conformer:
+                rc = lib.satb_dit_set_conformer(h, 1)
+                if rc != 0:
+                    msg = lib.satb_last_error()
+                    lib.satb_dit_destroy(h)
+                    raise _native.NativeError(f"satb200 error {rc}: {msg.decode() if msg else '?'}")
             self.__dict__["_h"] = h
         if self.__dict__["_weights_dirty"]:
             st = _native.stream_ptr(device)

@@ -16,6 +16,8 @@ from torch import nn
 
 # Attention head widths the native attention kernel and RoPE epilogue are built for (csrc/attention_tc.cu, gemm.cuh).
 SUPPORTED_HEAD_DIMS = (32, 64, 96, 128)
+# Widest model whose conformer branch the native depthwise-convolution kernel runs (csrc/conformer.cu).
+CONFORMER_MAX_DIM = 1536
 
 
 def check_head_dim(dim_heads, qk_norm=False):
@@ -115,13 +117,34 @@ class Attention(_FusedModule):
             nn.init.zeros_(self.to_out.weight)
 
 
+class ConformerModule(_FusedModule):
+    """Reference transformer.py:557-591: in_norm -> pointwise_conv (1x1) -> GLU (SiLU gate) -> depthwise_conv (17 taps,
+    zero padding 8, over the token axis) -> mid_norm -> SiLU -> pointwise_conv_2 (1x1).  Natively, pointwise_conv is
+    folded into glu.proj (one GEMM) and the depthwise convolution, mid_norm and SiLU are one kernel
+    (csrc/conformer.cu); its GEMMs take 16-bit operands in every operand_dtype, fp16 in the "fp8" mode."""
+
+    def __init__(self, dim, norm_kwargs={}):
+        super().__init__()
+        if dim > CONFORMER_MAX_DIM:
+            raise NotImplementedError(f"conformer blocks are on the native hot path up to dim {CONFORMER_MAX_DIM} "
+                                      f"(got {dim})")
+        self.dim = dim
+        self.in_norm = LayerNorm(dim, **norm_kwargs)
+        self.pointwise_conv = nn.Conv1d(dim, dim, kernel_size=1, bias=False)
+        self.glu = GLU(dim, dim, nn.SiLU())
+        self.depthwise_conv = nn.Conv1d(dim, dim, kernel_size=17, groups=dim, padding=8, bias=False)
+        self.mid_norm = LayerNorm(dim, **norm_kwargs)
+        self.swish = nn.SiLU()
+        self.pointwise_conv_2 = nn.Conv1d(dim, dim, kernel_size=1, bias=False)
+
+
 class TransformerBlock(_FusedModule):
     def __init__(self, dim, dim_heads=64, cross_attend=False, dim_context=None, global_cond_dim=None, causal=False,
                  zero_init_branch_outputs=True, conformer=False, layer_ix=-1, remove_norms=False, attn_kwargs={},
                  ff_kwargs={}, norm_kwargs={}):
         super().__init__()
-        if conformer or remove_norms:
-            raise NotImplementedError("conformer / norm-free blocks are outside the native hot path")
+        if remove_norms:
+            raise NotImplementedError("norm-free blocks are outside the native hot path")
         self.dim, self.dim_heads = dim, dim_heads
         self.cross_attend, self.dim_context = cross_attend, dim_context
         self.global_cond_dim, self.layer_ix = global_cond_dim, layer_ix
@@ -134,6 +157,8 @@ class TransformerBlock(_FusedModule):
                                         zero_init_output=zero_init_branch_outputs, **attn_kwargs)
         self.ff_norm = LayerNorm(dim, **norm_kwargs)
         self.ff = FeedForward(dim, zero_init_output=zero_init_branch_outputs, **ff_kwargs)
+        # x = x + conformer(x) between cross-attention and the feed-forward (reference transformer.py:680-681,697-698)
+        self.conformer = ConformerModule(dim, norm_kwargs=norm_kwargs) if conformer else None
         if global_cond_dim:
             self.to_scale_shift_gate = nn.Sequential(nn.SiLU(), nn.Linear(global_cond_dim, dim * 6, bias=False))
             nn.init.zeros_(self.to_scale_shift_gate[1].weight)

@@ -76,6 +76,12 @@ void satb_add_launch_count(unsigned long long n);
  *      (models/transformer.py:705-809) behind DiTWrapper.forward (models/diffusion.py:491-529) */
 int satb_dit_create(const SatbDitConfig* cfg, SatbDit** out);
 void satb_dit_destroy(SatbDit* h);
+/* conformer=True models (ContinuousTransformer / TransformerBlock kwarg, models/transformer.py:557-591,645,680-681,
+ * 697-698): enable != 0 adds the conformer branch x += conformer(x) between cross-attention and the feed-forward of
+ * every block.  Call after satb_dit_create and before the first satb_dit_load_weight; embed_dim <= 1536.  finalize then
+ * requires the nine "transformer.layers.{i}.conformer.*" tensors of every layer.  Its GEMMs take 16-bit operands in
+ * every operand_dtype (fp16 in the fp8 mode).  A handle that never calls this runs the model without the branch. */
+int satb_dit_set_conformer(SatbDit* h, int enable);
 /* One state-dict entry (key relative to DiffusionTransformer, e.g.
  * "transformer.layers.0.self_attn.to_qkv.weight"); src: device fp32, contiguous.
  * Replaces nn.Module.load_state_dict for this module (models/pretrained.py:24). */
@@ -103,7 +109,7 @@ int satb_dit_forward_debug(SatbDit* h, const float* x, const float* t, float* ou
 
 /* Per-kernel-class CUDA-event timing used by bench.py's roofline line: enable, run forwards,
  * then read ms[8]/count[8] (0 ff_in GEMM, 1 ff_out GEMM, 2 qkv GEMM, 3 self-attention core,
- * 4 attention out GEMM, 5 cross-attention, 6 LayerNorm, 7 unused). */
+ * 4 attention out GEMM, 5 cross-attention, 6 LayerNorm, 7 conformer branch (conformer models only)). */
 int satb_dit_profile(SatbDit* h, int enable);
 int satb_dit_profile_read(SatbDit* h, float* ms, int* count);
 
@@ -193,6 +199,13 @@ typedef struct SatbAttentionProbe {
   int q_col, k_col, v_col;
 } SatbAttentionProbe;
 int satb_attention_probe(const SatbAttentionProbe* p, void* stream);
+
+/* Test entry point: the kernel of the conformer branch, out = silu(LayerNorm(depthwise_conv(g))) per item
+ * (transformer.py:583-586): g, out [items * n_seq, D] 16-bit (fp16/bf16 bits), 16-byte aligned; the convolution runs
+ * over the n_seq rows of each item with 17 taps and 8 zero rows of padding at both ends; w [D, 1, 17] fp32 (device),
+ * gamma, beta [D] fp32 (beta may be NULL), eps 1e-5.  D a multiple of 128, <= 1536. */
+int satb_conformer_dwconv(const void* g16, const float* w, const float* gamma, const float* beta, void* out16, int items,
+                          int n_seq, int D, int bf16, void* stream);
 
 /* ---- Oobleck VAE: replaces OobleckDecoder / OobleckEncoder.forward
  *      (models/autoencoders.py:119-194) behind AudioAutoencoder.encode/decode (:268-343) */
