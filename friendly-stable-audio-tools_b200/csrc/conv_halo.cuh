@@ -29,10 +29,10 @@ struct HaloShape {
   int N;         // output channels (rows of W per tap)
 };
 
-struct ResUnitPre {      // FUSE: the inner conv7 -> snake2 step
+struct ResUnitPre {      // FUSE: the inner conv7 -> snake2 step (ELU instead when Epi::kAct is kActElu)
   const float* bias7;    // [N] or null
-  const float* sn2_a;    // e^alpha of snake2
-  const float* sn2_ib;   // 1/(e^beta + 1e-9) of snake2
+  const float* sn2_a;    // e^alpha of snake2 (unused by ELU)
+  const float* sn2_ib;   // 1/(e^beta + 1e-9) of snake2 (unused by ELU)
 };
 
 constexpr int kHaloMax = 54;   // halo rows beyond the tile: 6 taps x dilation 9
@@ -183,19 +183,23 @@ conv_halo_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       }
       if constexpr (FUSE) {
         named_bar_sync(3, 256);   // both warpgroups have read the previous tile's accumulator staging (same region)
-        // acc -> + bias7 -> snake2 -> 16-bit -> rows [64 cw, 64 cw + 64) of the A2 tile (K-major, 128B-swizzled atoms)
+        // acc -> + bias7 -> snake2 (or ELU: Epi::kAct) -> 16-bit -> rows [64 cw, 64 cw + 64) of the A2 tile (K-major,
+        // 128B-swizzled atoms)
+        constexpr int ACT = Epi::kAct;
         const int fr = 64 * cw + 16 * (warp & 3) + (lane >> 2), fc = 2 * (lane & 3);
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
           const int col = 8 * j + fc;
           const float b0 = pre.bias7 ? __ldg(pre.bias7 + col) : 0.f, b1 = pre.bias7 ? __ldg(pre.bias7 + col + 1) : 0.f;
-          const float a0 = __ldg(pre.sn2_a + col), a1 = __ldg(pre.sn2_a + col + 1);
-          const float i0 = __ldg(pre.sn2_ib + col), i1 = __ldg(pre.sn2_ib + col + 1);
+          const float a0 = ACT == kActSnake ? __ldg(pre.sn2_a + col) : 0.f;
+          const float a1 = ACT == kActSnake ? __ldg(pre.sn2_a + col + 1) : 0.f;
+          const float i0 = ACT == kActSnake ? __ldg(pre.sn2_ib + col) : 0.f;
+          const float i1 = ACT == kActSnake ? __ldg(pre.sn2_ib + col + 1) : 0.f;
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const int r = fr + 8 * h;
-            const uint32_t v = Op16<BF16>::pack(snake_fast(acc[4 * j + 2 * h] + b0, a0, i0),
-                                                snake_fast(acc[4 * j + 2 * h + 1] + b1, a1, i1));
+            const uint32_t v = Op16<BF16>::pack(act_fast<ACT>(acc[4 * j + 2 * h] + b0, a0, i0),
+                                                act_fast<ACT>(acc[4 * j + 2 * h + 1] + b1, a1, i1));
             const int chunk = (col & 63) >> 3;
             *reinterpret_cast<uint32_t*>(shared + (col >> 6) * (kBlockM * 128) + r * 128 + ((chunk ^ (r & 7)) << 4) +
                                          (col & 7) * 2) = v;
@@ -229,8 +233,10 @@ int launch_conv_halo(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUten
   using Cfg = HaloCfg<BN, Epi::kCols, Epi::kStageBytes, FUSE>;
   SATB_REQUIRE(s.K % kBlockK == 0 && s.n_taps % 2 == 1 && (s.n_taps - 1) * s.dil <= kHaloMax && s.N <= BN,
                "halo convolution: unsupported shape");
-  SATB_REQUIRE(!FUSE || (tmB1 != nullptr && s.N == BN && s.K == BN && pre.sn2_a && pre.sn2_ib),
-               "fused ResidualUnit: needs the 1x1 weights, channels = tile width, and snake2");
+  if constexpr (FUSE) {
+    SATB_REQUIRE(tmB1 != nullptr && s.N == BN && s.K == BN && (Epi::kAct == kActElu || (pre.sn2_a && pre.sn2_ib)),
+                 "fused ResidualUnit: needs the 1x1 weights, channels = tile width, and snake2");
+  }
   auto kern = conv_halo_wgmma_kernel<Epi, BN, BF16, FUSE>;
   static PerDeviceOnce attr;
   if (attr.first()) SATB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));

@@ -751,6 +751,39 @@ __device__ __forceinline__ uint64_t snake_fast2(uint64_t v, uint64_t a, uint64_t
   return f2_fma(ib, f2_mul(sn, sn), v);
 }
 
+// The activation a convolution epilogue applies to the 16-bit copy it writes (the consuming layer's activation,
+// models/autoencoders.py:29-42): a template parameter of every kernel that applies one.
+constexpr int kActSnake = 0;   // SnakeBeta (use_snake=True), per-channel a = e^alpha, ib = 1/(e^beta + 1e-9)
+constexpr int kActElu = 1;     // nn.ELU() (use_snake=False), alpha 1, no parameters
+
+// ELU: v > 0 ? v : e^v - 1.  e^v - 1 through the SFU exponential (ex2.approx) carries an absolute error of up to
+// ~2^-21.8, which near 0 exceeds the value's own 16-bit rounding (below |v| ~ 2^-12).  For -2^-6 < v <= 0 the cubic
+// Taylor polynomial is used instead: its truncation is < v^4 / 24, i.e. < 2^-22.6 |v| there.  Below -2^-6 the SFU
+// value's 2^-21.8 is < 2^-15.8 |e^v - 1|.  Same formulation in every instance (scalar and pair).  The exponential
+// flushes subnormal results (e^v < 2^-126, where e^v - 1 is -1 either way), which saves __expf's subnormal fix-up.
+__device__ __forceinline__ float elu_fast(float v) {
+  float e;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(v * 1.4426950409f));
+  e -= 1.0f;
+  const float p = v * fmaf(v, fmaf(v, 0.16666667f, 0.5f), 1.0f);
+  return v > 0.0f ? v : (v > -0.015625f ? p : e);
+}
+template <int ACT>
+__device__ __forceinline__ float act_fast(float v, float a, float ib) {
+  if constexpr (ACT == kActElu) return elu_fast(v);
+  else return snake_fast(v, a, ib);
+}
+template <int ACT>
+__device__ __forceinline__ uint64_t act_fast2(uint64_t v, uint64_t a, uint64_t ib) {
+  if constexpr (ACT == kActElu) {
+    float x0, x1;
+    f2_unpack(v, x0, x1);
+    return f2_pack(elu_fast(x0), elu_fast(x1));
+  } else {
+    return snake_fast2(v, a, ib);
+  }
+}
+
 // Epilogue of every tensor-core convolution of the Oobleck VAE (models/autoencoders.py:45-116):
 //   y = acc + bias[co] (+ resid[pos, co])            ResidualUnit skip :66-68
 //   raw_out[pos, co] = y (fp32, optional)            kept only where a later skip needs it
@@ -762,7 +795,8 @@ struct EpiConvParams {
   const void* resid;    // raw skip stream [B*L_out, cout] (fp32, or 16-bit when raw16) or null
   void* raw_out;        // raw stream out, same type, or null
   void* s16_out;        // 16-bit [B*L_out, cout] or null
-  const float* sn_a;    // [cout] e^alpha of the consumer's Snake, or null (plain cast)
+  const float* sn_a;    // [cout] e^alpha of the consumer's Snake, or null (plain cast); ELU instances ignore sn_a /
+                        // sn_ib and always apply ELU to s16_out
   const float* sn_ib;   // [cout] 1/(e^beta + 1e-9)
   int cout;
   int L_out;            // output positions per batch item
@@ -780,14 +814,19 @@ struct EpiConvParams {
 // idx0 + i * stride), keeps per-segment validity as a bit mask and makes Snake and the 16-bit raw streams
 // unconditional.  Compiled next to the general path in one kernel it pays ~200 bytes of spills in the persistent GEMM
 // kernels (long-scoreboard stalls on the reloads, profiles/r02_ncu_convT_s2.txt).
-template <bool BF16, bool MASKED = false>
-struct EpiConv {
+//
+// ACT: the activation of the 16-bit output (kActSnake / kActElu).  The body is EpiConvT; the instances are the two
+// derived names below, so the Snake instances keep the kernel symbols they had before ACT existed.
+template <bool BF16, bool MASKED, int ACT>
+struct EpiConvT {
   static constexpr int kCols = 32;
   static constexpr int kStageBytes = 32 * 36 * 4;   // per-warp [32 rows][32 + 4 pad] fp32 transpose tile
+  static constexpr int kAct = ACT;
+  static constexpr bool kMasked = MASKED;
   typedef EpiConvParams Params;
-  // Snake-activated 16-bit output, raw streams (if any) in the 16-bit type, no lo copy: what the default fp16 decode runs
+  // activated 16-bit output, raw streams (if any) in the 16-bit type, no lo copy: what the default fp16 decode runs
   __host__ __device__ static bool fast_flags(const Params& p) {
-    return p.s16_out != nullptr && p.sn_a != nullptr && p.s16_lo_out == nullptr &&
+    return p.s16_out != nullptr && (ACT == kActElu || p.sn_a != nullptr) && p.s16_lo_out == nullptr &&
            (p.raw16 != 0 || (p.resid == nullptr && p.raw_out == nullptr));
   }
   // Warp-cooperative: the accumulator chunk (thread = row, 32 columns) is transposed through the
@@ -862,8 +901,8 @@ struct EpiConv {
     __syncwarp();
     ulonglong2 b2 = make_ulonglong2(0ull, 0ull);
     if (p.bias) b2 = __ldg(reinterpret_cast<const ulonglong2*>(p.bias + pl.co));
-    const ulonglong2 a2 = __ldg(reinterpret_cast<const ulonglong2*>(p.sn_a + pl.co));
-    const ulonglong2 ib2 = __ldg(reinterpret_cast<const ulonglong2*>(p.sn_ib + pl.co));
+    const ulonglong2 a2 = ACT == kActSnake ? __ldg(reinterpret_cast<const ulonglong2*>(p.sn_a + pl.co)) : b2;
+    const ulonglong2 ib2 = ACT == kActSnake ? __ldg(reinterpret_cast<const ulonglong2*>(p.sn_ib + pl.co)) : b2;
     uint16_t* raw_o = static_cast<uint16_t*>(p.raw_out) + pl.idx0;
     uint16_t* s_o = static_cast<uint16_t*>(p.s16_out) + pl.idx0;
     uint32_t ld_addr = st + (r0 * 36 + 4 * g) * 4;
@@ -885,8 +924,8 @@ struct EpiConv {
         if (ok) *reinterpret_cast<uint2*>(raw_o) = make_uint2(Op16<BF16>::pack(y0, y1), Op16<BF16>::pack(y2, y3));
         raw_o += pl.stride;
       }
-      v01 = snake_fast2(v01, a2.x, ib2.x);
-      v23 = snake_fast2(v23, a2.y, ib2.y);
+      v01 = act_fast2<ACT>(v01, a2.x, ib2.x);
+      v23 = act_fast2<ACT>(v23, a2.y, ib2.y);
       float x0, x1, x2, x3;
       f2_unpack(v01, x0, x1);
       f2_unpack(v23, x2, x3);
@@ -949,8 +988,8 @@ struct EpiConv {
     const int co = sg.co;
     ulonglong2 b2 = make_ulonglong2(0ull, 0ull), a2 = b2, ib2 = b2;   // (x,y) and (z,w) pairs; 0 bits = 0.f
     if (p.bias) b2 = __ldg(reinterpret_cast<const ulonglong2*>(p.bias + co));
-    const bool snake = p.s16_out != nullptr && p.sn_a != nullptr;
-    if (snake) {
+    const bool act = p.s16_out != nullptr && (ACT == kActElu || p.sn_a != nullptr);
+    if (ACT == kActSnake && act) {
       a2 = __ldg(reinterpret_cast<const ulonglong2*>(p.sn_a + co));
       ib2 = __ldg(reinterpret_cast<const ulonglong2*>(p.sn_ib + co));
     }
@@ -982,9 +1021,9 @@ struct EpiConv {
           }
         }
         if (p.s16_out) {
-          if (snake) {
-            v01 = snake_fast2(v01, a2.x, ib2.x);
-            v23 = snake_fast2(v23, a2.y, ib2.y);
+          if (act) {
+            v01 = act_fast2<ACT>(v01, a2.x, ib2.x);
+            v23 = act_fast2<ACT>(v23, a2.y, ib2.y);
           }
           float x0, x1, x2, x3;
           f2_unpack(v01, x0, x1);
@@ -1009,6 +1048,12 @@ struct EpiConv {
     finish(p, c, r, rs);
   }
 };
+template <bool BF16, bool MASKED = false>
+struct EpiConv : EpiConvT<BF16, MASKED, kActSnake> {};
+template <bool BF16, bool MASKED = false>
+struct EpiConvElu : EpiConvT<BF16, MASKED, kActElu> {};
+template <bool BF16, bool MASKED, int ACT>
+using EpiConvFor = typename std::conditional<ACT == kActElu, EpiConvElu<BF16, MASKED>, EpiConv<BF16, MASKED>>::type;
 
 // out[b, n, l] (NCL fp32) = acc + bias[n]; consecutive lanes hold consecutive l, so every
 // per-column store is a coalesced 128 B line.

@@ -12,6 +12,9 @@
 // one (128 -> 2) runs through the same GEMM with a mostly empty N tile.
 // Weight-norm (w = g * v / ||v||, torch.nn.utils.weight_norm via dac.nn.layers) is folded
 // once at load time.
+// Block options (satb_oobleck_create_variant): ELU instead of Snake (use_snake=False) is the ACT template parameter of
+// every kernel that activates (kActElu: no per-channel parameters); nearest-neighbour upsampling + conv k = 2s 'same'
+// (use_nearest_upsample=True) is a 3-tap GEMM over the low-rate input with N = s*Cout (run_conv_gemm kind 3).
 #include <algorithm>
 #include <cmath>
 #include <tuple>
@@ -123,8 +126,8 @@ __global__ void __launch_bounds__(256) ncl_to_nlc16_kernel(const float* __restri
 
 // Encoder input convolution (audio NCL fp32, Cin = 1 or 2 -> C channels, k taps, pad k/2):
 // bandwidth-bound; one thread per output channel, a tile of positions per block.
-// Writes raw fp32 and the Snake-activated 16-bit copy, channels-last.
-template <bool BF16>
+// Writes raw fp32 and the activated (Snake or ELU: ACT) 16-bit copy, channels-last.
+template <bool BF16, int ACT>
 __global__ void __launch_bounds__(256) conv_in_kernel(const float* __restrict__ audio, const float* __restrict__ w,
                                                       const float* __restrict__ bias, const float* __restrict__ sn_a,
                                                       const float* __restrict__ sn_ib, void* __restrict__ raw,
@@ -145,7 +148,7 @@ __global__ void __launch_bounds__(256) conv_in_kernel(const float* __restrict__ 
     float wr[16];  // Cin * kk <= 16 (stereo k7 = 14)
     for (int i = 0; i < Cin * kk; ++i) wr[i] = w[static_cast<size_t>(co) * Cin * kk + i];
     const float bb = bias ? bias[co] : 0.f;
-    const float a = sn_a[co], ib = sn_ib[co];
+    const float a = ACT == kActSnake ? sn_a[co] : 0.f, ib = ACT == kActSnake ? sn_ib[co] : 0.f;
     for (int j = 0; j < kTile; ++j) {
       const int64_t l = l0 + j;
       if (l >= T) break;
@@ -159,7 +162,7 @@ __global__ void __launch_bounds__(256) conv_in_kernel(const float* __restrict__ 
       } else {
         static_cast<float*>(raw)[o] = acc;
       }
-      const float act = snake_fast(acc, a, ib);
+      const float act = act_fast<ACT>(acc, a, ib);
       typename Op16<BF16>::T h = Op16<BF16>::from_float(act);
       s16[o] = *reinterpret_cast<uint16_t*>(&h);
       if (s16_lo) {
@@ -169,12 +172,44 @@ __global__ void __launch_bounds__(256) conv_in_kernel(const float* __restrict__ 
     }
   }
 }
+// Nearest-neighbour upsampling by `up` followed by a Conv1d v [cout, cin, 2 up] with padding 'same' (up - 1 zeros on
+// the left, up on the right; models/autoencoders.py:95-100) is a 3-tap convolution of the low-rate input over
+// N = up * cout columns: output position up * m + ph reads x[m + o], o = -1, 0, 1, through
+//   dst[o + 1][ph * cout + co][ci] = sum_{k : floor((ph + k - up + 1) / up) = o} v[co, ci, k] * scale[co]
+// The sum runs in fp64 and is rounded to fp32 once; the fp32 value is then stored like every other conv weight (its
+// 16-bit rounding, and the 16-bit rounding of the remainder as the lo block in split-operand mode).
+template <bool BF16>
+__global__ void nearest_w_prep_kernel(const float* __restrict__ v, const float* __restrict__ scale,
+                                      uint16_t* __restrict__ dst, uint16_t* __restrict__ dst_lo, int cin, int cout,
+                                      int up, size_t total) {
+  for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const int ci = static_cast<int>(i % cin);
+    const size_t rest = i / cin;
+    const int n = static_cast<int>(rest % (static_cast<size_t>(up) * cout));
+    const int o = static_cast<int>(rest / (static_cast<size_t>(up) * cout)) - 1;
+    const int ph = n / cout, co = n - ph * cout;
+    // floor((ph + k - up + 1) / up) = o  <=>  k in [(o + 1) up - ph - 1, (o + 2) up - ph - 1), clipped to [0, 2 up)
+    const int k0 = max((o + 1) * up - ph - 1, 0), k1 = min((o + 2) * up - ph - 1, 2 * up);
+    const float* vr = v + (static_cast<size_t>(co) * cin + ci) * (2 * up);
+    double acc = 0.0;
+    for (int k = k0; k < k1; ++k) acc += static_cast<double>(vr[k]) * static_cast<double>(scale[co]);
+    const float w = static_cast<float>(acc);
+    typename Op16<BF16>::T h = Op16<BF16>::from_float(w);
+    dst[i] = *reinterpret_cast<uint16_t*>(&h);
+    if (dst_lo) {
+      typename Op16<BF16>::T l = Op16<BF16>::from_float(w - Op16<BF16>::to_float(h));
+      dst_lo[i] = *reinterpret_cast<uint16_t*>(&l);
+    }
+  }
+}
 
 }  // namespace
 
 struct ConvW {
   int cin = 0, cout = 0, k = 0;
   bool transposed = false, small = false, has_bias = true;
+  bool nearest = false;     // nearest-upsample conv (k = 2 * up), stored folded as 3 taps over up * cout rows
   std::string pfx;
   uint16_t* w16 = nullptr;  // [taps][n][cin]
   float* w32 = nullptr;     // small convs: folded [cout][cin][k]
@@ -192,6 +227,8 @@ using namespace satb;
 
 struct SatbOobleck {
   SatbOobleckConfig cfg;
+  int act = kActSnake;             // the blocks' activation (use_snake): kActSnake or kActElu
+  bool nearest = false;            // decoder upsampling: nearest + conv (use_nearest_upsample) instead of ConvTranspose1d
   bool bf16 = false;
   int raw16 = 0;                   // 1: the raw skip stream is carried in the 16-bit operand type (fp16 mode), 0: fp32
   bool split3 = false;             // operand_dtype 2 ("fp16x3"): every product as (hi, hi) + (lo, hi) + (hi, lo), see GemmShape
@@ -287,7 +324,43 @@ int prep_conv(SatbOobleck* h, const std::string& pfx, int cin, int cout, int k, 
   return 0;
 }
 
+// Conv1d k = 2 up after a nearest x up upsample (no bias), folded to the 3-tap block of nearest_w_prep_kernel.
+int prep_conv_nearest(SatbOobleck* h, const std::string& pfx, int cin, int cout, int up, cudaStream_t st) {
+  ConvW c;
+  c.cin = cin; c.cout = cout; c.k = 2 * up; c.has_bias = false; c.nearest = true; c.pfx = pfx;
+  float *g, *v;
+  const int slice = cin * c.k;
+  SATB_PROPAGATE(get_raw(h, pfx + "weight_g", cout, &g));
+  SATB_PROPAGATE(get_raw(h, pfx + "weight_v", static_cast<long long>(cout) * slice, &v));
+  float* scale;
+  SATB_PROPAGATE(h->alloc_bytes(reinterpret_cast<void**>(&scale), static_cast<size_t>(cout) * 4));
+  wn_scale_kernel<<<cout, 256, 0, st>>>(g, v, scale, slice);
+  count_launch();
+  const size_t total = static_cast<size_t>(3) * up * cout * cin;
+  const size_t parts = h->split3 ? 2 : 1;      // [hi block | lo block]
+  SATB_PROPAGATE(h->alloc_bytes(reinterpret_cast<void**>(&c.w16), parts * total * 2 + 256 * 128));  // slack for box overreach
+  SATB_CHECK_CUDA(cudaMemsetAsync(c.w16, 0, parts * total * 2 + 256 * 128, st));
+  uint16_t* w_lo = h->split3 ? c.w16 + total : nullptr;
+  int grid = static_cast<int>(ceil_div64(total, 256));
+  if (grid > 8192) grid = 8192;
+  if (h->bf16)
+    nearest_w_prep_kernel<true><<<grid, 256, 0, st>>>(v, scale, c.w16, w_lo, cin, cout, up, total);
+  else
+    nearest_w_prep_kernel<false><<<grid, 256, 0, st>>>(v, scale, c.w16, w_lo, cin, cout, up, total);
+  count_launch();
+  SATB_CHECK_CUDA(cudaGetLastError());
+  h->convs[pfx] = c;
+  return 0;
+}
+
+// elements of a finalized conv's stored weight block (one part)
+size_t conv_w_elems(const ConvW& c) {
+  const size_t n = static_cast<size_t>(c.cin) * c.cout;
+  return c.nearest ? n * 3 * (c.k / 2) : n * c.k;
+}
+
 int prep_snake(SatbOobleck* h, const std::string& pfx, int c, cudaStream_t st) {
+  if (h->act != kActSnake) return 0;     // nn.ELU has no parameters: nothing to look up
   SnakeW s;
   s.c = c; s.pfx = pfx;
   float *al, *be;
@@ -301,6 +374,14 @@ int prep_snake(SatbOobleck* h, const std::string& pfx, int c, cudaStream_t st) {
   h->snakes[pfx] = s;
   return 0;
 }
+
+// The parameters of the activation at `pfx`: the Snake's, or null in an ELU model (nn.ELU sits at the same index of
+// the Sequential and has none).
+const SnakeW* act_params(const SatbOobleck* h, const std::string& pfx) {
+  return h->act == kActSnake ? &h->snakes.at(pfx) : nullptr;
+}
+const float* act_a(const SnakeW* s) { return s ? s->a : nullptr; }
+const float* act_ib(const SnakeW* s) { return s ? s->ib : nullptr; }
 
 int get_tmap_a(SatbOobleck* h, const void* in16, int cin, int a_rows, int B, int L_in, int a_stride, const CUtensorMap** out,
                int box_rows = kBlockM) {
@@ -332,17 +413,21 @@ int get_tmap_b(SatbOobleck* h, const ConvW& cw, int b_rows, int box, const CUten
 //   kind 0: conv k taps, dilation dil, "same" padding           (L_out = L_in)
 //   kind 1: transposed conv k = 2*up, stride up, pad ceil(up/2)  (L_out = L_in * up)
 //   kind 2: strided conv k = 2*st, stride st, pad ceil(st/2)     (L_out = L_in / st)
+//   kind 3: nearest x up then conv k = 2*up, 'same' padding, as 3 taps over N = up*cout  (L_out = L_in * up)
 template <class Epi, bool BF16>
 int run_conv_gemm(SatbOobleck* h, const ConvW& cw, const void* in16, int B, int L_in, int kind, int dil, int factor,
                   const typename Epi::Params& ep, cudaStream_t st) {
   // the default 16-bit decode / encode runs the lean-epilogue instantiation of the GEMM kernels (EpiConv<.., MASKED>)
-  if constexpr (std::is_same<Epi, EpiConv<BF16, false>>::value) {
+  constexpr bool kGeneralConv =
+      std::is_same<Epi, EpiConv<BF16, false>>::value || std::is_same<Epi, EpiConvElu<BF16, false>>::value;
+  constexpr bool kLeanConv = std::is_same<Epi, EpiConv<BF16, true>>::value || std::is_same<Epi, EpiConvElu<BF16, true>>::value;
+  if constexpr (kGeneralConv) {
     if (Epi::fast_flags(ep))
-      return run_conv_gemm<EpiConv<BF16, true>, BF16>(h, cw, in16, B, L_in, kind, dil, factor, ep, st);
+      return run_conv_gemm<EpiConvFor<BF16, true, Epi::kAct>, BF16>(h, cw, in16, B, L_in, kind, dil, factor, ep, st);
   }
-  h->routes |= std::is_same<Epi, EpiStoreNCL>::value          ? SATB_OOB_ROUTE_GEMM_NCL
-               : std::is_same<Epi, EpiConv<BF16, true>>::value ? SATB_OOB_ROUTE_GEMM_LEAN
-                                                               : SATB_OOB_ROUTE_GEMM;
+  h->routes |= std::is_same<Epi, EpiStoreNCL>::value ? SATB_OOB_ROUTE_GEMM_NCL
+               : kLeanConv                           ? SATB_OOB_ROUTE_GEMM_LEAN
+                                                     : SATB_OOB_ROUTE_GEMM;
   GemmShape s;
   s.batches = B;
   s.b_static = 1;   // folded weight-norm weights, written at finalize time
@@ -353,6 +438,10 @@ int run_conv_gemm(SatbOobleck* h, const ConvW& cw, const void* in16, int B, int 
     s.stride = 1;
   } else if (kind == 1) {
     s.L = L_in + 1; s.N = factor * cw.cout; s.n_taps = 2; s.tap_base = 0; s.tap_step = -1; s.b_tap_rows = factor * cw.cout;
+    s.stride = 1;
+  } else if (kind == 3) {
+    SATB_REQUIRE(cw.nearest && cw.k == 2 * factor, "nearest upsample: needs the folded 3-tap weights of stride factor");
+    s.L = L_in; s.N = factor * cw.cout; s.n_taps = 3; s.tap_base = -1; s.tap_step = 1; s.b_tap_rows = factor * cw.cout;
     s.stride = 1;
   } else {
     SATB_REQUIRE(L_in % factor == 0, "strided conv: length must be a multiple of the stride");
@@ -387,13 +476,14 @@ int run_conv_gemm(SatbOobleck* h, const ConvW& cw, const void* in16, int B, int 
 // ResidualUnit (models/autoencoders.py:45-68).  In: snake1(x) as 16-bit in sA, x as fp32 in raw.
 // Out: y = x + conv1(snake2(conv7(.))) as fp32 in raw (if keep_raw) and snake_next(y) as 16-bit in sA;
 // sT is scratch (the two pointers are swapped when the fused kernel wrote its output there).
-template <bool BF16>
+// ACT: the model's activation (snake1 / snake2 / the next one are ELUs in an ELU model, with null parameters).
+template <bool BF16, int ACT>
 int residual_unit(SatbOobleck* h, const std::string& pfx, int C, int B, int L, int dil, void* raw, void*& sA, void*& sT,
                   const SnakeW* next_snake, bool keep_raw, cudaStream_t st) {
   const ConvW& c7 = h->convs.at(pfx + "layers.1.");
   const ConvW& c1 = h->convs.at(pfx + "layers.3.");
-  const SnakeW& s2 = h->snakes.at(pfx + "layers.2.");
-  typedef EpiConv<BF16> E;
+  const SnakeW* s2 = act_params(h, pfx + "layers.2.");
+  typedef EpiConvFor<BF16, false, ACT> E;
   typename E::Params e1{c1.bias, raw, keep_raw ? raw : nullptr, sA, next_snake ? next_snake->a : nullptr,
                         next_snake ? next_snake->ib : nullptr, C, L, 1, 0, h->split3 ? static_cast<char*>(sA) + h->lo_off : nullptr, h->raw16};
   if ((C == 128 || C == 256) && c7.k == 7 && 6 * dil <= kHaloMax && !h->split3) {
@@ -404,10 +494,10 @@ int residual_unit(SatbOobleck* h, const std::string& pfx, int C, int B, int L, i
     SATB_PROPAGATE(get_tmap_b(h, c1, C, C, &tb1));
     e1.s16_out = sT;
     const HaloShape hs{L, B, C, 7, dil, C};
-    const ResUnitPre pre{c7.bias, s2.a, s2.ib};
+    const ResUnitPre pre{c7.bias, act_a(s2), act_ib(s2)};
     h->routes |= E::fast_flags(e1) ? SATB_OOB_ROUTE_FUSED_LEAN : SATB_OOB_ROUTE_FUSED;
     if (E::fast_flags(e1)) {
-      typedef EpiConv<BF16, true> EM;
+      typedef EpiConvFor<BF16, true, ACT> EM;
       SATB_PROPAGATE(C == 128 ? (launch_conv_halo<EM, 128, BF16, true>(*ta, *tb7, tb1, hs, pre, e1, st))
                               : (launch_conv_halo<EM, 256, BF16, true>(*ta, *tb7, tb1, hs, pre, e1, st)));
     } else {
@@ -418,7 +508,7 @@ int residual_unit(SatbOobleck* h, const std::string& pfx, int C, int B, int L, i
     return 0;
   }
   // conv7(dil) on sA -> snake2 -> sT ; conv1 on sT -> + x -> raw, snake_next -> sA
-  typename E::Params e7{c7.bias, nullptr, nullptr, sT, s2.a, s2.ib, C, L, 1, 0, h->split3 ? static_cast<char*>(sT) + h->lo_off : nullptr, h->raw16};
+  typename E::Params e7{c7.bias, nullptr, nullptr, sT, act_a(s2), act_ib(s2), C, L, 1, 0, h->split3 ? static_cast<char*>(sT) + h->lo_off : nullptr, h->raw16};
   SATB_PROPAGATE((run_conv_gemm<E, BF16>(h, c7, sA, B, L, 0, dil, 1, e7, st)));
   SATB_PROPAGATE((run_conv_gemm<E, BF16>(h, c1, sT, B, L, 0, 1, 1, e1, st)));
   return 0;
@@ -430,8 +520,8 @@ void* lo_half(const SatbOobleck* h, void* p16) { return h->split3 ? static_cast<
 // satb_oobleck_probe runs one of them on caller-owned buffers.  Blocks b = 1 .. n, units j = 0 .. 2.
 
 // Decoder input: latents z NCL fp32 [B, latent_dim, L] -> channels-last 16-bit in tmp16 -> conv k7 latent -> chans[n],
-// whose epilogue applies block 1's leading Snake, into out16.
-template <bool BF16>
+// whose epilogue applies block 1's leading activation, into out16.
+template <bool BF16, int ACT>
 int dec_input(SatbOobleck* h, const float* z, void* tmp16, void* out16, int B, int L, cudaStream_t st) {
   const SatbOobleckConfig& c = h->cfg;
   {
@@ -440,45 +530,49 @@ int dec_input(SatbOobleck* h, const float* z, void* tmp16, void* out16, int B, i
                                                     static_cast<uint16_t*>(lo_half(h, tmp16)), c.latent_dim, L);
     count_launch();
   }
+  typedef EpiConvFor<BF16, false, ACT> E;
   const ConvW& c0 = h->convs.at("layers.0.");
-  const SnakeW& sn = h->snakes.at("layers.1.layers.0.");
-  typename EpiConv<BF16>::Params ep{c0.bias, nullptr, nullptr, out16, sn.a, sn.ib, c0.cout, L, 1, 0, lo_half(h, out16), h->raw16};
+  const SnakeW* sn = act_params(h, "layers.1.layers.0.");
+  typename E::Params ep{c0.bias, nullptr, nullptr, out16, act_a(sn), act_ib(sn), c0.cout, L, 1, 0, lo_half(h, out16), h->raw16};
   h->wrote_raw = false;
-  return run_conv_gemm<EpiConv<BF16>, BF16>(h, c0, tmp16, B, L, 0, 1, 1, ep, st);
+  return run_conv_gemm<E, BF16>(h, c0, tmp16, B, L, 0, 1, 1, ep, st);
 }
 
-// Decoder block b: transposed conv of in16 [B, L_in, chans[n-b+1]] -> raw and snake(unit 0) into out16, both
-// [B, L_in * stride, chans[n-b]].
-template <bool BF16>
+// Decoder block b: transposed conv (or nearest upsample + conv, folded to 3 taps) of in16 [B, L_in, chans[n-b+1]] ->
+// raw and act(unit 0) into out16, both [B, L_in * stride, chans[n-b]].
+template <bool BF16, int ACT>
 int dec_upsample(SatbOobleck* h, int b, const void* in16, void* raw, void* out16, int B, int L_in, cudaStream_t st) {
   const int n = h->cfg.n_stages, cout = h->chans[n - b], s = h->cfg.strides[n - b];
   const std::string bp = "layers." + std::to_string(b) + ".";
-  const ConvW& ct = h->convs.at(bp + "layers.1.");
-  const SnakeW& s_ru0 = h->snakes.at(bp + "layers.2.layers.0.");
+  const ConvW& ct = h->convs.at(bp + (h->nearest ? "layers.1.1." : "layers.1."));
+  const SnakeW* s_ru0 = act_params(h, bp + "layers.2.layers.0.");
   const int64_t Lo = static_cast<int64_t>(L_in) * s;
   SATB_REQUIRE(Lo < (int64_t(1) << 31) && static_cast<int64_t>(B) * Lo * cout < (int64_t(1) << 40), "decoder: sequence too long");
-  typename EpiConv<BF16>::Params et{ct.bias, nullptr, raw, out16, s_ru0.a, s_ru0.ib, cout, static_cast<int>(Lo), s, (s + 1) / 2, lo_half(h, out16), h->raw16};
+  typedef EpiConvFor<BF16, false, ACT> E;
+  // nearest: output position s m + ph is row m, column ph * cout + co (no padding to drop, no bias)
+  typename E::Params et{ct.bias, nullptr, raw, out16, act_a(s_ru0), act_ib(s_ru0), cout, static_cast<int>(Lo), s,
+                        h->nearest ? 0 : (s + 1) / 2, lo_half(h, out16), h->raw16};
   h->wrote_raw = true;
-  return run_conv_gemm<EpiConv<BF16>, BF16>(h, ct, in16, B, L_in, 1, 1, s, et, st);
+  return run_conv_gemm<E, BF16>(h, ct, in16, B, L_in, h->nearest ? 3 : 1, 1, s, et, st);
 }
 
-// Decoder ResidualUnit j of block b over [B, L, chans[n-b]]; the Snake applied to its output is the next unit's, then
-// the next block's, then the final one.
-template <bool BF16>
+// Decoder ResidualUnit j of block b over [B, L, chans[n-b]]; the activation applied to its output is the next unit's,
+// then the next block's, then the final one.
+template <bool BF16, int ACT>
 int dec_residual(SatbOobleck* h, int b, int j, int B, int L, void* raw, void*& sA, void*& sT, cudaStream_t st) {
   static const int dils[3] = {1, 3, 9};
   const int n = h->cfg.n_stages;
   const std::string bp = "layers." + std::to_string(b) + ".";
   const SnakeW* next;
   if (j < 2)
-    next = &h->snakes.at(bp + "layers." + std::to_string(3 + j) + ".layers.0.");
+    next = act_params(h, bp + "layers." + std::to_string(3 + j) + ".layers.0.");
   else if (b < n)
-    next = &h->snakes.at("layers." + std::to_string(b + 1) + ".layers.0.");
+    next = act_params(h, "layers." + std::to_string(b + 1) + ".layers.0.");
   else
-    next = &h->snakes.at("layers." + std::to_string(n + 1) + ".");
+    next = act_params(h, "layers." + std::to_string(n + 1) + ".");
   h->wrote_raw = j < 2;   // the last unit's raw output has no reader: the next step is a transposed or final conv
-  return residual_unit<BF16>(h, bp + "layers." + std::to_string(2 + j) + ".", h->chans[n - b], B, L, dils[j], raw, sA, sT,
-                             next, j < 2, st);
+  return residual_unit<BF16, ACT>(h, bp + "layers." + std::to_string(2 + j) + ".", h->chans[n - b], B, L, dils[j], raw,
+                                  sA, sT, next, j < 2, st);
 }
 
 // Decoder final conv k7 chans[0] -> audio channels (no bias, optional tanh) of in16 [B, L, chans[0]] into audio NCL.
@@ -501,49 +595,51 @@ int dec_output(SatbOobleck* h, const void* in16, float* audio, int B, int L, cud
   return run_conv_gemm<EpiStoreNCL, BF16>(h, cf, in16, B, L, 0, 1, 1, ep, st);
 }
 
-// Encoder input conv k7 audio NCL [B, in_channels, T] -> chans[0] on CUDA cores: raw, and block 1 / unit 0's Snake
-// into out16.
-template <bool BF16>
+// Encoder input conv k7 audio NCL [B, in_channels, T] -> chans[0] on CUDA cores: raw, and block 1 / unit 0's
+// activation into out16.
+template <bool BF16, int ACT>
 int enc_input(SatbOobleck* h, const float* audio, void* raw, void* out16, int B, int64_t T, cudaStream_t st) {
   const ConvW& c0 = h->convs.at("layers.0.");
-  const SnakeW& sn = h->snakes.at("layers.1.layers.0.layers.0.");
+  const SnakeW* sn = act_params(h, "layers.1.layers.0.layers.0.");
   SATB_REQUIRE(c0.cin * c0.k <= 16, "encoder input conv: in_channels * kernel must be <= 16");
   const size_t smem = static_cast<size_t>(c0.cin) * (64 + c0.k - 1) * 4;
   dim3 grid(static_cast<unsigned>(ceil_div64(T, 64)), B);
-  conv_in_kernel<BF16><<<grid, 256, smem, st>>>(audio, c0.w32, c0.bias, sn.a, sn.ib, raw, static_cast<uint16_t*>(out16),
-                                                 static_cast<uint16_t*>(lo_half(h, out16)), c0.cin, c0.cout, T, c0.k,
-                                                 h->raw16);
+  conv_in_kernel<BF16, ACT><<<grid, 256, smem, st>>>(audio, c0.w32, c0.bias, act_a(sn), act_ib(sn), raw,
+                                                      static_cast<uint16_t*>(out16),
+                                                      static_cast<uint16_t*>(lo_half(h, out16)), c0.cin, c0.cout, T, c0.k,
+                                                      h->raw16);
   count_launch();
   h->routes |= SATB_OOB_ROUTE_CUDA_CORE;
   h->wrote_raw = true;
   return 0;
 }
 
-// Encoder ResidualUnit j of block b over [B, L, chans[b-1]]; the Snake applied to its output is the next unit's, then
-// the block's own before its strided conv.
-template <bool BF16>
+// Encoder ResidualUnit j of block b over [B, L, chans[b-1]]; the activation applied to its output is the next unit's,
+// then the block's own before its strided conv.
+template <bool BF16, int ACT>
 int enc_residual(SatbOobleck* h, int b, int j, int B, int L, void* raw, void*& sA, void*& sT, cudaStream_t st) {
   static const int dils[3] = {1, 3, 9};
   const std::string bp = "layers." + std::to_string(b) + ".";
-  const SnakeW* next = j < 2 ? &h->snakes.at(bp + "layers." + std::to_string(j + 1) + ".layers.0.")
-                             : &h->snakes.at(bp + "layers.3.");
+  const SnakeW* next = j < 2 ? act_params(h, bp + "layers." + std::to_string(j + 1) + ".layers.0.")
+                             : act_params(h, bp + "layers.3.");
   h->wrote_raw = j < 2;   // the strided conv that follows the last unit has no skip
-  return residual_unit<BF16>(h, bp + "layers." + std::to_string(j) + ".", h->chans[b - 1], B, L, dils[j], raw, sA, sT,
-                             next, j < 2, st);
+  return residual_unit<BF16, ACT>(h, bp + "layers." + std::to_string(j) + ".", h->chans[b - 1], B, L, dils[j], raw, sA,
+                                  sT, next, j < 2, st);
 }
 
-// Encoder block b: strided conv of in16 [B, L_in, chans[b-1]] (already Snake-activated) -> [B, L_in / s, chans[b]]:
-// raw (when a next block reads it as its first skip) and the next block's (or the final) Snake into out16.
-template <bool BF16>
+// Encoder block b: strided conv of in16 [B, L_in, chans[b-1]] (already activated) -> [B, L_in / s, chans[b]]:
+// raw (when a next block reads it as its first skip) and the next block's (or the final) activation into out16.
+template <bool BF16, int ACT>
 int enc_downsample(SatbOobleck* h, int b, const void* in16, void* raw, void* out16, int B, int L_in, cudaStream_t st) {
   const int n = h->cfg.n_stages, s = h->cfg.strides[b - 1];
   const ConvW& cs = h->convs.at("layers." + std::to_string(b) + ".layers.4.");
   const int Lo = L_in / s;
-  const SnakeW* nx = b < n ? &h->snakes.at("layers." + std::to_string(b + 1) + ".layers.0.layers.0.")
-                           : &h->snakes.at("layers." + std::to_string(n + 1) + ".");
-  typename EpiConv<BF16>::Params ep{cs.bias, nullptr, b < n ? raw : nullptr, out16, nx->a, nx->ib, cs.cout, Lo, 1, 0, lo_half(h, out16), h->raw16};
+  const SnakeW* nx = b < n ? act_params(h, "layers." + std::to_string(b + 1) + ".layers.0.layers.0.")
+                           : act_params(h, "layers." + std::to_string(n + 1) + ".");
+  typedef EpiConvFor<BF16, false, ACT> E;
+  typename E::Params ep{cs.bias, nullptr, b < n ? raw : nullptr, out16, act_a(nx), act_ib(nx), cs.cout, Lo, 1, 0, lo_half(h, out16), h->raw16};
   h->wrote_raw = b < n;
-  return run_conv_gemm<EpiConv<BF16>, BF16>(h, cs, in16, B, L_in, 2, 1, s, ep, st);
+  return run_conv_gemm<E, BF16>(h, cs, in16, B, L_in, 2, 1, s, ep, st);
 }
 
 // Encoder final conv k3 chans[n] -> latent_dim of in16 [B, L, chans[n]], NCL fp32 output
@@ -555,7 +651,7 @@ int enc_output(SatbOobleck* h, const void* in16, float* latents, int B, int L, c
   return run_conv_gemm<EpiStoreNCL, BF16>(h, cf, in16, B, L, 0, 1, 1, ep, st);
 }
 
-template <bool BF16>
+template <bool BF16, int ACT>
 int decode_impl(SatbOobleck* h, const float* z, float* audio, int B, int L, cudaStream_t st) {
   const SatbOobleckConfig& c = h->cfg;
   const int n = c.n_stages;
@@ -576,21 +672,21 @@ int decode_impl(SatbOobleck* h, const float* z, float* audio, int B, int L, cuda
   void* raw = h->buf_raw;
   void* sA = h->buf_a;
   void* sB = h->buf_b;
-  SATB_PROPAGATE(dec_input<BF16>(h, z, sB, sA, B, L, st));
+  SATB_PROPAGATE((dec_input<BF16, ACT>(h, z, sB, sA, B, L, st)));
   int64_t Lc = L;
   for (int b = 1; b <= n; ++b) {
     // transposed conv reads sA [B, Lc, cin], writes raw + snake(ru0) into sB
-    SATB_PROPAGATE(dec_upsample<BF16>(h, b, sA, raw, sB, B, static_cast<int>(Lc), st));
+    SATB_PROPAGATE((dec_upsample<BF16, ACT>(h, b, sA, raw, sB, B, static_cast<int>(Lc), st)));
     std::swap(sA, sB);  // sA now holds the residual units' input
     Lc *= c.strides[n - b];
-    for (int j = 0; j < 3; ++j) SATB_PROPAGATE(dec_residual<BF16>(h, b, j, B, static_cast<int>(Lc), raw, sA, sB, st));
+    for (int j = 0; j < 3; ++j) SATB_PROPAGATE((dec_residual<BF16, ACT>(h, b, j, B, static_cast<int>(Lc), raw, sA, sB, st)));
   }
   SATB_PROPAGATE(dec_output<BF16>(h, sA, audio, B, static_cast<int>(Lc), st));
   SATB_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
 
-template <bool BF16>
+template <bool BF16, int ACT>
 int encode_impl(SatbOobleck* h, const float* audio, float* latents, int B, int64_t T, cudaStream_t st) {
   const SatbOobleckConfig& c = h->cfg;
   const int n = c.n_stages;
@@ -613,12 +709,12 @@ int encode_impl(SatbOobleck* h, const float* audio, float* latents, int B, int64
   void* raw = h->buf_raw;
   void* sA = h->buf_a;
   void* sB = h->buf_b;
-  SATB_PROPAGATE(enc_input<BF16>(h, audio, raw, sA, B, T, st));
+  SATB_PROPAGATE((enc_input<BF16, ACT>(h, audio, raw, sA, B, T, st)));
   int64_t Lc = T;
   for (int b = 1; b <= n; ++b) {
-    for (int j = 0; j < 3; ++j) SATB_PROPAGATE(enc_residual<BF16>(h, b, j, B, static_cast<int>(Lc), raw, sA, sB, st));
+    for (int j = 0; j < 3; ++j) SATB_PROPAGATE((enc_residual<BF16, ACT>(h, b, j, B, static_cast<int>(Lc), raw, sA, sB, st)));
     // strided conv reads sA [B, Lc, cin] -> [B, Lc/s, cout] in sB
-    SATB_PROPAGATE(enc_downsample<BF16>(h, b, sA, raw, sB, B, static_cast<int>(Lc), st));
+    SATB_PROPAGATE((enc_downsample<BF16, ACT>(h, b, sA, raw, sB, B, static_cast<int>(Lc), st)));
     std::swap(sA, sB);
     Lc /= c.strides[b - 1];
   }
@@ -627,7 +723,7 @@ int encode_impl(SatbOobleck* h, const float* audio, float* latents, int B, int64
 }
 
 // One step on caller-owned buffers (satb_oobleck_probe).
-template <bool BF16>
+template <bool BF16, int ACT>
 int probe_impl(SatbOobleck* h, SatbOobleckProbe* p, cudaStream_t st) {
   const int b = p->block, j = p->unit, B = p->B, L = p->L;
   if (p->step == SATB_OOB_DEC_RES || p->step == SATB_OOB_ENC_RES) {
@@ -638,19 +734,32 @@ int probe_impl(SatbOobleck* h, SatbOobleckProbe* p, cudaStream_t st) {
                                       cudaMemcpyDeviceToDevice, st));
     void* sA = p->in;
     void* sT = p->scratch;
-    SATB_PROPAGATE(dec ? dec_residual<BF16>(h, b, j, B, L, p->raw_out, sA, sT, st)
-                       : enc_residual<BF16>(h, b, j, B, L, p->raw_out, sA, sT, st));
+    SATB_PROPAGATE((dec ? dec_residual<BF16, ACT>(h, b, j, B, L, p->raw_out, sA, sT, st)
+                       : enc_residual<BF16, ACT>(h, b, j, B, L, p->raw_out, sA, sT, st)));
     p->result_in_scratch = sA == p->scratch;
     return 0;
   }
   switch (p->step) {
-    case SATB_OOB_DEC_IN: return dec_input<BF16>(h, static_cast<const float*>(p->in), p->scratch, p->out16, B, L, st);
-    case SATB_OOB_DEC_UP: return dec_upsample<BF16>(h, b, p->in, p->raw_out, p->out16, B, L, st);
+    case SATB_OOB_DEC_IN: return dec_input<BF16, ACT>(h, static_cast<const float*>(p->in), p->scratch, p->out16, B, L, st);
+    case SATB_OOB_DEC_UP: return dec_upsample<BF16, ACT>(h, b, p->in, p->raw_out, p->out16, B, L, st);
     case SATB_OOB_DEC_OUT: return dec_output<BF16>(h, p->in, p->out32, B, L, st);
-    case SATB_OOB_ENC_IN: return enc_input<BF16>(h, static_cast<const float*>(p->in), p->raw_out, p->out16, B, L, st);
-    case SATB_OOB_ENC_DOWN: return enc_downsample<BF16>(h, b, p->in, p->raw_out, p->out16, B, L, st);
+    case SATB_OOB_ENC_IN: return enc_input<BF16, ACT>(h, static_cast<const float*>(p->in), p->raw_out, p->out16, B, L, st);
+    case SATB_OOB_ENC_DOWN: return enc_downsample<BF16, ACT>(h, b, p->in, p->raw_out, p->out16, B, L, st);
     default: return enc_output<BF16>(h, p->in, p->out32, B, L, st);
   }
+}
+
+template <int ACT>
+int decode_act(SatbOobleck* h, const float* z, float* audio, int B, int L, cudaStream_t st) {
+  return h->bf16 ? decode_impl<true, ACT>(h, z, audio, B, L, st) : decode_impl<false, ACT>(h, z, audio, B, L, st);
+}
+template <int ACT>
+int encode_act(SatbOobleck* h, const float* audio, float* latents, int B, int64_t T, cudaStream_t st) {
+  return h->bf16 ? encode_impl<true, ACT>(h, audio, latents, B, T, st) : encode_impl<false, ACT>(h, audio, latents, B, T, st);
+}
+template <int ACT>
+int probe_act(SatbOobleck* h, SatbOobleckProbe* p, cudaStream_t st) {
+  return h->bf16 ? probe_impl<true, ACT>(h, p, st) : probe_impl<false, ACT>(h, p, st);
 }
 
 }  // namespace
@@ -658,17 +767,37 @@ int probe_impl(SatbOobleck* h, SatbOobleckProbe* p, cudaStream_t st) {
 extern "C" {
 
 int satb_oobleck_create(const SatbOobleckConfig* cfg, SatbOobleck** out) {
+  return satb_oobleck_create_variant(cfg, SATB_OOB_ACT_SNAKE, 0, out);
+}
+
+int satb_oobleck_create_variant(const SatbOobleckConfig* cfg, int activation, int nearest_upsample, SatbOobleck** out) {
   SATB_REQUIRE(cfg && out, "null argument");
   SATB_REQUIRE(cfg->n_stages >= 1 && cfg->n_stages <= SATB_MAX_STAGES, "bad number of stages");
   SATB_REQUIRE(cfg->channels % 32 == 0, "channels must be a multiple of 32");
   SATB_REQUIRE(cfg->latent_dim % 8 == 0, "latent_dim must be a multiple of 8");
   SATB_REQUIRE(cfg->in_channels >= 1 && cfg->in_channels <= 2, "audio channels must be 1 or 2");
+  if (activation != SATB_OOB_ACT_SNAKE && activation != SATB_OOB_ACT_ELU) {
+    set_last_error("oobleck: unknown activation " + std::to_string(activation) + "; accepted: 0 (snake), 1 (elu)");
+    return -1;
+  }
+  if (nearest_upsample != 0 && nearest_upsample != 1) {
+    set_last_error("oobleck: nearest_upsample must be 0 or 1, got " + std::to_string(nearest_upsample));
+    return -1;
+  }
+  SATB_REQUIRE(!nearest_upsample || cfg->is_decoder,
+               "oobleck: nearest_upsample applies to a decoder only (an encoder has no upsampling)");
   // A block's conv has kernel 2s, stride s, padding ceil(s/2) (models/autoencoders.py:75,86).  Its output length is
   // L * s (decoder) and L / s (encoder) only for an even decoder stride and an encoder stride >= 2: an odd decoder
-  // stride gives L * s - 1, encoder stride 1 gives L + 1.
+  // stride gives L * s - 1, encoder stride 1 gives L + 1.  Nearest upsampling followed by a 'same' conv gives L * s
+  // for every s.
   for (int i = 0; i < cfg->n_stages; ++i) {
     const int s = cfg->strides[i];
-    if (cfg->is_decoder ? (s < 2 || s % 2 != 0) : s < 2) {
+    if (cfg->is_decoder && nearest_upsample) {
+      if (s < 2) {
+        set_last_error("decoder: stride " + std::to_string(s) + " is not supported: nearest upsampling needs strides >= 2");
+        return -1;
+      }
+    } else if (cfg->is_decoder ? (s < 2 || s % 2 != 0) : s < 2) {
       set_last_error(std::string(cfg->is_decoder ? "decoder" : "encoder") + ": stride " + std::to_string(s) +
                      " is not supported: " +
                      (cfg->is_decoder ? "strides must be even (a transposed conv with kernel 2s, padding ceil(s/2) "
@@ -680,6 +809,8 @@ int satb_oobleck_create(const SatbOobleckConfig* cfg, SatbOobleck** out) {
   }
   SatbOobleck* h = new SatbOobleck();
   h->cfg = *cfg;
+  h->act = activation == SATB_OOB_ACT_ELU ? kActElu : kActSnake;
+  h->nearest = nearest_upsample != 0;
   h->bf16 = cfg->operand_dtype == 1;
   h->split3 = cfg->operand_dtype == 2;
   // fp16 operands: the un-activated skip stream is carried in fp16 as well (8 instead of 12 bytes per element and
@@ -746,7 +877,10 @@ int satb_oobleck_finalize(SatbOobleck* h, void* stream) {
       const int cin = h->chans[n - b + 1], cout = h->chans[n - b], s = c.strides[n - b];
       const std::string bp = "layers." + std::to_string(b) + ".";
       SATB_PROPAGATE(prep_snake(h, bp + "layers.0.", cin, st));
-      SATB_PROPAGATE(prep_conv(h, bp + "layers.1.", cin, cout, 2 * s, true, false, true, s, st));
+      if (h->nearest)
+        SATB_PROPAGATE(prep_conv_nearest(h, bp + "layers.1.1.", cin, cout, s, st));
+      else
+        SATB_PROPAGATE(prep_conv(h, bp + "layers.1.", cin, cout, 2 * s, true, false, true, s, st));
       for (int j = 0; j < 3; ++j) SATB_PROPAGATE(res_unit(bp + "layers." + std::to_string(2 + j) + ".", cout));
     }
     SATB_PROPAGATE(prep_snake(h, "layers." + std::to_string(n + 1) + ".", h->chans[0], st));
@@ -774,7 +908,7 @@ int satb_oobleck_decode(SatbOobleck* h, const float* z, float* audio, int B, int
   SATB_REQUIRE(h->cfg.is_decoder, "oobleck: handle is an encoder");
   SATB_REQUIRE(z && audio && B >= 1 && L >= 1, "bad argument");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  return h->bf16 ? decode_impl<true>(h, z, audio, B, L, st) : decode_impl<false>(h, z, audio, B, L, st);
+  return h->act == kActElu ? decode_act<kActElu>(h, z, audio, B, L, st) : decode_act<kActSnake>(h, z, audio, B, L, st);
 }
 
 int satb_oobleck_encode(SatbOobleck* h, const float* audio, float* latents, int B, long long T, void* stream) {
@@ -782,7 +916,8 @@ int satb_oobleck_encode(SatbOobleck* h, const float* audio, float* latents, int 
   SATB_REQUIRE(!h->cfg.is_decoder, "oobleck: handle is a decoder");
   SATB_REQUIRE(audio && latents && B >= 1 && T >= 1, "bad argument");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  return h->bf16 ? encode_impl<true>(h, audio, latents, B, T, st) : encode_impl<false>(h, audio, latents, B, T, st);
+  return h->act == kActElu ? encode_act<kActElu>(h, audio, latents, B, T, st)
+                           : encode_act<kActSnake>(h, audio, latents, B, T, st);
 }
 
 int satb_oobleck_probe(SatbOobleck* h, SatbOobleckProbe* p, void* stream) {
@@ -832,7 +967,7 @@ int satb_oobleck_probe(SatbOobleck* h, SatbOobleckProbe* p, void* stream) {
   h->lo_off = h->split3 ? static_cast<size_t>(p->lo_off) : 0;
   h->routes = 0;
   p->result_in_scratch = 0;
-  const int rc = h->bf16 ? probe_impl<true>(h, p, st) : probe_impl<false>(h, p, st);
+  const int rc = h->act == kActElu ? probe_act<kActElu>(h, p, st) : probe_act<kActSnake>(h, p, st);
   p->wrote_raw = h->wrote_raw ? 1 : 0;
   p->routes = static_cast<int>(h->routes);
   SATB_PROPAGATE(rc);
@@ -848,7 +983,7 @@ int satb_oobleck_weights(SatbOobleck* h, const char* prefix, void* dst, long lon
     return -1;
   }
   const ConvW& c = it->second;
-  const size_t total = static_cast<size_t>(c.cin) * c.cout * c.k;
+  const size_t total = conv_w_elems(c);
   const size_t n = c.small ? total * 4 : total * 2 * (h->split3 ? 2 : 1);
   *bytes = static_cast<long long>(n);
   if (dst) {

@@ -63,6 +63,8 @@ class SatbAttentionProbe(ctypes.Structure):
 # satb_oobleck_probe / satb_oobleck_weights (tests only): steps, route bits and the parameter block of include/satb200.h
 OOB_DEC_IN, OOB_DEC_UP, OOB_DEC_RES, OOB_DEC_OUT, OOB_ENC_IN, OOB_ENC_RES, OOB_ENC_DOWN, OOB_ENC_OUT = range(8)
 OOB_ROUTES = {1: "gemm", 2: "gemm_lean", 4: "fused", 8: "fused_lean", 16: "halo_ncl", 32: "gemm_ncl", 64: "cuda_core"}
+# satb_oobleck_create_variant: the blocks' activation
+OOB_ACT_SNAKE, OOB_ACT_ELU = 0, 1
 
 
 class SatbOobleckProbe(ctypes.Structure):
@@ -101,6 +103,7 @@ SIGNATURES = {
     "satb_attention_probe": (_I, [ctypes.POINTER(SatbAttentionProbe), _VP]),
     "satb_conformer_dwconv": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _VP]),
     "satb_oobleck_create": (_I, [ctypes.POINTER(SatbOobleckConfig), ctypes.POINTER(_VP)]),
+    "satb_oobleck_create_variant": (_I, [ctypes.POINTER(SatbOobleckConfig), _I, _I, ctypes.POINTER(_VP)]),
     "satb_oobleck_destroy": (None, [_VP]),
     "satb_oobleck_load_weight": (_I, [_VP, ctypes.c_char_p, _VP, _LL, _VP]),
     "satb_oobleck_finalize": (_I, [_VP, _VP]),

@@ -8,8 +8,11 @@ decode with ``iterate_batch`` micro-batching, chunked ``encode_audio`` / ``decod
 ``reconstruct_audio`` with Bartlett cross-fades) and the config factories (:693-787).
 
 The encoder / decoder ``forward`` run in ``libsatb200.so`` (``satb_oobleck_*``): wgmma
-implicit-GEMM convolutions with Snake fused into the producing epilogue.  The inner blocks
-are parameter containers.  The chunking / cross-fade orchestration is host-side tensor
+implicit-GEMM convolutions with the activation (SnakeBeta for ``use_snake=True``, ELU otherwise)
+fused into the producing epilogue.  Decoders upsample by transposed convolution or, with
+``use_nearest_upsample=True``, by nearest-neighbour repetition + a 'same' convolution.  The
+inner blocks are parameter containers.  ``antialias_activation=True`` is refused: it needs
+``alias_free_torch``, which this package does not ship.  The chunking / cross-fade orchestration is host-side tensor
 slicing on the device, exactly as in the reference.
 """
 import ctypes
@@ -37,14 +40,24 @@ def WNConvTranspose1d(*args, **kwargs):
     return weight_norm(nn.ConvTranspose1d(*args, **kwargs))
 
 
+_ANTIALIAS_REFUSAL = ("antialias_activation=True is not supported: the anti-aliased activation (alias_free_torch's "
+                      "Activation1d) needs the alias_free_torch package, which this package does not ship")
+
+
 def get_activation(activation: str, antialias=False, channels=None) -> nn.Module:
     if antialias:
-        raise NotImplementedError("anti-aliased activations are outside the native hot path")
+        raise NotImplementedError(_ANTIALIAS_REFUSAL)
     if activation == "snake":
         return SnakeBeta(channels)
+    if activation == "elu":
+        return nn.ELU()
     if activation == "none":
         return nn.Identity()
-    raise NotImplementedError(f"activation '{activation}' is outside the native hot path (use_snake=True only)")
+    raise ValueError(f"Unknown activation {activation}")
+
+
+def _act(use_snake):
+    return "snake" if use_snake else "elu"
 
 
 class _Container(_FusedModule):
@@ -54,13 +67,11 @@ class _Container(_FusedModule):
 class ResidualUnit(_Container):
     def __init__(self, in_channels, out_channels, dilation, use_snake=False, antialias_activation=False):
         super().__init__()
-        if not use_snake:
-            raise NotImplementedError("only use_snake=True is on the native hot path")
         self.dilation = dilation
         self.layers = nn.Sequential(
-            get_activation("snake", antialias=antialias_activation, channels=out_channels),
+            get_activation(_act(use_snake), antialias=antialias_activation, channels=out_channels),
             WNConv1d(in_channels, out_channels, kernel_size=7, dilation=dilation, padding=(dilation * 6) // 2),
-            get_activation("snake", antialias=antialias_activation, channels=out_channels),
+            get_activation(_act(use_snake), antialias=antialias_activation, channels=out_channels),
             WNConv1d(out_channels, out_channels, kernel_size=1))
 
 
@@ -71,7 +82,7 @@ class EncoderBlock(_Container):
             ResidualUnit(in_channels, in_channels, 1, use_snake=use_snake),
             ResidualUnit(in_channels, in_channels, 3, use_snake=use_snake),
             ResidualUnit(in_channels, in_channels, 9, use_snake=use_snake),
-            get_activation("snake" if use_snake else "elu", antialias=antialias_activation, channels=in_channels),
+            get_activation(_act(use_snake), antialias=antialias_activation, channels=in_channels),
             WNConv1d(in_channels, out_channels, kernel_size=2 * stride, stride=stride, padding=math.ceil(stride / 2)))
 
 
@@ -80,22 +91,31 @@ class DecoderBlock(_Container):
                  use_nearest_upsample=False):
         super().__init__()
         if use_nearest_upsample:
-            raise NotImplementedError("nearest-neighbour upsampling is outside the native hot path")
+            # reference :95-100; the native decoder folds the pair into one 3-tap convolution of the low-rate input
+            upsample = nn.Sequential(
+                nn.Upsample(scale_factor=stride, mode="nearest"),
+                WNConv1d(in_channels, out_channels, kernel_size=2 * stride, stride=1, bias=False, padding="same"))
+        else:
+            upsample = WNConvTranspose1d(in_channels, out_channels, kernel_size=2 * stride, stride=stride,
+                                         padding=math.ceil(stride / 2))
         self.layers = nn.Sequential(
-            get_activation("snake" if use_snake else "elu", antialias=antialias_activation, channels=in_channels),
-            WNConvTranspose1d(in_channels, out_channels, kernel_size=2 * stride, stride=stride,
-                              padding=math.ceil(stride / 2)),
+            get_activation(_act(use_snake), antialias=antialias_activation, channels=in_channels),
+            upsample,
             ResidualUnit(out_channels, out_channels, 1, use_snake=use_snake),
             ResidualUnit(out_channels, out_channels, 3, use_snake=use_snake),
             ResidualUnit(out_channels, out_channels, 9, use_snake=use_snake))
 
 
-def _check_strides(strides, decoder):
+def _check_strides(strides, decoder, nearest=False):
     """A block's conv has kernel 2s, stride s, padding ceil(s/2) (reference :75,86).  Its output has L * s (decoder) or
     L / s (encoder) positions, which forward allocates, only for an even decoder stride and an encoder stride >= 2:
-    an odd decoder stride gives L * s - 1, encoder stride 1 gives L + 1."""
+    an odd decoder stride gives L * s - 1, encoder stride 1 gives L + 1.  A nearest-upsampling decoder block (nearest
+    x s, then a 'same' conv) gives L * s for every s >= 2."""
     for s in strides:
-        if decoder and (s < 2 or s % 2):
+        if decoder and nearest and s < 2:
+            raise NotImplementedError(f"OobleckDecoder: stride {s} is not supported: nearest upsampling needs strides "
+                                      ">= 2")
+        if decoder and not nearest and (s < 2 or s % 2):
             raise NotImplementedError(f"OobleckDecoder: stride {s} is not supported: strides must be even (a transposed "
                                       "conv with kernel 2s, padding ceil(s/2) gives L * s positions only for even s)")
         if not decoder and s < 2:
@@ -108,12 +128,14 @@ class _NativeOobleck(nn.Module):
 
     _is_decoder = False
 
-    def _init_native(self, audio_channels, channels, latent_dim, c_mults, strides, final_tanh, operand_dtype):
+    def _init_native(self, audio_channels, channels, latent_dim, c_mults, strides, final_tanh, operand_dtype,
+                     use_snake=True, use_nearest_upsample=False):
         self.__dict__["_h"] = None
         self.__dict__["_dirty"] = True
         self.__dict__["_ncfg"] = dict(audio_channels=audio_channels, channels=channels, latent_dim=latent_dim,
                                       c_mults=list(c_mults), strides=list(strides), final_tanh=bool(final_tanh),
-                                      operand_dtype=operand_dtype)
+                                      operand_dtype=operand_dtype, use_snake=bool(use_snake),
+                                      use_nearest_upsample=bool(use_nearest_upsample))
         # also fires when a parent module's load_state_dict recurses into this one (see models/dit.py)
         self.register_load_state_dict_post_hook(lambda module, incompatible: module.refresh_native_weights())
 
@@ -150,7 +172,9 @@ class _NativeOobleck(nn.Module):
                 raise ValueError(f"operand_dtype must be fp16, bf16 or fp16x3, got {nc['operand_dtype']}")
             cfg.operand_dtype = {"fp16": 0, "bf16": 1, "fp16x3": 2}[nc["operand_dtype"]]
             h = ctypes.c_void_p()
-            _native.check(lib.satb_oobleck_create(ctypes.byref(cfg), ctypes.byref(h)))
+            act = _native.OOB_ACT_SNAKE if nc["use_snake"] else _native.OOB_ACT_ELU
+            _native.check(lib.satb_oobleck_create_variant(ctypes.byref(cfg), act, int(nc["use_nearest_upsample"]),
+                                                          ctypes.byref(h)))
             self.__dict__["_h"] = h
         if self.__dict__["_dirty"]:
             st = _native.stream_ptr(device)
@@ -173,16 +197,16 @@ class OobleckEncoder(_NativeOobleck):
     def __init__(self, in_channels=2, channels=128, latent_dim=32, c_mults=[1, 2, 4, 8], strides=[2, 4, 8, 8],
                  use_snake=False, antialias_activation=False, operand_dtype="fp16"):
         super().__init__()
-        if not use_snake or antialias_activation:
-            raise NotImplementedError("only use_snake=True without anti-aliasing is on the native hot path")
+        if antialias_activation:
+            raise NotImplementedError(_ANTIALIAS_REFUSAL)
         _check_strides(strides, decoder=False)
-        self._init_native(in_channels, channels, latent_dim, c_mults, strides, False, operand_dtype)
+        self._init_native(in_channels, channels, latent_dim, c_mults, strides, False, operand_dtype, use_snake=use_snake)
         cm = [1] + list(c_mults)
         self.depth = len(cm)
         layers = [WNConv1d(in_channels, cm[0] * channels, kernel_size=7, padding=3)]
         for i in range(self.depth - 1):
             layers.append(EncoderBlock(cm[i] * channels, cm[i + 1] * channels, strides[i], use_snake=use_snake))
-        layers += [get_activation("snake", channels=cm[-1] * channels),
+        layers += [get_activation(_act(use_snake), channels=cm[-1] * channels),
                    WNConv1d(cm[-1] * channels, latent_dim, kernel_size=3, padding=1)]
         self.layers = nn.Sequential(*layers)
         self.downsampling_ratio = int(math.prod(strides))
@@ -210,10 +234,11 @@ class OobleckDecoder(_NativeOobleck):
                  use_snake=False, antialias_activation=False, use_nearest_upsample=False, final_tanh=True,
                  operand_dtype="fp16"):
         super().__init__()
-        if not use_snake or antialias_activation:
-            raise NotImplementedError("only use_snake=True without anti-aliasing is on the native hot path")
-        _check_strides(strides, decoder=True)
-        self._init_native(out_channels, channels, latent_dim, c_mults, strides, final_tanh, operand_dtype)
+        if antialias_activation:
+            raise NotImplementedError(_ANTIALIAS_REFUSAL)
+        _check_strides(strides, decoder=True, nearest=use_nearest_upsample)
+        self._init_native(out_channels, channels, latent_dim, c_mults, strides, final_tanh, operand_dtype,
+                          use_snake=use_snake, use_nearest_upsample=use_nearest_upsample)
         cm = [1] + list(c_mults)
         self.depth = len(cm)
         layers = [WNConv1d(latent_dim, cm[-1] * channels, kernel_size=7, padding=3)]
@@ -221,7 +246,7 @@ class OobleckDecoder(_NativeOobleck):
             layers.append(DecoderBlock(cm[i] * channels, cm[i - 1] * channels, strides[i - 1], use_snake=use_snake,
                                        antialias_activation=antialias_activation,
                                        use_nearest_upsample=use_nearest_upsample))
-        layers += [get_activation("snake", channels=cm[0] * channels),
+        layers += [get_activation(_act(use_snake), channels=cm[0] * channels),
                    WNConv1d(cm[0] * channels, out_channels, kernel_size=7, padding=3, bias=False),
                    nn.Tanh() if final_tanh else nn.Identity()]
         self.layers = nn.Sequential(*layers)

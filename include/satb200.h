@@ -210,6 +210,19 @@ int satb_conformer_dwconv(const void* g16, const float* w, const float* gamma, c
 /* ---- Oobleck VAE: replaces OobleckDecoder / OobleckEncoder.forward
  *      (models/autoencoders.py:119-194) behind AudioAutoencoder.encode/decode (:268-343) */
 int satb_oobleck_create(const SatbOobleckConfig* cfg, SatbOobleck** out);
+/* The same for the blocks' other options (models/autoencoders.py:29-116):
+ *   activation        SATB_OOB_ACT_SNAKE (use_snake=True: SnakeBeta, "alpha" / "beta" keys) or SATB_OOB_ACT_ELU
+ *                     (use_snake=False: nn.ELU(), no parameters, so finalize looks up no alpha / beta keys);
+ *   nearest_upsample  1: every decoder block upsamples by nearest-neighbour x s followed by a bias-free weight-normed
+ *                     Conv1d k = 2s, padding 'same' ("layers.{b}.layers.1.1.weight_g / weight_v"; use_nearest_upsample)
+ *                     instead of a ConvTranspose1d.  Any decoder stride >= 2 is accepted, odd ones included.  The conv
+ *                     runs as a 3-tap convolution of the low-rate input; finalize folds its weights (fp64 sums).
+ *                     Refused for an encoder.
+ * Unknown values are refused.  satb_oobleck_create(cfg, out) is satb_oobleck_create_variant(cfg, SNAKE, 0, out).  The
+ * options are fixed for the handle's lifetime: they decide which weights finalize expects. */
+#define SATB_OOB_ACT_SNAKE 0
+#define SATB_OOB_ACT_ELU 1
+int satb_oobleck_create_variant(const SatbOobleckConfig* cfg, int activation, int nearest_upsample, SatbOobleck** out);
 void satb_oobleck_destroy(SatbOobleck* h);
 /* State-dict entry relative to the encoder/decoder module ("layers.1.layers.1.weight_v" ...). */
 int satb_oobleck_load_weight(SatbOobleck* h, const char* name, const float* src, long long numel, void* stream);
