@@ -93,16 +93,40 @@ static int linear(TmapCache& tc, const void* A, int64_t lda, int M, int K, const
 // Picks the N tile (256 or 128) that wastes less of the last wave of the persistent grid; the
 // 128-wide tile streams as many smem bytes per MMA cycle as the tensor pipe can take, so it is
 // only preferred when it clearly wins on wave quantisation.
+static int auto_bn(int m_tiles, int N) {
+  const double sms = device_sm_count();
+  auto eff = [&](int bn) {
+    const double waves = static_cast<double>(m_tiles) * ceil_div(N, bn) / sms;
+    return waves / std::ceil(waves);
+  };
+  return N % 128 == 0 && eff(128) * 0.9 > eff(256) ? 128 : 256;
+}
+
 template <class Epi, bool BF16, bool FP8 = false>
 static int linear_auto(TmapCache& tc, const void* A, int64_t lda, int M, int K, const void* W, int N,
                        const typename Epi::Params& ep, cudaStream_t stream, const Fp8Scales& sc = Fp8Scales{}) {
-  const double sms = device_sm_count();
-  auto eff = [&](int bn) {
-    const double waves = static_cast<double>(ceil_div(M, kBlockM)) * ceil_div(N, bn) / sms;
-    return waves / std::ceil(waves);
-  };
-  if (N % 128 == 0 && eff(128) * 0.9 > eff(256)) return linear<Epi, 128, BF16, FP8>(tc, A, lda, M, K, W, N, ep, stream, 1, sc);
+  if (auto_bn(ceil_div(M, kBlockM), N) == 128) return linear<Epi, 128, BF16, FP8>(tc, A, lda, M, K, W, N, ep, stream, 1, sc);
   return linear<Epi, 256, BF16, FP8>(tc, A, lda, M, K, W, N, ep, stream, 1, sc);
+}
+
+// Convolution over the tokens of every item (FeedForward use_conv, models/transformer.py:262-271, padding k / 2):
+//   C[r * n_seq + l, n] = sum_t sum_c A[r, l + t - k / 2, c] * W[t * N + n, c]
+// on the Linears' GEMM instances (n_taps = k, batches = R).  Rows outside an item's n_seq read as zeros (TMA zero fill),
+// so each item, every CFG row included, is zero-padded at its own ends.  A: 16-bit [R, item_stride rows, K]; W: the
+// tap-major weight [k * N, K]; C rows are dense ([R * n_seq] in the epilogue's row space).  The tiles are per item
+// (ceil(n_seq / 128) m-tiles each).  bn: 0 picks the N tile as linear_auto does, over those m-tiles; else 128 or 256.
+template <class Epi, bool BF16>
+static int token_conv(TmapCache& tc, const void* A, int64_t item_stride, int R, int n_seq, int K, const void* W, int N,
+                      int k, const typename Epi::Params& ep, cudaStream_t stream, int bn = 0) {
+  if (bn == 0) bn = auto_bn(R * ceil_div(n_seq, kBlockM), N);
+  const CUtensorMap *ta, *tb;
+  SATB_PROPAGATE(tc.get_a(A, K, n_seq, R, K, item_stride * K, &ta));
+  GemmShape s;
+  s.L = n_seq; s.batches = R; s.N = N; s.K = K; s.n_taps = k; s.tap_base = -(k / 2); s.tap_step = 1; s.b_tap_rows = N;
+  s.stride = 1; s.b_static = 1;
+  SATB_PROPAGATE(tc.get_b(W, K, k * N, K, bn, &tb));
+  if (bn == 128) return launch_gemm<Epi, 128, BF16>(*ta, *tb, s, ep, stream);
+  return launch_gemm<Epi, 256, BF16>(*ta, *tb, s, ep, stream);
 }
 
 struct LayerW {
@@ -136,6 +160,12 @@ struct SatbDit {
   bool bf16, fp8, adaln, qk_norm = false;   // fp8: e4m3 operands for the QKV, cross q and FF-in GEMMs (fp16 elsewhere)
   bool conformer = false;     // every block runs the conformer branch (satb_dit_set_conformer)
   int* cf_perm = nullptr;     // SwiGLU row interleave of the folded [2D, D] conformer GLU weight
+  // feed-forward (satb_dit_set_feedforward; default: SwiGLU Linear, inner 4D, biased).  ffi above is ff_inner padded up
+  // to a multiple of 64.  ff_k: kernel size of the token convolutions, 0 = Linear (with ff_glu, FF-out only).  ff_bias:
+  // FF-out (and a plain FF-in) carry a bias; the SwiGLU projection always does.
+  int ff_inner = 0, ff_k = 0;
+  bool ff_set = false, ff_glu = true, ff_bias = true;
+  bool ff_conv_in() const { return !ff_glu && ff_k > 0; }
   int P;  // prepended tokens: 1 (the global-conditioning token; 0 in adaLN mode) + Pp
   std::vector<LayerW> layers;
   std::vector<void*> owned;   // every cudaMalloc of weight storage
@@ -239,6 +269,79 @@ static int fold_conformer_glu(SatbDit* d, LayerW& L, cudaStream_t st) {
   return 0;
 }
 
+// Stored fp32 layout of a feed-forward matrix of a satb_dit_set_feedforward variant, built on the host:
+//   W [G * out, in, taps] (a Linear: taps = 1) -> [taps * G * out_p, in_p],  row (t G + g) out_p + n = W[g out + n, :, t]
+// with zero rows and columns in the padding.  G = 2 for the GLU projection: its value and gate halves are padded
+// separately, so the SwiGLU row interleave then applies at out_p.  A Conv1d weight comes out tap-major and K-major.
+static std::vector<float> ff_stored_layout(const std::vector<float>& w, int G, int out, int in, int taps, int out_p,
+                                           int in_p) {
+  std::vector<float> s(static_cast<size_t>(taps) * G * out_p * in_p, 0.f);
+  for (int t = 0; t < taps; ++t)
+    for (int g = 0; g < G; ++g)
+      for (int n = 0; n < out; ++n) {
+        float* dst = s.data() + (static_cast<size_t>(t * G + g) * out_p + n) * in_p;
+        const float* row = w.data() + static_cast<size_t>(g * out + n) * in * taps;
+        for (int c = 0; c < in; ++c) dst[c] = row[static_cast<size_t>(c) * taps + t];
+      }
+  return s;
+}
+
+// One "ff.*" state-dict entry of a variant set by satb_dit_set_feedforward (the default keeps its own path in
+// satb_dit_load_weight).  Keys, per transformer.py:258-284: ff.ff.0.proj.{weight, bias} (GLU, always biased) or
+// ff.ff.0.1.weight [inner, D(, k)] (+ .bias); ff.ff.2.weight [D, inner(, k)] (+ .bias).  Returns 1 for a key the
+// variant does not have.  Synchronous (load time only).
+static int load_ff_weight(SatbDit* d, LayerW& L, const std::string& name, const std::string& k, const float* src,
+                          long long numel, cudaStream_t st) {
+  const int D = d->D, inner = d->ff_inner, ip = d->ffi, taps = d->ff_k > 0 ? d->ff_k : 1;
+  enum { W_IN, B_IN, W_OUT, B_OUT } what;
+  int G = 1, out, in = 1, tp = 1, out_p;
+  if (d->ff_glu && k == "ff.ff.0.proj.weight") { what = W_IN; G = 2; out = inner; in = D; out_p = ip; }
+  else if (d->ff_glu && k == "ff.ff.0.proj.bias") { what = B_IN; G = 2; out = inner; out_p = ip; }
+  else if (!d->ff_glu && k == "ff.ff.0.1.weight") { what = W_IN; out = inner; in = D; tp = d->ff_conv_in() ? taps : 1; out_p = ip; }
+  else if (!d->ff_glu && d->ff_bias && k == "ff.ff.0.1.bias") { what = B_IN; out = inner; out_p = ip; }
+  else if (k == "ff.ff.2.weight") { what = W_OUT; out = D; in = inner; tp = taps; out_p = D; }
+  else if (d->ff_bias && k == "ff.ff.2.bias") { what = B_OUT; out = D; out_p = D; }
+  else return 1;
+  SATB_REQUIRE(numel == static_cast<long long>(G) * out * in * tp, ("bad size for " + name).c_str());
+  const int in_p = what == W_OUT ? ip : in;
+  const int rows = tp * G * out_p;
+  if (G == 2 && !d->ff_perm) {
+    const std::vector<int> perm = swiglu_perm(ip);
+    SATB_PROPAGATE(d->alloc(&d->ff_perm, perm.size()));
+    SATB_CHECK_CUDA(cudaMemcpy(d->ff_perm, perm.data(), perm.size() * sizeof(int), cudaMemcpyHostToDevice));
+  }
+  std::vector<float> w(numel);
+  SATB_CHECK_CUDA(cudaMemcpyAsync(w.data(), src, numel * sizeof(float), cudaMemcpyDeviceToHost, st));
+  SATB_CHECK_CUDA(cudaStreamSynchronize(st));
+  const std::vector<float> s = ff_stored_layout(w, G, out, in, tp, out_p, in_p);
+  float* tmp = nullptr;
+  SATB_CHECK_CUDA(cudaMalloc(&tmp, s.size() * sizeof(float)));
+  int rc = 0;
+  if (cudaMemcpy(tmp, s.data(), s.size() * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) {
+    set_last_error("cudaMemcpy of a feed-forward weight failed");
+    rc = -2;
+  }
+  float** bias = what == B_IN ? &L.b_ff1 : &L.b_ff2;
+  uint16_t** w16 = what == W_IN ? &L.w_ff1 : &L.w_ff2;
+  if (rc == 0 && (what == B_IN || what == B_OUT)) {
+    if (!*bias) rc = d->alloc(bias, rows);
+    if (rc == 0 && G == 2) rc = launch_gather_f32(tmp, *bias, d->ff_perm, rows, st);
+    else if (rc == 0 && cudaMemcpyAsync(*bias, tmp, rows * sizeof(float), cudaMemcpyDeviceToDevice, st) != cudaSuccess) rc = -2;
+  } else if (rc == 0 && what == W_IN && d->fp8 && !d->ff_conv_in()) {   // e4m3 rows; the zero rows take scale 1
+    if (!L.w8_ff1) rc = d->alloc(&L.w8_ff1, static_cast<size_t>(rows) * in_p);
+    if (rc == 0 && !L.s_ff1) rc = d->alloc(&L.s_ff1, rows);
+    if (rc == 0) rc = launch_quant_rows_fp8(tmp, L.w8_ff1, L.s_ff1, G == 2 ? d->ff_perm : nullptr, rows, in_p, st);
+  } else if (rc == 0) {
+    if (!*w16) rc = d->alloc(w16, static_cast<size_t>(rows) * in_p);
+    if (rc == 0) rc = launch_cast_rows(tmp, *w16, G == 2 ? d->ff_perm : nullptr, rows, in_p, in_p, in_p, d->bf16, st);
+  }
+  const cudaError_t e = cudaStreamSynchronize(st);
+  cudaFree(tmp);
+  SATB_PROPAGATE(rc);
+  SATB_CHECK_CUDA(e);
+  return 0;
+}
+
 extern "C" {
 
 const char* satb_last_error(void) { return get_last_error(); }
@@ -274,6 +377,7 @@ int satb_dit_create(const SatbDitConfig* cfg, SatbDit** out) {
   d->gd = cfg->global_cond_dim;
   d->ge = cfg->project_global_cond ? d->D : d->gd;
   d->ffi = 4 * d->D;
+  d->ff_inner = d->ffi;
   d->depth = cfg->depth;
   d->F = 128;  // timestep_features_dim 256 = cos | sin of 128 frequencies (models/dit.py:41-43)
   const int rot = d->dh / 2 > 32 ? d->dh / 2 : 32;  // models/transformer.py:737
@@ -308,6 +412,27 @@ int satb_dit_set_conformer(SatbDit* d, int enable) {
   SATB_REQUIRE(d->loaded.empty(), "satb_dit_set_conformer must be called before the first weight is loaded");
   SATB_REQUIRE(!enable || d->D <= kConformerMaxDim, "conformer blocks are supported up to embed_dim 1536");
   d->conformer = enable != 0;
+  return 0;
+}
+
+// Feed-forward options (FeedForward, transformer.py:238-287): call before the first satb_dit_load_weight.
+int satb_dit_set_feedforward(SatbDit* d, int inner_dim, int glu, int conv_kernel_size, int bias) {
+  SATB_REQUIRE(d, "null handle");
+  SATB_REQUIRE(d->loaded.empty(), "satb_dit_set_feedforward must be called before the first weight is loaded");
+  SATB_REQUIRE(inner_dim >= 1, "feed-forward inner dim must be >= 1");
+  SATB_REQUIRE(glu == 0 || glu == 1, "glu must be 0 or 1");
+  SATB_REQUIRE(bias == 0 || bias == 1, "bias must be 0 or 1");
+  SATB_REQUIRE(conv_kernel_size >= 0, "conv_kernel_size must be 0 (Linear) or a positive odd kernel size");
+  SATB_REQUIRE(conv_kernel_size == 0 || conv_kernel_size % 2 == 1,
+               "conv_kernel_size must be odd: an even kernel gives one output position more than the sequence");
+  const long long inner_p = (static_cast<long long>(inner_dim) + 63) / 64 * 64;
+  SATB_REQUIRE(inner_p * d->D * std::max(conv_kernel_size, 2) <= 0x7fffffffLL, "feed-forward weight too large");
+  d->ff_set = true;
+  d->ff_inner = inner_dim;
+  d->ffi = static_cast<int>(inner_p);
+  d->ff_glu = glu != 0;
+  d->ff_k = conv_kernel_size;
+  d->ff_bias = bias != 0;
   return 0;
 }
 
@@ -382,6 +507,13 @@ int satb_dit_load_weight(SatbDit* d, const char* name_c, const float* src, long 
     if (k == "cross_attend_norm.beta") return copy_f32(&L.ca_b, D);
     if (k == "ff_norm.gamma") return copy_f32(&L.ff_g, D);
     if (k == "ff_norm.beta") return copy_f32(&L.ff_b, D);
+    if (d->ff_set && k.compare(0, 3, "ff.") == 0) {
+      const int rc = load_ff_weight(d, L, name, k, src, numel, st);
+      if (rc != 1) return rc;
+      d->loaded.erase(name);
+      set_last_error("unknown DiT weight key: " + name + " (not a key of this model's feed-forward variant)");
+      return -4;
+    }
     if (k == "self_attn.to_qkv.weight") {
       if (!d->qkv_perm && d->dh != 32 && d->dh != 64) {
         const std::vector<int> perm = qkv_head_perm(D, d->dh, d->nf);
@@ -472,6 +604,24 @@ int satb_dit_finalize(SatbDit* d, void* stream_v) {
       }
     }
   }
+  if (d->ff_set) {
+    const bool in8 = d->fp8 && !d->ff_conv_in();
+    for (int i = 0; i < d->depth; ++i) {
+      const LayerW& L = d->layers[i];
+      const std::string p = "transformer.layers." + std::to_string(i) + ".ff.ff.";
+      std::string miss;
+      auto need = [&](bool ok, const char* key) { if (!ok) miss += (miss.empty() ? "" : ", ") + p + key; };
+      need(in8 ? L.w8_ff1 != nullptr : L.w_ff1 != nullptr, d->ff_glu ? "0.proj.weight" : "0.1.weight");
+      if (d->ff_glu) need(L.b_ff1 != nullptr, "0.proj.bias");
+      else if (d->ff_bias) need(L.b_ff1 != nullptr, "0.1.bias");
+      need(L.w_ff2 != nullptr, "2.weight");
+      if (d->ff_bias) need(L.b_ff2 != nullptr, "2.bias");
+      if (!miss.empty()) {
+        set_last_error("feed-forward weights missing in layer " + std::to_string(i) + ": " + miss);
+        return -1;
+      }
+    }
+  }
   SATB_REQUIRE(d->ts_w && d->te0_w && d->te0_b && d->te2_w && d->te2_b, "timestep embedding weights missing");
   SATB_REQUIRE(d->pin_w && d->pout_w && d->pre_w && d->post_w, "project_in/out or pre/post conv weights missing");
   SATB_REQUIRE(d->inv_freq, "rotary inv_freq missing");
@@ -479,7 +629,9 @@ int satb_dit_finalize(SatbDit* d, void* stream_v) {
   if (d->gd > 0) SATB_REQUIRE(d->ge0_w && d->ge2_w, "to_global_embed weights missing");
   for (int i = 0; i < d->depth; ++i) {
     const LayerW& L = d->layers[i];
-    SATB_REQUIRE(L.pre_g && L.ff_g && (d->fp8 ? L.w8_qkv && L.w8_ff1 : L.w_qkv && L.w_ff1) && L.w_o && L.w_ff2,
+    const bool ff_in8 = d->fp8 && !d->ff_conv_in();   // a token-convolution FF-in keeps 16-bit weights in every mode
+    SATB_REQUIRE(L.pre_g && L.ff_g && (d->fp8 ? L.w8_qkv != nullptr : L.w_qkv != nullptr) &&
+                     (ff_in8 ? L.w8_ff1 != nullptr : L.w_ff1 != nullptr) && L.w_o && L.w_ff2,
                  "transformer layer weights missing");
     if (d->ct > 0)
       SATB_REQUIRE(L.ca_g && (d->fp8 ? L.w8_q != nullptr : L.w_q != nullptr) && L.w_kv && L.w_co,
@@ -559,7 +711,8 @@ int satb_dit_reserve(SatbDit* d, int R, int L) {
   SATB_PROPAGATE(d->ws_qkv.ensure(M * 3 * D * 2));
   SATB_PROPAGATE(d->ws_attn.ensure(M * D * 2));
   SATB_PROPAGATE(d->ws_q16.ensure(M * D * 2));
-  SATB_PROPAGATE(d->ws_ff.ensure(M * d->ffi * 2));
+  // the FF intermediate [M, ffi], and the conformer branch's two [M, D] intermediates
+  SATB_PROPAGATE(d->ws_ff.ensure(M * std::max(d->ffi, d->conformer ? 2 * D : 0) * 2));
   SATB_PROPAGATE(d->ws_ain.ensure(M * d->Cin * 2));
   SATB_PROPAGATE(d->ws_y.ensure(M * d->C * 4));
   if (d->fp8) {
@@ -838,24 +991,42 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
       EpiResidual::Params ep{h, D, nullptr, nullptr, N_seq, 0, 1};
       SATB_PROPAGATE((linear_auto<EpiResidual, BF16>(d->tmaps, cv, D, M, D, W.cf_w2, D, ep, st)));
     }
-    // ---- feed-forward: LN -> GEMM (+bias, SwiGLU) -> GEMM (+bias, +residual)
+    // ---- feed-forward: LN -> GEMM (+bias, SwiGLU) -> GEMM (+bias, +residual).  satb_dit_set_feedforward variants: a
+    // plain FF-in is the GEMM (+bias, SiLU); a token convolution (FF-in and / or FF-out) the k-tap GEMM over each item.
     {
       ProfScope ps(d, PROF_LN, st);
-      SATB_PROPAGATE(layernorm_in(W.ff_g, W.ff_b, M, ssg_l ? ssg_l + 3 * D : nullptr, ssg_l ? ssg_l + 4 * D : nullptr,
-                                  ssg_ld, B));
+      const float* mod_scale = ssg_l ? ssg_l + 3 * D : nullptr;
+      const float* mod_shift = ssg_l ? ssg_l + 4 * D : nullptr;
+      if (FP8 && d->ff_conv_in())   // the token convolution takes 16-bit (fp16) operands in every mode
+        SATB_PROPAGATE(launch_layernorm(h, W.ff_g, W.ff_b, a16, M, D, mod_scale, mod_shift, ssg_ld, N_seq, B, false, st));
+      else
+        SATB_PROPAGATE(layernorm_in(W.ff_g, W.ff_b, M, mod_scale, mod_shift, ssg_ld, B));
     }
     {
       ProfScope ps(d, PROF_FF_IN, st);
-      typedef EpiSwiglu<BF16> E;
-      typename E::Params ep{ff, d->ffi, W.b_ff1};
       const void* w = FP8 ? static_cast<const void*>(W.w8_ff1) : static_cast<const void*>(W.w_ff1);
-      SATB_PROPAGATE((linear<E, 256, BF16, FP8>(d->tmaps, a_in, D, M, D, w, 2 * d->ffi, ep, st, 1,
-                                                 Fp8Scales{a_scale, W.s_ff1})));
+      if (d->ff_glu) {
+        typedef EpiSwiglu<BF16> E;
+        typename E::Params ep{ff, d->ffi, W.b_ff1};
+        SATB_PROPAGATE((linear<E, 256, BF16, FP8>(d->tmaps, a_in, D, M, D, w, 2 * d->ffi, ep, st, 1,
+                                                   Fp8Scales{a_scale, W.s_ff1})));
+      } else if (d->ff_k == 0) {
+        typedef EpiStore16<BF16> E;   // silu(x W^T + b), transformer.py:262-268
+        typename E::Params ep{ff, d->ffi, W.b_ff1, 1};
+        SATB_PROPAGATE((linear_auto<E, BF16, FP8>(d->tmaps, a_in, D, M, D, w, d->ffi, ep, st, Fp8Scales{a_scale, W.s_ff1})));
+      } else {
+        typedef EpiStore16<BF16> E;
+        typename E::Params ep{ff, d->ffi, W.b_ff1, 1};
+        SATB_PROPAGATE((token_conv<E, BF16>(d->tmaps, a16, N_seq, R, N_seq, D, W.w_ff1, d->ffi, d->ff_k, ep, st)));
+      }
     }
     {
       ProfScope ps(d, PROF_FF_OUT, st);
       EpiResidual::Params ep{h, D, W.b_ff2, ssg_l ? ssg_l + 5 * D : nullptr, N_seq, static_cast<int>(ssg_ld), B};
-      SATB_PROPAGATE((linear_auto<EpiResidual, BF16>(d->tmaps, ff, d->ffi, M, d->ffi, W.w_ff2, D, ep, st)));
+      if (d->ff_k == 0)
+        SATB_PROPAGATE((linear_auto<EpiResidual, BF16>(d->tmaps, ff, d->ffi, M, d->ffi, W.w_ff2, D, ep, st)));
+      else
+        SATB_PROPAGATE((token_conv<EpiResidual, BF16>(d->tmaps, ff, N_seq, R, N_seq, d->ffi, W.w_ff2, D, d->ff_k, ep, st)));
     }
   }
   if (hidden_out)
@@ -1076,6 +1247,42 @@ int satb_gemm_probe_fp8(const void* a8, const void* w8, const float* a_scale, co
   set_last_error("gemm probe fp8: no such instance (epi " + std::to_string(p->epi) + ", BN " + std::to_string(bn) +
                  "); the forward's FP8 instances are qkv_rope and swiglu BN 256, store16 BN 128 / 256 and head_norm16 BN 128");
   return -1;
+}
+
+}  // extern "C"
+
+// The feed-forward's token convolutions, through token_conv as the forward calls it.
+template <bool BF16>
+static int token_conv_probe(const void* a, long long item_stride, const void* w, int R, int n_seq, int K, int N, int k,
+                            const SatbGemmProbe& p, cudaStream_t st) {
+  TmapCache tc;
+  if (p.epi == SATB_EPI_STORE16) {
+    typedef EpiStore16<BF16> E;
+    return token_conv<E, BF16>(tc, a, item_stride, R, n_seq, K, w, N, k, typename E::Params{p.out, p.ld, p.bias, p.act},
+                               st, p.bn);
+  }
+  const EpiResidual::Params ep{p.h, p.ld, p.bias, p.gate, p.rows_per_item, p.gate_ld, p.n_items};
+  return token_conv<EpiResidual, BF16>(tc, a, item_stride, R, n_seq, K, w, N, k, ep, st, p.bn);
+}
+
+extern "C" {
+
+int satb_token_conv_probe(const void* a16, long long item_stride, const void* w16, int R, int n_seq, int K, int N, int k,
+                          const SatbGemmProbe* p, void* stream) {
+  SATB_REQUIRE(a16 && w16 && p, "null argument");
+  SATB_REQUIRE(aligned16(a16) && aligned16(w16), "token conv probe: operands must be 16-byte aligned");
+  SATB_REQUIRE(R >= 1 && n_seq >= 1 && item_stride >= n_seq, "token conv probe: need R, n_seq >= 1 and item_stride >= n_seq");
+  SATB_REQUIRE(K >= 8 && K % 8 == 0 && N >= 32 && N % 32 == 0, "token conv probe: need K % 8 == 0 and N % 32 == 0");
+  SATB_REQUIRE(k >= 1 && k % 2 == 1, "token conv probe: the kernel size must be odd");
+  SATB_REQUIRE(p->epi == SATB_EPI_STORE16 || p->epi == SATB_EPI_RESIDUAL,
+               "token conv probe: the forward's convolutions run the store16 and residual epilogues only");
+  SATB_REQUIRE(p->bn == 0 || p->bn == 128 || p->bn == 256, "token conv probe: bn must be 0 (the forward's pick), 128 or 256");
+  SATB_REQUIRE(p->epi == SATB_EPI_STORE16 || !p->gate || (p->rows_per_item >= 1 && p->n_items >= 1 && p->gate_ld % 4 == 0),
+               "token conv probe: the gate needs rows_per_item, n_items >= 1 and gate_ld % 4 == 0");
+  SATB_PROPAGATE(probe_check_outputs(*p, N));
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return p->bf16 ? token_conv_probe<true>(a16, item_stride, w16, R, n_seq, K, N, k, *p, st)
+                 : token_conv_probe<false>(a16, item_stride, w16, R, n_seq, K, N, k, *p, st);
 }
 
 }  // extern "C"

@@ -82,6 +82,7 @@ SIGNATURES = {
     "satb_dit_create": (_I, [ctypes.POINTER(SatbDitConfig), ctypes.POINTER(_VP)]),
     "satb_dit_destroy": (None, [_VP]),
     "satb_dit_set_conformer": (_I, [_VP, _I]),
+    "satb_dit_set_feedforward": (_I, [_VP, _I, _I, _I, _I]),
     "satb_dit_load_weight": (_I, [_VP, ctypes.c_char_p, _VP, _LL, _VP]),
     "satb_dit_finalize": (_I, [_VP, _VP]),
     "satb_dit_reserve": (_I, [_VP, _I, _I]),
@@ -98,6 +99,7 @@ SIGNATURES = {
     "satb_linear_f32out": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _VP]),
     "satb_gemm_probe": (_I, [_VP, _VP, _I, _I, _I, ctypes.POINTER(SatbGemmProbe), _VP]),
     "satb_gemm_probe_fp8": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, ctypes.POINTER(SatbGemmProbe), _VP]),
+    "satb_token_conv_probe": (_I, [_VP, _LL, _VP, _I, _I, _I, _I, _I, ctypes.POINTER(SatbGemmProbe), _VP]),
     "satb_attention": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP]),
     "satb_attention_hd": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _VP]),
     "satb_attention_probe": (_I, [ctypes.POINTER(SatbAttentionProbe), _VP]),

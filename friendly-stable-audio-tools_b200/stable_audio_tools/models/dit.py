@@ -12,7 +12,10 @@ and parameter names, ``forward`` signature and CFG semantics); the arithmetic ru
 * rows whose context is all-zero (the uncond half without a negative prompt) skip
   cross-attention: the branch is bias-free, so its output is exactly 0 (SURVEY.md H5);
 * ``conformer=True`` models run the conformer branch of every block natively
-  (``satb_dit_set_conformer``, csrc/conformer.cu), with 16-bit GEMM operands in every ``operand_dtype``.
+  (``satb_dit_set_conformer``, csrc/conformer.cu), with 16-bit GEMM operands in every ``operand_dtype``;
+* ``ff_kwargs`` (any ``mult``, ``no_bias``, ``glu=False``, ``use_conv`` with an odd ``conv_kernel_size``) select the
+  native feed-forward variant (``satb_dit_set_feedforward``); its token convolutions run as k-tap GEMMs over each
+  item, with 16-bit operands in every ``operand_dtype``.
 
 There is no eager / CPU fallback: tensors must live on a CUDA device.
 """
@@ -112,6 +115,10 @@ class DiffusionTransformer(nn.Module):
         nn.init.zeros_(self.preprocess_conv.weight)
         self.postprocess_conv = nn.Conv1d(io_channels, io_channels, 1, bias=False)
         nn.init.zeros_(self.postprocess_conv.weight)
+        # ff_kwargs (ContinuousTransformer -> TransformerBlock -> FeedForward): the native feed-forward variant, handed
+        # to satb_dit_set_feedforward only when it differs from the default SwiGLU (mult 4, biased, Linear)
+        ff = self.transformer.layers[0].ff if depth > 0 else None
+        self.ff_spec = ff.native_spec() if ff is not None else (4 * embed_dim, 1, 0, 1)
 
         # native state (not part of the state dict)
         self.__dict__["_h"] = None
@@ -168,8 +175,13 @@ class DiffusionTransformer(nn.Module):
             cfg = self.native_config()
             h = ctypes.c_void_p()
             _native.check(lib.satb_dit_create(ctypes.byref(cfg), ctypes.byref(h)))
+            options = []
             if self.conformer:
-                rc = lib.satb_dit_set_conformer(h, 1)
+                options.append(lambda: lib.satb_dit_set_conformer(h, 1))
+            if self.ff_spec != (4 * self.embed_dim, 1, 0, 1):
+                options.append(lambda: lib.satb_dit_set_feedforward(h, *self.ff_spec))
+            for set_option in options:
+                rc = set_option()
                 if rc != 0:
                     msg = lib.satb_last_error()
                     lib.satb_dit_destroy(h)

@@ -78,19 +78,44 @@ class GLU(_FusedModule):
 
 
 class FeedForward(_FusedModule):
-    """SwiGLU MLP; keys ``ff.0.proj.{weight,bias}`` and ``ff.2.{weight,bias}``."""
+    """Reference transformer.py:238-287, every option but ``dim_out != dim``.  Keys: ``ff.0.proj.{weight,bias}`` (GLU,
+    the default SwiGLU: Linear(dim, 2 inner), always biased) or ``ff.0.1.{weight,bias}`` (``glu=False``: Linear, or
+    Conv1d with ``use_conv``, then SiLU); ``ff.2.{weight,bias}`` (Linear, or Conv1d with ``use_conv``); no biases but the
+    GLU's with ``no_bias``.  inner = int(dim * mult).  The ``Rearrange`` modules of the reference have no parameters and
+    are ``nn.Identity`` here.  Natively (``satb_dit_set_feedforward``) the convolutions run over each item's tokens as a
+    k-tap GEMM, with 16-bit operands in every ``operand_dtype``."""
 
     def __init__(self, dim, dim_out=None, mult=4, no_bias=False, glu=True, use_conv=False, conv_kernel_size=3,
                  zero_init_output=True):
         super().__init__()
-        if not glu or use_conv or no_bias or (dim_out not in (None, dim)) or mult != 4:
-            raise NotImplementedError("only the default SwiGLU feed-forward (mult 4, biased) is on the native hot path")
+        if dim_out not in (None, dim):
+            # the reference builds it, then fails at the residual add (transformer.py:692-700)
+            raise NotImplementedError(f"a feed-forward with dim_out {dim_out} != dim {dim} cannot be added to the "
+                                      "residual stream")
+        if use_conv and (conv_kernel_size < 1 or conv_kernel_size % 2 == 0):
+            # padding k // 2 keeps the length only for odd k: an even k gives L + 1 positions
+            raise NotImplementedError(f"conv_kernel_size must be odd and positive (got {conv_kernel_size})")
         inner = int(dim * mult)
-        linear_out = nn.Linear(inner, dim)
+        if inner < 1:
+            raise NotImplementedError(f"feed-forward inner dim int({dim} * {mult}) = {inner} must be >= 1")
+        self.inner_dim, self.glu, self.bias = inner, bool(glu), not no_bias
+        self.conv_kernel_size = conv_kernel_size if use_conv else 0
+        conv = lambda i, o: nn.Conv1d(i, o, conv_kernel_size, padding=conv_kernel_size // 2, bias=not no_bias)
+        if glu:
+            linear_in = GLU(dim, inner)                 # the reference builds GLU without use_conv (:260)
+        else:
+            linear_in = nn.Sequential(nn.Identity(), conv(dim, inner) if use_conv else nn.Linear(dim, inner, bias=not no_bias),
+                                      nn.Identity(), nn.SiLU())
+        linear_out = conv(inner, dim) if use_conv else nn.Linear(inner, dim, bias=not no_bias)
         if zero_init_output:
             nn.init.zeros_(linear_out.weight)
-            nn.init.zeros_(linear_out.bias)
-        self.ff = nn.Sequential(GLU(dim, inner), nn.Identity(), linear_out, nn.Identity())
+            if not no_bias:
+                nn.init.zeros_(linear_out.bias)
+        self.ff = nn.Sequential(linear_in, nn.Identity(), linear_out, nn.Identity())
+
+    def native_spec(self):
+        """The satb_dit_set_feedforward arguments: (inner_dim, glu, conv_kernel_size, bias)."""
+        return (self.inner_dim, int(self.glu), self.conv_kernel_size, int(self.bias))
 
 
 class Attention(_FusedModule):

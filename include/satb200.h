@@ -82,6 +82,18 @@ void satb_dit_destroy(SatbDit* h);
  * requires the nine "transformer.layers.{i}.conformer.*" tensors of every layer.  Its GEMMs take 16-bit operands in
  * every operand_dtype (fp16 in the fp8 mode).  A handle that never calls this runs the model without the branch. */
 int satb_dit_set_conformer(SatbDit* h, int enable);
+/* Feed-forward options (FeedForward kwargs via ff_kwargs, models/transformer.py:238-287,643): inner_dim = int(dim *
+ * mult); glu 1 = SwiGLU (FF-in "ff.ff.0.proj" Linear(dim, 2 inner), always biased), 0 = "ff.ff.0.1" then SiLU;
+ * conv_kernel_size 0 = Linear layers, else use_conv with that odd kernel size and padding k / 2: FF-out "ff.ff.2" becomes
+ * Conv1d(inner, dim, k) over the tokens, and so does a non-GLU FF-in (Conv1d(dim, inner, k)); the GLU projection stays
+ * a Linear.  bias 0 = no_bias (FF-out and a non-GLU FF-in lose their bias).  A convolution runs over each item's
+ * tokens (prepended ones included), zero-padded at the item's ends, every CFG row its own item; it takes 16-bit
+ * operands in every operand_dtype (fp16 in the fp8 mode, whose e4m3 FF-in is the Linear one).  The inner width is
+ * padded with zeros to a multiple of 64 at load time (exact).  Call after satb_dit_create and before the first
+ * satb_dit_load_weight; bad values (inner_dim < 1, an even or negative kernel size) and late calls are refused.
+ * finalize then requires the variant's keys and names the missing ones.  The default is (4 * embed_dim, 1, 0, 1): a
+ * handle that never calls this runs the default feed-forward. */
+int satb_dit_set_feedforward(SatbDit* h, int inner_dim, int glu, int conv_kernel_size, int bias);
 /* One state-dict entry (key relative to DiffusionTransformer, e.g.
  * "transformer.layers.0.self_attn.to_qkv.weight"); src: device fp32, contiguous.
  * Replaces nn.Module.load_state_dict for this module (models/pretrained.py:24). */
@@ -163,6 +175,15 @@ int satb_gemm_probe(const void* a16, const void* w16, int M, int N, int K, const
  * (fp16 outputs) and K a multiple of 128. */
 int satb_gemm_probe_fp8(const void* a8, const void* w8, const float* a_scale, const float* w_scale, int M, int N, int K,
                         const SatbGemmProbe* p, void* stream);
+/* Test entry point: the feed-forward's token convolution (satb_dit_set_feedforward with conv_kernel_size k), through
+ * the GEMM launch the DiT forward makes:
+ *   C[r * n_seq + l, n] = sum_t sum_c a16[r, l + t - k / 2, c] * w16[t * N + n, c]   (rows outside 0..n_seq-1: zero)
+ * a16: 16-bit [R, item_stride, K] (item_stride >= n_seq rows; rows n_seq.. of an item are never read); w16: tap-major
+ * [k * N, K]; C goes through p's epilogue: SATB_EPI_STORE16 (out [R * n_seq, ld], bias, act) or SATB_EPI_RESIDUAL (h,
+ * bias, gate).  p->bn: 0 = the N tile the forward picks for this shape, or 128 / 256; p->bf16 selects the instance.
+ * k odd, K % 8 == 0, N % 32 == 0; pointers 16-byte aligned. */
+int satb_token_conv_probe(const void* a16, long long item_stride, const void* w16, int R, int n_seq, int K, int N, int k,
+                          const SatbGemmProbe* p, void* stream);
 /* One step of the v-objective k-diffusion samplers in a single pass over the latents (replaces the
  * ~20 elementwise torch kernels of K.external.VDenoiser.forward + sample_dpmpp_{2m,3m}_sde's update,
  * reference call sites inference/sampling.py:159,225-228): with v = model(x * c_in, t),
