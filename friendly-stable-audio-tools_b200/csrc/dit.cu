@@ -166,6 +166,13 @@ struct SatbDit {
   int ff_inner = 0, ff_k = 0;
   bool ff_set = false, ff_glu = true, ff_bias = true;
   bool ff_conv_in() const { return !ff_glu && ff_k > 0; }
+  // positions (satb_dit_set_positions; default: rotary, no embedding).  pos_type 1: ScaledSinusoidalEmbedding (pos_scale
+  // [1], pos_inv [D / 2]); 2: AbsolutePositionalEmbedding (pos_emb [abs_max_len, D]).  ws_pos: the [pos_len, D] fp32
+  // table project_in adds, built by satb_dit_reserve (pos_len 0: stale).
+  bool rotary = true;
+  int pos_type = 0, abs_max_len = 0, pos_len = 0;
+  float *pos_scale = nullptr, *pos_inv = nullptr, *pos_emb = nullptr;
+  DevBuf ws_pos;
   int P;  // prepended tokens: 1 (the global-conditioning token; 0 in adaLN mode) + Pp
   std::vector<LayerW> layers;
   std::vector<void*> owned;   // every cudaMalloc of weight storage
@@ -436,6 +443,22 @@ int satb_dit_set_feedforward(SatbDit* d, int inner_dim, int glu, int conv_kernel
   return 0;
 }
 
+// Positional options (ContinuousTransformer rotary_pos_emb / use_sinusoidal_emb / use_abs_pos_emb, transformer.py:50-96,
+// 737-785): call before the first satb_dit_load_weight.
+int satb_dit_set_positions(SatbDit* d, int rotary, int pos_type, int abs_max_len) {
+  SATB_REQUIRE(d, "null handle");
+  SATB_REQUIRE(d->loaded.empty(), "satb_dit_set_positions must be called before the first weight is loaded");
+  SATB_REQUIRE(rotary == 0 || rotary == 1, "rotary must be 0 or 1");
+  SATB_REQUIRE(pos_type >= 0 && pos_type <= 2, "pos_type must be 0 (none), 1 (sinusoidal) or 2 (absolute)");
+  SATB_REQUIRE(pos_type == 2 ? abs_max_len >= 1 : abs_max_len == 0,
+               "abs_max_len must be >= 1 with the absolute embedding (pos_type 2) and 0 otherwise");
+  SATB_REQUIRE(static_cast<long long>(abs_max_len) * d->D <= 0x7fffffffLL, "absolute embedding too large");
+  d->rotary = rotary != 0;
+  d->pos_type = pos_type;
+  d->abs_max_len = abs_max_len;
+  return 0;
+}
+
 void satb_dit_destroy(SatbDit* d) {
   if (!d) return;
   for (void* p : d->owned) cudaFree(p);
@@ -446,6 +469,7 @@ void satb_dit_destroy(SatbDit* d) {
   d->ws_h.release(); d->ws_a16.release(); d->ws_qkv.release(); d->ws_attn.release(); d->ws_q16.release();
   d->ws_ff.release(); d->ws_ain.release(); d->ws_y.release(); d->ws_small.release(); d->ws_cond.release();
   d->ws_kv.release(); d->ws_rope.release(); d->ws_prep.release(); d->ws_a8.release(); d->ws_ascale.release();
+  d->ws_pos.release();
   delete d;
 }
 
@@ -492,7 +516,12 @@ int satb_dit_load_weight(SatbDit* d, const char* name_c, const float* src, long 
   if (name == "postprocess_conv.weight") return copy_f32(&d->post_w, static_cast<long long>(C) * C);
   if (name == "transformer.project_in.weight") return copy_f32(&d->pin_w, static_cast<long long>(D) * Cin);
   if (name == "transformer.project_out.weight") return copy_f32(&d->pout_w, static_cast<long long>(C) * D);
-  if (name == "transformer.rotary_pos_emb.inv_freq") return copy_f32(&d->inv_freq, d->nf);
+  if (name == "transformer.rotary_pos_emb.inv_freq" && d->rotary) return copy_f32(&d->inv_freq, d->nf);
+  // the sinusoid's inv_freq is a non-persistent buffer of the reference: the caller hands it over under this key
+  if (d->pos_type == 1 && name == "transformer.pos_emb.scale") return copy_f32(&d->pos_scale, 1);
+  if (d->pos_type == 1 && name == "transformer.pos_emb.inv_freq") return copy_f32(&d->pos_inv, D / 2);
+  if (d->pos_type == 2 && name == "transformer.pos_emb.emb.weight")
+    return copy_f32(&d->pos_emb, static_cast<long long>(d->abs_max_len) * D);
   const std::string lp = "transformer.layers.";
   if (name.compare(0, lp.size(), lp) == 0) {
     const size_t dot = name.find('.', lp.size());
@@ -622,9 +651,16 @@ int satb_dit_finalize(SatbDit* d, void* stream_v) {
       }
     }
   }
+  if (d->pos_type == 1 && !(d->pos_scale && d->pos_inv)) {
+    set_last_error(std::string("sinusoidal positional embedding missing: ") +
+                   (d->pos_scale ? "" : "transformer.pos_emb.scale ") + (d->pos_inv ? "" : "transformer.pos_emb.inv_freq"));
+    return -1;
+  }
+  if (d->pos_type == 2) SATB_REQUIRE(d->pos_emb, "absolute positional embedding missing: transformer.pos_emb.emb.weight");
   SATB_REQUIRE(d->ts_w && d->te0_w && d->te0_b && d->te2_w && d->te2_b, "timestep embedding weights missing");
   SATB_REQUIRE(d->pin_w && d->pout_w && d->pre_w && d->post_w, "project_in/out or pre/post conv weights missing");
-  SATB_REQUIRE(d->inv_freq, "rotary inv_freq missing");
+  if (d->rotary) SATB_REQUIRE(d->inv_freq, "rotary inv_freq missing");
+  d->pos_len = 0;   // rebuilt from the (re)loaded scale / embedding by the next satb_dit_reserve
   if (d->ct > 0) SATB_REQUIRE(d->ce0_w && d->ce2_w, "to_cond_embed weights missing");
   if (d->gd > 0) SATB_REQUIRE(d->ge0_w && d->ge2_w, "to_global_embed weights missing");
   for (int i = 0; i < d->depth; ++i) {
@@ -696,6 +732,40 @@ static int ensure_rope(SatbDit* d, int N_seq) {
   return 0;
 }
 
+// The [N_seq, D] fp32 table project_in adds (transformer.py:784-785), position p = row within the item, prepended rows
+// included.  Sinusoidal (:74-96): cat(sin(p inv_freq), cos(p inv_freq)) * scale, with the product p * inv_freq in fp32
+// and the reference's own inv_freq.  Absolute (:50-71): emb.weight[p] * fp32(D ** -0.5).
+static int ensure_pos(SatbDit* d, int N_seq) {
+  if (d->pos_len == N_seq) return 0;
+  const int D = d->D, half = D / 2;
+  std::vector<float> tab(static_cast<size_t>(N_seq) * D);
+  if (d->pos_type == 1) {
+    std::vector<float> inv(half);
+    float scale = 0.f;
+    SATB_CHECK_CUDA(cudaMemcpy(inv.data(), d->pos_inv, half * 4, cudaMemcpyDeviceToHost));
+    SATB_CHECK_CUDA(cudaMemcpy(&scale, d->pos_scale, 4, cudaMemcpyDeviceToHost));
+    for (int p = 0; p < N_seq; ++p)
+      for (int j = 0; j < half; ++j) {
+        const float f = static_cast<float>(p) * inv[j];
+        tab[static_cast<size_t>(p) * D + j] = sinf(f) * scale;
+        tab[static_cast<size_t>(p) * D + half + j] = cosf(f) * scale;
+      }
+  } else {
+    SATB_CHECK_CUDA(cudaMemcpy(tab.data(), d->pos_emb, tab.size() * 4, cudaMemcpyDeviceToHost));
+    const float s = static_cast<float>(std::pow(static_cast<double>(D), -0.5));
+    for (float& v : tab) v *= s;
+  }
+  SATB_PROPAGATE(d->ws_pos.ensure(tab.size() * 4));
+  SATB_CHECK_CUDA(cudaMemcpy(d->ws_pos.p, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice));
+  d->pos_len = N_seq;
+  return 0;
+}
+
+// The shape of the last reserve no longer fits, or the position table is stale (weights reloaded).
+static bool needs_reserve(const SatbDit* d, int R, int L) {
+  return R > d->res_R || L != d->res_L || d->P != d->res_P || (d->pos_type != 0 && d->pos_len != L + d->P);
+}
+
 extern "C" {
 
 // Reserve every activation buffer for R rows of L latent tokens (synchronous; call
@@ -704,6 +774,11 @@ int satb_dit_reserve(SatbDit* d, int R, int L) {
   SATB_REQUIRE(d && d->finalized, "weights not finalized");
   SATB_REQUIRE(R >= 1 && L >= 1, "bad shape");
   const int N_seq = L + d->P;
+  if (d->pos_type == 2 && N_seq > d->abs_max_len) {
+    set_last_error("sequence length " + std::to_string(N_seq) + " (latent tokens + prepended tokens) exceeds the absolute "
+                   "positional embedding's max length " + std::to_string(d->abs_max_len));
+    return -1;
+  }
   const size_t M = static_cast<size_t>(R) * N_seq;
   const int D = d->D;
   SATB_PROPAGATE(d->ws_h.ensure(M * D * 4));
@@ -719,7 +794,8 @@ int satb_dit_reserve(SatbDit* d, int R, int L) {
     SATB_PROPAGATE(d->ws_a8.ensure(M * D));
     SATB_PROPAGATE(d->ws_ascale.ensure(M * 4));
   }
-  SATB_PROPAGATE(ensure_rope(d, N_seq));
+  if (d->rotary) SATB_PROPAGATE(ensure_rope(d, N_seq));
+  if (d->pos_type != 0) SATB_PROPAGATE(ensure_pos(d, N_seq));
   d->tmaps.maps.clear();
   d->res_R = R;
   d->res_L = L;
@@ -885,8 +961,10 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
   uint16_t* ff = d->ws_ff.as<uint16_t>();
   uint16_t* ain = d->ws_ain.as<uint16_t>();
   float* y = d->ws_y.as<float>();
-  const float* cos_tab = d->ws_rope.as<float>();
-  const float* sin_tab = cos_tab + static_cast<size_t>(N_seq) * d->nf;
+  // rotary off (satb_dit_set_positions): null tables, which the QKV epilogues take as no rotation
+  const float* cos_tab = d->rotary ? d->ws_rope.as<float>() : nullptr;
+  const float* sin_tab = d->rotary ? cos_tab + static_cast<size_t>(N_seq) * d->nf : nullptr;
+  const float* pos_tab = d->pos_type != 0 ? d->ws_pos.as<float>() : nullptr;
 
   // timestep embedding (+ global embedding) -> conditioning token / adaLN vector  (dit.py:176-195)
   SATB_PROPAGATE(launch_fourier(t, d->ts_w, sw.fourier, B, d->F, st));
@@ -894,12 +972,18 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
   SATB_PROPAGATE(launch_skinny_linear(sw.fourier, d->te0_w, d->te0_b, nullptr, sw.te_h, B, 2 * d->F, D, 1, st));
   SATB_PROPAGATE(launch_skinny_linear(sw.te_h, d->te2_w, d->te2_b, d->has_global ? sw.ge : nullptr, sw.tok, B, D, D,
                                       d->adaln ? 1 : 0, st));
-  // latent -> token rows, project_in (with the 1x1 pre-conv folded), prepend token
+  // latent -> token rows, project_in (with the 1x1 pre-conv folded), prepend token; a positional embedding is added to
+  // every row, prepended ones included, in project_in's epilogue and by write_prepend
   SATB_PROPAGATE(launch_dit_pre(x, ain, R, B, d->Cin, L, P, BF16, st));
-  SATB_PROPAGATE((linear<EpiStore32, 256, BF16>(d->tmaps, ain, d->Cin, M, d->Cin, d->w_in16, D, EpiStore32::Params{h, D, nullptr}, st)));
+  if (pos_tab)
+    SATB_PROPAGATE((linear<EpiStore32Pos, 256, BF16>(d->tmaps, ain, d->Cin, M, d->Cin, d->w_in16, D,
+                                                     EpiStore32Pos::Params{h, D, nullptr, pos_tab, N_seq}, st)));
+  else
+    SATB_PROPAGATE((linear<EpiStore32, 256, BF16>(d->tmaps, ain, d->Cin, M, d->Cin, d->w_in16, D, EpiStore32::Params{h, D, nullptr}, st)));
   const int64_t ssg_ld = static_cast<int64_t>(d->depth) * 6 * D;
   if (P > 0) {
-    SATB_PROPAGATE(launch_write_prepend(sw.tok, d->Pp > 0 ? d->ws_prep.as<float>() : nullptr, h, R, B, N_seq, D, d->Pp, st));
+    SATB_PROPAGATE(launch_write_prepend(sw.tok, d->Pp > 0 ? d->ws_prep.as<float>() : nullptr, pos_tab, h, R, B, N_seq, D,
+                                        d->Pp, st));
   } else {
     // adaLN: all layers' scale/shift/gate in one skinny GEMM (transformer.py:648-651,667)
     SATB_PROPAGATE(launch_skinny_linear(sw.tok, d->w_ssg, nullptr, nullptr, sw.ssg, B, D, d->depth * 6 * D, 0, st));
@@ -1055,7 +1139,7 @@ int satb_dit_forward(SatbDit* d, const float* x, const float* t, float* out, int
   SATB_REQUIRE(d && d->finalized, "weights not finalized");
   SATB_REQUIRE(B == d->B, "batch size differs from satb_dit_prepare_cond");
   const int R = d->cfg_on ? 2 * B : B;
-  if (R > d->res_R || L != d->res_L || d->P != d->res_P) SATB_PROPAGATE(satb_dit_reserve(d, R, L));
+  if (needs_reserve(d, R, L)) SATB_PROPAGATE(satb_dit_reserve(d, R, L));
   cudaStream_t st = static_cast<cudaStream_t>(stream_v);
   return dit_forward_dispatch(d, x, t, out, B, L, cfg_scale, scale_phi, st, nullptr);
 }
@@ -1092,7 +1176,7 @@ int satb_dit_forward_debug(SatbDit* d, const float* x, const float* t, float* ou
   SATB_REQUIRE(d && d->finalized, "weights not finalized");
   SATB_REQUIRE(B == d->B, "batch size differs from satb_dit_prepare_cond");
   const int R = d->cfg_on ? 2 * B : B;
-  if (R > d->res_R || L != d->res_L || d->P != d->res_P) SATB_PROPAGATE(satb_dit_reserve(d, R, L));
+  if (needs_reserve(d, R, L)) SATB_PROPAGATE(satb_dit_reserve(d, R, L));
   cudaStream_t st = static_cast<cudaStream_t>(stream_v);
   return dit_forward_dispatch(d, x, t, out, B, L, cfg_scale, scale_phi, st, hidden);
 }
@@ -1113,7 +1197,7 @@ static int probe_run(const void* a, const void* w, int M, int N, int K, const ty
 }
 
 static int probe_check_outputs(const SatbGemmProbe& p, int N) {
-  const int out_elem = p.epi == SATB_EPI_STORE32 ? 4 : 2;
+  const int out_elem = p.epi == SATB_EPI_STORE32 || p.epi == SATB_EPI_STORE32_POS ? 4 : 2;
   if (p.epi != SATB_EPI_RESIDUAL) {
     SATB_REQUIRE(p.out && aligned16(p.out), "gemm probe: out must be a 16-byte aligned device pointer");
     SATB_REQUIRE(p.ld >= (p.epi == SATB_EPI_SWIGLU ? N / 2 : N) && (p.ld * out_elem) % 16 == 0,
@@ -1135,6 +1219,13 @@ static int gemm_probe(const void* a, const void* w, int M, int N, int K, const S
       const EpiStore32::Params ep{static_cast<float*>(p.out), p.ld, p.bias};
       if (bn == 64) return probe_run<EpiStore32, 64, BF16>(a, w, M, N, K, ep, p.b_static, st);
       if (bn == 256) return probe_run<EpiStore32, 256, BF16>(a, w, M, N, K, ep, p.b_static, st);
+      break;
+    }
+    case SATB_EPI_STORE32_POS: {
+      SATB_REQUIRE(p.pos_tab && aligned16(p.pos_tab) && p.seq_len >= 1,
+                   "gemm probe: store32_pos needs a 16-byte aligned pos_tab and seq_len >= 1");
+      const EpiStore32Pos::Params ep{static_cast<float*>(p.out), p.ld, p.bias, p.pos_tab, p.seq_len};
+      if (bn == 256) return probe_run<EpiStore32Pos, 256, BF16>(a, w, M, N, K, ep, p.b_static, st);
       break;
     }
     case SATB_EPI_STORE16: {
@@ -1183,7 +1274,7 @@ static int gemm_probe(const void* a, const void* w, int M, int N, int K, const S
   }
   set_last_error("gemm probe: no such instance (epi " + std::to_string(p.epi) + ", BN " + std::to_string(bn) +
                  "); the forward's instances are store32 BN 64/256, store16, head_norm16 and residual BN 128/256, "
-                 "qkv_rope and swiglu BN 256");
+                 "qkv_rope, swiglu and store32_pos BN 256");
   return -1;
 }
 

@@ -396,15 +396,18 @@ __global__ void __launch_bounds__(256) skinny_linear_kernel(const float* __restr
 }
 
 // rows 0 .. Pp-1 of every item: the prepend-conditioning tokens (conditional rows r < B; zeros for the unconditional CFG
-// rows, dit.py:309-311); row Pp: the global-conditioning token (dit.py:185-195)
-__global__ void write_prepend_kernel(const float* __restrict__ tok, const float* __restrict__ pre, float* __restrict__ h, int B,
-                                     int N_seq, int D, int Pp) {
+// rows, dit.py:309-311); row Pp: the global-conditioning token (dit.py:185-195).  pos (may be null): the positional
+// embedding table [N_seq, D]; row j gets pos[j] added, as the reference adds it after the prepend concat
+// (transformer.py:770-785).
+__global__ void write_prepend_kernel(const float* __restrict__ tok, const float* __restrict__ pre,
+                                     const float* __restrict__ pos, float* __restrict__ h, int B, int N_seq, int D, int Pp) {
   const int r = blockIdx.y, j = blockIdx.z;
   const int d = blockIdx.x * blockDim.x + threadIdx.x;
   if (d >= D) return;
   float v;
   if (j < Pp) v = (r < B && pre) ? pre[(static_cast<size_t>(r) * Pp + j) * D + d] : 0.f;
   else v = tok[static_cast<size_t>(r % B) * D + d];
+  if (pos) v += pos[static_cast<size_t>(j) * D + d];
   h[(static_cast<size_t>(r) * N_seq + j) * D + d] = v;
 }
 
@@ -643,10 +646,10 @@ int launch_skinny_linear(const float* in, const float* W, const float* bias, con
   return 0;
 }
 
-int launch_write_prepend(const float* tok, const float* pre, float* h, int R, int B, int N_seq, int D, int Pp,
-                         cudaStream_t stream) {
+int launch_write_prepend(const float* tok, const float* pre, const float* pos, float* h, int R, int B, int N_seq, int D,
+                         int Pp, cudaStream_t stream) {
   dim3 grid(ceil_div(D, 256), R, Pp + 1);
-  write_prepend_kernel<<<grid, 256, 0, stream>>>(tok, pre, h, B, N_seq, D, Pp);
+  write_prepend_kernel<<<grid, 256, 0, stream>>>(tok, pre, pos, h, B, N_seq, D, Pp);
   count_launch();
   SATB_CHECK_CUDA(cudaGetLastError());
   return 0;

@@ -432,6 +432,52 @@ struct EpiStore32 {
   }
 };
 
+// EpiStore32 plus one row of a position table: out32[row, col] = acc (+ bias) + pos[row % n_seq, col], pos [n_seq, N]
+// fp32.  The DiT's project_in runs it to add the positional embedding (transformer.py:784-785) to every item's n_seq
+// rows.  A type of its own, so that the plain EpiStore32 instances stay as they are.
+struct EpiStore32Pos {
+  static constexpr int kCols = 32;
+  static constexpr int kStageBytes = 0;
+  static constexpr bool kFragment = true;
+  struct Params {
+    float* out;
+    int ld;
+    const float* bias;  // may be null
+    const float* pos;
+    int n_seq;
+  };
+  template <int BN>
+  __device__ static __forceinline__ void apply_fragment(const Params& p, const float (&acc)[BN / 2], int L, int N,
+                                                        int row0, int n0, int batch, int lane) {
+    const int fc = 2 * (lane & 3);
+    const float* prow[2];
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr)
+      prow[rr] = p.pos + static_cast<size_t>((batch * L + row0 + 8 * rr) % p.n_seq) * N;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      if (n0 + 8 * j >= N) break;
+      const int col = n0 + 8 * j + fc;
+      float2 b = make_float2(0.f, 0.f);
+      if (p.bias) b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int l = row0 + 8 * rr;
+        if (l >= L) continue;
+        const float2 e = __ldg(reinterpret_cast<const float2*>(prow[rr] + col));
+        float2 v = make_float2(acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1]);
+        if (p.bias) {
+          v.x += b.x;
+          v.y += b.y;
+        }
+        v.x += e.x;
+        v.y += e.y;
+        *reinterpret_cast<float2*>(p.out + static_cast<size_t>(batch * L + l) * p.ld + col) = v;
+      }
+    }
+  }
+};
+
 // Residual stream update (models/transformer.py:692-700 and adaLN :670-689):
 //   h[row, col] += (acc + bias[col]) * gate[row / rows_per_item, col]
 // Runs on the accumulator fragment: each thread adds its column pairs (c, c + 1) of rows row0 and row0 + 8 with one

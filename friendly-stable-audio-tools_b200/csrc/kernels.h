@@ -42,9 +42,10 @@ int launch_fourier(const float* t, const float* w, float* out, int B, int F, cud
 // out[r, n] = act_out(sum_k in[r, k] * W[n, k] + bias[n] (+ add[r, n])); fp32 weights; act_out = SiLU if silu_out.
 int launch_skinny_linear(const float* in, const float* W, const float* bias, const float* add, float* out, int R,
                          int K, int N, int silu_out, cudaStream_t stream);
-// h[r*N_seq + j, :] = pre[r, j, :] (j < Pp; zeros for rows r >= B or pre == null), h[r*N_seq + Pp, :] = tok[r % B, :]
-int launch_write_prepend(const float* tok, const float* pre, float* h, int R, int B, int N_seq, int D, int Pp,
-                         cudaStream_t stream);
+// h[r*N_seq + j, :] = pre[r, j, :] (j < Pp; zeros for rows r >= B or pre == null), h[r*N_seq + Pp, :] = tok[r % B, :];
+// plus pos[j, :] on every row j <= Pp when pos (the [N_seq, D] positional embedding table) is given
+int launch_write_prepend(const float* tok, const float* pre, const float* pos, float* h, int R, int B, int N_seq, int D,
+                         int Pp, cudaStream_t stream);
 // in place: x = sigmoid(1 - x) on column ranges [c0, c0+D) and [c1, c1+D) of every 6D-wide layer block
 int launch_gate_sigmoid(float* ssg, int rows, int depth, int D, cudaStream_t stream);
 // y[R*N_seq, C] fp32 -> out[B, C, L] with CFG combine / rescale (models/dit.py:338-347)

@@ -43,13 +43,14 @@ _VP, _I, _LL, _F = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong, ctypes.c_fl
 # satb_gemm_probe (tests only): epilogue kinds and the parameter block, in the order of include/satb200.h
 EPI_STORE32, EPI_STORE16, EPI_HEAD_NORM16, EPI_QKV_ROPE, EPI_SWIGLU, EPI_RESIDUAL = range(6)
 EPI_RESIDUAL_LN = 6   # retired (the LayerNorm-fold residual epilogue): refused, and the number is not reused
+EPI_STORE32_POS = 7   # store32 plus a [seq_len, N] position-table row (project_in with a positional embedding)
 
 
 class SatbGemmProbe(ctypes.Structure):
     _fields_ = ([(n, _I) for n in ("epi", "bn", "bf16", "b_static")] + [("out", _VP), ("ld", _I), ("bias", _VP),
                 ("act", _I), ("h", _VP), ("gate", _VP)]
                 + [(n, _I) for n in ("rows_per_item", "gate_ld", "n_items", "rope_cols", "seq_len", "head_dim", "nf")]
-                + [("cos_tab", _VP), ("sin_tab", _VP), ("norm_cols", _I)])
+                + [("cos_tab", _VP), ("sin_tab", _VP), ("norm_cols", _I), ("pos_tab", _VP)])
 
 
 # satb_attention_probe (tests only): the parameter block of include/satb200.h
@@ -83,6 +84,7 @@ SIGNATURES = {
     "satb_dit_destroy": (None, [_VP]),
     "satb_dit_set_conformer": (_I, [_VP, _I]),
     "satb_dit_set_feedforward": (_I, [_VP, _I, _I, _I, _I]),
+    "satb_dit_set_positions": (_I, [_VP, _I, _I, _I]),
     "satb_dit_load_weight": (_I, [_VP, ctypes.c_char_p, _VP, _LL, _VP]),
     "satb_dit_finalize": (_I, [_VP, _VP]),
     "satb_dit_reserve": (_I, [_VP, _I, _I]),

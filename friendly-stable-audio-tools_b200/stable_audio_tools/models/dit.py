@@ -15,7 +15,9 @@ and parameter names, ``forward`` signature and CFG semantics); the arithmetic ru
   (``satb_dit_set_conformer``, csrc/conformer.cu), with 16-bit GEMM operands in every ``operand_dtype``;
 * ``ff_kwargs`` (any ``mult``, ``no_bias``, ``glu=False``, ``use_conv`` with an odd ``conv_kernel_size``) select the
   native feed-forward variant (``satb_dit_set_feedforward``); its token convolutions run as k-tap GEMMs over each
-  item, with 16-bit operands in every ``operand_dtype``.
+  item, with 16-bit operands in every ``operand_dtype``;
+* ``rotary_pos_emb=False``, ``use_sinusoidal_emb`` and ``use_abs_pos_emb`` select the native positional options
+  (``satb_dit_set_positions``); the embedding is added to every row, prepended ones included, in project_in's epilogue.
 
 There is no eager / CPU fallback: tensors must live on a CUDA device.
 """
@@ -119,6 +121,11 @@ class DiffusionTransformer(nn.Module):
         # to satb_dit_set_feedforward only when it differs from the default SwiGLU (mult 4, biased, Linear)
         ff = self.transformer.layers[0].ff if depth > 0 else None
         self.ff_spec = ff.native_spec() if ff is not None else (4 * embed_dim, 1, 0, 1)
+        # positions (ContinuousTransformer kwargs): the satb_dit_set_positions arguments (rotary, pos_type, abs_max_len),
+        # handed over only when they differ from the default (rotary, no embedding)
+        tr = self.transformer
+        self.pos_spec = (int(tr.rotary_pos_emb is not None), {None: 0, "sinusoidal": 1, "abs": 2}[tr.pos_type],
+                         tr.pos_emb.max_seq_len if tr.pos_type == "abs" else 0)
 
         # native state (not part of the state dict)
         self.__dict__["_h"] = None
@@ -180,6 +187,8 @@ class DiffusionTransformer(nn.Module):
                 options.append(lambda: lib.satb_dit_set_conformer(h, 1))
             if self.ff_spec != (4 * self.embed_dim, 1, 0, 1):
                 options.append(lambda: lib.satb_dit_set_feedforward(h, *self.ff_spec))
+            if self.pos_spec != (1, 0, 0):
+                options.append(lambda: lib.satb_dit_set_positions(h, *self.pos_spec))
             for set_option in options:
                 rc = set_option()
                 if rc != 0:
@@ -190,7 +199,12 @@ class DiffusionTransformer(nn.Module):
         if self.__dict__["_weights_dirty"]:
             st = _native.stream_ptr(device)
             with torch.no_grad():
-                for name, t in self.state_dict().items():
+                weights = list(self.state_dict().items())
+                if self.transformer.pos_type == "sinusoidal":
+                    # a non-persistent buffer, so not in the state dict: handed over as the module holds it (the native
+                    # table uses these very values rather than recomputing the powers)
+                    weights.append(("transformer.pos_emb.inv_freq", self.transformer.pos_emb.inv_freq))
+                for name, t in weights:
                     if name.endswith("rotary_pos_emb.scale") or t is None:
                         continue
                     if not t.is_cuda:
@@ -248,6 +262,14 @@ class DiffusionTransformer(nn.Module):
                              f"(input_concat_dim={self.input_concat_dim})")
         if self.training and cfg_dropout_prob > 0.0:
             raise NotImplementedError("training-time CFG dropout is outside the inference hot path")
+        if self.transformer.pos_type == "abs":
+            # AbsolutePositionalEmbedding's assertion (transformer.py:61-63) over the tokens after the prepend concat
+            n_seq = x.shape[2] // self.patch_size
+            if self.global_cond_type == "prepend":
+                n_seq += 1 + (prepend_cond.shape[1] if prepend_cond is not None else 0)
+            max_len = self.transformer.pos_emb.max_seq_len
+            assert n_seq <= max_len, (f"you are passing in a sequence length of {n_seq} but your absolute positional "
+                                      f"embedding has a max sequence length of {max_len}")
         if not x.is_cuda:
             raise _native.NativeError("DiffusionTransformer.forward needs CUDA tensors (no CPU fallback)")
         # masks are accepted and ignored exactly like the reference (dit.py:250-252,

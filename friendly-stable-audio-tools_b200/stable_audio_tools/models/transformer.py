@@ -52,6 +52,30 @@ class RotaryEmbedding(_FusedModule):
         self.dim = dim
 
 
+class ScaledSinusoidalEmbedding(_FusedModule):
+    """Reference transformer.py:74-96: ``scale`` (a Parameter [1], dim ** -0.5 at init) and ``inv_freq`` (a
+    non-persistent buffer [dim / 2]: not in the state dict, so DiffusionTransformer hands it to the native handle
+    itself).  The embedding of position p is cat(sin(p inv_freq), cos(p inv_freq)) * scale."""
+
+    def __init__(self, dim, theta=10000):
+        super().__init__()
+        assert (dim % 2) == 0, 'dimension must be divisible by 2'
+        self.scale = nn.Parameter(torch.ones(1) * dim ** -0.5)
+        half = dim // 2
+        self.register_buffer("inv_freq", theta ** -(torch.arange(half).float() / half), persistent=False)
+
+
+class AbsolutePositionalEmbedding(_FusedModule):
+    """Reference transformer.py:50-71: ``emb`` = nn.Embedding(max_seq_len, dim); position p adds emb.weight[p] *
+    dim ** -0.5.  Sequences longer than max_seq_len (prepended tokens included) fail its assertion."""
+
+    def __init__(self, dim, max_seq_len):
+        super().__init__()
+        self.scale = dim ** -0.5
+        self.max_seq_len = max_seq_len
+        self.emb = nn.Embedding(max_seq_len, dim)
+
+
 class LayerNorm(_FusedModule):
     """gamma (parameter, or buffer when ``fix_scale``) and beta (buffer unless ``bias``)."""
 
@@ -190,17 +214,28 @@ class TransformerBlock(_FusedModule):
 
 
 class ContinuousTransformer(_FusedModule):
+    """Reference transformer.py:705-809 without ``causal``.  Positions: rotary (``rotary_pos_emb``) and / or one
+    embedding added to the residual stream (``use_sinusoidal_emb`` or ``use_abs_pos_emb``)."""
+
     def __init__(self, dim, depth, *, dim_in=None, dim_out=None, dim_heads=64, cross_attend=False,
                  cond_token_dim=None, global_cond_dim=None, causal=False, rotary_pos_emb=True,
                  zero_init_branch_outputs=True, conformer=False, use_sinusoidal_emb=False, use_abs_pos_emb=False,
                  abs_pos_emb_max_length=10000, **kwargs):
         super().__init__()
-        if causal or use_sinusoidal_emb or use_abs_pos_emb or not rotary_pos_emb:
-            raise NotImplementedError("only the non-causal rotary configuration is on the native hot path")
+        assert not (use_sinusoidal_emb and use_abs_pos_emb), \
+            "Can't select both of sinusoidal/abs positional embedding type."
+        if causal:
+            raise NotImplementedError("causal attention is outside the native hot path")
         self.dim, self.depth = dim, depth
         self.project_in = nn.Linear(dim_in, dim, bias=False) if dim_in else nn.Identity()
         self.project_out = nn.Linear(dim, dim_out, bias=False) if dim_out else nn.Identity()
-        self.rotary_pos_emb = RotaryEmbedding(max(dim_heads // 2, 32))
+        self.rotary_pos_emb = RotaryEmbedding(max(dim_heads // 2, 32)) if rotary_pos_emb else None
+        # added to every row after the prepend concat (transformer.py:770-785); natively in project_in's epilogue
+        self.pos_type, self.pos_emb = None, None
+        if use_sinusoidal_emb:
+            self.pos_type, self.pos_emb = "sinusoidal", ScaledSinusoidalEmbedding(dim)
+        elif use_abs_pos_emb:
+            self.pos_type, self.pos_emb = "abs", AbsolutePositionalEmbedding(dim, abs_pos_emb_max_length)
         self.layers = nn.ModuleList([
             TransformerBlock(dim, dim_heads=dim_heads, cross_attend=cross_attend, dim_context=cond_token_dim,
                              global_cond_dim=global_cond_dim, causal=causal,

@@ -94,6 +94,18 @@ int satb_dit_set_conformer(SatbDit* h, int enable);
  * finalize then requires the variant's keys and names the missing ones.  The default is (4 * embed_dim, 1, 0, 1): a
  * handle that never calls this runs the default feed-forward. */
 int satb_dit_set_feedforward(SatbDit* h, int inner_dim, int glu, int conv_kernel_size, int bias);
+/* Positional options (ContinuousTransformer kwargs, models/transformer.py:50-96,737-785): rotary 1 = rotary_pos_emb
+ * (the "transformer.rotary_pos_emb.inv_freq" key), 0 = no RoPE (no inv_freq key; q and k are not rotated).  pos_type
+ * 0 = none, 1 = use_sinusoidal_emb (ScaledSinusoidalEmbedding: keys "transformer.pos_emb.scale" [1] and, since the
+ * reference keeps it out of the state dict, its inv_freq buffer [embed_dim / 2] under "transformer.pos_emb.inv_freq"),
+ * 2 = use_abs_pos_emb (AbsolutePositionalEmbedding: "transformer.pos_emb.emb.weight" [abs_max_len, embed_dim]).
+ * abs_max_len: abs_pos_emb_max_length with pos_type 2, else 0.  The embedding is added to every row after the prepend
+ * concat: positions count the prepended tokens (global-conditioning and prepend-conditioning ones) and, with patching,
+ * patched tokens.  Forwards whose latent + prepended tokens exceed abs_max_len are refused.  Call after
+ * satb_dit_create and before the first satb_dit_load_weight; bad values and late calls are refused.  finalize then
+ * requires the variant's keys and names the missing ones.  The default is (1, 0, 0): a handle that never calls this
+ * runs rotary positions only. */
+int satb_dit_set_positions(SatbDit* h, int rotary, int pos_type, int abs_max_len);
 /* One state-dict entry (key relative to DiffusionTransformer, e.g.
  * "transformer.layers.0.self_attn.to_qkv.weight"); src: device fp32, contiguous.
  * Replaces nn.Module.load_state_dict for this module (models/pretrained.py:24). */
@@ -144,7 +156,8 @@ int satb_layernorm_fp8(const float* x, const float* gamma, const float* beta, co
 int satb_linear_f32out(const void* a16, const void* w16, float* c, int M, int N, int K, int bf16, void* stream);
 /* Test entry point (no product path calls it): C = A[M, K] * W[N, K]^T through ONE of the fused-epilogue GEMM
  * instances the DiT forward launches, chosen by `epi`, `bn` and `bf16`.  The instances: store32 BN 64 / 256;
- * store16, head_norm16 and residual BN 128 / 256; qkv_rope and swiglu BN 256; anything else returns an error.  The
+ * store16, head_norm16 and residual BN 128 / 256; qkv_rope, swiglu and store32_pos BN 256; anything else returns an
+ * error.  The
  * remaining fields are the epilogue's parameters (csrc/gemm.cuh); all pointers are device pointers, 16-byte aligned;
  * fields an epilogue does not use are ignored. */
 #define SATB_EPI_STORE32 0      /* out fp32 = acc (+ bias) */
@@ -154,6 +167,8 @@ int satb_linear_f32out(const void* a16, const void* w16, float* c, int M, int N,
 #define SATB_EPI_SWIGLU 4       /* out[:, N / 2] = value * silu(gate), 32 / 32 interleaved columns */
 #define SATB_EPI_RESIDUAL 5     /* h += (acc (+ bias)) (* gate) */
 /* 6 was the LayerNorm-fold residual epilogue, since removed: it is refused, and the number is not reused. */
+#define SATB_EPI_STORE32_POS 7  /* out fp32 = acc (+ bias) + pos_tab[row % seq_len, :] (BN 256: DiT project_in with a
+                                   positional embedding) */
 typedef struct SatbGemmProbe {
   int epi, bn, bf16, b_static;      /* b_static 1: weight prefetch before the dependency wait, as the forward runs */
   void* out;                        /* store32 (fp32), store16, head_norm16, qkv_rope, swiglu (16-bit) */
@@ -167,6 +182,7 @@ typedef struct SatbGemmProbe {
   const float* cos_tab;
   const float* sin_tab;
   int norm_cols;                    /* head_norm16 */
+  const float* pos_tab;             /* store32_pos: [seq_len, N] fp32 */
 } SatbGemmProbe;
 int satb_gemm_probe(const void* a16, const void* w16, int M, int N, int K, const SatbGemmProbe* p, void* stream);
 /* Test entry point: the same through ONE of the FP8-mode instances of the DiT forward: a8 [M, K] and w8 [N, K] e4m3
