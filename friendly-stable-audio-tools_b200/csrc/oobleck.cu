@@ -9,7 +9,9 @@
 // over N = s*Cout columns; a strided convolution (k = 2s, stride s) is a 2s-tap GEMM whose
 // taps address the input as (phase, row) through a 4-D tensor map.  The encoder's first
 // convolution (2 -> 128 channels) is bandwidth-bound and stays on CUDA cores; the decoder's last
-// one (128 -> 2) runs through the same GEMM with a mostly empty N tile.
+// one (128 -> 2) runs through the same GEMM with a mostly empty N tile.  Behind a PQMF pretransform the
+// encoder reads and the decoder writes channels * num_bands sub-bands (a multiple of 8, up to 128): the
+// encoder's first convolution then runs as a GEMM over a 16-bit channels-last copy of its input.
 // Weight-norm (w = g * v / ||v||, torch.nn.utils.weight_norm via dac.nn.layers) is folded
 // once at load time.
 // Block options (satb_oobleck_create_variant): ELU instead of Snake (use_snake=False) is the ACT template parameter of
@@ -577,7 +579,8 @@ int dec_residual(SatbOobleck* h, int b, int j, int B, int L, void* raw, void*& s
 
 // Decoder final conv k7 chans[0] -> audio channels (no bias, optional tanh) of in16 [B, L, chans[0]] into audio NCL.
 // The 128 -> 2 contraction runs with the N tile mostly empty (8x wasted MMA work is still ~10x faster than the
-// shared-memory-bound CUDA-core version it replaces: 1.21 ms -> bandwidth-bound)
+// shared-memory-bound CUDA-core version it replaces: 1.21 ms -> bandwidth-bound).  Up to 64 outputs (audio, or the
+// sub-bands of a PQMF pretransform) take the halo-tile route; 65 .. 128 sub-bands take the implicit GEMM's 128 tile.
 template <bool BF16>
 int dec_output(SatbOobleck* h, const void* in16, float* audio, int B, int L, cudaStream_t st) {
   const ConvW& cf = h->convs.at("layers." + std::to_string(h->cfg.n_stages + 2) + ".");
@@ -595,12 +598,25 @@ int dec_output(SatbOobleck* h, const void* in16, float* audio, int B, int L, cud
   return run_conv_gemm<EpiStoreNCL, BF16>(h, cf, in16, B, L, 0, 1, 1, ep, st);
 }
 
-// Encoder input conv k7 audio NCL [B, in_channels, T] -> chans[0] on CUDA cores: raw, and block 1 / unit 0's
-// activation into out16.
+// Encoder input conv k7 audio NCL [B, in_channels, T] -> chans[0]: raw, and block 1 / unit 0's activation into out16.
+// 1 or 2 channels run on CUDA cores.  Wider inputs (the sub-bands of a PQMF pretransform, a multiple of 8 channels) are
+// cast to channels-last 16-bit in tmp16 and run as a 7-tap implicit GEMM with the same epilogue outputs.
 template <bool BF16, int ACT>
-int enc_input(SatbOobleck* h, const float* audio, void* raw, void* out16, int B, int64_t T, cudaStream_t st) {
+int enc_input(SatbOobleck* h, const float* audio, void* raw, void* out16, void* tmp16, int B, int64_t T,
+              cudaStream_t st) {
   const ConvW& c0 = h->convs.at("layers.0.");
   const SnakeW* sn = act_params(h, "layers.1.layers.0.layers.0.");
+  h->wrote_raw = true;
+  if (!c0.small) {
+    dim3 grid(static_cast<unsigned>(ceil_div64(T, 32)), ceil_div(c0.cin, 32), B);
+    ncl_to_nlc16_kernel<BF16><<<grid, 256, 0, st>>>(audio, static_cast<uint16_t*>(tmp16),
+                                                    static_cast<uint16_t*>(lo_half(h, tmp16)), c0.cin, static_cast<int>(T));
+    count_launch();
+    typedef EpiConvFor<BF16, false, ACT> E;
+    typename E::Params ep{c0.bias, nullptr, raw, out16, act_a(sn), act_ib(sn), c0.cout, static_cast<int>(T), 1, 0,
+                          lo_half(h, out16), h->raw16};
+    return run_conv_gemm<E, BF16>(h, c0, tmp16, B, static_cast<int>(T), 0, 1, 1, ep, st);
+  }
   SATB_REQUIRE(c0.cin * c0.k <= 16, "encoder input conv: in_channels * kernel must be <= 16");
   const size_t smem = static_cast<size_t>(c0.cin) * (64 + c0.k - 1) * 4;
   dim3 grid(static_cast<unsigned>(ceil_div64(T, 64)), B);
@@ -610,7 +626,6 @@ int enc_input(SatbOobleck* h, const float* audio, void* raw, void* out16, int B,
                                                       h->raw16);
   count_launch();
   h->routes |= SATB_OOB_ROUTE_CUDA_CORE;
-  h->wrote_raw = true;
   return 0;
 }
 
@@ -694,7 +709,7 @@ int encode_impl(SatbOobleck* h, const float* audio, float* latents, int B, int64
   for (int i = 0; i < n; ++i) ratio *= c.strides[i];
   SATB_REQUIRE(T % ratio == 0, "encoder: audio length must be a multiple of the downsampling ratio");
   SATB_REQUIRE(T < (int64_t(1) << 31), "encoder: sequence too long");
-  size_t max_elems = 0;
+  size_t max_elems = static_cast<size_t>(B) * T * c.in_channels;   // a wide input conv's 16-bit copy
   {
     int64_t l = T;
     for (int i = 0; i <= n; ++i) {
@@ -709,7 +724,7 @@ int encode_impl(SatbOobleck* h, const float* audio, float* latents, int B, int64
   void* raw = h->buf_raw;
   void* sA = h->buf_a;
   void* sB = h->buf_b;
-  SATB_PROPAGATE((enc_input<BF16, ACT>(h, audio, raw, sA, B, T, st)));
+  SATB_PROPAGATE((enc_input<BF16, ACT>(h, audio, raw, sA, sB, B, T, st)));
   int64_t Lc = T;
   for (int b = 1; b <= n; ++b) {
     for (int j = 0; j < 3; ++j) SATB_PROPAGATE((enc_residual<BF16, ACT>(h, b, j, B, static_cast<int>(Lc), raw, sA, sB, st)));
@@ -743,7 +758,8 @@ int probe_impl(SatbOobleck* h, SatbOobleckProbe* p, cudaStream_t st) {
     case SATB_OOB_DEC_IN: return dec_input<BF16, ACT>(h, static_cast<const float*>(p->in), p->scratch, p->out16, B, L, st);
     case SATB_OOB_DEC_UP: return dec_upsample<BF16, ACT>(h, b, p->in, p->raw_out, p->out16, B, L, st);
     case SATB_OOB_DEC_OUT: return dec_output<BF16>(h, p->in, p->out32, B, L, st);
-    case SATB_OOB_ENC_IN: return enc_input<BF16, ACT>(h, static_cast<const float*>(p->in), p->raw_out, p->out16, B, L, st);
+    case SATB_OOB_ENC_IN:
+      return enc_input<BF16, ACT>(h, static_cast<const float*>(p->in), p->raw_out, p->out16, p->scratch, B, L, st);
     case SATB_OOB_ENC_DOWN: return enc_downsample<BF16, ACT>(h, b, p->in, p->raw_out, p->out16, B, L, st);
     default: return enc_output<BF16>(h, p->in, p->out32, B, L, st);
   }
@@ -775,7 +791,12 @@ int satb_oobleck_create_variant(const SatbOobleckConfig* cfg, int activation, in
   SATB_REQUIRE(cfg->n_stages >= 1 && cfg->n_stages <= SATB_MAX_STAGES, "bad number of stages");
   SATB_REQUIRE(cfg->channels % 32 == 0, "channels must be a multiple of 32");
   SATB_REQUIRE(cfg->latent_dim % 8 == 0, "latent_dim must be a multiple of 8");
-  SATB_REQUIRE(cfg->in_channels >= 1 && cfg->in_channels <= 2, "audio channels must be 1 or 2");
+  if (!(cfg->in_channels >= 1 && cfg->in_channels <= 2) &&
+      !(cfg->in_channels % 8 == 0 && cfg->in_channels >= 8 && cfg->in_channels <= 128)) {
+    set_last_error("oobleck: in_channels must be 1, 2 (audio) or a multiple of 8 up to 128 (PQMF sub-bands), got " +
+                   std::to_string(cfg->in_channels));
+    return -1;
+  }
   if (activation != SATB_OOB_ACT_SNAKE && activation != SATB_OOB_ACT_ELU) {
     set_last_error("oobleck: unknown activation " + std::to_string(activation) + "; accepted: 0 (snake), 1 (elu)");
     return -1;
@@ -887,7 +908,7 @@ int satb_oobleck_finalize(SatbOobleck* h, void* stream) {
     SATB_PROPAGATE(prep_conv(h, "layers." + std::to_string(n + 2) + ".", h->chans[0], c.in_channels, 7, false, false, false, 1, st));
     SATB_REQUIRE(h->chans[0] % 2 == 0, "decoder: channels must be even");
   } else {
-    SATB_PROPAGATE(prep_conv(h, "layers.0.", c.in_channels, h->chans[0], 7, false, true, true, 1, st));
+    SATB_PROPAGATE(prep_conv(h, "layers.0.", c.in_channels, h->chans[0], 7, false, c.in_channels <= 2, true, 1, st));
     for (int b = 1; b <= n; ++b) {
       const int cin = h->chans[b - 1], cout = h->chans[b], s = c.strides[b - 1];
       const std::string bp = "layers." + std::to_string(b) + ".";
@@ -953,7 +974,7 @@ int satb_oobleck_probe(SatbOobleck* h, SatbOobleckProbe* p, void* stream) {
   const bool raw_out = step == SATB_OOB_DEC_UP || step == SATB_OOB_ENC_IN || step == SATB_OOB_ENC_DOWN || res;
   const bool out16 = step == SATB_OOB_DEC_IN || step == SATB_OOB_DEC_UP || step == SATB_OOB_ENC_IN || step == SATB_OOB_ENC_DOWN;
   const bool out32 = step == SATB_OOB_DEC_OUT || step == SATB_OOB_ENC_OUT;
-  const bool scratch = step == SATB_OOB_DEC_IN || res;
+  const bool scratch = step == SATB_OOB_DEC_IN || res || (step == SATB_OOB_ENC_IN && h->cfg.in_channels > 2);
   const struct { const char* name; const void* ptr; bool used; } bufs[] = {
       {"in", p->in, true}, {"raw_in", p->raw_in, res}, {"raw_out", p->raw_out, raw_out},
       {"out16", p->out16, out16}, {"scratch", p->scratch, scratch}, {"out32", p->out32, out32}};

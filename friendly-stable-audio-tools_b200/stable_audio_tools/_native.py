@@ -115,6 +115,11 @@ SIGNATURES = {
     "satb_oobleck_encode": (_I, [_VP, _VP, _VP, _I, _LL, _VP]),
     "satb_oobleck_probe": (_I, [_VP, ctypes.POINTER(SatbOobleckProbe), _VP]),
     "satb_oobleck_weights": (_I, [_VP, ctypes.c_char_p, _VP, ctypes.POINTER(_LL), _VP]),
+    "satb_pqmf_create": (_I, [_I, _I, ctypes.POINTER(_VP)]),
+    "satb_pqmf_destroy": (None, [_VP]),
+    "satb_pqmf_load_filter": (_I, [_VP, _VP, _VP]),
+    "satb_pqmf_analysis": (_I, [_VP, _VP, _VP, _I, _I, _LL, _VP]),
+    "satb_pqmf_synthesis": (_I, [_VP, _VP, _VP, _I, _I, _I, _VP]),
 }
 
 

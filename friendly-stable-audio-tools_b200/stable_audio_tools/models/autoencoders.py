@@ -13,7 +13,9 @@ fused into the producing epilogue.  Decoders upsample by transposed convolution 
 ``use_nearest_upsample=True``, by nearest-neighbour repetition + a 'same' convolution.  The
 inner blocks are parameter containers.  ``antialias_activation=True`` is refused: it needs
 ``alias_free_torch``, which this package does not ship.  The chunking / cross-fade orchestration is host-side tensor
-slicing on the device, exactly as in the reference.
+slicing on the device, exactly as in the reference.  A nested ``pqmf`` pretransform (``PQMFPretransform``) runs around
+the encoder and decoder where the reference runs it; the encoder then reads, and the decoder writes, io_channels x
+num_bands sub-bands.  Other nested pretransform kinds are refused.
 """
 import ctypes
 import math
@@ -28,6 +30,7 @@ from .. import _native
 from .blocks import SnakeBeta
 from .bottleneck import Bottleneck
 from .factory import create_bottleneck_from_config, create_pretransform_from_config
+from .pretransforms import PQMFPretransform
 from .transformer import _FusedModule
 
 
@@ -123,6 +126,15 @@ def _check_strides(strides, decoder, nearest=False):
                                       "kernel 2s, padding ceil(s/2) gives L / s positions only for s >= 2)")
 
 
+def check_oobleck_io_channels(c, what):
+    """The encoder input / decoder output widths the native Oobleck runs: 1 or 2 audio channels, or the channels x
+    bands of a PQMF pretransform when that is a multiple of 8 up to 128 (its first / last conv then runs on tensor
+    cores over 16-byte rows)."""
+    if not (c in (1, 2) or (c % 8 == 0 and 8 <= c <= 128)):
+        raise NotImplementedError(f"Oobleck: {what} = {c} channels is not supported: the encoder input / decoder "
+                                  "output must be 1 or 2 channels, or a multiple of 8 up to 128")
+
+
 class _NativeOobleck(nn.Module):
     """Shared native-handle plumbing of OobleckEncoder / OobleckDecoder."""
 
@@ -200,6 +212,7 @@ class OobleckEncoder(_NativeOobleck):
         if antialias_activation:
             raise NotImplementedError(_ANTIALIAS_REFUSAL)
         _check_strides(strides, decoder=False)
+        check_oobleck_io_channels(in_channels, "OobleckEncoder in_channels")
         self._init_native(in_channels, channels, latent_dim, c_mults, strides, False, operand_dtype, use_snake=use_snake)
         cm = [1] + list(c_mults)
         self.depth = len(cm)
@@ -237,6 +250,7 @@ class OobleckDecoder(_NativeOobleck):
         if antialias_activation:
             raise NotImplementedError(_ANTIALIAS_REFUSAL)
         _check_strides(strides, decoder=True, nearest=use_nearest_upsample)
+        check_oobleck_io_channels(out_channels, "OobleckDecoder out_channels")
         self._init_native(out_channels, channels, latent_dim, c_mults, strides, final_tanh, operand_dtype,
                           use_snake=use_snake, use_nearest_upsample=use_nearest_upsample)
         cm = [1] + list(c_mults)
@@ -292,13 +306,20 @@ class AudioAutoencoder(nn.Module):
         self.decoder = decoder
         self.bottleneck = bottleneck
         if pretransform is not None:
-            raise NotImplementedError("nested pretransforms are outside the native hot path")
-        self.pretransform = None
+            if not isinstance(pretransform, PQMFPretransform):
+                raise NotImplementedError("nested pretransforms are outside the native hot path")
+            # the encoder reads and the decoder writes io_channels * num_bands sub-bands
+            check_oobleck_io_channels(self.io_channels * pretransform.pqmf.num_bands,
+                                      f"io_channels {self.io_channels} x PQMF num_bands "
+                                      f"{pretransform.pqmf.num_bands}")
+        self.pretransform = pretransform
         self.soft_clip = soft_clip
         self.is_discrete = bool(self.bottleneck is not None and self.bottleneck.is_discrete)
 
     # -- plain encode / decode (reference :268-343) --------------------------------------
     def encode(self, audio, return_info=False, skip_pretransform=False, iterate_batch=False, **kwargs):
+        if self.pretransform is not None and not skip_pretransform:
+            audio = torch.cat([self.pretransform.encode(a) for a in _micro_batches(audio, iterate_batch)], dim=0)
         latents = audio
         if self.encoder is not None:
             latents = torch.cat([self.encoder(a) for a in _micro_batches(audio, iterate_batch)], dim=0)
@@ -312,6 +333,8 @@ class AudioAutoencoder(nn.Module):
         if self.bottleneck is not None:
             latents = torch.cat([self.bottleneck.decode(l) for l in _micro_batches(latents, iterate_batch)], dim=0)
         decoded = torch.cat([self.decoder(l) for l in _micro_batches(latents, iterate_batch)], dim=0)
+        if self.pretransform is not None:
+            decoded = torch.cat([self.pretransform.decode(d) for d in _micro_batches(decoded, iterate_batch)], dim=0)
         if self.soft_clip:
             decoded = torch.tanh(decoded)
         return decoded

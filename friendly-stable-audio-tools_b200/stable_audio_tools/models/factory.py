@@ -21,15 +21,23 @@ def create_model_from_config_path(model_config_path):
 
 def create_pretransform_from_config(pretransform_config, sample_rate):
     kind = pretransform_config["type"]
-    if kind != "autoencoder":
-        raise NotImplementedError(f"pretransform '{kind}' is outside the native hot path (autoencoder only)")
-    from .autoencoders import create_autoencoder_from_config
-    from .pretransforms import AutoencoderPretransform
-    # the autoencoder factory wants a top-level config carrying the sample rate
-    autoencoder = create_autoencoder_from_config({"sample_rate": sample_rate, "model": pretransform_config["config"]})
-    pretransform = AutoencoderPretransform(
-        autoencoder, scale=pretransform_config.get("scale", 1.0), model_half=pretransform_config.get("model_half", False),
-        iterate_batch=pretransform_config.get("iterate_batch", False), chunked=pretransform_config.get("chunked", False))
+    if kind == "autoencoder":
+        from .autoencoders import create_autoencoder_from_config
+        from .pretransforms import AutoencoderPretransform
+        # the autoencoder factory wants a top-level config carrying the sample rate
+        autoencoder = create_autoencoder_from_config({"sample_rate": sample_rate, "model": pretransform_config["config"]})
+        pretransform = AutoencoderPretransform(
+            autoencoder, scale=pretransform_config.get("scale", 1.0),
+            model_half=pretransform_config.get("model_half", False),
+            iterate_batch=pretransform_config.get("iterate_batch", False),
+            chunked=pretransform_config.get("chunked", False))
+    elif kind == "pqmf":
+        from .pretransforms import PQMFPretransform
+        pretransform = PQMFPretransform(**pretransform_config["config"])
+    else:
+        # wavelet needs pywt; dac_pretrained and audiocraft_pretrained need the dac / audiocraft packages and their
+        # downloaded checkpoints.  None of them is shipped with this package.
+        raise NotImplementedError(f"pretransform '{kind}' is outside the native hot path (autoencoder and pqmf only)")
     enable_grad = pretransform_config.get("enable_grad", False)
     pretransform.enable_grad = enable_grad
     pretransform.eval().requires_grad_(enable_grad)

@@ -24,6 +24,7 @@ extern "C" {
 
 typedef struct SatbDit SatbDit;
 typedef struct SatbOobleck SatbOobleck;
+typedef struct SatbPqmf SatbPqmf;
 
 /* Mirrors the constructor kwargs of DiffusionTransformer
  * (reference stable_audio_tools/models/dit.py:15-30) for the continuous_transformer backbone. */
@@ -51,7 +52,8 @@ typedef struct SatbDitConfig {
 /* Mirrors OobleckEncoder/OobleckDecoder kwargs (models/autoencoders.py:119-194). */
 #define SATB_MAX_STAGES 8
 typedef struct SatbOobleckConfig {
-  int in_channels;          /* audio channels (encoder input / decoder output) */
+  int in_channels;          /* encoder input / decoder output channels: 1 or 2 (audio), or a multiple of 8 up to 128
+                               (the channels * num_bands sub-bands of a PQMF pretransform) */
   int channels;
   int latent_dim;           /* decoder input channels / encoder output channels */
   int n_stages;             /* len(c_mults) == len(strides) */
@@ -280,7 +282,7 @@ int satb_oobleck_encode(SatbOobleck* h, const float* audio, float* latents, int 
  *   DEC_UP    block b: in (16-bit, L positions) -> raw_out, out16 (L * stride positions)
  *   DEC_RES   unit (b, j): in (16-bit), raw_in -> raw_out (if wrote_raw), the result in `in` or `scratch`
  *   DEC_OUT   in (16-bit) -> out32 (NCL fp32 audio)
- *   ENC_IN    in: fp32 NCL audio [B, in_channels, L] -> raw_out, out16
+ *   ENC_IN    in: fp32 NCL audio [B, in_channels, L] -> raw_out, out16; with in_channels > 2, scratch: its 16-bit copy
  *   ENC_RES   unit (b, j), as DEC_RES
  *   ENC_DOWN  block b: in (16-bit, L positions, a multiple of the stride) -> raw_out (if wrote_raw), out16
  *   ENC_OUT   in (16-bit) -> out32 (NCL fp32 pre-bottleneck)
@@ -321,6 +323,22 @@ int satb_oobleck_probe(SatbOobleck* h, SatbOobleckProbe* p, void* stream);
  * fp16x3 mode, its lo block right after it), or the fp32 [cout][cin][k] weights of a CUDA-core conv.  *bytes gets
  * the size; dst (device, may be NULL to ask for the size) receives the data. */
 int satb_oobleck_weights(SatbOobleck* h, const char* prefix, void* dst, long long* bytes, void* stream);
+
+/* ---- PQMF filterbank: replaces PQMF.forward / PQMF.inverse (models/pqmf.py) behind PQMFPretransform.encode / decode
+ *      (models/pretransforms.py:114-133), fp32 on the CUDA cores.
+ * num_bands: a power of 2 in [2, 256]; taps: the filter bank's length (the reference pads it to a power of two), a
+ * multiple of 2 * num_bands, at most 16384.  Every call checks its arguments before any CUDA call. */
+int satb_pqmf_create(int num_bands, int taps, SatbPqmf** out);
+void satb_pqmf_destroy(SatbPqmf* h);
+/* filter_bank: device [num_bands, taps] (the "pqmf.filter_bank" buffer).  Builds the handle's polyphase weights on
+ * `stream`; call it again after the buffer changes. */
+int satb_pqmf_load_filter(SatbPqmf* h, const float* filter_bank, void* stream);
+/* audio [B, C, T] -> bands [B, C * num_bands, ceil(T / num_bands)] (band k of channel c at row c * num_bands + k):
+ * the signal zero-padded to a multiple of num_bands, polyphase analysis, alias cancellation (PQMF.forward + the
+ * pretransform's "b c n t -> b (c n) t"). */
+int satb_pqmf_analysis(SatbPqmf* h, const float* audio, float* bands, int B, int C, long long T, void* stream);
+/* bands [B, C * num_bands, frames] -> audio [B, C, frames * num_bands] (PQMF.inverse). */
+int satb_pqmf_synthesis(SatbPqmf* h, const float* bands, float* audio, int B, int C, int frames, void* stream);
 
 #ifdef __cplusplus
 }
