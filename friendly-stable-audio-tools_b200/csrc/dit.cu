@@ -153,6 +153,10 @@ using namespace satb;
 struct SatbDit {
   SatbDitConfig cfg;
   int D, H, dh, C, Cin, ct, ce, gd, ge, ffi, depth, F, nf;   // C = output channels, Cin = C + input_concat_dim
+  // row pitches of project_in's input (Cin up to a multiple of 8: 16-byte TMA rows) and of project_out's output y (C up
+  // to a multiple of 32: EpiStore32's column chunk).  The folded weights carry zero columns / rows in the padding, so
+  // the padded products are exact; an aligned width pads nothing.
+  int Cin_p, C_p;
   int pdim = 0;               // prepend_cond_dim
   float *pe0_w = nullptr, *pe2_w = nullptr;   // to_prepend_embed (fp32, bias-free)
   int Pp = 0;                 // prepend-conditioning tokens of the current conditioning
@@ -364,9 +368,11 @@ int satb_dit_create(const SatbDitConfig* cfg, SatbDit** out) {
   const int dh = cfg->num_heads > 0 ? cfg->embed_dim / cfg->num_heads : 0;
   SATB_REQUIRE(dh == 32 || dh == 64 || dh == 96 || dh == 128, "head dim (embed_dim / num_heads) must be 32, 64, 96 or 128");
   SATB_REQUIRE(!(cfg->qk_norm && dh != 64), "qk_norm is supported with head dim 64 only");
-  SATB_REQUIRE(cfg->io_channels % 8 == 0 && cfg->io_channels % 32 == 0, "io_channels must be a multiple of 32");
+  SATB_REQUIRE(cfg->io_channels >= 1, "io_channels must be >= 1");
   SATB_REQUIRE(cfg->patch_size == 1, "patch_size 1 only");
-  SATB_REQUIRE(cfg->input_concat_dim >= 0 && cfg->input_concat_dim % 8 == 0, "input_concat_dim must be a multiple of 8");
+  SATB_REQUIRE(cfg->input_concat_dim >= 0, "input_concat_dim must be >= 0");
+  SATB_REQUIRE(static_cast<long long>(cfg->io_channels) + cfg->input_concat_dim <= 32768,
+               "io_channels + input_concat_dim must be at most 32768");
   SATB_REQUIRE(cfg->prepend_cond_dim >= 0 && cfg->prepend_cond_dim % 4 == 0, "prepend_cond_dim must be a multiple of 4");
   SATB_REQUIRE(!(cfg->prepend_cond_dim > 0 && cfg->global_cond_type == 1),
                "prepend conditioning is supported with global_cond_type \"prepend\" only");
@@ -378,6 +384,8 @@ int satb_dit_create(const SatbDitConfig* cfg, SatbDit** out) {
   d->dh = d->D / d->H;
   d->C = cfg->io_channels;
   d->Cin = cfg->io_channels + (cfg->input_concat_dim > 0 ? cfg->input_concat_dim : 0);
+  d->Cin_p = (d->Cin + 7) / 8 * 8;
+  d->C_p = (d->C + 31) / 32 * 32;
   d->pdim = cfg->prepend_cond_dim > 0 ? cfg->prepend_cond_dim : 0;
   d->ct = cfg->cond_token_dim;
   d->ce = cfg->project_cond_tokens ? d->D : d->ct;
@@ -682,12 +690,14 @@ int satb_dit_finalize(SatbDit* d, void* stream_v) {
   SATB_CHECK_CUDA(cudaMemcpy(pout.data(), d->pout_w, pout.size() * 4, cudaMemcpyDeviceToHost));
   SATB_CHECK_CUDA(cudaMemcpy(pre.data(), d->pre_w, pre.size() * 4, cudaMemcpyDeviceToHost));
   SATB_CHECK_CUDA(cudaMemcpy(post.data(), d->post_w, post.size() * 4, cudaMemcpyDeviceToHost));
-  std::vector<float> fin(static_cast<size_t>(D) * Cin), fout(static_cast<size_t>(C) * D);
+  // stored at the padded pitches: fin [D, Cin_p] with zero columns Cin .., fout [C_p, D] with zero rows C ..
+  const int Cin_p = d->Cin_p, C_p = d->C_p;
+  std::vector<float> fin(static_cast<size_t>(D) * Cin_p, 0.f), fout(static_cast<size_t>(C_p) * D, 0.f);
   for (int n = 0; n < D; ++n)
     for (int c = 0; c < Cin; ++c) {
       double acc = pin[static_cast<size_t>(n) * Cin + c];
       for (int j = 0; j < Cin; ++j) acc += static_cast<double>(pin[static_cast<size_t>(n) * Cin + j]) * pre[j * Cin + c];
-      fin[static_cast<size_t>(n) * Cin + c] = static_cast<float>(acc);
+      fin[static_cast<size_t>(n) * Cin_p + c] = static_cast<float>(acc);
     }
   for (int c = 0; c < C; ++c)
     for (int k = 0; k < D; ++k) {
@@ -702,8 +712,8 @@ int satb_dit_finalize(SatbDit* d, void* stream_v) {
   SATB_CHECK_CUDA(cudaMemcpy(tmp_out, fout.data(), fout.size() * 4, cudaMemcpyHostToDevice));
   if (!d->w_in16) SATB_PROPAGATE(d->alloc(&d->w_in16, fin.size()));
   if (!d->w_out16) SATB_PROPAGATE(d->alloc(&d->w_out16, fout.size()));
-  int rc = launch_cast_rows(tmp_in, d->w_in16, nullptr, D, Cin, Cin, Cin, d->bf16, st);
-  if (rc == 0) rc = launch_cast_rows(tmp_out, d->w_out16, nullptr, C, D, D, D, d->bf16, st);
+  int rc = launch_cast_rows(tmp_in, d->w_in16, nullptr, D, Cin_p, Cin_p, Cin_p, d->bf16, st);
+  if (rc == 0) rc = launch_cast_rows(tmp_out, d->w_out16, nullptr, C_p, D, D, D, d->bf16, st);
   cudaStreamSynchronize(st);
   cudaFree(tmp_in);
   cudaFree(tmp_out);
@@ -788,8 +798,8 @@ int satb_dit_reserve(SatbDit* d, int R, int L) {
   SATB_PROPAGATE(d->ws_q16.ensure(M * D * 2));
   // the FF intermediate [M, ffi], and the conformer branch's two [M, D] intermediates
   SATB_PROPAGATE(d->ws_ff.ensure(M * std::max(d->ffi, d->conformer ? 2 * D : 0) * 2));
-  SATB_PROPAGATE(d->ws_ain.ensure(M * d->Cin * 2));
-  SATB_PROPAGATE(d->ws_y.ensure(M * d->C * 4));
+  SATB_PROPAGATE(d->ws_ain.ensure(M * d->Cin_p * 2));
+  SATB_PROPAGATE(d->ws_y.ensure(M * d->C_p * 4));
   if (d->fp8) {
     SATB_PROPAGATE(d->ws_a8.ensure(M * D));
     SATB_PROPAGATE(d->ws_ascale.ensure(M * 4));
@@ -973,13 +983,15 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
   SATB_PROPAGATE(launch_skinny_linear(sw.te_h, d->te2_w, d->te2_b, d->has_global ? sw.ge : nullptr, sw.tok, B, D, D,
                                       d->adaln ? 1 : 0, st));
   // latent -> token rows, project_in (with the 1x1 pre-conv folded), prepend token; a positional embedding is added to
-  // every row, prepended ones included, in project_in's epilogue and by write_prepend
-  SATB_PROPAGATE(launch_dit_pre(x, ain, R, B, d->Cin, L, P, BF16, st));
+  // every row, prepended ones included, in project_in's epilogue and by write_prepend.  K is Cin_p: the pad columns of
+  // ain (zeroed by dit_pre) meet the zero columns of w_in16.
+  const int Kin = d->Cin_p;
+  SATB_PROPAGATE(launch_dit_pre(x, ain, R, B, d->Cin, Kin, L, P, BF16, st));
   if (pos_tab)
-    SATB_PROPAGATE((linear<EpiStore32Pos, 256, BF16>(d->tmaps, ain, d->Cin, M, d->Cin, d->w_in16, D,
+    SATB_PROPAGATE((linear<EpiStore32Pos, 256, BF16>(d->tmaps, ain, Kin, M, Kin, d->w_in16, D,
                                                      EpiStore32Pos::Params{h, D, nullptr, pos_tab, N_seq}, st)));
   else
-    SATB_PROPAGATE((linear<EpiStore32, 256, BF16>(d->tmaps, ain, d->Cin, M, d->Cin, d->w_in16, D, EpiStore32::Params{h, D, nullptr}, st)));
+    SATB_PROPAGATE((linear<EpiStore32, 256, BF16>(d->tmaps, ain, Kin, M, Kin, d->w_in16, D, EpiStore32::Params{h, D, nullptr}, st)));
   const int64_t ssg_ld = static_cast<int64_t>(d->depth) * 6 * D;
   if (P > 0) {
     SATB_PROPAGATE(launch_write_prepend(sw.tok, d->Pp > 0 ? d->ws_prep.as<float>() : nullptr, pos_tab, h, R, B, N_seq, D,
@@ -1115,10 +1127,12 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
   }
   if (hidden_out)
     SATB_CHECK_CUDA(cudaMemcpyAsync(hidden_out, h, static_cast<size_t>(M) * D * 4, cudaMemcpyDeviceToDevice, st));
-  // project_out (with the 1x1 post-conv folded) reads a 16-bit copy of h
+  // project_out (with the 1x1 post-conv folded) reads a 16-bit copy of h; its N is C_p (zero weight rows past C), and
+  // dit_post reads the C real channels of each y row
+  const int Cp = d->C_p;
   SATB_PROPAGATE(launch_cast_rows(h, a16, nullptr, M, D, D, D, BF16, st));
-  SATB_PROPAGATE((linear<EpiStore32, 64, BF16>(d->tmaps, a16, D, M, D, d->w_out16, C, EpiStore32::Params{y, C, nullptr}, st)));
-  SATB_PROPAGATE(launch_dit_post(y, out, B, C, L, N_seq, P, d->cfg_on ? 1 : 0, cfg_scale, scale_phi, st));
+  SATB_PROPAGATE((linear<EpiStore32, 64, BF16>(d->tmaps, a16, D, M, D, d->w_out16, Cp, EpiStore32::Params{y, Cp, nullptr}, st)));
+  SATB_PROPAGATE(launch_dit_post(y, Cp, out, B, C, L, N_seq, P, d->cfg_on ? 1 : 0, cfg_scale, scale_phi, st));
   return 0;
 }
 
@@ -1374,6 +1388,13 @@ int satb_token_conv_probe(const void* a16, long long item_stride, const void* w1
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   return p->bf16 ? token_conv_probe<true>(a16, item_stride, w16, R, n_seq, K, N, k, *p, st)
                  : token_conv_probe<false>(a16, item_stride, w16, R, n_seq, K, N, k, *p, st);
+}
+
+int satb_dit_pre_probe(const float* x, void* a16, int R, int B_src, int C, int lda, int L, int P, int bf16, void* stream) {
+  SATB_REQUIRE(x && a16, "null argument");
+  SATB_REQUIRE(R >= 1 && B_src >= 1 && C >= 1 && L >= 1 && P >= 0, "dit pre probe: need R, B_src, C, L >= 1 and P >= 0");
+  SATB_REQUIRE(lda >= C && lda % 8 == 0, "dit pre probe: need lda >= C and lda % 8 == 0");
+  return launch_dit_pre(x, a16, R, B_src, C, lda, L, P, bf16 != 0, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

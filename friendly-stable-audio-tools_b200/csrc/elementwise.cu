@@ -275,11 +275,13 @@ __global__ void __launch_bounds__(256) snake_beta_kernel(const float* __restrict
 }
 
 // ------------------------------------------------------------------ DiT pre
-// NCL fp32 latent -> token-major 16-bit rows [R*N_seq, C]; the P leading rows of every
-// item (the prepend slots) are zero so the project_in GEMM leaves them 0.
+// NCL fp32 latent -> token-major 16-bit rows [R*N_seq, lda]; the P leading rows of every
+// item (the prepend slots) are zero so the project_in GEMM leaves them 0.  Columns C .. lda-1
+// (the row pitch padded up to 16 bytes for TMA) are written as zeros on every call too, so the
+// zero-padded K of project_in never reads stale memory.
 template <bool BF16>
 __global__ void __launch_bounds__(256) dit_pre_kernel(const float* __restrict__ x, uint16_t* __restrict__ a, int B_src,
-                                                      int C, int L, int P) {
+                                                      int C, int lda, int L, int P) {
   __shared__ float tile[32][33];
   const int r = blockIdx.z;
   const int l0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
@@ -293,16 +295,16 @@ __global__ void __launch_bounds__(256) dit_pre_kernel(const float* __restrict__ 
   __syncthreads();
   for (int j = ty; j < 32; j += 8) {
     const int l = l0 + j, c = c0 + tx;
-    if (l < L && c < C)
+    if (l < L && c < lda)
     {
-      typename Op16<BF16>::T hv = Op16<BF16>::from_float(tile[tx][j]);
-      a[(static_cast<size_t>(r) * N_seq + P + l) * C + c] = *reinterpret_cast<uint16_t*>(&hv);
+      typename Op16<BF16>::T hv = Op16<BF16>::from_float(tile[tx][j]);   // tile holds 0 for c >= C
+      a[(static_cast<size_t>(r) * N_seq + P + l) * lda + c] = *reinterpret_cast<uint16_t*>(&hv);
     }
   }
   if (blockIdx.x == 0 && P > 0) {
     for (int j = ty; j < P; j += 8) {
       const int c = c0 + tx;
-      if (c < C) a[(static_cast<size_t>(r) * N_seq + j) * C + c] = 0;
+      if (c < lda) a[(static_cast<size_t>(r) * N_seq + j) * lda + c] = 0;
     }
   }
 }
@@ -424,20 +426,22 @@ __global__ void gate_sigmoid_kernel(float* __restrict__ ssg, int depth, int D) {
 
 // ------------------------------------------------------------------ DiT post
 // models/dit.py:219 (drop prepend), :338-347 (CFG combine, std rescale over channels).
-// y rows are token-major [R*N_seq, C]; one thread per (b, l).
-__global__ void __launch_bounds__(128) dit_post_kernel(const float* __restrict__ y, float* __restrict__ out, int B,
-                                                       int C, int L, int N_seq, int P, int cfg, float cfg_scale,
+// y rows are token-major [R*N_seq, ldy] (ldy >= C: project_out's N padded up to its store width; only the C real
+// channels are read); one thread per (b, l).  C = 1 with scale_phi != 0 gives NaN, as torch.std (unbiased) of one
+// channel does in the reference.
+__global__ void __launch_bounds__(128) dit_post_kernel(const float* __restrict__ y, int ldy, float* __restrict__ out,
+                                                       int B, int C, int L, int N_seq, int P, int cfg, float cfg_scale,
                                                        float scale_phi) {
   const int l = blockIdx.x * blockDim.x + threadIdx.x;
   const int b = blockIdx.y;
   if (l >= L) return;
-  const float* yc = y + (static_cast<size_t>(b) * N_seq + P + l) * C;
+  const float* yc = y + (static_cast<size_t>(b) * N_seq + P + l) * ldy;
   float* o = out + static_cast<size_t>(b) * C * L + l;
   if (!cfg) {
     for (int c = 0; c < C; ++c) o[static_cast<size_t>(c) * L] = yc[c];
     return;
   }
-  const float* yu = y + (static_cast<size_t>(B + b) * N_seq + P + l) * C;
+  const float* yu = y + (static_cast<size_t>(B + b) * N_seq + P + l) * ldy;
   if (scale_phi == 0.f) {
     for (int c = 0; c < C; ++c) {
       const float cv = yc[c], uv = yu[c];
@@ -614,12 +618,14 @@ int launch_snake_beta(const float* x, const float* alpha, const float* beta, flo
   return 0;
 }
 
-int launch_dit_pre(const float* x, void* a16, int R, int B_src, int C, int L, int P, bool bf16, cudaStream_t stream) {
-  dim3 grid(ceil_div(L, 32), ceil_div(C, 32), R);
+int launch_dit_pre(const float* x, void* a16, int R, int B_src, int C, int lda, int L, int P, bool bf16,
+                   cudaStream_t stream) {
+  SATB_REQUIRE(lda >= C, "dit_pre: the row pitch must cover the channels");
+  dim3 grid(ceil_div(L, 32), ceil_div(lda, 32), R);
   if (bf16)
-    dit_pre_kernel<true><<<grid, 256, 0, stream>>>(x, static_cast<uint16_t*>(a16), B_src, C, L, P);
+    dit_pre_kernel<true><<<grid, 256, 0, stream>>>(x, static_cast<uint16_t*>(a16), B_src, C, lda, L, P);
   else
-    dit_pre_kernel<false><<<grid, 256, 0, stream>>>(x, static_cast<uint16_t*>(a16), B_src, C, L, P);
+    dit_pre_kernel<false><<<grid, 256, 0, stream>>>(x, static_cast<uint16_t*>(a16), B_src, C, lda, L, P);
   count_launch();
   SATB_CHECK_CUDA(cudaGetLastError());
   return 0;
@@ -663,10 +669,11 @@ int launch_gate_sigmoid(float* ssg, int rows, int depth, int D, cudaStream_t str
   return 0;
 }
 
-int launch_dit_post(const float* y, float* out, int B, int C, int L, int N_seq, int P, int cfg, float cfg_scale,
-                    float scale_phi, cudaStream_t stream) {
+int launch_dit_post(const float* y, int ldy, float* out, int B, int C, int L, int N_seq, int P, int cfg,
+                    float cfg_scale, float scale_phi, cudaStream_t stream) {
+  SATB_REQUIRE(ldy >= C, "dit_post: the row pitch must cover the channels");
   dim3 grid(ceil_div(L, 128), B);
-  dit_post_kernel<<<grid, 128, 0, stream>>>(y, out, B, C, L, N_seq, P, cfg, cfg_scale, scale_phi);
+  dit_post_kernel<<<grid, 128, 0, stream>>>(y, ldy, out, B, C, L, N_seq, P, cfg, cfg_scale, scale_phi);
   count_launch();
   SATB_CHECK_CUDA(cudaGetLastError());
   return 0;

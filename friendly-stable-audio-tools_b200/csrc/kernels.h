@@ -35,8 +35,10 @@ int launch_sampler_update(const float* x, const float* v, const float* d1, const
 // SnakeBeta on [B, C, T] fp32 (log-scale alpha/beta per channel).
 int launch_snake_beta(const float* x, const float* alpha, const float* beta, float* y, int B, int C, int64_t T,
                       int logscale, cudaStream_t stream);
-// x[B_src, C, L] fp32 -> a16[(r*N_seq + P + l), c] (rows r*N_seq .. +P-1 zero), r < R, source row r % B_src.
-int launch_dit_pre(const float* x, void* a16, int R, int B_src, int C, int L, int P, bool bf16, cudaStream_t stream);
+// x[B_src, C, L] fp32 -> a16[(r*N_seq + P + l), c] at row pitch lda >= C (rows r*N_seq .. +P-1 and columns
+// C .. lda-1 zero), r < R, source row r % B_src.
+int launch_dit_pre(const float* x, void* a16, int R, int B_src, int C, int lda, int L, int P, bool bf16,
+                   cudaStream_t stream);
 // Fourier timestep features [B, 2*F]: cat(cos(2*pi*t*w), sin(2*pi*t*w)).
 int launch_fourier(const float* t, const float* w, float* out, int B, int F, cudaStream_t stream);
 // out[r, n] = act_out(sum_k in[r, k] * W[n, k] + bias[n] (+ add[r, n])); fp32 weights; act_out = SiLU if silu_out.
@@ -48,9 +50,9 @@ int launch_write_prepend(const float* tok, const float* pre, const float* pos, f
                          int Pp, cudaStream_t stream);
 // in place: x = sigmoid(1 - x) on column ranges [c0, c0+D) and [c1, c1+D) of every 6D-wide layer block
 int launch_gate_sigmoid(float* ssg, int rows, int depth, int D, cudaStream_t stream);
-// y[R*N_seq, C] fp32 -> out[B, C, L] with CFG combine / rescale (models/dit.py:338-347)
-int launch_dit_post(const float* y, float* out, int B, int C, int L, int N_seq, int P, int cfg, float cfg_scale,
-                    float scale_phi, cudaStream_t stream);
+// y[R*N_seq, ldy] fp32 (its first C columns) -> out[B, C, L] with CFG combine / rescale (models/dit.py:338-347)
+int launch_dit_post(const float* y, int ldy, float* out, int B, int C, int L, int N_seq, int P, int cfg,
+                    float cfg_scale, float scale_phi, cudaStream_t stream);
 // generic fp32 -> 16-bit cast with row gather: dst[r, :] = src[perm ? perm[r] : r, :] * row_scale
 int launch_cast_rows(const float* src, void* dst, const int* perm, int rows, int cols, int64_t src_ld, int64_t dst_ld,
                      bool bf16, cudaStream_t stream);

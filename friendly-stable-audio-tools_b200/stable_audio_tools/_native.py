@@ -102,6 +102,7 @@ SIGNATURES = {
     "satb_gemm_probe": (_I, [_VP, _VP, _I, _I, _I, ctypes.POINTER(SatbGemmProbe), _VP]),
     "satb_gemm_probe_fp8": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, ctypes.POINTER(SatbGemmProbe), _VP]),
     "satb_token_conv_probe": (_I, [_VP, _LL, _VP, _I, _I, _I, _I, _I, ctypes.POINTER(SatbGemmProbe), _VP]),
+    "satb_dit_pre_probe": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _I, _I, _VP]),
     "satb_attention": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP]),
     "satb_attention_hd": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _VP]),
     "satb_attention_probe": (_I, [ctypes.POINTER(SatbAttentionProbe), _VP]),

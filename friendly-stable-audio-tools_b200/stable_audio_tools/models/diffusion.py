@@ -112,7 +112,19 @@ def create_diffusion_cond_from_config(config: tp.Dict[str, tp.Any]):
     diff_cfg = model_cfg["diffusion"]
     if diff_cfg["type"] != "dit":
         raise NotImplementedError(f"diffusion backbone '{diff_cfg['type']}' is outside the native hot path (DiT only)")
-    if model_type not in ("diffusion_cond", "diffusion_cond_inpaint"):
+    extra = {}
+    if model_type in ("diffusion_cond", "diffusion_cond_inpaint"):
+        wrapper_fn = ConditionedDiffusionModelWrapper
+        extra["diffusion_objective"] = diff_cfg.get("diffusion_objective", "v")
+    elif model_type == "diffusion_prior":
+        # reference diffusion.py:636-641: the prior wrapper gets no diffusion_objective, so it keeps the default "v"
+        prior_type = model_cfg["prior_type"]
+        if prior_type != "mono_stereo":
+            raise NotImplementedError(f"prior_type '{prior_type}' is not a diffusion prior of the reference "
+                                      "(mono_stereo only)")
+        from .diffusion_prior import MonoToStereoDiffusionPrior
+        wrapper_fn = MonoToStereoDiffusionPrior
+    else:
         raise NotImplementedError(f"model_type '{model_type}' is outside the native hot path")
     denoiser = DiTWrapper(**diff_cfg["config"])
     conditioner = None
@@ -125,9 +137,9 @@ def create_diffusion_cond_from_config(config: tp.Dict[str, tp.Any]):
         pretransform = create_pretransform_from_config(pretransform, config["sample_rate"])
         min_len = pretransform.downsampling_ratio
     min_len *= denoiser.model.patch_size
-    return ConditionedDiffusionModelWrapper(
+    return wrapper_fn(
         denoiser, conditioner, min_input_length=min_len, sample_rate=config["sample_rate"],
         cross_attn_cond_ids=diff_cfg.get("cross_attention_cond_ids", []),
         global_cond_ids=diff_cfg.get("global_cond_ids", []), input_concat_ids=diff_cfg.get("input_concat_ids", []),
         prepend_cond_ids=diff_cfg.get("prepend_cond_ids", []), pretransform=pretransform,
-        io_channels=model_cfg["io_channels"], diffusion_objective=diff_cfg.get("diffusion_objective", "v"))
+        io_channels=model_cfg["io_channels"], **extra)

@@ -17,7 +17,9 @@ and parameter names, ``forward`` signature and CFG semantics); the arithmetic ru
   native feed-forward variant (``satb_dit_set_feedforward``); its token convolutions run as k-tap GEMMs over each
   item, with 16-bit operands in every ``operand_dtype``;
 * ``rotary_pos_emb=False``, ``use_sinusoidal_emb`` and ``use_abs_pos_emb`` select the native positional options
-  (``satb_dit_set_positions``); the embedding is added to every row, prepended ones included, in project_in's epilogue.
+  (``satb_dit_set_positions``); the embedding is added to every row, prepended ones included, in project_in's epilogue;
+* any ``io_channels`` and ``input_concat_dim`` (an inpainting DiT's latent + 1 mask channel, PQMF sub-bands, raw audio):
+  the library pads project_in's K to a multiple of 8 and project_out's N to a multiple of 32 with zero weights.
 
 There is no eager / CPU fallback: tensors must live on a CUDA device.
 """
@@ -70,6 +72,12 @@ class DiffusionTransformer(nn.Module):
         check_head_dim(embed_dim // num_heads, bool(kwargs.get("attn_kwargs", {}).get("qk_norm", False)))
         if patch_size < 1:
             raise ValueError("patch_size must be >= 1")
+        # any width runs natively (project_in's K and project_out's N are zero-padded inside the library); these are
+        # the only widths it refuses
+        if io_channels < 1:
+            raise ValueError(f"io_channels must be >= 1, got {io_channels}")
+        if input_concat_dim < 0:
+            raise ValueError(f"input_concat_dim must be >= 0, got {input_concat_dim}")
         if global_cond_type not in ("prepend", "adaLN"):
             raise ValueError(f"unknown global_cond_type {global_cond_type}")
         if operand_dtype not in OPERAND_DTYPES:

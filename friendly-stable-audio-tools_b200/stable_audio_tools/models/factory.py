@@ -7,11 +7,12 @@ def create_model_from_config(model_config):
     if model_type == "autoencoder":
         from .autoencoders import create_autoencoder_from_config
         return create_autoencoder_from_config(model_config)
-    if model_type in ("diffusion_cond", "diffusion_cond_inpaint"):
+    if model_type in ("diffusion_cond", "diffusion_cond_inpaint", "diffusion_prior"):
         from .diffusion import create_diffusion_cond_from_config
         return create_diffusion_cond_from_config(model_config)
     raise NotImplementedError(
-        f"model_type '{model_type}' is outside the H100-native hot path (supported: autoencoder, diffusion_cond)")
+        f"model_type '{model_type}' is outside the H100-native hot path (supported: autoencoder, diffusion_cond, "
+        "diffusion_cond_inpaint, diffusion_prior)")
 
 
 def create_model_from_config_path(model_config_path):

@@ -202,6 +202,10 @@ int satb_gemm_probe_fp8(const void* a8, const void* w8, const float* a_scale, co
  * k odd, K % 8 == 0, N % 32 == 0; pointers 16-byte aligned. */
 int satb_token_conv_probe(const void* a16, long long item_stride, const void* w16, int R, int n_seq, int K, int N, int k,
                           const SatbGemmProbe* p, void* stream);
+/* Test entry point: the DiT forward's token-row kernel (the project_in GEMM's A operand).  x [B_src, C, L] fp32 ->
+ * a16 [R * (P + L), lda] 16-bit (bf16 or fp16) with lda >= C, lda % 8 == 0: row r * (P + L) + P + l, column c holds
+ * x[r % B_src, c, l]; the P leading rows of every item and the columns C .. lda-1 of every row are written as zeros. */
+int satb_dit_pre_probe(const float* x, void* a16, int R, int B_src, int C, int lda, int L, int P, int bf16, void* stream);
 /* One step of the v-objective k-diffusion samplers in a single pass over the latents (replaces the
  * ~20 elementwise torch kernels of K.external.VDenoiser.forward + sample_dpmpp_{2m,3m}_sde's update,
  * reference call sites inference/sampling.py:159,225-228): with v = model(x * c_in, t),
