@@ -6,6 +6,11 @@
 
 using namespace satb;
 
+namespace {
+inline bool aligned_to(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
+constexpr int kMaxGridYZ = 65535;
+}  // namespace
+
 extern "C" {
 
 int satb_snake_beta(const float* x, const float* alpha, const float* beta, float* y, int B, int C, long long T,
@@ -29,6 +34,81 @@ int satb_layernorm_fp8(const float* x, const float* gamma, const float* beta, co
                "adaLN modulation needs shift, rows_per_item >= 1, n_items >= 1 and mod_stride % 4 == 0");
   return launch_layernorm_fp8(x, gamma, beta, out8, row_scale, rows, D, mod_scale, mod_shift, mod_stride,
                               rows_per_item, n_items, static_cast<cudaStream_t>(stream));
+}
+
+// ---- test entry points of the small kernels: argument checks, then the launch function the forward calls
+int satb_layernorm_mod(const float* x, const float* gamma, const float* beta, const float* mod_scale,
+                       const float* mod_shift, long long mod_stride, int rows_per_item, int n_items, void* out16,
+                       int rows, int D, int bf16, void* stream) {
+  SATB_REQUIRE(x && gamma && out16, "null argument");
+  SATB_REQUIRE(!mod_scale || (mod_shift && rows_per_item >= 1 && n_items >= 1 && mod_stride % 4 == 0),
+               "adaLN modulation needs shift, rows_per_item >= 1, n_items >= 1 and mod_stride % 4 == 0");
+  SATB_REQUIRE(aligned_to(x, 16) && aligned_to(gamma, 16) && aligned_to(beta, 16) && aligned_to(mod_scale, 16) &&
+                   aligned_to(mod_shift, 16) && aligned_to(out16, 8),
+               "LayerNorm: x, gamma, beta and the modulation must be 16-byte aligned, out 8-byte aligned");
+  SATB_REQUIRE(rows >= 0, "LayerNorm: negative row count");
+  return launch_layernorm(x, gamma, beta, out16, rows, D, mod_scale, mod_shift, mod_stride, mod_scale ? rows_per_item : 1,
+                          mod_scale ? n_items : 1, bf16 != 0, static_cast<cudaStream_t>(stream));
+}
+
+int satb_fourier_probe(const float* t, const float* w, float* out, int B, int F, void* stream) {
+  SATB_REQUIRE(t && w && out, "null argument");
+  SATB_REQUIRE(B >= 1 && F >= 1 && static_cast<long long>(B) * F <= (1 << 30), "fourier probe: need B, F >= 1");
+  return launch_fourier(t, w, out, B, F, static_cast<cudaStream_t>(stream));
+}
+
+int satb_skinny_linear_probe(const float* in, const float* W, const float* bias, const float* add, float* out, int R,
+                             int K, int N, int silu_out, void* stream) {
+  SATB_REQUIRE(in && W && out, "null argument");
+  SATB_REQUIRE(aligned_to(in, 16) && aligned_to(W, 16), "skinny linear probe: in and W must be 16-byte aligned");
+  SATB_REQUIRE(K >= 4 && N >= 1, "skinny linear probe: need K >= 4 and N >= 1");
+  return launch_skinny_linear(in, W, bias, add, out, R, K, N, silu_out, static_cast<cudaStream_t>(stream));
+}
+
+int satb_write_prepend_probe(const float* tok, const float* pre, const float* pos, float* h, int R, int B, int N_seq,
+                             int D, int Pp, void* stream) {
+  SATB_REQUIRE(tok && h, "null argument");
+  SATB_REQUIRE(B >= 1 && R >= 1 && R <= kMaxGridYZ && D >= 1, "write prepend probe: need B, D >= 1 and 1 <= R <= 65535");
+  SATB_REQUIRE(Pp >= 0 && Pp < kMaxGridYZ && N_seq > Pp, "write prepend probe: need 0 <= Pp < N_seq");
+  return launch_write_prepend(tok, pre, pos, h, R, B, N_seq, D, Pp, static_cast<cudaStream_t>(stream));
+}
+
+int satb_gate_sigmoid_probe(float* ssg, int rows, int depth, int D, void* stream) {
+  SATB_REQUIRE(ssg, "null argument");
+  SATB_REQUIRE(rows >= 1 && rows <= kMaxGridYZ && depth >= 1 && D >= 1 &&
+                   static_cast<long long>(depth) * 6 * D <= (1 << 30),
+               "gate sigmoid probe: need 1 <= rows <= 65535 and depth, D >= 1");
+  return launch_gate_sigmoid(ssg, rows, depth, D, static_cast<cudaStream_t>(stream));
+}
+
+int satb_dit_post_probe(const float* y, int ldy, float* out, int B, int C, int L, int N_seq, int P, int cfg,
+                        float cfg_scale, float scale_phi, void* stream) {
+  SATB_REQUIRE(y && out, "null argument");
+  SATB_REQUIRE(B >= 1 && B <= kMaxGridYZ && C >= 1 && L >= 1 && P >= 0, "dit post probe: need 1 <= B <= 65535, C, L >= 1 and P >= 0");
+  SATB_REQUIRE(N_seq >= P && N_seq - P >= L, "dit post probe: need N_seq >= P + L");
+  return launch_dit_post(y, ldy, out, B, C, L, N_seq, P, cfg != 0, cfg_scale, scale_phi, static_cast<cudaStream_t>(stream));
+}
+
+int satb_cast_rows_probe(const float* src, void* dst16, const int* perm, int rows, int cols, long long src_ld,
+                         long long dst_ld, int bf16, void* stream) {
+  SATB_REQUIRE(src && dst16, "null argument");
+  SATB_REQUIRE(rows >= 1 && cols >= 1, "cast rows probe: need rows, cols >= 1");
+  SATB_REQUIRE(src_ld >= cols && dst_ld >= cols, "cast rows probe: the row pitches must cover the columns");
+  return launch_cast_rows(src, dst16, perm, rows, cols, src_ld, dst_ld, bf16 != 0, static_cast<cudaStream_t>(stream));
+}
+
+int satb_quant_rows_fp8_probe(const float* src, void* dst8, float* row_scale, const int* perm, int rows, int cols,
+                              void* stream) {
+  SATB_REQUIRE(src && dst8 && row_scale, "null argument");
+  SATB_REQUIRE(rows >= 1 && cols >= 4, "FP8 row quantisation probe: need rows >= 1 and cols >= 4");
+  SATB_REQUIRE(aligned_to(dst8, 4), "FP8 row quantisation probe: dst must be 4-byte aligned");
+  return launch_quant_rows_fp8(src, dst8, row_scale, perm, rows, cols, static_cast<cudaStream_t>(stream));
+}
+
+int satb_matmul_f64_probe(const float* A, const float* B, float* C, int M, int N, int K, void* stream) {
+  SATB_REQUIRE(A && B && C, "null argument");
+  SATB_REQUIRE(M >= 1 && N >= 1 && K >= 1 && (M + 63) / 64 <= kMaxGridYZ, "matmul probe: need M, N, K >= 1 and M <= 64 * 65535");
+  return launch_matmul_f64(A, B, C, M, N, K, static_cast<cudaStream_t>(stream));
 }
 
 int satb_linear_f32out(const void* a16, const void* w16, float* c, int M, int N, int K, int bf16, void* stream) {

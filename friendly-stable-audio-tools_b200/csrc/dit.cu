@@ -364,6 +364,10 @@ int satb_abi_version(void) { return SATB_ABI_VERSION; }
 int satb_dit_create(const SatbDitConfig* cfg, SatbDit** out) {
   SATB_REQUIRE(cfg && out, "null argument");
   SATB_REQUIRE(cfg->embed_dim % 128 == 0, "embed_dim must be a multiple of 128");
+  // the LayerNorm holds a row in registers (<= 2048 wide); the conditioning MLPs stage K % 4 == 0, K <= 6400 inputs
+  SATB_REQUIRE(cfg->embed_dim >= 128 && cfg->embed_dim <= 2048, "embed_dim must be between 128 and 2048");
+  SATB_REQUIRE(cfg->global_cond_dim >= 0 && cfg->global_cond_dim % 4 == 0 && cfg->global_cond_dim <= 6400,
+               "global_cond_dim must be a multiple of 4, at most 6400");
   SATB_REQUIRE(cfg->num_heads > 0 && cfg->embed_dim % cfg->num_heads == 0, "embed_dim must be a multiple of num_heads");
   const int dh = cfg->num_heads > 0 ? cfg->embed_dim / cfg->num_heads : 0;
   SATB_REQUIRE(dh == 32 || dh == 64 || dh == 96 || dh == 128, "head dim (embed_dim / num_heads) must be 32, 64, 96 or 128");
@@ -373,7 +377,8 @@ int satb_dit_create(const SatbDitConfig* cfg, SatbDit** out) {
   SATB_REQUIRE(cfg->input_concat_dim >= 0, "input_concat_dim must be >= 0");
   SATB_REQUIRE(static_cast<long long>(cfg->io_channels) + cfg->input_concat_dim <= 32768,
                "io_channels + input_concat_dim must be at most 32768");
-  SATB_REQUIRE(cfg->prepend_cond_dim >= 0 && cfg->prepend_cond_dim % 4 == 0, "prepend_cond_dim must be a multiple of 4");
+  SATB_REQUIRE(cfg->prepend_cond_dim >= 0 && cfg->prepend_cond_dim % 4 == 0 && cfg->prepend_cond_dim <= 6400,
+               "prepend_cond_dim must be a multiple of 4, at most 6400");
   SATB_REQUIRE(!(cfg->prepend_cond_dim > 0 && cfg->global_cond_type == 1),
                "prepend conditioning is supported with global_cond_type \"prepend\" only");
   SATB_REQUIRE(cfg->operand_dtype >= 0 && cfg->operand_dtype <= 2, "operand_dtype must be 0 (fp16), 1 (bf16) or 2 (fp8)");

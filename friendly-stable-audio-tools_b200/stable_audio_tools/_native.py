@@ -103,6 +103,15 @@ SIGNATURES = {
     "satb_gemm_probe_fp8": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, ctypes.POINTER(SatbGemmProbe), _VP]),
     "satb_token_conv_probe": (_I, [_VP, _LL, _VP, _I, _I, _I, _I, _I, ctypes.POINTER(SatbGemmProbe), _VP]),
     "satb_dit_pre_probe": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _I, _I, _VP]),
+    "satb_layernorm_mod": (_I, [_VP, _VP, _VP, _VP, _VP, _LL, _I, _I, _VP, _I, _I, _I, _VP]),
+    "satb_fourier_probe": (_I, [_VP, _VP, _VP, _I, _I, _VP]),
+    "satb_skinny_linear_probe": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _VP]),
+    "satb_write_prepend_probe": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _VP]),
+    "satb_gate_sigmoid_probe": (_I, [_VP, _I, _I, _I, _VP]),
+    "satb_dit_post_probe": (_I, [_VP, _I, _VP, _I, _I, _I, _I, _I, _I, _F, _F, _VP]),
+    "satb_cast_rows_probe": (_I, [_VP, _VP, _VP, _I, _I, _LL, _LL, _I, _VP]),
+    "satb_quant_rows_fp8_probe": (_I, [_VP, _VP, _VP, _VP, _I, _I, _VP]),
+    "satb_matmul_f64_probe": (_I, [_VP, _VP, _VP, _I, _I, _I, _VP]),
     "satb_attention": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP]),
     "satb_attention_hd": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _VP]),
     "satb_attention_probe": (_I, [ctypes.POINTER(SatbAttentionProbe), _VP]),

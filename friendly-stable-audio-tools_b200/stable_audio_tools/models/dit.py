@@ -78,6 +78,13 @@ class DiffusionTransformer(nn.Module):
             raise ValueError(f"io_channels must be >= 1, got {io_channels}")
         if input_concat_dim < 0:
             raise ValueError(f"input_concat_dim must be >= 0, got {input_concat_dim}")
+        # the native LayerNorm keeps a row in registers, and the conditioning MLPs stage their input rows in shared
+        # memory four floats at a time (satb_dit_create refuses the same)
+        if embed_dim > 2048:
+            raise NotImplementedError(f"embed_dim {embed_dim} is above 2048, the widest the native path runs")
+        for name, dim in (("global_cond_dim", global_cond_dim), ("prepend_cond_dim", prepend_cond_dim)):
+            if dim < 0 or dim % 4 != 0 or dim > 6400:
+                raise NotImplementedError(f"{name} {dim}: the native path needs a multiple of 4, at most 6400")
         if global_cond_type not in ("prepend", "adaLN"):
             raise ValueError(f"unknown global_cond_type {global_cond_type}")
         if operand_dtype not in OPERAND_DTYPES:

@@ -206,6 +206,42 @@ int satb_token_conv_probe(const void* a16, long long item_stride, const void* w1
  * a16 [R * (P + L), lda] 16-bit (bf16 or fp16) with lda >= C, lda % 8 == 0: row r * (P + L) + P + l, column c holds
  * x[r % B_src, c, l]; the P leading rows of every item and the columns C .. lda-1 of every row are written as zeros. */
 int satb_dit_pre_probe(const float* x, void* a16, int R, int B_src, int C, int lda, int L, int P, int bf16, void* stream);
+/* Test entry points (no product path calls them): the DiT forward's small kernels, each through the launch function the
+ * forward itself calls.  Every one checks its arguments before any CUDA call; device pointers are fp32 unless stated.
+ *
+ * satb_layernorm_mod: satb_layernorm with the adaLN modulation of satb_layernorm_fp8: out16[r, :] = 16-bit of
+ * LayerNorm(x[r, :]) * (1 + mod_scale[item, :]) + mod_shift[item, :], item = (r / rows_per_item) % n_items, vector of
+ * item i at mod_scale + i * mod_stride (mod_scale NULL: no modulation, mod_* ignored).  x, gamma, beta, mod_* 16-byte
+ * aligned, out16 8-byte aligned; D a multiple of 128, <= 2048. */
+int satb_layernorm_mod(const float* x, const float* gamma, const float* beta, const float* mod_scale,
+                       const float* mod_shift, long long mod_stride, int rows_per_item, int n_items, void* out16,
+                       int rows, int D, int bf16, void* stream);
+/* Timestep features (models/blocks.py:95-97): t [B], w [F] -> out [B, 2 F] = [cos(2 pi t w) | sin(2 pi t w)]. */
+int satb_fourier_probe(const float* t, const float* w, float* out, int B, int F, void* stream);
+/* out[r, n] = act(sum_k in[r, k] W[n, k] (+ bias[n]) (+ add[r, n])), act = SiLU when silu_out: in [R, K], W [N, K] (both
+ * 16-byte aligned), bias [N] / add [R, N] may be NULL.  1 <= R <= 4096, K a multiple of 4, 4 <= K <= 6400. */
+int satb_skinny_linear_probe(const float* in, const float* W, const float* bias, const float* add, float* out, int R,
+                             int K, int N, int silu_out, void* stream);
+/* The prepended rows of the residual stream h [R, N_seq, D]: rows j < Pp of item r get pre[r, j, :] (r < B and pre given;
+ * else zeros), row Pp gets tok[r % B, :]; pos [N_seq, D] (may be NULL) adds pos[j, :].  Rows past Pp are not written. */
+int satb_write_prepend_probe(const float* tok, const float* pre, const float* pos, float* h, int R, int B, int N_seq,
+                             int D, int Pp, void* stream);
+/* ssg [rows, depth * 6 D], in place: g -> sigmoid(1 - g) on chunks 2 and 5 of every 6 D-wide layer block. */
+int satb_gate_sigmoid_probe(float* ssg, int rows, int depth, int D, void* stream);
+/* y [R * N_seq, ldy] (R = B, or 2 B with cfg: conditional rows first; only columns < C are read) -> out [B, C, L]:
+ * the P leading rows of every item dropped, the CFG combine and std rescale of models/dit.py:338-347 when cfg != 0. */
+int satb_dit_post_probe(const float* y, int ldy, float* out, int B, int C, int L, int N_seq, int P, int cfg,
+                        float cfg_scale, float scale_phi, void* stream);
+/* dst16[r, c] = 16-bit (fp16 / bf16, round to nearest even) of src[perm ? perm[r] : r, c], c < cols, at row pitches
+ * src_ld / dst_ld (elements); perm: device int32 [rows] or NULL.  Any number of rows. */
+int satb_cast_rows_probe(const float* src, void* dst16, const int* perm, int rows, int cols, long long src_ld,
+                         long long dst_ld, int bf16, void* stream);
+/* The FP8 mode's weight quantiser: dst8[r, :] = e4m3_rn(src[perm ? perm[r] : r, :] / row_scale[r]) with the row-scale
+ * rule of satb_layernorm_fp8.  src [*, cols] 16-byte aligned, dst8 4-byte aligned, cols a multiple of 4. */
+int satb_quant_rows_fp8_probe(const float* src, void* dst8, float* row_scale, const int* perm, int rows, int cols,
+                              void* stream);
+/* C [M, N] = A [M, K] B [K, N], fp32 row-major, float64 products and sums (the conformer weight fold). */
+int satb_matmul_f64_probe(const float* A, const float* B, float* C, int M, int N, int K, void* stream);
 /* One step of the v-objective k-diffusion samplers in a single pass over the latents (replaces the
  * ~20 elementwise torch kernels of K.external.VDenoiser.forward + sample_dpmpp_{2m,3m}_sde's update,
  * reference call sites inference/sampling.py:159,225-228): with v = model(x * c_in, t),
