@@ -139,6 +139,15 @@ int satb_sampler_update(const float* x, const float* v, const float* den_1, cons
                                c_in_next, static_cast<cudaStream_t>(stream));
 }
 
+int satb_vdiffusion_update(const float* x, const float* v, const float* noise, float* x_next, float* pred, long long n,
+                           float alpha, float sigma, float alpha_next, float adj_sigma, float ddim_sigma, void* stream) {
+  SATB_REQUIRE(x && v, "null argument");
+  SATB_REQUIRE(x_next || pred, "v-diffusion update: x_next and pred are both null (nothing to write)");
+  SATB_REQUIRE(n >= 1, "v-diffusion update: element count must be positive");
+  return launch_vdiffusion_update(x, v, noise, x_next, pred, n, alpha, sigma, alpha_next, adj_sigma, ddim_sigma,
+                                  static_cast<cudaStream_t>(stream));
+}
+
 int satb_attention(const void* q16, const void* k16, const void* v16, void* o16, int B, int H, int Hkv, int Nq, int Nk,
                    int bf16, void* stream) {
   return satb_attention_hd(q16, k16, v16, o16, B, H, Hkv, Nq, Nk, 64, bf16, stream);

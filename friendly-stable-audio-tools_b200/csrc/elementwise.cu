@@ -604,6 +604,44 @@ int launch_sampler_update(const float* x, const float* v, const float* d1, const
   return 0;
 }
 
+// One step of the v-diffusion DDIM sampler (reference inference/sampling.py:64-118) as a single pass over the state:
+//   pred = x alpha - v sigma;  eps = x sigma + v alpha;  x_next = pred alpha_next + eps adj_sigma (+ noise ddim_sigma)
+// Every product and sum is rounded on its own (the _rn intrinsics keep nvcc from contracting them into FMAs), in the
+// order of the reference's fp32 tensor expressions, so a step equals their torch evaluation bit for bit.  pred and
+// x_next may each be null (the last step writes pred only); noise may be null.
+__global__ void __launch_bounds__(256) vdiffusion_update_kernel(const float* __restrict__ x, const float* __restrict__ v,
+                                                                const float* __restrict__ nz, float* __restrict__ x_next,
+                                                                float* __restrict__ pred, long long n, float alpha,
+                                                                float sigma, float alpha_next, float adj_sigma,
+                                                                float ddim_sigma) {
+  pdl_launch_dependents();
+  pdl_wait();
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const float xv = x[i], vv = v[i];
+    const float p = __fsub_rn(__fmul_rn(xv, alpha), __fmul_rn(vv, sigma));
+    if (pred) pred[i] = p;
+    if (x_next) {
+      const float e = __fadd_rn(__fmul_rn(xv, sigma), __fmul_rn(vv, alpha));
+      float o = __fadd_rn(__fmul_rn(p, alpha_next), __fmul_rn(e, adj_sigma));
+      if (nz) o = __fadd_rn(o, __fmul_rn(nz[i], ddim_sigma));
+      x_next[i] = o;
+    }
+  }
+}
+
+int launch_vdiffusion_update(const float* x, const float* v, const float* nz, float* x_next, float* pred, long long n,
+                             float alpha, float sigma, float alpha_next, float adj_sigma, float ddim_sigma,
+                             cudaStream_t stream) {
+  SATB_REQUIRE(n > 0, "v-diffusion update: element count must be positive");
+  int grid = static_cast<int>(ceil_div64(n, 256));
+  if (grid > 4 * device_sm_count()) grid = 4 * device_sm_count();
+  SATB_CHECK_CUDA(launch_pdl(vdiffusion_update_kernel, dim3(grid), dim3(256), 0, stream, x, v, nz, x_next, pred, n, alpha,
+                             sigma, alpha_next, adj_sigma, ddim_sigma));
+  count_launch();
+  return 0;
+}
+
 int launch_snake_beta(const float* x, const float* alpha, const float* beta, float* y, int B, int C, int64_t T,
                       int logscale, cudaStream_t stream) {
   if (B <= 0 || C <= 0 || T <= 0) return 0;

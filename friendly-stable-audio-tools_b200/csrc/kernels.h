@@ -32,6 +32,10 @@ int launch_quant_rows_fp8(const float* src, void* dst, float* row_scale, const i
 int launch_sampler_update(const float* x, const float* v, const float* d1, const float* d2, const float* nz, float* den,
                           float* x_next, float* x_in, long long n, float c_skip, float c_out, float A, float B, float C,
                           float D, float S, float c_in_next, cudaStream_t stream);
+// One v-diffusion DDIM step in the reference's fp32 operation order (see elementwise.cu).
+int launch_vdiffusion_update(const float* x, const float* v, const float* nz, float* x_next, float* pred, long long n,
+                             float alpha, float sigma, float alpha_next, float adj_sigma, float ddim_sigma,
+                             cudaStream_t stream);
 // SnakeBeta on [B, C, T] fp32 (log-scale alpha/beta per channel).
 int launch_snake_beta(const float* x, const float* alpha, const float* beta, float* y, int B, int C, int64_t T,
                       int logscale, cudaStream_t stream);

@@ -96,6 +96,7 @@ SIGNATURES = {
     "satb_dit_profile_read": (_I, [_VP, _VP, _VP]),
     "satb_snake_beta": (_I, [_VP, _VP, _VP, _VP, _I, _I, _LL, _I, _VP]),
     "satb_sampler_update": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _LL] + [_F] * 8 + [_VP]),
+    "satb_vdiffusion_update": (_I, [_VP, _VP, _VP, _VP, _VP, _LL] + [_F] * 5 + [_VP]),
     "satb_layernorm": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _VP]),
     "satb_layernorm_fp8": (_I, [_VP, _VP, _VP, _VP, _VP, _LL, _I, _I, _VP, _VP, _I, _I, _VP]),
     "satb_linear_f32out": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _VP]),

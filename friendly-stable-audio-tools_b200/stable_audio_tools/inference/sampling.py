@@ -1,6 +1,7 @@
 """Samplers for the v-objective denoiser.
 
-``sample_k`` keeps the reference signature and behaviour (``inference/sampling.py:144-228``):
+``sample`` is the reference's v-diffusion DDIM sampler (``inference/sampling.py:64-118``), the decode loop of
+diffusion autoencoders.  ``sample_k`` keeps the reference signature and behaviour (``inference/sampling.py:144-228``):
 polyexponential sigma schedule, initial noise scaled by sigma_0, variation / inpainting
 initialisation and the inpainting callback, sampler dispatch by name.  The k-diffusion 0.1.1
 pieces it relies on (``VDenoiser``, ``get_sigmas_polyexponential``, DPM-Solver++(2M/3M) SDE, and
@@ -498,6 +499,85 @@ def sample_k(model_fn, noise, init_data=None, mask=None, steps=100, sampler_type
                                    callback=wrapped_callback, extra_args=extra_args)
     return SAMPLERS[sampler_type](denoiser, x, sigmas, disable=disable_tqdm, callback=wrapped_callback,
                                   extra_args=extra_args, noise_sampler=noise_sampler)
+
+
+def get_alphas_sigmas(t):
+    """The scales of the clean signal (alpha) and of the noise (sigma) at timestep t (reference sampling.py:10-13)."""
+    return torch.cos(t * math.pi / 2), torch.sin(t * math.pi / 2)
+
+
+def vdiffusion_schedule(steps, eta):
+    """Per-step scalars of ``sample`` as Python floats: (t, alpha, sigma, alpha_next, adjusted_sigma, ddim_sigma) for
+    every step, the last step's three next-step values None.  Computed once per call with the reference's fp32 CPU
+    tensor expressions (sampling.py:69-70,94-96), so the floats are the very values its fp32 loop multiplies by."""
+    t = torch.linspace(1, 0, steps + 1)[:-1]
+    alphas, sigmas = get_alphas_sigmas(t)
+    out = []
+    for i in range(steps):
+        nxt = (None, None, None)
+        if i < steps - 1:
+            ddim_sigma = eta * (sigmas[i + 1] ** 2 / sigmas[i] ** 2).sqrt() * (1 - alphas[i] ** 2 / alphas[i + 1] ** 2).sqrt()
+            adjusted_sigma = (sigmas[i + 1] ** 2 - ddim_sigma ** 2).sqrt()
+            nxt = (float(alphas[i + 1]), float(adjusted_sigma), float(ddim_sigma))
+        out.append((float(t[i]), float(alphas[i]), float(sigmas[i])) + nxt)
+    return out
+
+
+@torch.no_grad()
+def sample(model, x, steps, eta, verbose: bool = True, noise_sampler=None, **extra_args):
+    """v-diffusion DDIM sampling from the start noise x (reference sampling.py:64-118): with alpha, sigma = cos, sin of
+    t pi / 2 over t = linspace(1, 0, steps + 1)[:-1] and v = model(x, t_i, **extra_args),
+        pred = x alpha_i - v sigma_i,  eps = x sigma_i + v alpha_i,
+        x = pred alpha_{i+1} + eps adjusted_sigma + ddim_sigma noise   (every step but the last),
+    and returns the last step's pred.  ``noise_sampler(i)`` returns step i's noise (default ``torch.randn_like(x)``;
+    drawn only when eta != 0).  ``verbose`` is accepted for the reference's signature; no progress is printed (the
+    reference times every tenth step with a device synchronise).
+
+    CUDA fp32 state: each step's update is one launch of ``satb_vdiffusion_update``, which equals the fp32 torch
+    expressions below bit for bit, and a native DiT (a DiTWrapper or a DiffusionTransformer) runs each forward as one
+    CUDA-graph replay.  Other inputs (CPU tensors, other dtypes) take the torch expressions themselves."""
+    if steps < 1:
+        raise ValueError(f"sample needs steps >= 1, got {steps}")
+    sched = vdiffusion_schedule(steps, eta)
+    noise = noise_sampler if noise_sampler is not None else (lambda i: torch.randn_like(x))
+    ones = x.new_ones([x.shape[0]])
+    fused = x.is_cuda and x.dtype == torch.float32
+    graph_dit = None
+    if fused:
+        for cand in (model, getattr(model, "model", None)):
+            if cand is not None and hasattr(cand, "cuda_graph") and hasattr(cand, "_graph_forward"):
+                graph_dit = cand
+    prev = None
+    if graph_dit is not None:
+        prev, graph_dit.cuda_graph = graph_dit.cuda_graph, True
+    try:
+        pred = None
+        for i, (t_i, a, s, a_next, adj, ddim) in enumerate(sched):
+            v = model(x, ones * t_i, **extra_args).float()
+            last = a_next is None
+            nz = noise(i) if (not last and eta) else None
+            if fused:
+                from .. import _native
+                xc, vc = x.contiguous(), v.contiguous()
+                pred = torch.empty_like(xc) if last else None
+                x_next = None if last else torch.empty_like(xc)
+                _native.check(_native.lib().satb_vdiffusion_update(
+                    _native.ptr(xc), _native.ptr(vc), _native.ptr(nz.float().contiguous() if nz is not None else None),
+                    _native.ptr(x_next), _native.ptr(pred), xc.numel(), a, s, a_next or 0.0, adj or 0.0, ddim or 0.0,
+                    _native.stream_ptr(x.device)))
+                if not last:
+                    x = x_next
+            else:
+                pred = x * a - v * s
+                if not last:
+                    eps = x * s + v * a
+                    x = pred * a_next + eps * adj
+                    if nz is not None:
+                        x += nz * ddim
+    finally:
+        if graph_dit is not None:
+            graph_dit.cuda_graph = prev
+    return pred
 
 
 @torch.no_grad()

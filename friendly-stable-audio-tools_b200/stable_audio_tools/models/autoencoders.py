@@ -5,7 +5,8 @@ Interface parity with reference ``models/autoencoders.py`` for the Oobleck path:
 ``OobleckDecoder`` (:45-194, same constructor kwargs and state-dict keys incl. the
 weight-norm ``weight_g`` / ``weight_v`` pairs), ``AudioAutoencoder`` (:234-645: encode /
 decode with ``iterate_batch`` micro-batching, chunked ``encode_audio`` / ``decode_audio`` /
-``reconstruct_audio`` with Bartlett cross-fades) and the config factories (:693-787).
+``reconstruct_audio`` with Bartlett cross-fades), ``DiffusionAutoencoder`` (:648-690, a DiT decoder sampled with
+``inference.sampling.sample``) and the config factories (:693-847).
 
 The encoder / decoder ``forward`` run in ``libsatb200.so`` (``satb_oobleck_*``): wgmma
 implicit-GEMM convolutions with the activation (SnakeBeta for ``use_snake=True``, ELU otherwise)
@@ -30,7 +31,7 @@ from .. import _native
 from .blocks import SnakeBeta
 from .bottleneck import Bottleneck
 from .factory import create_bottleneck_from_config, create_pretransform_from_config
-from .pretransforms import PQMFPretransform
+from .pretransforms import AutoencoderPretransform, PQMFPretransform
 from .transformer import _FusedModule
 
 
@@ -454,3 +455,91 @@ def create_autoencoder_from_config(config: tp.Dict[str, tp.Any]):
         sample_rate=config["sample_rate"], bottleneck=create_bottleneck_from_config(bottleneck) if bottleneck else None,
         pretransform=pretransform, in_channels=ae.get("in_channels"), out_channels=ae.get("out_channels"),
         soft_clip=ae["decoder"].get("soft_clip", False))
+
+
+# ---------------------------------------------------------------------------------- diffusion autoencoder
+class DiffusionAutoencoder(AudioAutoencoder):
+    """reference models/autoencoders.py:648-690: an (optional) Oobleck encoder and bottleneck, and a DiT decoder that
+    samples the pretransform's input (raw audio, PQMF sub-bands or an Oobleck autoencoder's latents) from noise, with
+    the upsampled latents as its input-concat conditioning.  ``encode`` is the inherited one.  State-dict keys are the
+    reference's: ``encoder.*``, ``diffusion.model.*``, and the bottleneck's and pretransform's.
+
+    The pretransform may be None, a ``PQMFPretransform`` or an ``AutoencoderPretransform``; the DiT then diffuses the
+    signal that pretransform decodes, so its io_channels are the audio channels, the channels x bands, or the inner
+    autoencoder's latent_dim."""
+
+    def __init__(self, diffusion, diffusion_downsampling_ratio, *args, decoder=None, pretransform=None, **kwargs):
+        if decoder is not None:
+            raise NotImplementedError(_DIFFAE_DECODER_REFUSAL)
+        # AudioAutoencoder accepts a PQMF pretransform only, and checks its width as the input of an Oobleck encoder
+        # over channels x bands; here the pretransform wraps the DiT's signal instead, so it is attached afterwards
+        super().__init__(*args, decoder=None, pretransform=None, **kwargs)
+        if pretransform is not None and not isinstance(pretransform, (PQMFPretransform, AutoencoderPretransform)):
+            raise NotImplementedError("DiffusionAutoencoder: the pretransform must be pqmf or an Oobleck autoencoder")
+        self.pretransform = pretransform
+        dit = getattr(diffusion, "model", None)
+        if dit is not None and hasattr(dit, "input_concat_dim"):
+            concat = self.latent_dim + getattr(self.bottleneck, "noise_augment_dim", 0)
+            if dit.io_channels != self.io_channels or dit.input_concat_dim != concat:
+                raise ValueError(f"DiffusionAutoencoder: the DiT has io_channels {dit.io_channels} and input_concat_dim "
+                                 f"{dit.input_concat_dim}; the model needs {self.io_channels} and {concat} (latent_dim "
+                                 "plus the bottleneck's noise channels)")
+        self.diffusion = diffusion
+        self.min_length = self.downsampling_ratio * diffusion_downsampling_ratio
+        if self.encoder is not None:
+            # shrink the initial encoder parameters to avoid saturated latents (reference :661-665)
+            with torch.no_grad():
+                for param in self.encoder.parameters():
+                    param *= 0.5
+            self.encoder.refresh_native_weights()
+
+    def decode(self, latents, steps=100, noise=None, **kwargs):
+        """latents [B, latent_dim, n] -> bottleneck decode, nearest upsample to n * downsampling_ratio, ``steps``
+        v-diffusion steps of the DiT from ``noise`` [B, io_channels, n * downsampling_ratio] (default: a torch.randn
+        draw on the latents' device, as the reference draws it), then the pretransform's decode."""
+        from ..inference.sampling import sample
+        upsampled_length = latents.shape[2] * self.downsampling_ratio
+        if self.bottleneck is not None:
+            latents = self.bottleneck.decode(latents)
+        if latents.shape[2] != upsampled_length:
+            latents = F.interpolate(latents, size=upsampled_length, mode="nearest")
+        shape = (latents.shape[0], self.io_channels, upsampled_length)
+        if noise is None:
+            noise = torch.randn(*shape, device=latents.device)
+        elif tuple(noise.shape) != shape:
+            raise ValueError(f"noise has shape {tuple(noise.shape)}, the decode needs {shape}")
+        decoded = sample(self.diffusion, noise, steps, 0, input_concat_cond=latents)
+        if self.pretransform is not None:
+            with torch.no_grad():
+                decoded = self.pretransform.decode(decoded)
+        return decoded
+
+
+_DIFFAE_DECODER_REFUSAL = (
+    "DiffusionAutoencoder with a 'decoder' is not supported: the reference's decode passes the latents to "
+    "self.decode itself in that case (models/autoencoders.py:673-674), which recurses without end, so there is no "
+    "behaviour to reproduce")
+
+
+def create_diffAE_from_config(config: tp.Dict[str, tp.Any]):
+    """reference models/autoencoders.py:790-847 with a DiT diffusion block (``DiTWrapper``, diffusion downsampling 1)."""
+    from .diffusion import DiTWrapper
+    diffae = config["model"]
+    if "decoder" in diffae:
+        raise NotImplementedError(_DIFFAE_DECODER_REFUSAL)
+    kind = diffae["diffusion"]["type"]
+    if kind in ("DAU1d", "adp_1d"):
+        raise NotImplementedError(f"diffusion block '{kind}' is not supported: the ADP U-Nets are outside this "
+                                  "package (DESIGN.md section 7); the diffusion block must be 'dit'")
+    if kind != "dit":
+        raise NotImplementedError(f"No such model type: '{kind}'")
+    encoder = create_encoder_from_config(diffae["encoder"]) if "encoder" in diffae else None
+    diffusion = DiTWrapper(**diffae["diffusion"]["config"])
+    bottleneck = diffae.get("bottleneck")
+    pretransform = diffae.get("pretransform")
+    if pretransform:
+        pretransform = create_pretransform_from_config(pretransform, config["sample_rate"])
+    return DiffusionAutoencoder(
+        encoder=encoder, diffusion=diffusion, io_channels=diffae["io_channels"], sample_rate=config["sample_rate"],
+        latent_dim=diffae["latent_dim"], downsampling_ratio=diffae["downsampling_ratio"], diffusion_downsampling_ratio=1,
+        bottleneck=create_bottleneck_from_config(bottleneck) if bottleneck else None, pretransform=pretransform or None)

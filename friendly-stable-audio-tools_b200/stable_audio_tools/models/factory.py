@@ -10,9 +10,12 @@ def create_model_from_config(model_config):
     if model_type in ("diffusion_cond", "diffusion_cond_inpaint", "diffusion_prior"):
         from .diffusion import create_diffusion_cond_from_config
         return create_diffusion_cond_from_config(model_config)
+    if model_type == "diffusion_autoencoder":
+        from .autoencoders import create_diffAE_from_config
+        return create_diffAE_from_config(model_config)
     raise NotImplementedError(
         f"model_type '{model_type}' is outside the H100-native hot path (supported: autoencoder, diffusion_cond, "
-        "diffusion_cond_inpaint, diffusion_prior)")
+        "diffusion_cond_inpaint, diffusion_prior, diffusion_autoencoder)")
 
 
 def create_model_from_config_path(model_config_path):
@@ -53,8 +56,15 @@ def create_bottleneck_from_config(bottleneck_config):
     elif kind == "tanh":
         from .bottleneck import TanhBottleneck
         bottleneck = TanhBottleneck()
+    elif kind == "l2_norm":
+        from .bottleneck import L2Bottleneck
+        bottleneck = L2Bottleneck()
+    elif kind == "wasserstein":
+        from .bottleneck import WassersteinBottleneck
+        bottleneck = WassersteinBottleneck(**bottleneck_config.get("config", {}))
     else:
-        raise NotImplementedError(f"bottleneck '{kind}' is outside the native hot path (vae / tanh only)")
+        raise NotImplementedError(f"bottleneck '{kind}' is outside the native hot path "
+                                  "(vae / tanh / l2_norm / wasserstein only)")
     if not bottleneck_config.get("requires_grad", True):
         for p in bottleneck.parameters():
             p.requires_grad = False

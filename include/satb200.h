@@ -250,6 +250,13 @@ int satb_matmul_f64_probe(const float* A, const float* B, float* C, int M, int N
 int satb_sampler_update(const float* x, const float* v, const float* den_1, const float* den_2, const float* noise,
                         float* den, float* x_next, float* x_in_next, long long n, float c_skip, float c_out, float a,
                         float b, float c, float d, float s, float c_in_next, void* stream);
+/* One step of the v-diffusion DDIM sampler (reference inference/sampling.py:64-118) in a single pass, with the
+ * reference's fp32 rounding (every product and sum rounded on its own, in its order):
+ *   pred = x alpha - v sigma;  eps = x sigma + v alpha;  x_next = pred alpha_next + eps adj_sigma + noise ddim_sigma.
+ * noise may be NULL (no noise term); x_next and pred may each be NULL (the last step writes pred only), not both.
+ * All tensors fp32 with n >= 1 elements; outputs must not overlap the inputs. */
+int satb_vdiffusion_update(const float* x, const float* v, const float* noise, float* x_next, float* pred, long long n,
+                           float alpha, float sigma, float alpha_next, float adj_sigma, float ddim_sigma, void* stream);
 /* softmax(q k^T / sqrt(64)) v (transformer.py:496-536): q [B, Nq, H*64], k/v [B, Nk, Hkv*64],
  * out [B, Nq, H*64]; 16-bit, contiguous. */
 int satb_attention(const void* q16, const void* k16, const void* v16, void* o16, int B, int H, int Hkv, int Nq, int Nk,
