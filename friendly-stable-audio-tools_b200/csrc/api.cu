@@ -175,4 +175,31 @@ int satb_attention_probe(const SatbAttentionProbe* p, void* stream) {
                              p->Nk, p->head_dim, p->bf16 != 0, static_cast<cudaStream_t>(stream));
 }
 
+// FP8 self-attention pieces (attention_fp8.cu), as the DiT forward launches them, on caller-owned buffers
+int satb_attention_fp8_vt(const void* v16, void* vt8, float* sv, int B, int H, int N, int bf16, void* stream) {
+  SATB_REQUIRE(v16 && vt8 && sv, "null argument");
+  SATB_REQUIRE(B >= 1 && B <= kMaxGridYZ && H >= 1 && H <= kMaxGridYZ && N >= 1,
+               "FP8 attention V quantiser: need 1 <= B, H <= 65535 and N >= 1");
+  const int64_t D = static_cast<int64_t>(H) * 64;
+  const AttnFp8Bufs b{nullptr, nullptr, nullptr, nullptr, static_cast<uint8_t*>(vt8), sv};
+  return launch_attention_fp8_vt(v16, D, N * D, b, B, H, N, bf16 != 0, static_cast<cudaStream_t>(stream));
+}
+
+int satb_attention_fp8_core(const void* q8, const void* k8, const float* sq, const float* sk, const void* vt8,
+                            const float* sv, void* o16, int B, int H, int Nq, int Nk, int bf16, void* stream) {
+  SATB_REQUIRE(q8 && k8 && sq && sk && vt8 && sv && o16, "null argument");
+  SATB_REQUIRE(B >= 1 && B <= kMaxGridYZ && H >= 1 && H <= kMaxGridYZ && Nq >= 1 && Nk >= 1,
+               "FP8 attention: need 1 <= B, H <= 65535 and Nq, Nk >= 1");
+  SATB_REQUIRE(aligned_to(q8, 16) && aligned_to(k8, 16) && aligned_to(sq, 16) && aligned_to(sk, 16) &&
+                   aligned_to(vt8, 16) && aligned_to(sv, 8),
+               "FP8 attention: q8, k8, vt8 and the row scales must be 16-byte aligned, sv 8-byte aligned");
+  const AttnFp8Bufs b{const_cast<uint8_t*>(static_cast<const uint8_t*>(q8)), const_cast<uint8_t*>(static_cast<const uint8_t*>(k8)),
+                      const_cast<float*>(sq), const_cast<float*>(sk), const_cast<uint8_t*>(static_cast<const uint8_t*>(vt8)),
+                      const_cast<float*>(sv)};
+  AttnFp8Maps maps;
+  SATB_PROPAGATE(make_attention_fp8_maps(&maps, b, B, H, Nq, Nk));
+  const int64_t D = static_cast<int64_t>(H) * 64;
+  return launch_attention_fp8(maps, b, o16, D, Nq * D, B, H, Nq, Nk, bf16 != 0, static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

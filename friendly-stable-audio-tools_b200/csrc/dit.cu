@@ -163,6 +163,7 @@ struct SatbDit {
   DevBuf ws_prep;             // their embeddings [B, Pp, D] + scratch
   bool bf16, fp8, adaln, qk_norm = false;   // fp8: e4m3 operands for the QKV, cross q and FF-in GEMMs (fp16 elsewhere)
   bool conformer = false;     // every block runs the conformer branch (satb_dit_set_conformer)
+  bool attn_fp8 = false;      // self-attention with e4m3 q, k, v and P (satb_dit_set_attention_fp8)
   int* cf_perm = nullptr;     // SwiGLU row interleave of the folded [2D, D] conformer GLU weight
   // feed-forward (satb_dit_set_feedforward; default: SwiGLU Linear, inner 4D, biased).  ffi above is ff_inner padded up
   // to a multiple of 64.  ff_k: kernel size of the token convolutions, 0 = Linear (with ff_glu, FF-out only).  ff_bias:
@@ -198,6 +199,8 @@ struct SatbDit {
   TmapCache tmaps;
   DevBuf ws_h, ws_a16, ws_qkv, ws_attn, ws_q16, ws_ff, ws_ain, ws_y, ws_small, ws_cond, ws_kv, ws_rope;
   DevBuf ws_a8, ws_ascale;   // FP8 mode: e4m3 LayerNorm rows [M, D] and their scales [M]
+  DevBuf ws_attn8;            // FP8 self-attention operands (attn_fp8_bufs), with their tensor maps for res_R rows
+  AttnFp8Maps attn8_maps;
   int rope_len = 0;
   int res_R = 0, res_L = 0, res_P = -1;
   // optional per-category CUDA-event timing (bench.py roofline)
@@ -472,6 +475,17 @@ int satb_dit_set_positions(SatbDit* d, int rotary, int pos_type, int abs_max_len
   return 0;
 }
 
+// FP8 self-attention (attention_fp8.cu): call before satb_dit_finalize.
+int satb_dit_set_attention_fp8(SatbDit* d, int enable) {
+  SATB_REQUIRE(d, "null handle");
+  SATB_REQUIRE(enable == 0 || enable == 1, "enable must be 0 or 1");
+  SATB_REQUIRE(!d->finalized, "satb_dit_set_attention_fp8 must be called before satb_dit_finalize");
+  SATB_REQUIRE(!enable || d->dh == 64, "FP8 self-attention is supported with head dim 64 only");
+  d->attn_fp8 = enable != 0;
+  d->res_R = 0;   // the next forward reserves (and sizes the FP8 operands)
+  return 0;
+}
+
 void satb_dit_destroy(SatbDit* d) {
   if (!d) return;
   for (void* p : d->owned) cudaFree(p);
@@ -482,7 +496,7 @@ void satb_dit_destroy(SatbDit* d) {
   d->ws_h.release(); d->ws_a16.release(); d->ws_qkv.release(); d->ws_attn.release(); d->ws_q16.release();
   d->ws_ff.release(); d->ws_ain.release(); d->ws_y.release(); d->ws_small.release(); d->ws_cond.release();
   d->ws_kv.release(); d->ws_rope.release(); d->ws_prep.release(); d->ws_a8.release(); d->ws_ascale.release();
-  d->ws_pos.release();
+  d->ws_pos.release(); d->ws_attn8.release();
   delete d;
 }
 
@@ -809,6 +823,13 @@ int satb_dit_reserve(SatbDit* d, int R, int L) {
     SATB_PROPAGATE(d->ws_a8.ensure(M * D));
     SATB_PROPAGATE(d->ws_ascale.ensure(M * 4));
   }
+  if (d->attn_fp8) {
+    SATB_PROPAGATE(d->ws_attn8.ensure(attn_fp8_workspace_bytes(R, d->H, N_seq, N_seq)));
+    // the q / k scales past each item's tokens are never written (the core masks those keys): zero, once
+    SATB_CHECK_CUDA(cudaMemset(d->ws_attn8.p, 0, attn_fp8_workspace_bytes(R, d->H, N_seq, N_seq)));
+    SATB_PROPAGATE(make_attention_fp8_maps(&d->attn8_maps, attn_fp8_bufs(d->ws_attn8.p, R, d->H, N_seq, N_seq), R, d->H,
+                                           N_seq, N_seq));
+  }
   if (d->rotary) SATB_PROPAGATE(ensure_rope(d, N_seq));
   if (d->pos_type != 0) SATB_PROPAGATE(ensure_pos(d, N_seq));
   d->tmaps.maps.clear();
@@ -1019,26 +1040,44 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
       ProfScope ps(d, PROF_QKV, st);
       const void* w = FP8 ? static_cast<const void*>(W.w8_qkv) : static_cast<const void*>(W.w_qkv);
       const Fp8Scales sc{a_scale, W.s_qkv};
+      // FP8 self-attention: q and k leave the epilogue as e4m3 with their scales, v in 16 bits as always
+      const AttnFp8Bufs b8 = d->attn_fp8 ? attn_fp8_bufs(d->ws_attn8.p, d->res_R, H, N_seq, N_seq) : AttnFp8Bufs{};
+      const QkE4m3Out o8{b8.q8, b8.k8, b8.sq, b8.sk, H, attn_fp8_pad(N_seq)};
       if (d->qk_norm) {
         typedef EpiHeadNorm16<BF16> E;   // q, k heads L2-normalised, then rotary
         typename E::Params ep{qkv, 3 * D, 2 * D, 2 * D, N_seq, cos_tab, sin_tab};
         // FP8: BN 128 (the instance the cross q GEMM also runs; the BN 256 one spills a few registers)
         constexpr int kBn = FP8 ? 128 : 256;
-        SATB_PROPAGATE((linear<E, kBn, BF16, FP8>(d->tmaps, a_in, D, M, D, w, 3 * D, ep, st, 1, sc)));
+        if (d->attn_fp8)
+          SATB_PROPAGATE((linear<EpiHeadNormE4m3<BF16>, kBn, BF16, FP8>(d->tmaps, a_in, D, M, D, w, 3 * D,
+                                                                         {ep, o8}, st, 1, sc)));
+        else
+          SATB_PROPAGATE((linear<E, kBn, BF16, FP8>(d->tmaps, a_in, D, M, D, w, 3 * D, ep, st, 1, sc)));
       } else {
         typedef EpiQkvRope<BF16> E;
         typename E::Params ep{qkv, 3 * D, 2 * D, N_seq, d->dh, d->nf, cos_tab, sin_tab};
-        SATB_PROPAGATE((linear<E, 256, BF16, FP8>(d->tmaps, a_in, D, M, D, w, 3 * D, ep, st, 1, sc)));
+        if (d->attn_fp8)
+          SATB_PROPAGATE((linear<EpiQkvRopeE4m3<BF16>, 256, BF16, FP8>(d->tmaps, a_in, D, M, D, w, 3 * D, {ep, o8}, st,
+                                                                        1, sc)));
+        else
+          SATB_PROPAGATE((linear<E, 256, BF16, FP8>(d->tmaps, a_in, D, M, D, w, 3 * D, ep, st, 1, sc)));
       }
     }
     {
       ProfScope ps(d, PROF_ATTN_SELF, st);
       const int64_t qs = static_cast<int64_t>(N_seq) * 3 * D;
-      const CUtensorMap* tm = nullptr;   // q, k and v are column ranges of one buffer: one map
-      if (d->dh == 64) SATB_PROPAGATE(d->tmaps.get_a(qkv, 3 * D, N_seq, R, 3 * D, qs, &tm));
-      SATB_PROPAGATE(launch_attention_tc(qkv, qkv, qkv, att, 3 * D, 3 * D, 3 * D, D, qs, qs, qs,
-                                         static_cast<int64_t>(N_seq) * D, 3 * D, 3 * D, 3 * D, 0, D, 2 * D, R, H, H,
-                                         N_seq, N_seq, d->dh, BF16, st, tm, tm, tm));
+      if (d->attn_fp8) {   // e4m3 operands in the workspace carved for res_R rows; the maps were made for them
+        const AttnFp8Bufs b8 = attn_fp8_bufs(d->ws_attn8.p, d->res_R, H, N_seq, N_seq);
+        SATB_PROPAGATE(launch_attention_fp8_vt(qkv + 2 * D, 3 * D, qs, b8, R, H, N_seq, BF16, st));
+        SATB_PROPAGATE(launch_attention_fp8(d->attn8_maps, b8, att, D, static_cast<int64_t>(N_seq) * D, R, H, N_seq,
+                                            N_seq, BF16, st));
+      } else {
+        const CUtensorMap* tm = nullptr;   // q, k and v are column ranges of one buffer: one map
+        if (d->dh == 64) SATB_PROPAGATE(d->tmaps.get_a(qkv, 3 * D, N_seq, R, 3 * D, qs, &tm));
+        SATB_PROPAGATE(launch_attention_tc(qkv, qkv, qkv, att, 3 * D, 3 * D, 3 * D, D, qs, qs, qs,
+                                           static_cast<int64_t>(N_seq) * D, 3 * D, 3 * D, 3 * D, 0, D, 2 * D, R, H, H,
+                                           N_seq, N_seq, d->dh, BF16, st, tm, tm, tm));
+      }
     }
     {
       ProfScope ps(d, PROF_ATTN_OUT, st);
@@ -1356,6 +1395,52 @@ int satb_gemm_probe_fp8(const void* a8, const void* w8, const float* a_scale, co
   }
   set_last_error("gemm probe fp8: no such instance (epi " + std::to_string(p->epi) + ", BN " + std::to_string(bn) +
                  "); the forward's FP8 instances are qkv_rope and swiglu BN 256, store16 BN 128 / 256 and head_norm16 BN 128");
+  return -1;
+}
+
+// The e4m3 QKV epilogues of FP8 self-attention (EpiQkvRopeE4m3 BN 256, EpiHeadNormE4m3 BN 256 / FP8 BN 128), as the
+// forward launches them: 16-bit operands when a_scale is null, e4m3 operands with their row scales otherwise.
+int satb_gemm_probe_qk8(const void* a, const void* w, const float* a_scale, const float* w_scale, int M, int N, int K,
+                        const SatbGemmProbe* p, const SatbQkE4m3* o, void* stream) {
+  SATB_REQUIRE(a && w && p && o && o->q8 && o->k8 && o->sq && o->sk, "null argument");
+  const bool fp8 = a_scale != nullptr;
+  SATB_REQUIRE(!fp8 || w_scale, "gemm probe qk8: a_scale needs w_scale");
+  SATB_REQUIRE(aligned16(a) && aligned16(w) && aligned16(o->q8) && aligned16(o->k8) && (!fp8 || aligned16(w_scale)),
+               "gemm probe qk8: operands and q8 / k8 must be 16-byte aligned");
+  SATB_REQUIRE(M >= 1 && K >= 8 && K % (fp8 ? 128 : 8) == 0, "gemm probe qk8: need M >= 1 and K % 8 == 0 (FP8: 128)");
+  SATB_REQUIRE(o->heads >= 1 && N % 64 == 0 && N >= 128 * o->heads, "gemm probe qk8: N must be a multiple of 64 holding "
+               "the 2 heads * 64 q / k columns");
+  SATB_REQUIRE(p->seq_len >= 1 && o->scale_ld >= p->seq_len, "gemm probe qk8: need seq_len >= 1 and scale_ld >= seq_len");
+  SATB_REQUIRE(!fp8 || !p->bf16, "gemm probe qk8: the FP8 instances store fp16");
+  SATB_REQUIRE(p->out && aligned16(p->out) && p->ld >= N && p->ld % 8 == 0, "gemm probe qk8: out must be 16-byte aligned, ld >= N");
+  SATB_REQUIRE(!p->cos_tab || (p->sin_tab && aligned16(p->cos_tab) && aligned16(p->sin_tab)),
+               "gemm probe qk8: rotary needs 16-byte aligned cos_tab and sin_tab");
+  const QkE4m3Out q{static_cast<uint8_t*>(o->q8), static_cast<uint8_t*>(o->k8), o->sq, o->sk, o->heads, o->scale_ld};
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const Fp8Scales sc{a_scale, w_scale};
+  const int bn = p->bn;
+  auto rope = [&](auto bf) -> int {
+    constexpr bool BF16 = decltype(bf)::value;
+    typedef EpiQkvRopeE4m3<BF16> E;
+    const typename E::Params ep{{p->out, p->ld, p->rope_cols, p->seq_len, 64, 16, p->cos_tab, p->sin_tab}, q};
+    if constexpr (!BF16)   // the FP8 instances store fp16
+      if (fp8) return probe_run<E, 256, false, true>(a, w, M, N, K, ep, p->b_static, st, sc);
+    return probe_run<E, 256, BF16>(a, w, M, N, K, ep, p->b_static, st);
+  };
+  auto norm = [&](auto bf) -> int {
+    constexpr bool BF16 = decltype(bf)::value;
+    typedef EpiHeadNormE4m3<BF16> E;
+    const typename E::Params ep{{p->out, p->ld, 128 * o->heads, p->rope_cols, p->seq_len, p->cos_tab, p->sin_tab}, q};
+    if constexpr (!BF16)
+      if (fp8) return probe_run<E, 128, false, true>(a, w, M, N, K, ep, p->b_static, st, sc);
+    return probe_run<E, 256, BF16>(a, w, M, N, K, ep, p->b_static, st);
+  };
+  if (p->epi == SATB_EPI_QKV_ROPE_E4M3 && bn == 256)
+    return p->bf16 ? rope(std::true_type{}) : rope(std::false_type{});
+  if (p->epi == SATB_EPI_HEAD_NORM_E4M3 && bn == (fp8 ? 128 : 256))
+    return p->bf16 ? norm(std::true_type{}) : norm(std::false_type{});
+  set_last_error("gemm probe qk8: no such instance (epi " + std::to_string(p->epi) + ", BN " + std::to_string(bn) +
+                 "); the forward's are qkv_rope_e4m3 BN 256 and head_norm_e4m3 BN 256 (FP8 operands: BN 128)");
   return -1;
 }
 

@@ -18,6 +18,7 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "fp8.cuh"
 #include "ptx.cuh"
 
 namespace satb {
@@ -684,6 +685,179 @@ struct EpiHeadNorm16 {
                               Op16<BF16>::pack(__uint_as_float(q[4]) * inv, __uint_as_float(q[5]) * inv),
                               Op16<BF16>::pack(__uint_as_float(q[6]) * inv, __uint_as_float(q[7]) * inv));
     }
+  }
+};
+
+// Where the e4m3 QKV epilogues below put q and k (FP8 self-attention, attention_fp8.cu): columns [0, 64 H) are q and
+// [64 H, 128 H) k, stored as e4m3 [rows, 64 H] in q8 / k8 with one power-of-two scale per (row, head) (fp8_row_exp of
+// the head's 16-bit values) at s[(item H + head) * scale_ld + token], item = row / seq_len, token = row % seq_len.
+struct QkE4m3Out {
+  uint8_t *q8, *k8;
+  float *sq, *sk;
+  int heads;
+  int scale_ld;
+};
+// e4m3 bytes and scale of the (row, head) a value belongs to; `which` 0 = q, 1 = k
+__device__ __forceinline__ uint8_t* qk8_row(const QkE4m3Out& o, int which, int row, int head) {
+  return (which ? o.k8 : o.q8) + static_cast<size_t>(row) * (64 * o.heads) + 64 * head;
+}
+__device__ __forceinline__ float* qk8_scale(const QkE4m3Out& o, int which, int row, int head, int seq_len) {
+  return (which ? o.sk : o.sq) + static_cast<size_t>(row / seq_len * o.heads + head) * o.scale_ld + row % seq_len;
+}
+
+// EpiQkvRope at head dim 64 (nf 16) with q and k stored as e4m3 (QkE4m3Out): the 16-bit values it computes - the same
+// row permutation, rotary arithmetic and rounding, so the same bits - are quantised instead of stored.  A head's 64
+// columns of a fragment row lie in one quad (8 groups of 8 columns, 2 per lane), so its amax takes two shfl_xor.  v
+// columns (>= 128 H) are stored in 16 bits as by EpiQkvRope.  N must be a multiple of 64.
+template <bool BF16>
+struct EpiQkvRopeE4m3 {
+  static constexpr int kCols = 64;
+  static constexpr int kStageBytes = 0;
+  static constexpr bool kFragment = true;
+  struct Params {
+    typename EpiQkvRope<BF16>::Params base;   // head_dim 64, nf 16
+    QkE4m3Out o;
+  };
+  template <int BN>
+  __device__ static __forceinline__ void apply_fragment(const Params& pp, const float (&acc)[BN / 2], int L, int N,
+                                                        int row0, int n0, int batch, int lane) {
+    const typename EpiQkvRope<BF16>::Params& p = pp.base;
+    const int fc = 2 * (lane & 3);
+    const int qk_cols = 128 * pp.o.heads;
+    float2 tc[2][2], ts[2][2];   // [jj][rr]: (cos, sin) of pair columns 8 jj + fc, + 1 (chunk 0 of every head)
+    const bool tile_rot = n0 < p.rope_cols && p.cos_tab;
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      const int pos = (batch * L + row0 + 8 * rr) % p.seq_len;
+#pragma unroll
+      for (int jj = 0; jj < 2; ++jj) {
+        tc[jj][rr] = ts[jj][rr] = make_float2(0.f, 0.f);
+        if (tile_rot) {
+          const int t = pos * p.nf + 8 * jj + fc;
+          tc[jj][rr] = __ldg(reinterpret_cast<const float2*>(p.cos_tab + t));
+          ts[jj][rr] = __ldg(reinterpret_cast<const float2*>(p.sin_tab + t));
+        }
+      }
+    }
+#pragma unroll
+    for (int hd = 0; hd < BN / 64; ++hd) {
+      const int col0 = n0 + 64 * hd;
+      if (col0 >= N) break;
+      const bool rot = col0 < p.rope_cols && p.cos_tab;
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int l = row0 + 8 * rr;
+        const int row = batch * L + l;
+        uint32_t w[8];   // 16-bit pairs of the head's 8 column groups, this row
+#pragma unroll
+        for (int jj = 0; jj < 2; ++jj) {   // chunk 0: pairs (i, i + 16), i = 8 jj + fc, + 1, all rotated
+          const int ia = 4 * (8 * hd + jj) + 2 * rr, ib = ia + 8;
+          float a0 = acc[ia], a1 = acc[ia + 1], b0 = acc[ib], b1 = acc[ib + 1];
+          if (rot) {
+            EpiQkvRope<BF16>::rotate(a0, b0, tc[jj][rr].x, ts[jj][rr].x);
+            EpiQkvRope<BF16>::rotate(a1, b1, tc[jj][rr].y, ts[jj][rr].y);
+          }
+          w[jj] = Op16<BF16>::pack(a0, a1);
+          w[jj + 2] = Op16<BF16>::pack(b0, b1);
+        }
+#pragma unroll
+        for (int g = 4; g < 8; ++g) {      // chunk 1: passes through
+          const int ia = 4 * (8 * hd + g) + 2 * rr;
+          w[g] = Op16<BF16>::pack(acc[ia], acc[ia + 1]);
+        }
+        if (col0 < qk_cols) {              // warp-uniform
+          float v[16], amax = 0.f;
+#pragma unroll
+          for (int g = 0; g < 8; ++g) {
+            const float2 f = Op16<BF16>::unpack(w[g]);
+            v[2 * g] = f.x;
+            v[2 * g + 1] = f.y;
+            amax = fmaxf(amax, fmaxf(fabsf(f.x), fabsf(f.y)));
+          }
+          amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
+          amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
+          const int e = fp8_row_exp(amax);
+          const float inv = pow2f(-e);
+          if (l < L) {
+            const int which = col0 >= 64 * pp.o.heads, head = (col0 >> 6) - which * pp.o.heads;
+            uint8_t* dst = qk8_row(pp.o, which, row, head) + fc;
+#pragma unroll
+            for (int g = 0; g < 8; ++g)
+              *reinterpret_cast<uint16_t*>(dst + 8 * g) = static_cast<uint16_t>(
+                  __nv_cvt_float2_to_fp8x2(make_float2(v[2 * g] * inv, v[2 * g + 1] * inv), __NV_SATFINITE, __NV_E4M3));
+            if (fc == 0) *qk8_scale(pp.o, which, row, head, p.seq_len) = pow2f(e);
+          }
+        } else {
+          uint16_t* out = static_cast<uint16_t*>(p.out) + static_cast<size_t>(row) * p.ld;
+#pragma unroll
+          for (int q = 0; q < 4; ++q) store16_group_pair(out, col0 + 16 * q, w[2 * q], w[2 * q + 1], lane, l < L);
+        }
+      }
+    }
+  }
+};
+
+// EpiHeadNorm16 with q and k stored as e4m3 (QkE4m3Out; norm_cols must be 128 H): the same normalised and rotated
+// 16-bit values, quantised per (row, head) instead of stored; v columns are stored in 16 bits as by EpiHeadNorm16.
+template <bool BF16>
+struct EpiHeadNormE4m3 {
+  static constexpr int kCols = 64;
+  static constexpr int kStageBytes = 0;
+  struct Params {
+    typename EpiHeadNorm16<BF16>::Params base;
+    QkE4m3Out o;
+  };
+  __device__ static __forceinline__ void apply(const Params& pp, const EpiCtx& c, const uint32_t (&r)[64]) {
+    const typename EpiHeadNorm16<BF16>::Params& p = pp.base;
+    if (c.col0 >= p.norm_cols) {
+      EpiHeadNorm16<BF16>::apply(p, c, r);
+      return;
+    }
+    if (!c.valid) return;
+    float ss = 0.f;
+#pragma unroll
+    for (int j = 0; j < 64; ++j) ss = fmaf(__uint_as_float(r[j]), __uint_as_float(r[j]), ss);
+    const float inv = 1.f / fmaxf(sqrtf(ss), 1e-12f);
+    float v[64];
+#pragma unroll
+    for (int j = 0; j < 64; ++j) v[j] = __uint_as_float(r[j]) * inv;
+    if (c.col0 < p.rope_cols && p.cos_tab) {
+      const int pos = c.row % p.seq_len;
+      const float4* ct = reinterpret_cast<const float4*>(p.cos_tab + pos * 16);
+      const float4* st = reinterpret_cast<const float4*>(p.sin_tab + pos * 16);
+#pragma unroll
+      for (int j4 = 0; j4 < 4; ++j4) {
+        const float4 cs = __ldg(ct + j4), sn = __ldg(st + j4);
+        const float cc[4] = {cs.x, cs.y, cs.z, cs.w}, ss4[4] = {sn.x, sn.y, sn.z, sn.w};
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          const int j = j4 * 4 + u;
+          const float a = v[j], b = v[j + 16];
+          v[j] = a * cc[u] - b * ss4[u];
+          v[j + 16] = b * cc[u] + a * ss4[u];
+        }
+      }
+    }
+    float amax = 0.f;
+#pragma unroll
+    for (int j = 0; j < 64; j += 2) {   // the values EpiHeadNorm16 stores
+      const float2 f = Op16<BF16>::unpack(Op16<BF16>::pack(v[j], v[j + 1]));
+      v[j] = f.x;
+      v[j + 1] = f.y;
+      amax = fmaxf(amax, fmaxf(fabsf(f.x), fabsf(f.y)));
+    }
+    const int e = fp8_row_exp(amax);
+    const float s = pow2f(-e);
+    const int which = c.col0 >= 64 * pp.o.heads, head = (c.col0 >> 6) - which * pp.o.heads;
+    uint4* dst = reinterpret_cast<uint4*>(qk8_row(pp.o, which, c.row, head));
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float* x = v + 16 * j;
+      dst[j] = make_uint4(e4m3x4(x[0] * s, x[1] * s, x[2] * s, x[3] * s), e4m3x4(x[4] * s, x[5] * s, x[6] * s, x[7] * s),
+                          e4m3x4(x[8] * s, x[9] * s, x[10] * s, x[11] * s),
+                          e4m3x4(x[12] * s, x[13] * s, x[14] * s, x[15] * s));
+    }
+    *qk8_scale(pp.o, which, c.row, head, p.seq_len) = pow2f(e);
   }
 };
 

@@ -15,6 +15,36 @@ int launch_attention_tc(const void* q, const void* k, const void* v, void* o, in
                         int head_dim, bool bf16, cudaStream_t stream, const CUtensorMap* tmq = nullptr,
                         const CUtensorMap* tmk = nullptr, const CUtensorMap* tmv = nullptr);
 
+// ---- attention_fp8.cu (FP8 self-attention, head dim 64, one kv head per head)
+// Operands of B items, H heads, Nq query / Nk key rows per item; pad(n) = n rounded up to a multiple of 128:
+//   q8 [B, Nq, H * 64], k8 [B, Nk, H * 64] e4m3 rows;  sq [B * H, pad(Nq)], sk [B * H, pad(Nk)] their power-of-two
+//   (row, head) scales;  vt8 [B * H, 64, pad(Nk)] e4m3 V^T (keys of each 32-key group in fp8_key_of order, zero past
+//   Nk);  sv [B * H, 64] the (item, head, channel) scales of v.
+struct AttnFp8Bufs {
+  uint8_t *q8, *k8;
+  float *sq, *sk;
+  uint8_t* vt8;
+  float* sv;
+};
+struct AttnFp8Maps {
+  CUtensorMap q, k, vt, sk;
+};
+__host__ __device__ constexpr int attn_fp8_pad(int n) { return (n + 127) / 128 * 128; }
+size_t attn_fp8_workspace_bytes(int B, int H, int Nq, int Nk);
+AttnFp8Bufs attn_fp8_bufs(void* ws, int B, int H, int Nq, int Nk);   // carves a workspace of the size above
+// V^T and its channel scales from 16-bit v [B, N, ld] (item stride bs, head h at column
+// h * 64); q8 / k8 and their scales come from the QKV GEMM's e4m3 epilogues (gemm.cuh QkE4m3Out)
+int launch_attention_fp8_vt(const void* v, int64_t ld, int64_t bs, const AttnFp8Bufs& o, int B, int H, int N, bool bf16,
+                            cudaStream_t stream);
+int make_attention_fp8_maps(AttnFp8Maps* m, const AttnFp8Bufs& bufs, int B, int H, int Nq, int Nk);
+// o [B, Nq, ldo] 16-bit (item stride o_bs), head h at column h * 64
+int launch_attention_fp8(const AttnFp8Maps& maps, const AttnFp8Bufs& bufs, void* o, int64_t ldo, int64_t o_bs, int B,
+                         int H, int Nq, int Nk, bool bf16, cudaStream_t stream);
+
+// ---- runtime.cu: a 2-D / 3-D tensor map (dims[0] innermost, strides of dims 1.. in bytes), zero OOB fill
+int make_tmap_nd(CUtensorMap* m, const void* ptr, int rank, int dtype, const uint64_t* dims, const uint64_t* strides_bytes,
+                 const uint32_t* box, int swizzle);
+
 // ---- elementwise.cu
 // LayerNorm over the last dim (eps 1e-5), optional adaLN modulation y*(1+scale)+shift, 16-bit output.
 int launch_layernorm(const float* x, const float* gamma, const float* beta, void* out16, int rows, int D,

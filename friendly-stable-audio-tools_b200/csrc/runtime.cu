@@ -98,4 +98,28 @@ int make_tmap_b(CUtensorMap* m, const void* ptr, int K, int rows, int64_t row_st
   return 0;
 }
 
+// Generic 2-D / 3-D map (rank = number of dims given, 2 or 3): dims[0] innermost (elements), strides in bytes of dims 1
+// and 2, box per dim; zero OOB fill.  dtype: CU_TENSOR_MAP_DATA_TYPE_UINT8 or _FLOAT32.
+int make_tmap_nd(CUtensorMap* m, const void* ptr, int rank, int dtype, const uint64_t* dims, const uint64_t* strides_bytes,
+                 const uint32_t* box, int swizzle) {
+  EncodeTiledFn fn = get_encode_fn();
+  SATB_REQUIRE(fn != nullptr, "cuTensorMapEncodeTiled entry point unavailable");
+  SATB_REQUIRE(rank == 2 || rank == 3, "tensor map rank must be 2 or 3");
+  SATB_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & 15) == 0, "TMA base must be 16B aligned");
+  for (int i = 0; i + 1 < rank; ++i) SATB_REQUIRE(strides_bytes[i] % 16 == 0, "TMA strides must be 16B multiples");
+  cuuint64_t d[3], s[2];
+  cuuint32_t b[3], e[3] = {1, 1, 1};
+  for (int i = 0; i < rank; ++i) { d[i] = dims[i]; b[i] = box[i]; }
+  for (int i = 0; i + 1 < rank; ++i) s[i] = strides_bytes[i];
+  CUresult r = fn(m, static_cast<CUtensorMapDataType>(dtype), rank, const_cast<void*>(ptr), d, s, b, e,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, static_cast<CUtensorMapSwizzle>(swizzle),
+                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_last_error("cuTensorMapEncodeTiled failed with CUresult " + std::to_string(static_cast<int>(r)) + " dims " +
+                   std::to_string(dims[0]) + " x " + std::to_string(dims[1]) + (rank == 3 ? " x " + std::to_string(dims[2]) : ""));
+    return -3;
+  }
+  return 0;
+}
+
 }  // namespace satb

@@ -44,6 +44,12 @@ _VP, _I, _LL, _F = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong, ctypes.c_fl
 EPI_STORE32, EPI_STORE16, EPI_HEAD_NORM16, EPI_QKV_ROPE, EPI_SWIGLU, EPI_RESIDUAL = range(6)
 EPI_RESIDUAL_LN = 6   # retired (the LayerNorm-fold residual epilogue): refused, and the number is not reused
 EPI_STORE32_POS = 7   # store32 plus a [seq_len, N] position-table row (project_in with a positional embedding)
+# satb_gemm_probe_qk8 only: the e4m3 QKV epilogues of FP8 self-attention
+EPI_QKV_ROPE_E4M3, EPI_HEAD_NORM_E4M3 = 8, 9
+
+
+class SatbQkE4m3(ctypes.Structure):
+    _fields_ = [(n, _VP) for n in ("q8", "k8", "sq", "sk")] + [("heads", _I), ("scale_ld", _I)]
 
 
 class SatbGemmProbe(ctypes.Structure):
@@ -85,6 +91,7 @@ SIGNATURES = {
     "satb_dit_set_conformer": (_I, [_VP, _I]),
     "satb_dit_set_feedforward": (_I, [_VP, _I, _I, _I, _I]),
     "satb_dit_set_positions": (_I, [_VP, _I, _I, _I]),
+    "satb_dit_set_attention_fp8": (_I, [_VP, _I]),
     "satb_dit_load_weight": (_I, [_VP, ctypes.c_char_p, _VP, _LL, _VP]),
     "satb_dit_finalize": (_I, [_VP, _VP]),
     "satb_dit_reserve": (_I, [_VP, _I, _I]),
@@ -116,6 +123,10 @@ SIGNATURES = {
     "satb_attention": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP]),
     "satb_attention_hd": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _VP]),
     "satb_attention_probe": (_I, [ctypes.POINTER(SatbAttentionProbe), _VP]),
+    "satb_attention_fp8_vt": (_I, [_VP] * 3 + [_I, _I, _I, _I, _VP]),
+    "satb_gemm_probe_qk8": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, ctypes.POINTER(SatbGemmProbe), ctypes.POINTER(SatbQkE4m3),
+                                 _VP]),
+    "satb_attention_fp8_core": (_I, [_VP] * 7 + [_I, _I, _I, _I, _I, _VP]),
     "satb_conformer_dwconv": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _VP]),
     "satb_oobleck_create": (_I, [ctypes.POINTER(SatbOobleckConfig), ctypes.POINTER(_VP)]),
     "satb_oobleck_create_variant": (_I, [ctypes.POINTER(SatbOobleckConfig), _I, _I, ctypes.POINTER(_VP)]),

@@ -39,6 +39,10 @@ from .transformer import SUPPORTED_HEAD_DIMS, ContinuousTransformer, check_head_
 # conformer branch included; a precision choice with its own tolerance (DESIGN.md section 5), not a second path to the
 # fp16 result.
 OPERAND_DTYPES = {"fp16": 0, "bf16": 1, "fp8": 2}
+# attention_dtype: None (default) keeps the 16-bit self-attention of the operand mode.  "fp8": self-attention on e4m3
+# q, k, v and probabilities with power-of-two scales (satb_dit_set_attention_fp8), head dim 64 only, with any
+# operand_dtype; cross-attention stays 16-bit.  A precision choice with its own tolerance (DESIGN.md section 5).
+ATTENTION_DTYPES = (None, "fp8")
 
 
 class DiffusionTransformer(nn.Module):
@@ -57,6 +61,7 @@ class DiffusionTransformer(nn.Module):
                  transformer_type: str = "x-transformers",
                  global_cond_type: str = "prepend",
                  operand_dtype: str = "fp16",
+                 attention_dtype=None,
                  **kwargs):
         super().__init__()
         if transformer_type != "continuous_transformer":
@@ -89,6 +94,10 @@ class DiffusionTransformer(nn.Module):
             raise ValueError(f"unknown global_cond_type {global_cond_type}")
         if operand_dtype not in OPERAND_DTYPES:
             raise ValueError(f"operand_dtype must be one of {', '.join(OPERAND_DTYPES)}, got {operand_dtype!r}")
+        if attention_dtype not in ATTENTION_DTYPES:
+            raise ValueError(f"attention_dtype must be None or 'fp8', got {attention_dtype!r}")
+        if attention_dtype == "fp8" and embed_dim // num_heads != 64:
+            raise NotImplementedError(f"attention_dtype='fp8' needs head dim 64 (got {embed_dim // num_heads})")
         self.patch_size = patch_size
         self.cond_token_dim = cond_token_dim
         self.input_concat_dim = input_concat_dim
@@ -103,6 +112,7 @@ class DiffusionTransformer(nn.Module):
         self.transformer_type = transformer_type
         self.global_cond_type = global_cond_type
         self.operand_dtype = operand_dtype
+        self.attention_dtype = attention_dtype
         self.qk_norm = bool(kwargs.get("attn_kwargs", {}).get("qk_norm", False))
         # conformer=True (ContinuousTransformer kwarg): every block adds the conformer branch (satb_dit_set_conformer)
         self.conformer = bool(kwargs.get("conformer", False))
@@ -200,6 +210,8 @@ class DiffusionTransformer(nn.Module):
             options = []
             if self.conformer:
                 options.append(lambda: lib.satb_dit_set_conformer(h, 1))
+            if self.attention_dtype == "fp8":
+                options.append(lambda: lib.satb_dit_set_attention_fp8(h, 1))
             if self.ff_spec != (4 * self.embed_dim, 1, 0, 1):
                 options.append(lambda: lib.satb_dit_set_feedforward(h, *self.ff_spec))
             if self.pos_spec != (1, 0, 0):

@@ -108,6 +108,12 @@ int satb_dit_set_feedforward(SatbDit* h, int inner_dim, int glu, int conv_kernel
  * requires the variant's keys and names the missing ones.  The default is (1, 0, 0): a handle that never calls this
  * runs rotary positions only. */
 int satb_dit_set_positions(SatbDit* h, int rotary, int pos_type, int abs_max_len);
+/* FP8 self-attention (DiffusionTransformer attention_dtype "fp8"; DESIGN.md section 5): enable 1 runs every block's
+ * self-attention on e4m3 q, k, v and probabilities (power-of-two scales per (token, head) for q and k, per (item, head,
+ * channel) for v), with an fp32 accumulator and the 16-bit output of the operand mode; cross-attention stays 16-bit.
+ * Head dim 64 only; works with every operand_dtype.  Call before satb_dit_finalize; a later call, another head dim
+ * with enable 1, and an enable other than 0 or 1 are refused.  Default 0. */
+int satb_dit_set_attention_fp8(SatbDit* h, int enable);
 /* One state-dict entry (key relative to DiffusionTransformer, e.g.
  * "transformer.layers.0.self_attn.to_qkv.weight"); src: device fp32, contiguous.
  * Replaces nn.Module.load_state_dict for this module (models/pretrained.py:24). */
@@ -171,6 +177,9 @@ int satb_linear_f32out(const void* a16, const void* w16, float* c, int M, int N,
 /* 6 was the LayerNorm-fold residual epilogue, since removed: it is refused, and the number is not reused. */
 #define SATB_EPI_STORE32_POS 7  /* out fp32 = acc (+ bias) + pos_tab[row % seq_len, :] (BN 256: DiT project_in with a
                                    positional embedding) */
+/* e4m3 QKV epilogues of FP8 self-attention (satb_gemm_probe_qk8 only; the other probes refuse them): */
+#define SATB_EPI_QKV_ROPE_E4M3 8   /* qkv_rope at head dim 64 (nf 16), q / k columns stored e4m3 (SatbQkE4m3), v 16-bit */
+#define SATB_EPI_HEAD_NORM_E4M3 9  /* head_norm16 with norm_cols = 128 heads, q / k stored e4m3 (SatbQkE4m3), v 16-bit */
 typedef struct SatbGemmProbe {
   int epi, bn, bf16, b_static;      /* b_static 1: weight prefetch before the dependency wait, as the forward runs */
   void* out;                        /* store32 (fp32), store16, head_norm16, qkv_rope, swiglu (16-bit) */
@@ -285,6 +294,34 @@ typedef struct SatbAttentionProbe {
   int q_col, k_col, v_col;
 } SatbAttentionProbe;
 int satb_attention_probe(const SatbAttentionProbe* p, void* stream);
+
+/* Test entry points of the FP8 self-attention (satb_dit_set_attention_fp8), head dim 64, one kv head per head.
+ * pad(n) = n rounded up to a multiple of 128; buffers device, 16-byte aligned (sv 8-byte).  Operand layouts:
+ *   q8, k8 [B, N, H*64] e4m3 = e4m3_rn(x / s), s = 2^e per (token, head), e the smallest integer with amax <= 448 * 2^e,
+ *   e >= -126, s = 1 for an all-zero head (x: the 16-bit values the QKV epilogue would store); sq, sk [B*H, pad(N)]
+ *   those s at [item * H + head, token];
+ *   vt8 [B*H, 64, pad(N)] e4m3 of v^T / sv per (item, head, channel) over the item's N tokens, same rule; within every
+ *   32-key group, stored position j holds key 16 (j/16) + 8 ((j%4)/2) + 2 ((j/4)%4) + j%2; zero past N;  sv [B*H, 64].
+ * satb_attention_fp8_vt: v16 [B, N, H*64] 16-bit -> vt8, sv.
+ * satb_attention_fp8_core: o16 [B, Nq, H*64] = softmax((q8 sq)(k8 sk)^T / 8) (vt8^T sv) with P in e4m3 (see the
+ *   header comment of csrc/attention_fp8.cu) on operands of that layout (q8 / sq with Nq rows, k8 / sk / vt8 with Nk).
+ * satb_gemm_probe_qk8: the QKV GEMM with SATB_EPI_QKV_ROPE_E4M3 (bn 256) or SATB_EPI_HEAD_NORM_E4M3 (bn 256; 128 with
+ *   FP8 operands) as the forward runs it: A [M, K], W [N, K] 16-bit (a_scale NULL) or e4m3 with row scales a_scale [M],
+ *   w_scale [N] (fp16 out only); p gives out / ld (v columns >= 128 heads, 16-bit), bf16, b_static, rope_cols,
+ *   seq_len, cos_tab / sin_tab ([seq_len, 16]); q columns [0, 64 heads) -> o->q8, k columns -> o->k8 (row pitch
+ *   64 heads), scales at (row / seq_len * heads + head) * scale_ld + row % seq_len.  N a multiple of 64. */
+typedef struct SatbQkE4m3 {
+  void* q8;
+  void* k8;
+  float* sq;
+  float* sk;
+  int heads, scale_ld;
+} SatbQkE4m3;
+int satb_attention_fp8_vt(const void* v16, void* vt8, float* sv, int B, int H, int N, int bf16, void* stream);
+int satb_attention_fp8_core(const void* q8, const void* k8, const float* sq, const float* sk, const void* vt8,
+                            const float* sv, void* o16, int B, int H, int Nq, int Nk, int bf16, void* stream);
+int satb_gemm_probe_qk8(const void* a, const void* w, const float* a_scale, const float* w_scale, int M, int N, int K,
+                        const SatbGemmProbe* p, const SatbQkE4m3* o, void* stream);
 
 /* Test entry point: the kernel of the conformer branch, out = silu(LayerNorm(depthwise_conv(g))) per item
  * (transformer.py:583-586): g, out [items * n_seq, D] 16-bit (fp16/bf16 bits), 16-byte aligned; the convolution runs
