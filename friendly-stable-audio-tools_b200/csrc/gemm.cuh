@@ -923,6 +923,96 @@ struct EpiSwiglu {
   }
 };
 
+// ------------------------------------------------------- T5 feed-forward epilogues (t5.cu)
+// Two 16-bit pairs of the T5 encoder's FF-in activations.  In fp16 the values saturate to +-65504 instead of rounding
+// to infinity (cvt .satfinite; a NaN stays NaN): the encoder's overflow behaviour, where the reference's fp16 model
+// clamps its infinities afterwards (modeling_t5.py:451-456).  bf16 has the range of fp32 and is stored as is.
+template <bool BF16>
+__device__ __forceinline__ uint32_t pack16_satfinite(float a, float b) {
+  if constexpr (BF16) {
+    return Op16<true>::pack(a, b);
+  } else {
+    uint32_t r;
+    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));
+    return r;
+  }
+}
+
+// T5 FF-in with the ReLU of T5DenseActDense (modeling_t5.py:84-103): out16[row, col] = max(acc, 0), saturating.  A type
+// of its own so that EpiStore16 keeps no runtime activation branch for it.  N a multiple of 32.
+template <bool BF16>
+struct EpiRelu16 {
+  static constexpr int kCols = 32;
+  static constexpr int kStageBytes = 0;
+  static constexpr bool kFragment = true;
+  struct Params {
+    void* out;
+    int ld;
+  };
+  template <int BN>
+  __device__ static __forceinline__ void apply_fragment(const Params& p, const float (&acc)[BN / 2], int L, int N,
+                                                        int row0, int n0, int batch, int lane) {
+#pragma unroll
+    for (int j = 0; j < BN / 8; j += 2) {
+      if (n0 + 8 * j >= N) break;
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int l = row0 + 8 * rr;
+        uint32_t w[2];
+#pragma unroll
+        for (int g = 0; g < 2; ++g)
+          w[g] = pack16_satfinite<BF16>(fmaxf(acc[4 * (j + g) + 2 * rr], 0.f), fmaxf(acc[4 * (j + g) + 2 * rr + 1], 0.f));
+        store16_group_pair(static_cast<uint16_t*>(p.out) + static_cast<size_t>(batch * L + l) * p.ld, n0 + 8 * j, w[0],
+                           w[1], lane, l < L);
+      }
+    }
+  }
+};
+
+// gelu_new (the tanh form, transformers activations.NewGELUActivation): 0.5 x (1 + tanh(sqrt(2 / pi) (x + 0.044715 x^3)))
+__device__ __forceinline__ float gelu_tanh_f(float x) {
+  return 0.5f * x * (1.0f + tanhf(0.7978845608028654f * fmaf(0.044715f * x, x * x, x)));
+}
+
+// T5 FF-in of T5DenseGatedActDense (modeling_t5.py:106-130): out16[row, c] = gelu_new(x wi_0[c]) * (x wi_1[c]),
+// saturating.  The weight is [wi_1; wi_0] interleaved at load time as swiglu_perm does (every 64 rows: 32 rows of wi_1,
+// then the same 32 rows of wi_0), so value column c and gate column c + 32 sit in one thread's fragment as in EpiSwiglu.
+// N (= 2 d_ff) a multiple of 64; out [M, N / 2].
+template <bool BF16>
+struct EpiGeglu16 {
+  static constexpr int kCols = 64;
+  static constexpr int kStageBytes = 0;
+  static constexpr bool kFragment = true;
+  struct Params {
+    void* out;
+    int ld;   // d_ff (N / 2)
+  };
+  template <int BN>
+  __device__ static __forceinline__ void apply_fragment(const Params& p, const float (&acc)[BN / 2], int L, int N,
+                                                        int row0, int n0, int batch, int lane) {
+#pragma unroll
+    for (int g = 0; g < BN / 64; ++g) {
+      const int col0 = n0 + 64 * g;
+      if (col0 >= N) break;
+#pragma unroll
+      for (int jp = 0; jp < 4; jp += 2) {
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          const int l = row0 + 8 * rr;
+          uint32_t w[2];
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int av = 4 * (8 * g + jp + h) + 2 * rr, ag = av + 16;
+            w[h] = pack16_satfinite<BF16>(acc[av] * gelu_tanh_f(acc[ag]), acc[av + 1] * gelu_tanh_f(acc[ag + 1]));
+          }
+          store16_group_pair(static_cast<uint16_t*>(p.out) + static_cast<size_t>(batch * L + l) * p.ld,
+                             (col0 >> 1) + 8 * jp, w[0], w[1], lane, l < L);
+        }
+      }
+    }
+  }
+};
+
 // ------------------------------------------------------- convolution epilogues
 // SnakeBeta (models/blocks.py:318-319) with precomputed a = e^alpha, ib = 1/(e^beta + 1e-9):
 // v + ib * sin^2(a v) with the SFU sine (sin.approx = multiply by 1/2pi + MUFU.SIN, which is periodic

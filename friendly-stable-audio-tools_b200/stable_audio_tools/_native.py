@@ -30,6 +30,17 @@ class SatbDitConfig(ctypes.Structure):
 SATB_MAX_STAGES = 8
 
 
+class SatbT5Config(ctypes.Structure):
+    _fields_ = ([(n, ctypes.c_int) for n in (
+        "vocab_size", "d_model", "d_kv", "num_heads", "d_ff", "num_layers", "relative_attention_num_buckets",
+        "relative_attention_max_distance", "feed_forward_proj")]
+        + [("layer_norm_epsilon", ctypes.c_float), ("operand_dtype", ctypes.c_int)])
+
+
+# SatbT5Config.feed_forward_proj
+T5_FF_RELU, T5_FF_GATED_GELU = 0, 1
+
+
 class SatbOobleckConfig(ctypes.Structure):
     _fields_ = [("in_channels", ctypes.c_int), ("channels", ctypes.c_int), ("latent_dim", ctypes.c_int),
                 ("n_stages", ctypes.c_int), ("c_mults", ctypes.c_int * SATB_MAX_STAGES),
@@ -46,6 +57,8 @@ EPI_RESIDUAL_LN = 6   # retired (the LayerNorm-fold residual epilogue): refused,
 EPI_STORE32_POS = 7   # store32 plus a [seq_len, N] position-table row (project_in with a positional embedding)
 # satb_gemm_probe_qk8 only: the e4m3 QKV epilogues of FP8 self-attention
 EPI_QKV_ROPE_E4M3, EPI_HEAD_NORM_E4M3 = 8, 9
+# satb_t5_gemm_probe only: the T5 encoder's FF-in epilogues
+EPI_RELU16, EPI_GEGLU16 = 10, 11
 
 
 class SatbQkE4m3(ctypes.Structure):
@@ -142,6 +155,16 @@ SIGNATURES = {
     "satb_pqmf_load_filter": (_I, [_VP, _VP, _VP]),
     "satb_pqmf_analysis": (_I, [_VP, _VP, _VP, _I, _I, _LL, _VP]),
     "satb_pqmf_synthesis": (_I, [_VP, _VP, _VP, _I, _I, _I, _VP]),
+    "satb_t5_create": (_I, [ctypes.POINTER(SatbT5Config), ctypes.POINTER(_VP)]),
+    "satb_t5_destroy": (None, [_VP]),
+    "satb_t5_load_weight": (_I, [_VP, ctypes.c_char_p, _VP, _LL, _VP]),
+    "satb_t5_set_buckets": (_I, [_VP, _VP, _I]),
+    "satb_t5_set_proj_out": (_I, [_VP, _VP, _VP, _I, _VP]),
+    "satb_t5_finalize": (_I, [_VP, _VP]),
+    "satb_t5_encode": (_I, [_VP, _VP, _VP, _I, _I, _VP, _VP]),
+    "satb_t5_rmsnorm_probe": (_I, [_VP, _VP, _VP, _I, _I, _F, _I, _VP]),
+    "satb_t5_attention_probe": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _VP, _VP]),
+    "satb_t5_gemm_probe": (_I, [_VP, _VP, _I, _I, _I, ctypes.POINTER(SatbGemmProbe), _VP]),
 }
 
 

@@ -6,7 +6,9 @@ They run once per generation, not per denoise step, so they stay plain PyTorch m
 (:39-61), ``T5Conditioner`` (frozen fp16 HF T5 encoder, padded to ``max_length``, masked
 positions zeroed, :261-346) and ``MultiConditioner`` (:505-549); state-dict keys match the
 reference (``conditioner.conditioners.<id>.embedder.embedding.0.weights`` ...).  The T5 encoder
-needs the HF model files locally or a network, exactly like the reference.
+needs the HF model files locally or a network, exactly like the reference.  ``T5Conditioner(native=True)`` (a JSON
+conditioner "config" may carry it) runs the same weights on the native packed encoder (models/t5.py) instead of HF's
+eager fp16 module.
 """
 import logging
 import math
@@ -100,11 +102,20 @@ class T5Conditioner(Conditioner):
                      "google/flan-t5-xl": 2048, "google/flan-t5-xxl": 4096}
 
     def __init__(self, output_dim: int, t5_model_name: str = "t5-base", max_length: int = 128,
-                 enable_grad: bool = False, project_out: bool = False):
+                 enable_grad: bool = False, project_out: bool = False, native: bool = False):
+        """native=True: the encoder runs on the native kernels (models/t5.py), inference only.  The HF model is still
+        loaded (and cast to fp16) exactly as with native=False; its weights are handed to the native encoder by
+        set_device, and the HF module itself stays on the CPU.  proj_out and the mask multiply run inside the native
+        encode."""
         assert t5_model_name in self.T5_MODEL_DIMS, f"Unknown T5 model name: {t5_model_name}"
+        if native and enable_grad:
+            raise NotImplementedError("T5Conditioner: native=True is inference only (enable_grad=True is refused)")
+        if native and max_length > 512:
+            raise NotImplementedError(f"T5Conditioner: the native encoder takes max_length <= 512, not {max_length}")
         super().__init__(self.T5_MODEL_DIMS[t5_model_name], output_dim, project_out=project_out)
         from transformers import AutoTokenizer, T5EncoderModel
         self.max_length, self.enable_grad, self.device = max_length, enable_grad, "cpu"
+        self.native = native
         prev = logging.root.manager.disable
         logging.disable(logging.ERROR)
         try:
@@ -119,17 +130,41 @@ class T5Conditioner(Conditioner):
             self.model = model
         else:
             self.__dict__["model"] = model     # frozen: kept out of the state dict like the reference
+        if native:
+            from .t5 import T5Encoder
+            self.__dict__["native_encoder"] = T5Encoder.from_config(model.config, operand_dtype="fp16")
 
     def set_device(self, device):
         self.to(device)
-        self.model.to(device)
+        if self.native:
+            self._load_native(device)
+        else:
+            self.model.to(device)
         self.device = device
+
+    def _load_native(self, device):
+        """Loads the HF module's (fp16) weights into the native encoder on `device` (once per device), and proj_out."""
+        from .._native import NativeError
+        enc = self.__dict__["native_encoder"]
+        device = torch.device(device)
+        if device.type != "cuda":
+            raise NativeError("T5Conditioner(native=True) runs on a CUDA device only (no CPU fallback)")
+        if device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device())
+        if enc.device != device:
+            enc.load_state_dict(self.model.state_dict(), device=device)
+        if isinstance(self.proj_out, nn.Linear):   # its current parameters (a state dict may have been loaded since)
+            enc.set_proj_out(self.proj_out.weight, self.proj_out.bias)
 
     def forward(self, texts: tp.List[str]):
         enc = self.tokenizer(texts, truncation=True, max_length=self.max_length, padding="max_length",
                              return_tensors="pt")
         ids = enc["input_ids"].to(self.device)
         mask = enc["attention_mask"].to(self.device).to(torch.bool)
+        if self.native:
+            self._load_native(self.device)
+            with torch.no_grad():
+                return self.__dict__["native_encoder"](ids, mask), mask
         self.model.eval()
         with torch.set_grad_enabled(self.enable_grad):
             emb = self.model(input_ids=ids, attention_mask=mask)["last_hidden_state"]

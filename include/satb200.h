@@ -424,6 +424,65 @@ int satb_pqmf_analysis(SatbPqmf* h, const float* audio, float* bands, int B, int
 /* bands [B, C * num_bands, frames] -> audio [B, C, frames * num_bands] (PQMF.inverse). */
 int satb_pqmf_synthesis(SatbPqmf* h, const float* bands, float* audio, int B, int C, int frames, void* stream);
 
+/* ---- T5 encoder: replaces Hugging Face T5EncoderModel.forward (transformers models/t5/modeling_t5.py) behind
+ *      T5Conditioner.forward (models/conditioners.py).  Prompts are packed (sum of lengths rows, nothing computed for
+ *      padding); fp32 residual stream, 16-bit GEMM operands; csrc/t5.cu describes the launches.
+ * Mirrors the T5Config fields the encoder uses.  Refused by satb_t5_create: d_kv other than 64 or 128, feed_forward_proj
+ * other than relu / gated-gelu, d_model not a multiple of 128 or above 4096, d_ff not a multiple of 32. */
+#define SATB_T5_FF_RELU 0          /* "relu": DenseReluDense.wi, ReLU, wo */
+#define SATB_T5_FF_GATED_GELU 1    /* "gated-gelu": gelu_new(wi_0 x) * (wi_1 x), wo */
+typedef struct SatbT5Config {
+  int vocab_size;
+  int d_model;
+  int d_kv;
+  int num_heads;
+  int d_ff;
+  int num_layers;
+  int relative_attention_num_buckets;
+  int relative_attention_max_distance;   /* informational: the buckets come from satb_t5_set_buckets */
+  int feed_forward_proj;                 /* SATB_T5_FF_* */
+  float layer_norm_epsilon;
+  int operand_dtype;                     /* 0 = fp16 (the reference's dtype), 1 = bf16 */
+} SatbT5Config;
+typedef struct SatbT5 SatbT5;
+int satb_t5_create(const SatbT5Config* cfg, SatbT5** out);
+void satb_t5_destroy(SatbT5* h);
+/* One T5EncoderModel state-dict entry by its HF key ("shared.weight" or "encoder.embed_tokens.weight",
+ * "encoder.block.{i}.layer.0.SelfAttention.{q,k,v,o}.weight", block 0's "...SelfAttention.relative_attention_bias.weight",
+ * "encoder.block.{i}.layer.1.DenseReluDense.{wi | wi_0, wi_1, wo}.weight", "encoder.block.{i}.layer.{0,1}.layer_norm.weight",
+ * "encoder.final_layer_norm.weight"); src: device fp32, contiguous. */
+int satb_t5_load_weight(SatbT5* h, const char* name, const float* src, long long numel, void* stream);
+/* buckets (host) [1023]: the bucket of relative position j - i = k - 511 at index k, as
+ * T5Attention._relative_position_bucket(bidirectional=True, num_buckets, max_distance) gives it; each in
+ * [0, num_buckets).  Required before satb_t5_finalize. */
+int satb_t5_set_buckets(SatbT5* h, const int* buckets, int n);
+/* Optional output projection (the conditioner's proj_out Linear): W [out_dim, d_model], b [out_dim], device fp32;
+ * out_dim a multiple of 8.  Without it the encoder writes d_model columns. */
+int satb_t5_set_proj_out(SatbT5* h, const float* W, const float* b, int out_dim, void* stream);
+/* Checks that every weight and the buckets are there and builds the bias table (synchronous). */
+int satb_t5_finalize(SatbT5* h, void* stream);
+/* ids_dev [B, L] int64 (device), lengths_host [B]: item b is the right-padded prefix ids[b, :lengths[b]] (0 <= length
+ * <= L); 1 <= L <= 512.  out_dev [B, L, out_dim or d_model] fp32: the encoder's last hidden state (projected when
+ * proj_out is set) at valid positions, exact zeros at padded ones.  Ids outside [0, vocab_size) are clamped to the table
+ * (the Python layer refuses them). */
+int satb_t5_encode(SatbT5* h, const long long* ids_dev, const int* lengths_host, int B, int L, float* out_dev,
+                   void* stream);
+/* Test entry points (no product path calls them), through the launches the encode makes:
+ * satb_t5_rmsnorm_probe: out[r, :] = w * (x[r, :] * rsqrt(mean(x[r, :]^2) + eps)); x [rows, D] fp32; out_kind 0 = fp16
+ *   (saturating at +-65504), 1 = bf16, 2 = fp32; D a multiple of 4, at most 4096; pointers 16-byte aligned.
+ * satb_t5_attention_probe: qkv16 [M, 3 H d_kv] packed rows (M = sum of lengths_host[B], each at most 512): q of head h
+ *   at column h d_kv, k at (H + h) d_kv, v at (2 H + h) d_kv; bias_tab [H, 1023] fp32, entry k the bias of key j for
+ *   query i with k = j - i + 511; o16 [M, H d_kv] = softmax(q k^T + bias) v per item and head (no scale).
+ * satb_t5_gemm_probe: C = A[M, K] W[N, K]^T through one of the encoder's own FF-in epilogues (p->epi, p->bn 128 / 256,
+ *   p->bf16, p->out, p->ld); the other GEMM probes refuse these ids and this one refuses theirs. */
+#define SATB_EPI_RELU16 10    /* out 16-bit = max(acc, 0), saturating in fp16 */
+#define SATB_EPI_GEGLU16 11   /* out[:, N / 2] = value * gelu_new(gate), 32 / 32 interleaved columns, saturating in fp16 */
+int satb_t5_rmsnorm_probe(const float* x, const float* w, void* out, int rows, int D, float eps, int out_kind,
+                          void* stream);
+int satb_t5_attention_probe(const void* qkv16, const float* bias_tab, const int* lengths_host, int B, int H, int d_kv,
+                            int bf16, void* o16, void* stream);
+int satb_t5_gemm_probe(const void* a16, const void* w16, int M, int N, int K, const SatbGemmProbe* p, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
