@@ -742,3 +742,71 @@ int satb_t5_gemm_probe(const void* a16, const void* w16, int M, int N, int K, co
 }
 
 }  // extern "C"
+
+// Every GEMM of an encode through t5_linear, with the parameters t5_encode_impl passes.
+template <bool BF16>
+static int t5_linear_probe(const void* a16, int a_rows, const void* w16, int M, int N, int K, const SatbGemmProbe& p,
+                           cudaStream_t st) {
+  TmapCache tc;
+  const int bn = p.bn;
+  auto out_ok = [&](int cols, int elem) {
+    return p.out && (reinterpret_cast<uintptr_t>(p.out) & 15) == 0 && p.ld >= cols && (p.ld * elem) % 16 == 0;
+  };
+  switch (p.epi) {
+    case SATB_EPI_STORE16:   // QKV
+      SATB_REQUIRE(N % 32 == 0 && out_ok(N, 2), "T5 linear probe store16: N % 32 == 0, out 16-byte aligned, ld >= N");
+      return t5_linear<EpiStore16<BF16>, BF16>(tc, a16, a_rows, M, K, w16, N,
+                                              typename EpiStore16<BF16>::Params{p.out, p.ld, nullptr, 0}, st, bn);
+    case SATB_EPI_RESIDUAL:  // o-projection, FF-out
+      SATB_REQUIRE(N % 8 == 0 && p.h && (reinterpret_cast<uintptr_t>(p.h) & 15) == 0 && p.ld >= N && p.ld % 4 == 0,
+                   "T5 linear probe residual: N % 8 == 0, h 16-byte aligned, ld >= N, ld % 4 == 0");
+      return t5_linear<EpiResidual, BF16>(tc, a16, a_rows, M, K, w16, N,
+                                          EpiResidual::Params{p.h, p.ld, nullptr, nullptr, 1, 0, 1}, st, bn);
+    case SATB_EPI_STORE32:   // proj_out
+      SATB_REQUIRE(N % 8 == 0 && out_ok(N, 4) && p.bias && (reinterpret_cast<uintptr_t>(p.bias) & 15) == 0,
+                   "T5 linear probe store32: N % 8 == 0, out and bias 16-byte aligned, ld >= N");
+      return t5_linear<EpiStore32, BF16>(tc, a16, a_rows, M, K, w16, N,
+                                         EpiStore32::Params{static_cast<float*>(p.out), p.ld, p.bias}, st, bn);
+    case SATB_EPI_RELU16:    // FF-in, relu
+      SATB_REQUIRE(N % 32 == 0 && out_ok(N, 2), "T5 linear probe relu16: N % 32 == 0, out 16-byte aligned, ld >= N");
+      return t5_linear<EpiRelu16<BF16>, BF16>(tc, a16, a_rows, M, K, w16, N,
+                                             typename EpiRelu16<BF16>::Params{p.out, p.ld}, st, bn);
+    case SATB_EPI_GEGLU16:   // FF-in, gated-gelu
+      SATB_REQUIRE(N % 64 == 0 && out_ok(N / 2, 2),
+                   "T5 linear probe geglu16: N % 64 == 0, out 16-byte aligned, ld >= N / 2");
+      return t5_linear<EpiGeglu16<BF16>, BF16>(tc, a16, a_rows, M, K, w16, N,
+                                              typename EpiGeglu16<BF16>::Params{p.out, p.ld}, st, bn);
+    default:
+      break;
+  }
+  set_last_error("T5 linear probe: no such instance (epi " + std::to_string(p.epi) +
+                 "); an encode runs store16 (1), residual (5), store32 (0), relu16 (10) and geglu16 (11)");
+  return -1;
+}
+
+extern "C" {
+
+int satb_t5_linear_probe(const void* a16, int a_rows, const void* w16, int M, int N, int K, const SatbGemmProbe* p,
+                         void* stream) {
+  SATB_REQUIRE(a16 && w16 && p, "null argument");
+  SATB_REQUIRE(M >= 1 && a_rows >= M && N >= 8 && K >= 8 && K % 8 == 0,
+               "T5 linear probe: need 1 <= M <= a_rows, N >= 8 and K % 8 == 0");
+  SATB_REQUIRE((reinterpret_cast<uintptr_t>(a16) & 15) == 0 && (reinterpret_cast<uintptr_t>(w16) & 15) == 0,
+               "T5 linear probe: operands must be 16-byte aligned");
+  SATB_REQUIRE(p->bn == 0 || p->bn == 128 || p->bn == 256, "T5 linear probe: bn must be 0 (auto_bn), 128 or 256");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return p->bf16 ? t5_linear_probe<true>(a16, a_rows, w16, M, N, K, *p, st)
+                 : t5_linear_probe<false>(a16, a_rows, w16, M, N, K, *p, st);
+}
+
+int satb_t5_bias_table(SatbT5* t, float* dst, void* stream) {
+  SATB_REQUIRE(t && dst, "null argument");
+  SATB_REQUIRE(t->finalized, "T5: call satb_t5_finalize first (it builds the bias table)");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  SATB_CHECK_CUDA(cudaMemcpyAsync(dst, t->bias_tab, static_cast<size_t>(t->H) * kT5BiasSpan * sizeof(float),
+                                  cudaMemcpyDeviceToDevice, st));
+  SATB_CHECK_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+}  // extern "C"

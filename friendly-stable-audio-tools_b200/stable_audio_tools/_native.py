@@ -165,6 +165,8 @@ SIGNATURES = {
     "satb_t5_rmsnorm_probe": (_I, [_VP, _VP, _VP, _I, _I, _F, _I, _VP]),
     "satb_t5_attention_probe": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _VP, _VP]),
     "satb_t5_gemm_probe": (_I, [_VP, _VP, _I, _I, _I, ctypes.POINTER(SatbGemmProbe), _VP]),
+    "satb_t5_linear_probe": (_I, [_VP, _I, _VP, _I, _I, _I, ctypes.POINTER(SatbGemmProbe), _VP]),
+    "satb_t5_bias_table": (_I, [_VP, _VP, _VP]),
 }
 
 

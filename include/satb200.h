@@ -482,6 +482,16 @@ int satb_t5_rmsnorm_probe(const float* x, const float* w, void* out, int rows, i
 int satb_t5_attention_probe(const void* qkv16, const float* bias_tab, const int* lengths_host, int B, int H, int d_kv,
                             int bf16, void* o16, void* stream);
 int satb_t5_gemm_probe(const void* a16, const void* w16, int M, int N, int K, const SatbGemmProbe* p, void* stream);
+/* satb_t5_linear_probe: C = A[M, K] W[N, K]^T through the encoder's own GEMM launch with the parameters an encode
+ *   passes: SATB_EPI_STORE16 (QKV; out, ld), SATB_EPI_RESIDUAL (o-projection and FF-out: h[M, ld] += C, no bias, no
+ *   gate), SATB_EPI_STORE32 (proj_out: out = C + bias, bias required), SATB_EPI_RELU16 / SATB_EPI_GEGLU16 (FF-in).
+ *   A's tensor map spans a_rows >= M rows, as the encoder's spans its workspace; the tiles cover M.  p->bn: 128, 256,
+ *   or 0 for the tile the encoder picks at this (M, N).  p->bf16 selects the operand type.
+ * satb_t5_bias_table: copies the finalized relative-position bias table [H, 1023] fp32 (entry k of head h: the bias of
+ *   relative position k - 511, rel[bucket, h]) to the device buffer dst (synchronous). */
+int satb_t5_linear_probe(const void* a16, int a_rows, const void* w16, int M, int N, int K, const SatbGemmProbe* p,
+                         void* stream);
+int satb_t5_bias_table(SatbT5* h, float* dst, void* stream);
 
 #ifdef __cplusplus
 }

@@ -199,6 +199,96 @@ def test_attention_checker_is_sharp(dk):
         assert t5_ref.check_attention(bad, ref, out)[0] > 1.0
 
 
+def _attention_dense(qkv16, bias_tab, lengths, H, dk):
+    """t5_ref.attention's earlier formulation, all heads at once with the [H, n, n, dk] difference tensor."""
+    x = qkv16.double()
+    inner = H * dk
+    o = torch.zeros(x.shape[0], inner, dtype=torch.float64)
+    t1, t2 = torch.zeros_like(o), torch.zeros_like(o)
+    r0 = 0
+    for n in lengths:
+        if n == 0:
+            continue
+        rows = x[r0:r0 + n]
+        q = rows[:, :inner].view(n, H, dk).transpose(0, 1)
+        k = rows[:, inner:2 * inner].view(n, H, dk).transpose(0, 1)
+        v = rows[:, 2 * inner:].view(n, H, dk).transpose(0, 1)
+        i = torch.arange(n)
+        b = bias_tab.double()[:, (i[None, :] - i[:, None]) + 511]
+        s = q @ k.transpose(1, 2) + b
+        p = torch.softmax(s, dim=-1)
+        oh = p @ v
+        ds = (dk / 16 + 1) * 2.0 ** -22 * (q.abs() @ k.abs().transpose(1, 2)) + 2.0 ** -22 * s.abs()
+        dv = (v[:, None, :, :] - oh[:, :, None, :]).abs()
+        o[r0:r0 + n] = oh.transpose(0, 1).reshape(n, inner)
+        t1[r0:r0 + n] = (p @ v.abs()).transpose(0, 1).reshape(n, inner)
+        t2[r0:r0 + n] = ((p * ds)[..., None] * dv).sum(2).transpose(0, 1).reshape(n, inner)
+        r0 += n
+    return o, t1, t2
+
+
+@pytest.mark.parametrize("dk", [64, 128])
+def test_attention_reference_equals_the_dense_formulation(dk):
+    """The head-by-head, query-block-by-block evaluation computes the same three terms to float64 rounding."""
+    g = torch.Generator().manual_seed(3)
+    H, lengths = 3, [1, 0, 17, 64, 65, 150]
+    qkv = (torch.randn(sum(lengths), 3 * H * dk, generator=g) * 0.3).half()
+    bias = torch.randn(H, 1023, generator=g) * 2
+    new = t5_ref.attention(qkv, bias, lengths, H, dk)
+    for a, b in zip(new, _attention_dense(qkv, bias, lengths, H, dk)):
+        assert torch.allclose(a, b, rtol=1e-12, atol=0), float(((a - b).abs() / b.abs().clamp_min(1e-300)).max())
+
+
+@pytest.mark.parametrize("dk", [64, 128])
+def test_attention_checker_is_sharp_at_128_heads(dk):
+    """t5-11b's head count: a head that reads its neighbour's q columns, a mirrored bias and keys of the wrong item
+    are each rejected."""
+    g = torch.Generator().manual_seed(4)
+    H, lengths = 128, [1, 17, 40]
+    M, inner = sum(lengths), H * dk
+    qkv = (torch.randn(M, 3 * inner, generator=g) * 0.25).half()
+    rel = torch.randn(32, H, generator=g)
+    pos = torch.arange(-511, 512)
+    bias = rel[to.relative_position_bucket(pos, 32, 128)].T.contiguous()
+    ref = t5_ref.attention(qkv, bias, lengths, H, dk)
+    assert t5_ref.check_attention(ref[0].half(), ref, "fp16")[0] <= 1.0
+    neighbour = qkv.clone()
+    neighbour[:, :inner] = qkv[:, :inner].roll(-dk, dims=1)            # head h reads head h + 1's q
+    bad = t5_ref.attention(neighbour, bias, lengths, H, dk)[0].half()
+    assert t5_ref.check_attention(bad, ref, "fp16")[0] > 1.0
+    bad = t5_ref.attention(qkv, bias, lengths, H, dk, bias_sign=-1)[0].half()
+    assert t5_ref.check_attention(bad, ref, "fp16")[0] > 1.0
+    bad = t5_ref.attention(qkv, bias, [M], H, dk)[0].half()              # keys of the wrong item
+    assert t5_ref.check_attention(bad, ref, "fp16")[0] > 1.0
+
+
+def test_gemm_bound_rejects_a_dropped_k_block_at_k65536():
+    """t5-11b's FF-out (K = 65536, residual into the fp32 stream) on t5_ref.gemm_operand's rows: an accumulator that
+    loses any one 64-wide k-block fails the bound, the float64 sum rounded to fp32 passes."""
+    K, N = 65536, 32
+    M = K // 64                        # every k-block is heavy in one row
+    g = torch.Generator().manual_seed(5)
+    a = t5_ref.both_16bit(t5_ref.gemm_operand(M, K, g))
+    w = t5_ref.both_16bit(torch.randn(N, K, generator=g) * K ** -0.5)
+    h0 = torch.randn(M, N, generator=g)
+    acc, S = R.accumulate(a, w)
+    exp = R.epi_residual(acc, S, h0)
+    assert R.check((h0.double() + acc).float(), exp, K, "fp32").ok
+    for blk in (0, 1, 511, 1023):
+        c = slice(64 * blk, 64 * blk + 64)
+        dropped = acc - a[:, c].double() @ w[:, c].double().T
+        assert not R.check((h0.double() + dropped).float(), exp, K, "fp32").ok, blk
+
+
+def test_operands_shared_by_fp16_and_bf16_are_exact_in_both():
+    g = torch.Generator().manual_seed(6)
+    x = t5_ref.both_16bit(torch.cat([torch.randn(4096, generator=g) * s for s in (1e-6, 1e-3, 1, 300)]))
+    assert torch.equal(x.half().float(), x) and torch.equal(x.bfloat16().float(), x)
+    a = t5_ref.gemm_operand(40, 4096, g)
+    heavy = a.abs().view(40, 64, 64).mean(-1).argmax(-1)
+    assert torch.equal(heavy, torch.arange(40) % 64)
+
+
 @pytest.mark.parametrize("out", ["fp16", "bf16"])
 def test_ff_in_epilogue_checkers_are_sharp(out):
     g = torch.Generator().manual_seed(2)
@@ -209,6 +299,13 @@ def test_ff_in_epilogue_checkers_are_sharp(out):
     e = t5_ref.epi_relu(acc, S, out)
     assert R.check(e.ref.to(dt), e, 128, out).ok
     assert not R.check(acc.to(dt), e, 128, out).ok                          # no ReLU
+    # an exact accumulator a hair below zero whose fp32 one, off by half the rounding bound, lands above it
+    tiny = acc.clone()
+    tiny[0, 0] = -0.25 * R.e_acc(128) * S[0, 0]
+    e = t5_ref.epi_relu(tiny, S, out)
+    kernel = tiny.clone()
+    kernel[0, 0] = 0.25 * R.e_acc(128) * S[0, 0]
+    assert R.check(kernel.clamp_min(0).to(dt), e, 128, out).ok
     e = t5_ref.epi_geglu(acc, S, out)
     assert R.check(e.ref.to(dt), e, 128, out, col_scale=2).ok
     n = 128
