@@ -1013,6 +1013,46 @@ struct EpiGeglu16 {
   }
 };
 
+// ------------------------------------------------------- RoBERTa feed-forward epilogue (roberta.cu)
+// The exact erf GELU of transformers' ACT2FN["gelu"] (GELUActivation, torch.nn.functional.gelu), not gelu_new.
+__device__ __forceinline__ float gelu_erf_f(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
+
+// RoBERTa FF-in (RobertaIntermediate): out16[row, col] = gelu(acc + bias[col]), saturating in fp16 like EpiRelu16.
+// N a multiple of 32.
+template <bool BF16>
+struct EpiBiasGelu16 {
+  static constexpr int kCols = 32;
+  static constexpr int kStageBytes = 0;
+  static constexpr bool kFragment = true;
+  struct Params {
+    void* out;
+    int ld;
+    const float* bias;
+  };
+  template <int BN>
+  __device__ static __forceinline__ void apply_fragment(const Params& p, const float (&acc)[BN / 2], int L, int N,
+                                                        int row0, int n0, int batch, int lane) {
+    const int fc = 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < BN / 8; j += 2) {
+      if (n0 + 8 * j >= N) break;
+      const float2 b[2] = {__ldg(reinterpret_cast<const float2*>(p.bias + n0 + 8 * j + fc)),
+                           __ldg(reinterpret_cast<const float2*>(p.bias + n0 + 8 * j + 8 + fc))};
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int l = row0 + 8 * rr;
+        uint32_t w[2];
+#pragma unroll
+        for (int g = 0; g < 2; ++g)
+          w[g] = pack16_satfinite<BF16>(gelu_erf_f(acc[4 * (j + g) + 2 * rr] + b[g].x),
+                                        gelu_erf_f(acc[4 * (j + g) + 2 * rr + 1] + b[g].y));
+        store16_group_pair(static_cast<uint16_t*>(p.out) + static_cast<size_t>(batch * L + l) * p.ld, n0 + 8 * j, w[0],
+                           w[1], lane, l < L);
+      }
+    }
+  }
+};
+
 // ------------------------------------------------------- convolution epilogues
 // SnakeBeta (models/blocks.py:318-319) with precomputed a = e^alpha, ib = 1/(e^beta + 1e-9):
 // v + ib * sin^2(a v) with the SFU sine (sin.approx = multiply by 1/2pi + MUFU.SIN, which is periodic

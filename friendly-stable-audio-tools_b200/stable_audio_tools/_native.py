@@ -41,6 +41,13 @@ class SatbT5Config(ctypes.Structure):
 T5_FF_RELU, T5_FF_GATED_GELU = 0, 1
 
 
+class SatbRobertaConfig(ctypes.Structure):
+    _fields_ = ([(n, ctypes.c_int) for n in (
+        "vocab_size", "hidden_size", "num_heads", "intermediate_size", "num_layers", "max_position_embeddings",
+        "type_vocab_size", "pad_token_id")]
+        + [("layer_norm_eps", ctypes.c_float), ("operand_dtype", ctypes.c_int)])
+
+
 class SatbOobleckConfig(ctypes.Structure):
     _fields_ = [("in_channels", ctypes.c_int), ("channels", ctypes.c_int), ("latent_dim", ctypes.c_int),
                 ("n_stages", ctypes.c_int), ("c_mults", ctypes.c_int * SATB_MAX_STAGES),
@@ -59,6 +66,8 @@ EPI_STORE32_POS = 7   # store32 plus a [seq_len, N] position-table row (project_
 EPI_QKV_ROPE_E4M3, EPI_HEAD_NORM_E4M3 = 8, 9
 # satb_t5_gemm_probe only: the T5 encoder's FF-in epilogues
 EPI_RELU16, EPI_GEGLU16 = 10, 11
+# satb_roberta_linear_probe only: the RoBERTa encoder's FF-in epilogue
+EPI_BIAS_GELU16 = 12
 
 
 class SatbQkE4m3(ctypes.Structure):
@@ -167,6 +176,16 @@ SIGNATURES = {
     "satb_t5_gemm_probe": (_I, [_VP, _VP, _I, _I, _I, ctypes.POINTER(SatbGemmProbe), _VP]),
     "satb_t5_linear_probe": (_I, [_VP, _I, _VP, _I, _I, _I, ctypes.POINTER(SatbGemmProbe), _VP]),
     "satb_t5_bias_table": (_I, [_VP, _VP, _VP]),
+    "satb_roberta_create": (_I, [ctypes.POINTER(SatbRobertaConfig), ctypes.POINTER(_VP)]),
+    "satb_roberta_destroy": (None, [_VP]),
+    "satb_roberta_load_weight": (_I, [_VP, ctypes.c_char_p, _VP, _LL, _VP]),
+    "satb_roberta_set_proj_out": (_I, [_VP, _VP, _VP, _I, _VP]),
+    "satb_roberta_finalize": (_I, [_VP, _VP]),
+    "satb_roberta_encode": (_I, [_VP, _VP, _VP, _I, _I, _VP, _VP]),
+    "satb_roberta_embed_probe": (_I, [_VP, _I, _I, _VP, _I, _VP, _I, _VP, _VP, _VP, _I, _I, _F, _VP, _VP, _I, _VP]),
+    "satb_roberta_layernorm_probe": (_I, [_VP, _VP, _VP, _I, _I, _F, _VP, _VP, _I, _VP]),
+    "satb_roberta_attention_probe": (_I, [_VP, _VP, _I, _I, _I, _I, _VP, _VP]),
+    "satb_roberta_linear_probe": (_I, [_VP, _VP, _I, _I, _I, ctypes.POINTER(SatbGemmProbe), _VP]),
 }
 
 

@@ -8,7 +8,8 @@ positions zeroed, :261-346) and ``MultiConditioner`` (:505-549); state-dict keys
 reference (``conditioner.conditioners.<id>.embedder.embedding.0.weights`` ...).  The T5 encoder
 needs the HF model files locally or a network, exactly like the reference.  ``T5Conditioner(native=True)`` (a JSON
 conditioner "config" may carry it) runs the same weights on the native packed encoder (models/t5.py) instead of HF's
-eager fp16 module.
+eager fp16 module.  ``CLAPTextConditioner`` (:105-192, ``"clap_text"``) returns hidden states of CLAP's RoBERTa
+text branch computed by the native encoder (models/roberta.py); it needs the roberta-base tokenizer files locally.
 """
 import logging
 import math
@@ -172,6 +173,99 @@ class T5Conditioner(Conditioner):
         return emb, mask
 
 
+def _clap_text_branch(clap_ckpt_path: str) -> tp.Dict[str, torch.Tensor]:
+    """The ``text_branch.*`` entries of a CLAP checkpoint, prefix removed, read as laion_clap's
+    ``clap_module.factory.load_state_dict`` reads it: ``torch.load``, the ``"state_dict"`` entry if there is one, and
+    a leading ``module.`` stripped from every key."""
+    ckpt = torch.load(clap_ckpt_path, map_location="cpu", weights_only=False)
+    sd = ckpt["state_dict"] if isinstance(ckpt, dict) and "state_dict" in ckpt else ckpt
+    if next(iter(sd.items()))[0].startswith("module"):
+        sd = {k[7:]: v for k, v in sd.items()}
+    pre = "text_branch."
+    return {k[len(pre):]: v for k, v in sd.items() if k.startswith(pre)}
+
+
+class CLAPTextConditioner(Conditioner):
+    """CLAP text features (the reference's ``use_text_features=True`` path): hidden state ``feature_layer_ix`` of
+    CLAP's RoBERTa text branch at every one of the 77 token positions, then ``proj_out``, with the tokenizer's
+    attention mask.  Padded positions keep their features, as in the reference.  The encoder runs on the native
+    kernels (models/roberta.py) with fp16 operands, inference only; the text branch's weights stay out of the state
+    dict, only ``proj_out`` is in it.
+
+    The text branch is roberta-base (every laion_clap checkpoint); its depth, vocabulary, FF width and position table
+    are read from the checkpoint's shapes.  ``audio_model_type`` and ``enable_fusion`` only shape CLAP's audio branch,
+    which the reference deletes, so they are accepted and ignored.  Refused: ``use_text_features=False`` (the pooled
+    embedding goes through laion_clap's own ``text_projection`` head) and ``finetune=True``."""
+
+    MAX_LENGTH = 77   # laion_clap's tokenizer: padding="max_length", truncation=True, max_length=77
+
+    def __init__(self, output_dim: int, clap_ckpt_path: str, use_text_features=False, feature_layer_ix: int = -1,
+                 audio_model_type="HTSAT-base", enable_fusion=True, project_out: bool = False, finetune: bool = False):
+        if not use_text_features:
+            raise NotImplementedError("CLAPTextConditioner: use_text_features=False (the pooled CLAP text embedding) "
+                                      "goes through laion_clap's text_projection head, which this build does not run")
+        if finetune:
+            raise NotImplementedError("CLAPTextConditioner: the native text encoder is inference only "
+                                      "(finetune=True is refused)")
+        super().__init__(768, output_dim, project_out=project_out)
+        from transformers import RobertaTokenizer
+        from .roberta import RobertaEncoder
+        self.use_text_features, self.feature_layer_ix, self.finetune = use_text_features, feature_layer_ix, finetune
+        self.device = "cpu"
+        prev = logging.root.manager.disable
+        logging.disable(logging.ERROR)
+        try:
+            with warnings.catch_warnings():
+                warnings.simplefilter("ignore")
+                self.tokenizer = RobertaTokenizer.from_pretrained("roberta-base")
+        finally:
+            logging.disable(prev)
+        sd = _clap_text_branch(clap_ckpt_path)
+        if not sd:
+            raise ValueError(f"{clap_ckpt_path} holds no text_branch.* weights")
+        D = sd["embeddings.word_embeddings.weight"].shape[1]
+        if D != self.dim:
+            raise NotImplementedError(f"CLAPTextConditioner: the text branch is {D} wide; CLAP's RoBERTa is 768")
+        cfg = dict(vocab_size=sd["embeddings.word_embeddings.weight"].shape[0], hidden_size=D,
+                   num_hidden_layers=1 + max(int(k.split(".")[2]) for k in sd if k.startswith("encoder.layer.")),
+                   num_attention_heads=D // 64, intermediate_size=sd["encoder.layer.0.intermediate.dense.weight"].shape[0],
+                   max_position_embeddings=sd["embeddings.position_embeddings.weight"].shape[0],
+                   type_vocab_size=sd["embeddings.token_type_embeddings.weight"].shape[0], pad_token_id=1,
+                   layer_norm_eps=1e-5, hidden_act="gelu")
+        self.__dict__["text_branch_state"] = sd       # frozen: kept out of the state dict like the reference
+        self.__dict__["native_encoder"] = RobertaEncoder.from_config(cfg, feature_layer_ix=feature_layer_ix)
+
+    def set_device(self, device):
+        self.to(device)
+        self._load_native(device)
+        self.device = device
+
+    def _load_native(self, device):
+        """Loads the text branch into the native encoder on `device` (once per device), and proj_out."""
+        from .._native import NativeError
+        enc = self.__dict__["native_encoder"]
+        device = torch.device(device)
+        if device.type != "cuda":
+            raise NativeError("CLAPTextConditioner runs on a CUDA device only (no CPU fallback)")
+        if device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device())
+        if enc.device != device:
+            enc.load_state_dict(self.__dict__["text_branch_state"], device=device)
+        if isinstance(self.proj_out, nn.Linear):   # its current parameters (a state dict may have been loaded since)
+            enc.set_proj_out(self.proj_out.weight, self.proj_out.bias)
+
+    def forward(self, texts: tp.List[str]):
+        # the reference tokenizes a single prompt together with "" (laion_clap's tokenizer squeezes a batch of one)
+        batch = [texts[0], ""] if len(texts) == 1 else list(texts)
+        enc = self.tokenizer(batch, padding="max_length", truncation=True, max_length=self.MAX_LENGTH,
+                             return_tensors="pt")
+        ids = enc["input_ids"][:len(texts)].to(self.device)
+        mask = enc["attention_mask"][:len(texts)].to(self.device)
+        self._load_native(self.device)
+        with torch.no_grad():
+            return [self.__dict__["native_encoder"](ids, mask), mask]
+
+
 class MultiConditioner(nn.Module):
     """Applies one conditioner per key of the per-item metadata dicts."""
 
@@ -200,7 +294,7 @@ class MultiConditioner(nn.Module):
         return out
 
 
-_TYPES = {"t5": T5Conditioner, "number": NumberConditioner, "int": IntConditioner}
+_TYPES = {"t5": T5Conditioner, "clap_text": CLAPTextConditioner, "number": NumberConditioner, "int": IntConditioner}
 
 
 def create_multi_conditioner_from_conditioning_config(config: tp.Dict[str, tp.Any]) -> MultiConditioner:

@@ -493,6 +493,64 @@ int satb_t5_linear_probe(const void* a16, int a_rows, const void* w16, int M, in
                          void* stream);
 int satb_t5_bias_table(SatbT5* h, float* dst, void* stream);
 
+/* ---- RoBERTa encoder: replaces Hugging Face RobertaModel(output_hidden_states=True).hidden_states[n] (transformers
+ *      models/roberta/modeling_roberta.py), the text branch behind the CLAP text conditioner's features
+ *      (models/conditioners.py CLAPTextConditioner).  All B L rows are computed, keys limited to each item's valid
+ *      prefix; fp32 residual stream, 16-bit GEMM operands; csrc/roberta.cu describes the launches.
+ * Mirrors the RobertaConfig fields the encoder uses, with num_layers the number of layers an encode runs (n: index n of
+ * hidden_states, 0 = the embedding output).  Refused by satb_roberta_create: hidden_size not a multiple of 128 or above
+ * 1024, head dim (hidden_size / num_heads) other than 64, intermediate_size not a multiple of 32. */
+typedef struct SatbRobertaConfig {
+  int vocab_size;
+  int hidden_size;
+  int num_heads;
+  int intermediate_size;
+  int num_layers;                 /* layers run */
+  int max_position_embeddings;
+  int type_vocab_size;
+  int pad_token_id;               /* also the padding_idx of the position ids */
+  float layer_norm_eps;
+  int operand_dtype;              /* 0 = fp16, 1 = bf16 */
+} SatbRobertaConfig;
+typedef struct SatbRoberta SatbRoberta;
+int satb_roberta_create(const SatbRobertaConfig* cfg, SatbRoberta** out);
+void satb_roberta_destroy(SatbRoberta* h);
+/* One RobertaModel state-dict entry by its HF key ("embeddings.{word,position,token_type}_embeddings.weight",
+ * "embeddings.LayerNorm.{weight,bias}", "encoder.layer.{i}.attention.self.{query,key,value}.{weight,bias}",
+ * "encoder.layer.{i}.attention.output.{dense,LayerNorm}.{weight,bias}", "encoder.layer.{i}.intermediate.dense.{weight,bias}",
+ * "encoder.layer.{i}.output.{dense,LayerNorm}.{weight,bias}", i < num_layers); src: device fp32, contiguous. */
+int satb_roberta_load_weight(SatbRoberta* h, const char* name, const float* src, long long numel, void* stream);
+/* Optional output projection (the conditioner's proj_out Linear): W [out_dim, hidden_size], b [out_dim], device fp32;
+ * out_dim a multiple of 8.  Without it the encoder writes hidden_size columns. */
+int satb_roberta_set_proj_out(SatbRoberta* h, const float* W, const float* b, int out_dim, void* stream);
+/* Checks that every weight is there (synchronous). */
+int satb_roberta_finalize(SatbRoberta* h, void* stream);
+/* ids_dev [B, L] int64 (device), lengths_host [B]: the keys of item b are positions [0, lengths[b]) (1 <= length <= L);
+ * 1 <= L <= 512 and L + pad_token_id < max_position_embeddings.  out_dev [B, L, out_dim or hidden_size] fp32: hidden
+ * state n (projected when proj_out is set) at every position, padded ones included.  Ids outside [0, vocab_size) are
+ * clamped to the table (the Python layer refuses them). */
+int satb_roberta_encode(SatbRoberta* h, const long long* ids_dev, const int* lengths_host, int B, int L, float* out_dev,
+                        void* stream);
+/* Test entry points (no product path calls them), through the launches the encode makes:
+ * satb_roberta_embed_probe: y[b L + t] = LayerNorm(word[ids[b, t]] + tok[0] + pos[p]) with p the position id of
+ *   create_position_ids_from_input_ids (padding_idx pad); y32 fp32 and y16 16-bit (fp16 saturating, or bf16) [B L, D].
+ * satb_roberta_layernorm_probe: y = LayerNorm(x) (gamma, beta) of x [rows, D] fp32 into y32 (may be x) and y16.
+ * satb_roberta_attention_probe: qkv16 [B L, 3 H 64] (q of head h at column 64 h, k at 64 (H + h), v at 64 (2 H + h));
+ *   o16 [B L, H 64] = softmax(q k^T / 8) v over keys [0, lengths_host[b]) of item b, for every one of its L rows.
+ * satb_roberta_linear_probe: C = A[M, K] W[N, K]^T through the encoder's GEMM launch with the parameters an encode
+ *   passes (bias required, ld == N): SATB_EPI_STORE16 (QKV), SATB_EPI_RESIDUAL (out-proj and FF-out: h += C + bias),
+ *   SATB_EPI_STORE32 (proj_out), SATB_EPI_BIAS_GELU16 (FF-in); p->bf16 selects the operand type. */
+#define SATB_EPI_BIAS_GELU16 12   /* out 16-bit = gelu(acc + bias) with the erf GELU, saturating in fp16 */
+int satb_roberta_embed_probe(const long long* ids, int B, int L, const float* word, int vocab, const float* pos,
+                             int max_pos, const float* tok, const float* gamma, const float* beta, int D, int pad,
+                             float eps, float* y32, void* y16, int bf16, void* stream);
+int satb_roberta_layernorm_probe(const float* x, const float* gamma, const float* beta, int rows, int D, float eps,
+                                 float* y32, void* y16, int bf16, void* stream);
+int satb_roberta_attention_probe(const void* qkv16, const int* lengths_host, int B, int L, int H, int bf16, void* o16,
+                                 void* stream);
+int satb_roberta_linear_probe(const void* a16, const void* w16, int M, int N, int K, const SatbGemmProbe* p,
+                              void* stream);
+
 #ifdef __cplusplus
 }
 #endif
