@@ -705,16 +705,12 @@ static bool needs_reserve(const SatbDit* d, int R, int L) {
   return R > d->res_R || L != d->res_L || d->P != d->res_P || (d->pos_type != 0 && d->pos_len != L + d->P);
 }
 
-extern "C" {
-
-// Reserve every activation buffer for R rows of L latent tokens (synchronous; call
-// before capturing a CUDA graph).  Grow-only.
-int satb_dit_reserve(SatbDit* d, int R, int L) {
-  SATB_REQUIRE(d && d->finalized, "weights not finalized");
-  SATB_REQUIRE(R >= 1 && L >= 1, "bad shape");
-  const int N_seq = L + d->P;
-  if (d->pos_type == 2 && N_seq > d->abs_max_len) {
-    set_last_error("sequence length " + std::to_string(N_seq) + " (latent tokens + prepended tokens) exceeds the absolute "
+// Every activation buffer for R rows of n tokens, and the rotary / positional tables for tab_len positions (n = tab_len
+// for the single-device forward; a rank of a group forward holds n of the tab_len tokens).  Grow-only.
+static int reserve_rows(SatbDit* d, int R, int n, int tab_len) {
+  const int N_seq = n;
+  if (d->pos_type == 2 && tab_len > d->abs_max_len) {
+    set_last_error("sequence length " + std::to_string(tab_len) + " (latent tokens + prepended tokens) exceeds the absolute "
                    "positional embedding's max length " + std::to_string(d->abs_max_len));
     return -1;
   }
@@ -740,9 +736,20 @@ int satb_dit_reserve(SatbDit* d, int R, int L) {
     SATB_PROPAGATE(make_attention_fp8_maps(&d->attn8_maps, attn_fp8_bufs(d->ws_attn8.p, R, d->H, N_seq, N_seq), R, d->H,
                                            N_seq, N_seq));
   }
-  if (d->rotary) SATB_PROPAGATE(ensure_rope(d, N_seq));
-  if (d->pos_type != 0) SATB_PROPAGATE(ensure_pos(d, N_seq));
+  if (d->rotary) SATB_PROPAGATE(ensure_rope(d, tab_len));
+  if (d->pos_type != 0) SATB_PROPAGATE(ensure_pos(d, tab_len));
   d->tmaps.maps.clear();
+  return 0;
+}
+
+extern "C" {
+
+// Reserve every activation buffer for R rows of L latent tokens (synchronous; call
+// before capturing a CUDA graph).  Grow-only.
+int satb_dit_reserve(SatbDit* d, int R, int L) {
+  SATB_REQUIRE(d && d->finalized, "weights not finalized");
+  SATB_REQUIRE(R >= 1 && L >= 1, "bad shape");
+  SATB_PROPAGATE(reserve_rows(d, R, L + d->P, L + d->P));
   d->res_R = R;
   d->res_L = L;
   d->res_P = d->P;
@@ -879,121 +886,180 @@ struct ProfScope {
 };
 enum { PROF_FF_IN = 0, PROF_FF_OUT, PROF_QKV, PROF_ATTN_SELF, PROF_ATTN_OUT, PROF_CROSS, PROF_LN, PROF_CONFORMER, PROF_NCAT };
 
+// The token rows one forward runs on one handle: R rows (B items, doubled under CFG) of n tokens each, the first P of
+// which are the prepended ones (global-conditioning and prepend-conditioning tokens).  The tokens are positions
+// pos0 .. pos0 + n - 1 of the rotary and positional tables, which hold tab_len positions.  The single-device forward is
+// the one shard that holds every token: P = d->P, n = tab_len = L + P, pos0 = 0.  A rank of a group forward holds a
+// contiguous range of every item's tokens, with the prepended ones on rank 0 only.
+struct FwdShape {
+  int B, R, L, P, n, pos0, tab_len;
+};
+
+// One forward as its stages: input (timestep embedding, project_in, prepended rows), then per block self_qkv, self_attn
+// and block_rest (cross-attention, conformer branch, feed-forward), then output (project_out, CFG combine).  The
+// single-device forward runs them in that order on one stream; the group forward interleaves the ranks' stages with the
+// K/V gather between self_qkv and self_attn.
 // FP8 = true: the QKV, cross-attention q and FF-in GEMMs read e4m3 LayerNorm rows (a8, one scale per row in a_scale)
 // and the e4m3 weights; everything else runs as in fp16 mode (BF16 = false).
 template <bool BF16, bool FP8 = false>
-static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* out, int B, int L, float cfg_scale,
-                            float scale_phi, cudaStream_t st, float* hidden_out) {
-  const int D = d->D, C = d->C, H = d->H, P = d->P;
-  const int R = d->cfg_on ? 2 * B : B;
-  const int N_seq = L + P;
-  const int M = R * N_seq;
-  const int Mc = d->Rc * N_seq;  // rows running cross-attention (a prefix of the row space)
-  SmallWs sw = small_ws(d, 2 * d->B);
-  float* h = d->ws_h.as<float>();
-  uint16_t* a16 = d->ws_a16.as<uint16_t>();
-  uint8_t* a8 = d->ws_a8.as<uint8_t>();
-  float* a_scale = d->ws_ascale.as<float>();
-  // LayerNorm rows for one of the three FP8-capable GEMMs: e4m3 + row scales in FP8 mode, 16-bit otherwise
-  auto layernorm_in = [&](const float* g, const float* b, int rows, const float* mod_scale, const float* mod_shift,
-                          int64_t mod_ld, int n_items) -> int {
-    if (FP8) return launch_layernorm_fp8(h, g, b, a8, a_scale, rows, D, mod_scale, mod_shift, mod_ld, N_seq, n_items, st);
-    return launch_layernorm(h, g, b, a16, rows, D, mod_scale, mod_shift, mod_ld, N_seq, n_items, BF16, st);
-  };
-  const void* a_in = FP8 ? static_cast<const void*>(a8) : static_cast<const void*>(a16);
-  uint16_t* qkv = d->ws_qkv.as<uint16_t>();
-  uint16_t* att = d->ws_attn.as<uint16_t>();
-  uint16_t* q16 = d->ws_q16.as<uint16_t>();
-  uint16_t* ff = d->ws_ff.as<uint16_t>();
-  uint16_t* ain = d->ws_ain.as<uint16_t>();
-  float* y = d->ws_y.as<float>();
-  // rotary off (satb_dit_set_positions): null tables, which the QKV epilogues take as no rotation
-  const float* cos_tab = d->rotary ? d->ws_rope.as<float>() : nullptr;
-  const float* sin_tab = d->rotary ? cos_tab + static_cast<size_t>(N_seq) * d->nf : nullptr;
-  const float* pos_tab = d->pos_type != 0 ? d->ws_pos.as<float>() : nullptr;
+struct DitFwd {
+  SatbDit* d;
+  FwdShape s;
+  cudaStream_t st;
+  int D, C, H, M, Mc;   // Mc: rows running cross-attention (a prefix of the row space)
+  int64_t ssg_ld;
+  SmallWs sw;
+  float* h;
+  uint16_t* a16;
+  uint8_t* a8;
+  float* a_scale;
+  const void* a_in;
+  uint16_t *qkv, *att, *q16, *ff, *ain;
+  float* y;
+  const float *cos_tab, *sin_tab, *pos_tab;
 
-  // timestep embedding (+ global embedding) -> conditioning token / adaLN vector  (dit.py:176-195)
-  SATB_PROPAGATE(launch_fourier(t, d->ts_w, sw.fourier, B, d->F, st));
-  // te_h = silu(W0 f + b0); tok = W2 te_h + b2 (+ global embed); in adaLN mode only silu(tok) is consumed
-  SATB_PROPAGATE(launch_skinny_linear(sw.fourier, d->te0_w, d->te0_b, nullptr, sw.te_h, B, 2 * d->F, D, 1, st));
-  SATB_PROPAGATE(launch_skinny_linear(sw.te_h, d->te2_w, d->te2_b, d->has_global ? sw.ge : nullptr, sw.tok, B, D, D,
-                                      d->adaln ? 1 : 0, st));
-  // latent -> token rows, project_in (with the 1x1 pre-conv folded), prepend token; a positional embedding is added to
-  // every row, prepended ones included, in project_in's epilogue and by write_prepend.  K is Cin_p: the pad columns of
-  // ain (zeroed by dit_pre) meet the zero columns of w_in16.
-  const int Kin = d->Cin_p;
-  SATB_PROPAGATE(launch_dit_pre(x, ain, R, B, d->Cin, Kin, L, P, BF16, st));
-  if (pos_tab)
-    SATB_PROPAGATE((linear<EpiStore32Pos, 256, BF16>(d->tmaps, ain, Kin, M, Kin, d->w_in16, D,
-                                                     EpiStore32Pos::Params{h, D, nullptr, pos_tab, N_seq}, st)));
-  else
-    SATB_PROPAGATE((linear<EpiStore32, 256, BF16>(d->tmaps, ain, Kin, M, Kin, d->w_in16, D, EpiStore32::Params{h, D, nullptr}, st)));
-  const int64_t ssg_ld = static_cast<int64_t>(d->depth) * 6 * D;
-  if (P > 0) {
-    SATB_PROPAGATE(launch_write_prepend(sw.tok, d->Pp > 0 ? d->ws_prep.as<float>() : nullptr, pos_tab, h, R, B, N_seq, D,
-                                        d->Pp, st));
-  } else {
-    // adaLN: all layers' scale/shift/gate in one skinny GEMM (transformer.py:648-651,667)
-    SATB_PROPAGATE(launch_skinny_linear(sw.tok, d->w_ssg, nullptr, nullptr, sw.ssg, B, D, d->depth * 6 * D, 0, st));
-    SATB_PROPAGATE(launch_gate_sigmoid(sw.ssg, B, d->depth, D, st));
+  DitFwd(SatbDit* d_, const FwdShape& s_, cudaStream_t st_) : d(d_), s(s_), st(st_) {
+    D = d->D; C = d->C; H = d->H;
+    M = s.R * s.n;
+    Mc = d->Rc * s.n;
+    ssg_ld = static_cast<int64_t>(d->depth) * 6 * D;
+    sw = small_ws(d, 2 * d->B);
+    h = d->ws_h.as<float>();
+    a16 = d->ws_a16.as<uint16_t>();
+    a8 = d->ws_a8.as<uint8_t>();
+    a_scale = d->ws_ascale.as<float>();
+    a_in = FP8 ? static_cast<const void*>(a8) : static_cast<const void*>(a16);
+    qkv = d->ws_qkv.as<uint16_t>();
+    att = d->ws_attn.as<uint16_t>();
+    q16 = d->ws_q16.as<uint16_t>();
+    ff = d->ws_ff.as<uint16_t>();
+    ain = d->ws_ain.as<uint16_t>();
+    y = d->ws_y.as<float>();
+    // rotary off (satb_dit_set_positions): null tables, which the QKV epilogues take as no rotation
+    const float* rope = d->ws_rope.as<float>();
+    cos_tab = d->rotary ? rope + static_cast<size_t>(s.pos0) * d->nf : nullptr;
+    sin_tab = d->rotary ? rope + static_cast<size_t>(s.tab_len + s.pos0) * d->nf : nullptr;
+    pos_tab = d->pos_type != 0 ? d->ws_pos.as<float>() + static_cast<size_t>(s.pos0) * D : nullptr;
   }
 
-  for (int i = 0; i < d->depth; ++i) {
+  // LayerNorm rows for one of the three FP8-capable GEMMs: e4m3 + row scales in FP8 mode, 16-bit otherwise
+  int layernorm_in(const float* g, const float* b, int rows, const float* mod_scale, const float* mod_shift,
+                   int64_t mod_ld, int n_items) {
+    if (FP8) return launch_layernorm_fp8(h, g, b, a8, a_scale, rows, D, mod_scale, mod_shift, mod_ld, s.n, n_items, st);
+    return launch_layernorm(h, g, b, a16, rows, D, mod_scale, mod_shift, mod_ld, s.n, n_items, BF16, st);
+  }
+
+  const float* ssg(int i) const { return d->adaln ? sw.ssg + static_cast<size_t>(i) * 6 * D : nullptr; }
+
+  int input(const float* x, const float* t) {
+    const int B = s.B;
+    // timestep embedding (+ global embedding) -> conditioning token / adaLN vector  (dit.py:176-195)
+    SATB_PROPAGATE(launch_fourier(t, d->ts_w, sw.fourier, B, d->F, st));
+    // te_h = silu(W0 f + b0); tok = W2 te_h + b2 (+ global embed); in adaLN mode only silu(tok) is consumed
+    SATB_PROPAGATE(launch_skinny_linear(sw.fourier, d->te0_w, d->te0_b, nullptr, sw.te_h, B, 2 * d->F, D, 1, st));
+    SATB_PROPAGATE(launch_skinny_linear(sw.te_h, d->te2_w, d->te2_b, d->has_global ? sw.ge : nullptr, sw.tok, B, D, D,
+                                        d->adaln ? 1 : 0, st));
+    // latent -> token rows, project_in (with the 1x1 pre-conv folded), prepend token; a positional embedding is added
+    // to every row, prepended ones included, in project_in's epilogue and by write_prepend.  K is Cin_p: the pad
+    // columns of ain (zeroed by dit_pre) meet the zero columns of w_in16.
+    const int Kin = d->Cin_p;
+    SATB_PROPAGATE(launch_dit_pre(x, ain, s.R, B, d->Cin, Kin, s.L, s.P, BF16, st));
+    if (pos_tab)
+      SATB_PROPAGATE((linear<EpiStore32Pos, 256, BF16>(d->tmaps, ain, Kin, M, Kin, d->w_in16, D,
+                                                       EpiStore32Pos::Params{h, D, nullptr, pos_tab, s.n}, st)));
+    else
+      SATB_PROPAGATE((linear<EpiStore32, 256, BF16>(d->tmaps, ain, Kin, M, Kin, d->w_in16, D, EpiStore32::Params{h, D, nullptr}, st)));
+    if (d->P > 0) {
+      if (s.P > 0)
+        SATB_PROPAGATE(launch_write_prepend(sw.tok, d->Pp > 0 ? d->ws_prep.as<float>() : nullptr, pos_tab, h, s.R, B,
+                                            s.n, D, d->Pp, st));
+    } else {
+      // adaLN: all layers' scale/shift/gate in one skinny GEMM (transformer.py:648-651,667)
+      SATB_PROPAGATE(launch_skinny_linear(sw.tok, d->w_ssg, nullptr, nullptr, sw.ssg, B, D, d->depth * 6 * D, 0, st));
+      SATB_PROPAGATE(launch_gate_sigmoid(sw.ssg, B, d->depth, D, st));
+    }
+    return 0;
+  }
+
+  // ---- self-attention, first half: LN -> QKV GEMM (+RoPE) into qkv
+  int self_qkv(int i) {
     const LayerW& W = d->layers[i];
-    const float* ssg_l = d->adaln ? sw.ssg + static_cast<size_t>(i) * 6 * D : nullptr;
-    // ---- self-attention: LN -> QKV GEMM (+RoPE) -> attention -> out-proj (+residual)
+    const float* ssg_l = ssg(i);
     {
       ProfScope ps(d, PROF_LN, st);
-      SATB_PROPAGATE(layernorm_in(W.pre_g, W.pre_b, M, ssg_l, ssg_l ? ssg_l + D : nullptr, ssg_ld, B));
+      SATB_PROPAGATE(layernorm_in(W.pre_g, W.pre_b, M, ssg_l, ssg_l ? ssg_l + D : nullptr, ssg_ld, s.B));
     }
-    {
-      ProfScope ps(d, PROF_QKV, st);
-      const void* w = FP8 ? static_cast<const void*>(W.w8_qkv) : static_cast<const void*>(W.w_qkv);
-      const Fp8Scales sc{a_scale, W.s_qkv};
-      // FP8 self-attention: q and k leave the epilogue as e4m3 with their scales, v in 16 bits as always
-      const AttnFp8Bufs b8 = d->attn_fp8 ? attn_fp8_bufs(d->ws_attn8.p, d->res_R, H, N_seq, N_seq) : AttnFp8Bufs{};
-      const QkE4m3Out o8{b8.q8, b8.k8, b8.sq, b8.sk, H, attn_fp8_pad(N_seq)};
-      if (d->qk_norm) {
-        typedef EpiHeadNorm16<BF16> E;   // q, k heads L2-normalised, then rotary
-        typename E::Params ep{qkv, 3 * D, 2 * D, 2 * D, N_seq, cos_tab, sin_tab};
-        // FP8: BN 128 (the instance the cross q GEMM also runs; the BN 256 one spills a few registers)
-        constexpr int kBn = FP8 ? 128 : 256;
-        if (d->attn_fp8)
-          SATB_PROPAGATE((linear<EpiHeadNormE4m3<BF16>, kBn, BF16, FP8>(d->tmaps, a_in, D, M, D, w, 3 * D,
-                                                                         {ep, o8}, st, 1, sc)));
-        else
-          SATB_PROPAGATE((linear<E, kBn, BF16, FP8>(d->tmaps, a_in, D, M, D, w, 3 * D, ep, st, 1, sc)));
-      } else {
-        typedef EpiQkvRope<BF16> E;
-        typename E::Params ep{qkv, 3 * D, 2 * D, N_seq, d->dh, d->nf, cos_tab, sin_tab};
-        if (d->attn_fp8)
-          SATB_PROPAGATE((linear<EpiQkvRopeE4m3<BF16>, 256, BF16, FP8>(d->tmaps, a_in, D, M, D, w, 3 * D, {ep, o8}, st,
-                                                                        1, sc)));
-        else
-          SATB_PROPAGATE((linear<E, 256, BF16, FP8>(d->tmaps, a_in, D, M, D, w, 3 * D, ep, st, 1, sc)));
-      }
+    ProfScope ps(d, PROF_QKV, st);
+    const void* w = FP8 ? static_cast<const void*>(W.w8_qkv) : static_cast<const void*>(W.w_qkv);
+    const Fp8Scales sc{a_scale, W.s_qkv};
+    // FP8 self-attention: q and k leave the epilogue as e4m3 with their scales, v in 16 bits as always
+    const AttnFp8Bufs b8 = d->attn_fp8 ? attn_fp8_bufs(d->ws_attn8.p, d->res_R, H, s.n, s.n) : AttnFp8Bufs{};
+    const QkE4m3Out o8{b8.q8, b8.k8, b8.sq, b8.sk, H, attn_fp8_pad(s.n)};
+    if (d->qk_norm) {
+      typedef EpiHeadNorm16<BF16> E;   // q, k heads L2-normalised, then rotary
+      typename E::Params ep{qkv, 3 * D, 2 * D, 2 * D, s.n, cos_tab, sin_tab};
+      // FP8: BN 128 (the instance the cross q GEMM also runs; the BN 256 one spills a few registers)
+      constexpr int kBn = FP8 ? 128 : 256;
+      if (d->attn_fp8)
+        SATB_PROPAGATE((linear<EpiHeadNormE4m3<BF16>, kBn, BF16, FP8>(d->tmaps, a_in, D, M, D, w, 3 * D,
+                                                                       {ep, o8}, st, 1, sc)));
+      else
+        SATB_PROPAGATE((linear<E, kBn, BF16, FP8>(d->tmaps, a_in, D, M, D, w, 3 * D, ep, st, 1, sc)));
+    } else {
+      typedef EpiQkvRope<BF16> E;
+      typename E::Params ep{qkv, 3 * D, 2 * D, s.n, d->dh, d->nf, cos_tab, sin_tab};
+      if (d->attn_fp8)
+        SATB_PROPAGATE((linear<EpiQkvRopeE4m3<BF16>, 256, BF16, FP8>(d->tmaps, a_in, D, M, D, w, 3 * D, {ep, o8}, st,
+                                                                      1, sc)));
+      else
+        SATB_PROPAGATE((linear<E, 256, BF16, FP8>(d->tmaps, a_in, D, M, D, w, 3 * D, ep, st, 1, sc)));
     }
+    return 0;
+  }
+
+  // ---- self-attention, second half: attention core -> out-proj (+residual).  kv null: the keys and values are the
+  // k / v columns of this handle's own qkv (the single-device forward).  Else kv [R, Nk, 2D] holds every token's k | v
+  // (the group forward's gathered buffer) and the local queries attend to all of them.
+  int self_attn(int i, const uint16_t* kv, int Nk) {
+    const LayerW& W = d->layers[i];
+    const float* ssg_l = ssg(i);
     {
       ProfScope ps(d, PROF_ATTN_SELF, st);
-      const int64_t qs = static_cast<int64_t>(N_seq) * 3 * D;
+      const int64_t qs = static_cast<int64_t>(s.n) * 3 * D;
       if (d->attn_fp8) {   // e4m3 operands in the workspace carved for res_R rows; the maps were made for them
-        const AttnFp8Bufs b8 = attn_fp8_bufs(d->ws_attn8.p, d->res_R, H, N_seq, N_seq);
-        SATB_PROPAGATE(launch_attention_fp8_vt(qkv + 2 * D, 3 * D, qs, b8, R, H, N_seq, BF16, st));
-        SATB_PROPAGATE(launch_attention_fp8(d->attn8_maps, b8, att, D, static_cast<int64_t>(N_seq) * D, R, H, N_seq,
-                                            N_seq, BF16, st));
-      } else {
+        const AttnFp8Bufs b8 = attn_fp8_bufs(d->ws_attn8.p, d->res_R, H, s.n, s.n);
+        SATB_PROPAGATE(launch_attention_fp8_vt(qkv + 2 * D, 3 * D, qs, b8, s.R, H, s.n, BF16, st));
+        SATB_PROPAGATE(launch_attention_fp8(d->attn8_maps, b8, att, D, static_cast<int64_t>(s.n) * D, s.R, H, s.n,
+                                            s.n, BF16, st));
+      } else if (!kv) {
         const CUtensorMap* tm = nullptr;   // q, k and v are column ranges of one buffer: one map
-        if (d->dh == 64) SATB_PROPAGATE(d->tmaps.get_a(qkv, 3 * D, N_seq, R, 3 * D, qs, &tm));
+        if (d->dh == 64) SATB_PROPAGATE(d->tmaps.get_a(qkv, 3 * D, s.n, s.R, 3 * D, qs, &tm));
         SATB_PROPAGATE(launch_attention_tc(qkv, qkv, qkv, att, 3 * D, 3 * D, 3 * D, D, qs, qs, qs,
-                                           static_cast<int64_t>(N_seq) * D, 3 * D, 3 * D, 3 * D, 0, D, 2 * D, R, H, H,
-                                           N_seq, N_seq, d->dh, BF16, st, tm, tm, tm));
+                                           static_cast<int64_t>(s.n) * D, 3 * D, 3 * D, 3 * D, 0, D, 2 * D, s.R, H, H,
+                                           s.n, s.n, d->dh, BF16, st, tm, tm, tm));
+      } else {
+        const int64_t kvs = static_cast<int64_t>(Nk) * 2 * D;
+        const CUtensorMap *tq = nullptr, *tkv = nullptr;   // k and v are column ranges of one buffer: one map
+        if (d->dh == 64) {
+          SATB_PROPAGATE(d->tmaps.get_a(qkv, 3 * D, s.n, s.R, 3 * D, qs, &tq));
+          SATB_PROPAGATE(d->tmaps.get_a(kv, 2 * D, Nk, s.R, 2 * D, kvs, &tkv));
+        }
+        SATB_PROPAGATE(launch_attention_tc(qkv, kv, kv, att, 3 * D, 2 * D, 2 * D, D, qs, kvs, kvs,
+                                           static_cast<int64_t>(s.n) * D, 3 * D, 2 * D, 2 * D, 0, 0, D, s.R, H, H,
+                                           s.n, Nk, d->dh, BF16, st, tq, tkv, tkv));
       }
     }
-    {
-      ProfScope ps(d, PROF_ATTN_OUT, st);
-      EpiResidual::Params ep{h, D, nullptr, ssg_l ? ssg_l + 2 * D : nullptr, N_seq, static_cast<int>(ssg_ld), B};
-      SATB_PROPAGATE((linear_auto<EpiResidual, BF16>(d->tmaps, att, D, M, D, W.w_o, D, ep, st)));
-    }
+    ProfScope ps(d, PROF_ATTN_OUT, st);
+    EpiResidual::Params ep{h, D, nullptr, ssg_l ? ssg_l + 2 * D : nullptr, s.n, static_cast<int>(ssg_ld), s.B};
+    SATB_PROPAGATE((linear_auto<EpiResidual, BF16>(d->tmaps, att, D, M, D, W.w_o, D, ep, st)));
+    return 0;
+  }
+
+  // ---- the rest of a block: cross-attention, conformer branch, feed-forward
+  int block_rest(int i) {
+    const LayerW& W = d->layers[i];
+    const float* ssg_l = ssg(i);
+    const int n = s.n;
     // ---- cross-attention on the rows that have a non-null context
     if (Mc > 0) {
       ProfScope ps(d, PROF_CROSS, st);
@@ -1003,7 +1069,7 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
       const Fp8Scales sc{a_scale, W.s_q};
       if (d->qk_norm) {
         typedef EpiHeadNorm16<BF16> E;
-        typename E::Params ep{q16, D, D, 0, N_seq, nullptr, nullptr};
+        typename E::Params ep{q16, D, D, 0, n, nullptr, nullptr};
         if (FP8)   // BN 128 only, as for the QKV GEMM above
           SATB_PROPAGATE((linear<E, 128, BF16, FP8>(d->tmaps, a_in, D, Mc, D, wq, D, ep, st, 1, sc)));
         else
@@ -1017,13 +1083,13 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
       const int64_t kvs = static_cast<int64_t>(d->Mctx) * 2 * d->ce;
       const CUtensorMap *tq = nullptr, *tkv = nullptr;   // k and v are column ranges of one buffer: one map
       if (d->dh == 64) {
-        SATB_PROPAGATE(d->tmaps.get_a(q16, D, N_seq, d->Rc, D, static_cast<int64_t>(N_seq) * D, &tq));
+        SATB_PROPAGATE(d->tmaps.get_a(q16, D, n, d->Rc, D, static_cast<int64_t>(n) * D, &tq));
         SATB_PROPAGATE(d->tmaps.get_a(kv, 2 * d->ce, d->Mctx, d->Rc, 2 * d->ce, kvs, &tkv));
       }
-      SATB_PROPAGATE(launch_attention_tc(q16, kv, kv, att, D, 2 * d->ce, 2 * d->ce, D, static_cast<int64_t>(N_seq) * D,
-                                         kvs, kvs, static_cast<int64_t>(N_seq) * D, D, 2 * d->ce, 2 * d->ce, 0, 0,
-                                         d->ce, d->Rc, H, Hkv, N_seq, d->Mctx, d->dh, BF16, st, tq, tkv, tkv));
-      EpiResidual::Params ep{h, D, nullptr, nullptr, N_seq, 0, 1};
+      SATB_PROPAGATE(launch_attention_tc(q16, kv, kv, att, D, 2 * d->ce, 2 * d->ce, D, static_cast<int64_t>(n) * D,
+                                         kvs, kvs, static_cast<int64_t>(n) * D, D, 2 * d->ce, 2 * d->ce, 0, 0,
+                                         d->ce, d->Rc, H, Hkv, n, d->Mctx, d->dh, BF16, st, tq, tkv, tkv));
+      EpiResidual::Params ep{h, D, nullptr, nullptr, n, 0, 1};
       SATB_PROPAGATE((linear_auto<EpiResidual, BF16>(d->tmaps, att, D, Mc, D, W.w_co, D, ep, st)));
     }
     // ---- conformer branch (transformer.py:576-591, added at :680-681 / :697-698 with no modulation or gate):
@@ -1034,11 +1100,11 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
       ProfScope ps(d, PROF_CONFORMER, st);
       uint16_t* glu = ff;
       uint16_t* cv = ff + static_cast<size_t>(M) * D;
-      SATB_PROPAGATE(launch_layernorm(h, W.cf_in_g, W.cf_in_b, a16, M, D, nullptr, nullptr, 0, N_seq, 1, BF16, st));
+      SATB_PROPAGATE(launch_layernorm(h, W.cf_in_g, W.cf_in_b, a16, M, D, nullptr, nullptr, 0, n, 1, BF16, st));
       typedef EpiSwiglu<BF16> E;
       SATB_PROPAGATE((linear<E, 256, BF16>(d->tmaps, a16, D, M, D, W.cf_w1, 2 * D, typename E::Params{glu, D, W.cf_b1}, st)));
-      SATB_PROPAGATE(launch_conformer_dwconv(glu, W.cf_dw, W.cf_mid_g, W.cf_mid_b, cv, R, N_seq, D, BF16, st));
-      EpiResidual::Params ep{h, D, nullptr, nullptr, N_seq, 0, 1};
+      SATB_PROPAGATE(launch_conformer_dwconv(glu, W.cf_dw, W.cf_mid_g, W.cf_mid_b, cv, s.R, n, D, BF16, st));
+      EpiResidual::Params ep{h, D, nullptr, nullptr, n, 0, 1};
       SATB_PROPAGATE((linear_auto<EpiResidual, BF16>(d->tmaps, cv, D, M, D, W.cf_w2, D, ep, st)));
     }
     // ---- feed-forward: LN -> GEMM (+bias, SwiGLU) -> GEMM (+bias, +residual).  satb_dit_set_feedforward variants: a
@@ -1048,9 +1114,9 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
       const float* mod_scale = ssg_l ? ssg_l + 3 * D : nullptr;
       const float* mod_shift = ssg_l ? ssg_l + 4 * D : nullptr;
       if (FP8 && d->ff_conv_in())   // the token convolution takes 16-bit (fp16) operands in every mode
-        SATB_PROPAGATE(launch_layernorm(h, W.ff_g, W.ff_b, a16, M, D, mod_scale, mod_shift, ssg_ld, N_seq, B, false, st));
+        SATB_PROPAGATE(launch_layernorm(h, W.ff_g, W.ff_b, a16, M, D, mod_scale, mod_shift, ssg_ld, n, s.B, false, st));
       else
-        SATB_PROPAGATE(layernorm_in(W.ff_g, W.ff_b, M, mod_scale, mod_shift, ssg_ld, B));
+        SATB_PROPAGATE(layernorm_in(W.ff_g, W.ff_b, M, mod_scale, mod_shift, ssg_ld, s.B));
     }
     {
       ProfScope ps(d, PROF_FF_IN, st);
@@ -1067,27 +1133,43 @@ static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* o
       } else {
         typedef EpiStore16<BF16> E;
         typename E::Params ep{ff, d->ffi, W.b_ff1, 1};
-        SATB_PROPAGATE((token_conv<E, BF16>(d->tmaps, a16, N_seq, R, N_seq, D, W.w_ff1, d->ffi, d->ff_k, ep, st)));
+        SATB_PROPAGATE((token_conv<E, BF16>(d->tmaps, a16, n, s.R, n, D, W.w_ff1, d->ffi, d->ff_k, ep, st)));
       }
     }
-    {
-      ProfScope ps(d, PROF_FF_OUT, st);
-      EpiResidual::Params ep{h, D, W.b_ff2, ssg_l ? ssg_l + 5 * D : nullptr, N_seq, static_cast<int>(ssg_ld), B};
-      if (d->ff_k == 0)
-        SATB_PROPAGATE((linear_auto<EpiResidual, BF16>(d->tmaps, ff, d->ffi, M, d->ffi, W.w_ff2, D, ep, st)));
-      else
-        SATB_PROPAGATE((token_conv<EpiResidual, BF16>(d->tmaps, ff, N_seq, R, N_seq, d->ffi, W.w_ff2, D, d->ff_k, ep, st)));
-    }
+    ProfScope ps(d, PROF_FF_OUT, st);
+    EpiResidual::Params ep{h, D, W.b_ff2, ssg_l ? ssg_l + 5 * D : nullptr, n, static_cast<int>(ssg_ld), s.B};
+    if (d->ff_k == 0)
+      SATB_PROPAGATE((linear_auto<EpiResidual, BF16>(d->tmaps, ff, d->ffi, M, d->ffi, W.w_ff2, D, ep, st)));
+    else
+      SATB_PROPAGATE((token_conv<EpiResidual, BF16>(d->tmaps, ff, n, s.R, n, d->ffi, W.w_ff2, D, d->ff_k, ep, st)));
+    return 0;
   }
-  if (hidden_out)
-    SATB_CHECK_CUDA(cudaMemcpyAsync(hidden_out, h, static_cast<size_t>(M) * D * 4, cudaMemcpyDeviceToDevice, st));
-  // project_out (with the 1x1 post-conv folded) reads a 16-bit copy of h; its N is C_p (zero weight rows past C), and
-  // dit_post reads the C real channels of each y row
-  const int Cp = d->C_p;
-  SATB_PROPAGATE(launch_cast_rows(h, a16, nullptr, M, D, D, D, BF16, st));
-  SATB_PROPAGATE((linear<EpiStore32, 64, BF16>(d->tmaps, a16, D, M, D, d->w_out16, Cp, EpiStore32::Params{y, Cp, nullptr}, st)));
-  SATB_PROPAGATE(launch_dit_post(y, Cp, out, B, C, L, N_seq, P, d->cfg_on ? 1 : 0, cfg_scale, scale_phi, st));
-  return 0;
+
+  int output(float* out, float cfg_scale, float scale_phi, float* hidden_out) {
+    if (hidden_out)
+      SATB_CHECK_CUDA(cudaMemcpyAsync(hidden_out, h, static_cast<size_t>(M) * D * 4, cudaMemcpyDeviceToDevice, st));
+    // project_out (with the 1x1 post-conv folded) reads a 16-bit copy of h; its N is C_p (zero weight rows past C), and
+    // dit_post reads the C real channels of each y row
+    const int Cp = d->C_p;
+    SATB_PROPAGATE(launch_cast_rows(h, a16, nullptr, M, D, D, D, BF16, st));
+    SATB_PROPAGATE((linear<EpiStore32, 64, BF16>(d->tmaps, a16, D, M, D, d->w_out16, Cp, EpiStore32::Params{y, Cp, nullptr}, st)));
+    SATB_PROPAGATE(launch_dit_post(y, Cp, out, s.B, C, s.L, s.n, s.P, d->cfg_on ? 1 : 0, cfg_scale, scale_phi, st));
+    return 0;
+  }
+};
+
+template <bool BF16, bool FP8 = false>
+static int dit_forward_impl(SatbDit* d, const float* x, const float* t, float* out, int B, int L, float cfg_scale,
+                            float scale_phi, cudaStream_t st, float* hidden_out) {
+  const int N_seq = L + d->P;
+  DitFwd<BF16, FP8> f(d, FwdShape{B, d->cfg_on ? 2 * B : B, L, d->P, N_seq, 0, N_seq}, st);
+  SATB_PROPAGATE(f.input(x, t));
+  for (int i = 0; i < d->depth; ++i) {
+    SATB_PROPAGATE(f.self_qkv(i));
+    SATB_PROPAGATE(f.self_attn(i, nullptr, N_seq));
+    SATB_PROPAGATE(f.block_rest(i));
+  }
+  return f.output(out, cfg_scale, scale_phi, hidden_out);
 }
 
 static int dit_forward_dispatch(SatbDit* d, const float* x, const float* t, float* out, int B, int L, float cfg_scale,
@@ -1147,6 +1229,255 @@ int satb_dit_forward_debug(SatbDit* d, const float* x, const float* t, float* ou
   if (needs_reserve(d, R, L)) SATB_PROPAGATE(satb_dit_reserve(d, R, L));
   cudaStream_t st = static_cast<cudaStream_t>(stream_v);
   return dit_forward_dispatch(d, x, t, out, B, L, cfg_scale, scale_phi, st, hidden);
+}
+
+// ---- Token-sharded forward: one process drives `world` ranks, each a finalized handle with a full copy of the weights
+// on its device (several ranks may share a device).  Rank r holds tokens token_begin[r] .. token_begin[r + 1] - 1 of
+// every item, the prepended ones on rank 0.  Every stage works per token except self-attention, which needs every
+// token's k and v: once per layer each rank gathers them into its kv buffer [R, N, 2D] and attends its own queries
+// against all N keys.
+int satb_dit_group_plan(int world, int n_prepend, int L, int* token_begin) {
+  SATB_REQUIRE(token_begin, "null argument");
+  SATB_REQUIRE(world >= 1 && world <= kKvGatherMaxRanks, "world must be 1 .. 8");
+  SATB_REQUIRE(n_prepend >= 0 && L >= 1, "need n_prepend >= 0 and L >= 1");
+  const int N = n_prepend + L;
+  if (world > N) {
+    set_last_error("world " + std::to_string(world) + " exceeds the " + std::to_string(N) +
+                   " tokens of an item: every rank needs at least one token");
+    return -1;
+  }
+  // as even as possible in units of `unit` tokens, rank 0 taking at least the prepended tokens
+  auto split = [&](int unit) -> int {
+    const int nu = ceil_div(N, unit);   // units; the last may be partial
+    const int p0 = ceil_div(n_prepend, unit);
+    for (int r = 0; r <= world; ++r) token_begin[r] = static_cast<int>(static_cast<long long>(r) * nu / world) * unit;
+    if (token_begin[1] < n_prepend) {   // rank 0 takes the prepended units, the others share the rest evenly
+      if (nu - p0 < world - 1) return -1;
+      for (int r = 1; r <= world; ++r)
+        token_begin[r] = (p0 + static_cast<int>(static_cast<long long>(r - 1) * (nu - p0) / (world - 1))) * unit;
+    }
+    token_begin[world] = N;
+    return 0;
+  };
+  // GEMM row tiles and attention query tiles are 128 rows (kBlockM): whole tiles per rank when every rank can have one
+  if (N >= kBlockM * world && split(kBlockM) == 0) return 0;
+  if (split(1) == 0) return 0;
+  set_last_error("the " + std::to_string(n_prepend) + " prepended tokens leave fewer than one token for each of the other " +
+                 std::to_string(world - 1) + " ranks");
+  return -1;
+}
+
+}  // extern "C"
+
+struct SatbDitGroup {
+  int world = 0;
+  std::vector<SatbDit*> h;
+  std::vector<int> dev;
+  std::vector<DevBuf> kv;                    // per rank, on its device: [R, N, 2D] 16-bit
+  std::vector<cudaEvent_t> ev_qkv, ev_read;  // per rank: its QKV GEMM done / its gather done (the last enqueued)
+  int res_R = 0, res_L = 0, res_P = -1;
+};
+
+// The option a group forward cannot run on this handle, or null.  Token convolutions (conformer blocks, use_conv
+// feed-forwards) need the neighbouring ranks' tokens (halos); FP8 self-attention's v channel scales span all of an
+// item's tokens.
+static const char* group_refusal(const SatbDit* d) {
+  if (d->conformer) return "conformer blocks are not supported by the token-sharded forward (their depthwise "
+                           "convolution needs the neighbouring ranks' tokens)";
+  if (d->ff_k > 0) return "use_conv feed-forwards are not supported by the token-sharded forward (their token "
+                          "convolution needs the neighbouring ranks' tokens)";
+  if (d->attn_fp8) return "attention_dtype \"fp8\" is not supported by the token-sharded forward (its v channel scales "
+                          "span all of an item's tokens)";
+  return nullptr;
+}
+
+static bool same_model(const SatbDit* a, const SatbDit* b) {
+  return std::memcmp(&a->cfg, &b->cfg, sizeof(SatbDitConfig)) == 0 && a->ff_inner == b->ff_inner &&
+         a->ff_glu == b->ff_glu && a->ff_bias == b->ff_bias && a->ff_k == b->ff_k && a->rotary == b->rotary &&
+         a->pos_type == b->pos_type && a->abs_max_len == b->abs_max_len && a->conformer == b->conformer &&
+         a->attn_fp8 == b->attn_fp8;
+}
+
+static void group_release(SatbDitGroup* g) {
+  int cur = 0;
+  cudaGetDevice(&cur);
+  for (int r = 0; r < g->world; ++r) {
+    cudaSetDevice(g->dev[r]);
+    if (r < static_cast<int>(g->kv.size())) g->kv[r].release();
+    if (r < static_cast<int>(g->ev_qkv.size()) && g->ev_qkv[r]) cudaEventDestroy(g->ev_qkv[r]);
+    if (r < static_cast<int>(g->ev_read.size()) && g->ev_read[r]) cudaEventDestroy(g->ev_read[r]);
+  }
+  cudaSetDevice(cur);
+}
+
+// Sets each rank's device in turn and restores the caller's on scope exit.
+struct DeviceRestore {
+  int cur = 0;
+  DeviceRestore() { cudaGetDevice(&cur); }
+  ~DeviceRestore() { cudaSetDevice(cur); }
+};
+
+// The group forward, layer-major across the ranks.  Hazards between ranks, ordered with events only:
+//   RAW: rank r's gather of layer l reads every rank's qkv, so it waits for every rank's QKV GEMM of layer l (ev_qkv).
+//   WAR: rank s's QKV GEMM of layer l + 1 overwrites its qkv, so it waits until every rank has finished gathering
+//        layer l (ev_read).  The first layer of a call waits likewise for the last gathers of the previous call.
+// Within a rank, its own stream orders everything else (its kv buffer is rewritten only after its own attention of the
+// previous layer, on the same stream).
+template <bool BF16, bool FP8>
+static int group_forward_impl(SatbDitGroup* g, const float* const* x, const float* const* t, float* const* out, int B,
+                              int L, float cfg_scale, float scale_phi, cudaStream_t const* st, const int* tb) {
+  const int W = g->world, P = g->h[0]->P, N = L + P;
+  const int R = g->h[0]->cfg_on ? 2 * B : B;
+  std::vector<DitFwd<BF16, FP8>> f;
+  f.reserve(W);
+  std::vector<const void*> qkv(W);
+  for (int r = 0; r < W; ++r) {
+    const int p = r == 0 ? P : 0, n = tb[r + 1] - tb[r];
+    f.emplace_back(g->h[r], FwdShape{B, R, n - p, p, n, tb[r], N}, st[r]);
+    qkv[r] = g->h[r]->ws_qkv.p;
+  }
+  for (int r = 0; r < W; ++r) {
+    SATB_CHECK_CUDA(cudaSetDevice(g->dev[r]));
+    SATB_PROPAGATE(f[r].input(x[r], t[r]));
+  }
+  const int D = g->h[0]->D;
+  for (int i = 0; i < g->h[0]->depth; ++i) {
+    for (int r = 0; r < W; ++r) {
+      SATB_CHECK_CUDA(cudaSetDevice(g->dev[r]));
+      for (int s = 0; s < W; ++s) SATB_CHECK_CUDA(cudaStreamWaitEvent(st[r], g->ev_read[s], 0));   // WAR
+      SATB_PROPAGATE(f[r].self_qkv(i));
+      SATB_CHECK_CUDA(cudaEventRecord(g->ev_qkv[r], st[r]));
+    }
+    for (int r = 0; r < W; ++r) {
+      SATB_CHECK_CUDA(cudaSetDevice(g->dev[r]));
+      for (int s = 0; s < W; ++s) SATB_CHECK_CUDA(cudaStreamWaitEvent(st[r], g->ev_qkv[s], 0));    // RAW
+      SATB_PROPAGATE(launch_kv_gather(qkv.data(), tb, W, g->kv[r].p, R, D, st[r]));
+      SATB_CHECK_CUDA(cudaEventRecord(g->ev_read[r], st[r]));
+      SATB_PROPAGATE(f[r].self_attn(i, g->kv[r].as<uint16_t>(), N));
+      SATB_PROPAGATE(f[r].block_rest(i));
+    }
+  }
+  for (int r = 0; r < W; ++r) {
+    SATB_CHECK_CUDA(cudaSetDevice(g->dev[r]));
+    SATB_PROPAGATE(f[r].output(out[r], cfg_scale, scale_phi, nullptr));
+  }
+  return 0;
+}
+
+extern "C" {
+
+int satb_dit_group_create(SatbDit* const* handles, const int* devices, int world, SatbDitGroup** out) {
+  SATB_REQUIRE(handles && devices && out, "null argument");
+  SATB_REQUIRE(world >= 1 && world <= kKvGatherMaxRanks, "world must be 1 .. 8");
+  for (int r = 0; r < world; ++r) {
+    SATB_REQUIRE(handles[r], "null handle");
+    const char* why = group_refusal(handles[r]);
+    if (why) {
+      set_last_error(why);
+      return -5;
+    }
+    if (!same_model(handles[0], handles[r])) {
+      set_last_error("rank " + std::to_string(r) + "'s handle has another config or model option than rank 0's");
+      return -1;
+    }
+    for (int s = 0; s < r; ++s)
+      SATB_REQUIRE(handles[s] != handles[r], "every rank needs its own handle (its own workspace)");
+  }
+  for (int r = 0; r < world; ++r) SATB_REQUIRE(handles[r]->finalized, "weights not finalized");
+  DeviceRestore restore;
+  int n_dev = 0;
+  SATB_CHECK_CUDA(cudaGetDeviceCount(&n_dev));
+  for (int r = 0; r < world; ++r) SATB_REQUIRE(devices[r] >= 0 && devices[r] < n_dev, "no such device");
+  // every rank reads every other rank's qkv: peer access between each pair of distinct devices
+  for (int r = 0; r < world; ++r)
+    for (int s = 0; s < world; ++s) {
+      if (devices[r] == devices[s]) continue;
+      int ok = 0;
+      SATB_CHECK_CUDA(cudaDeviceCanAccessPeer(&ok, devices[r], devices[s]));
+      if (!ok) {
+        set_last_error("device " + std::to_string(devices[r]) + " cannot access device " + std::to_string(devices[s]) +
+                       " peer to peer: the token-sharded forward reads every rank's K/V over peer links");
+        return -1;
+      }
+    }
+  for (int r = 0; r < world; ++r) {
+    SATB_CHECK_CUDA(cudaSetDevice(devices[r]));
+    for (int s = 0; s < world; ++s) {
+      if (devices[r] == devices[s]) continue;
+      const cudaError_t e = cudaDeviceEnablePeerAccess(devices[s], 0);   // this process's context only
+      if (e == cudaErrorPeerAccessAlreadyEnabled) {
+        cudaGetLastError();
+      } else {
+        SATB_CHECK_CUDA(e);
+      }
+    }
+  }
+  SatbDitGroup* g = new SatbDitGroup();
+  g->world = world;
+  g->h.assign(handles, handles + world);
+  g->dev.assign(devices, devices + world);
+  g->kv.resize(world);
+  g->ev_qkv.assign(world, nullptr);
+  g->ev_read.assign(world, nullptr);
+  for (int r = 0; r < world; ++r) {
+    cudaError_t e = cudaSetDevice(devices[r]);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&g->ev_qkv[r], cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&g->ev_read[r], cudaEventDisableTiming);
+    if (e != cudaSuccess) {
+      group_release(g);
+      delete g;
+      set_last_error(std::string("cudaEventCreate failed: ") + cudaGetErrorString(e));
+      return -2;
+    }
+  }
+  *out = g;
+  return 0;
+}
+
+void satb_dit_group_destroy(SatbDitGroup* g) {
+  if (!g) return;
+  group_release(g);
+  delete g;
+}
+
+int satb_dit_group_forward(SatbDitGroup* g, const float* const* x, const float* const* t, float* const* out, int B,
+                           int L, float cfg_scale, float scale_phi, void* const* streams) {
+  SATB_REQUIRE(g && x && t && out && streams, "null argument");
+  const int W = g->world;
+  SatbDit* d0 = g->h[0];
+  for (int r = 0; r < W; ++r) {
+    const SatbDit* d = g->h[r];
+    SATB_REQUIRE(d->finalized, "weights not finalized");
+    SATB_REQUIRE(x[r] && t[r] && out[r], "null argument");
+    SATB_REQUIRE(B == d->B, "batch size differs from satb_dit_prepare_cond");
+    SATB_REQUIRE(d->cfg_on == d0->cfg_on && d->P == d0->P && d->Rc == d0->Rc && d->Mctx == d0->Mctx &&
+                     d->has_global == d0->has_global,
+                 "every rank needs the same conditioning (satb_dit_set_prepend_cond / satb_dit_prepare_cond)");
+  }
+  SATB_REQUIRE(L >= 1, "bad shape");
+  int tb[kKvGatherMaxRanks + 1];
+  SATB_PROPAGATE(satb_dit_group_plan(W, d0->P, L, tb));
+  const int N = L + d0->P, R = d0->cfg_on ? 2 * B : B;
+  DeviceRestore restore;
+  const bool fresh = R <= g->res_R && L == g->res_L && d0->P == g->res_P;
+  for (int r = 0; r < W; ++r) {
+    SatbDit* d = g->h[r];
+    // res_R 0: no single-device forward has reserved since; and the table check of needs_reserve (a reload of the
+    // weights marks the position table stale)
+    if (fresh && d->res_R == 0 && !(d->pos_type != 0 && d->pos_len != N)) continue;
+    SATB_CHECK_CUDA(cudaSetDevice(g->dev[r]));
+    SATB_PROPAGATE(reserve_rows(d, R, tb[r + 1] - tb[r], N));
+    SATB_PROPAGATE(g->kv[r].ensure(static_cast<size_t>(R) * N * 2 * d->D * 2));
+    d->res_R = 0;   // the workspace no longer has the single-device forward's shape: its next call reserves again
+  }
+  g->res_R = std::max(g->res_R, R);
+  g->res_L = L;
+  g->res_P = d0->P;
+  cudaStream_t st[kKvGatherMaxRanks];
+  for (int r = 0; r < W; ++r) st[r] = static_cast<cudaStream_t>(streams[r]);
+  if (d0->fp8) return group_forward_impl<false, true>(g, x, t, out, B, L, cfg_scale, scale_phi, st, tb);
+  return d0->bf16 ? group_forward_impl<true, false>(g, x, t, out, B, L, cfg_scale, scale_phi, st, tb)
+                  : group_forward_impl<false, false>(g, x, t, out, B, L, cfg_scale, scale_phi, st, tb);
 }
 
 }  // extern "C"

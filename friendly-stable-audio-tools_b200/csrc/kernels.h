@@ -93,6 +93,14 @@ int launch_cast_rows(const float* src, void* dst, const int* perm, int rows, int
 int launch_gather_f32(const float* src, float* dst, const int* perm, int n, cudaStream_t stream);
 int launch_zero(void* p, size_t bytes, cudaStream_t stream);
 
+// ---- kv_gather.cu (token-sharded DiT forward)
+// kv [R, N, 2D] 16-bit = the k | v columns (D .. 3D - 1) of every rank's qkv [R, n_s, 3D], rank s's rows at tokens
+// token_begin[s] .. token_begin[s + 1] - 1 of each item (N = token_begin[world]).  qkv[s] may live on another device
+// (a peer pointer).
+constexpr int kKvGatherMaxRanks = 8;
+int launch_kv_gather(const void* const* qkv, const int* token_begin, int world, void* kv, int R, int D,
+                     cudaStream_t stream);
+
 // ---- conformer.cu
 // out16 = silu(LayerNorm(depthwise_conv17(g16))) per item of n_seq rows (zero padding at each item's ends, eps 1e-5):
 // g16, out16 [items * n_seq, D] 16-bit; w fp32 [D][17]; gamma, beta [D] (beta may be null).  D <= kConformerMaxDim.

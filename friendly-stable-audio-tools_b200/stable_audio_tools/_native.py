@@ -121,6 +121,11 @@ SIGNATURES = {
     "satb_dit_prepare_cond": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _VP]),
     "satb_dit_forward": (_I, [_VP, _VP, _VP, _VP, _I, _I, _F, _F, _VP]),
     "satb_dit_forward_debug": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _F, _F, _VP]),
+    "satb_dit_group_plan": (_I, [_I, _I, _I, _VP]),
+    "satb_dit_group_create": (_I, [_VP, _VP, _I, ctypes.POINTER(_VP)]),
+    "satb_dit_group_destroy": (None, [_VP]),
+    "satb_dit_group_forward": (_I, [_VP, _VP, _VP, _VP, _I, _I, _F, _F, _VP]),
+    "satb_kv_gather": (_I, [_VP, _VP, _I, _VP, _I, _I, _VP]),
     "satb_dit_profile": (_I, [_VP, _I]),
     "satb_dit_profile_read": (_I, [_VP, _VP, _VP]),
     "satb_snake_beta": (_I, [_VP, _VP, _VP, _VP, _I, _I, _LL, _I, _VP]),
@@ -227,6 +232,14 @@ def dev_f32(t, name="tensor"):
 
 def ptr(t):
     return ctypes.c_void_p(t.data_ptr()) if t is not None else None
+
+
+def group_plan(world, n_prepend, L):
+    """The token split of a sharded DiT forward (satb_dit_group_plan): token_begin[world + 1] over the n_prepend + L
+    tokens of an item; rank r holds tokens token_begin[r] .. token_begin[r + 1] - 1.  Host only."""
+    tb = (ctypes.c_int * (world + 1))()
+    check(lib().satb_dit_group_plan(int(world), int(n_prepend), int(L), tb))
+    return list(tb)
 
 
 def launch_count():

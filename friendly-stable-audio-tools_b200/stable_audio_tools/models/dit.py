@@ -19,7 +19,10 @@ and parameter names, ``forward`` signature and CFG semantics); the arithmetic ru
 * ``rotary_pos_emb=False``, ``use_sinusoidal_emb`` and ``use_abs_pos_emb`` select the native positional options
   (``satb_dit_set_positions``); the embedding is added to every row, prepended ones included, in project_in's epilogue;
 * any ``io_channels`` and ``input_concat_dim`` (an inpainting DiT's latent + 1 mask channel, PQMF sub-bands, raw audio):
-  the library pads project_in's K to a multiple of 8 and project_out's N to a multiple of 32 with zero weights.
+  the library pads project_in's K to a multiple of 8 and project_out's N to a multiple of 32 with zero weights;
+* ``shard_tokens(devices)`` splits every call's tokens over several ranks (``satb_dit_group_*``): each rank holds a full
+  copy of the weights and a contiguous range of every item's tokens, and gathers every rank's self-attention K / V once
+  per layer, so one prompt can use several GPUs.
 
 There is no eager / CPU fallback: tensors must live on a CUDA device.
 """
@@ -159,6 +162,8 @@ class DiffusionTransformer(nn.Module):
         self.__dict__["_keepalive"] = None
         self.__dict__["_neg_masked"] = None
         self.__dict__["_graph"] = None
+        self.__dict__["_shard"] = None           # shard_tokens state: devices, rank handles, group, streams
+        self.__dict__["_shard_dirty"] = True
         # cuda_graph = True: one denoiser call = ONE CUDA-graph launch (the ~280 kernel launches of a forward are
         # captured once per (shape, guidance, conditioning) and replayed).  The returned tensor is then a static
         # buffer that the NEXT call overwrites - fine for the samplers, which consume it at once; off by default.
@@ -172,13 +177,19 @@ class DiffusionTransformer(nn.Module):
     # ------------------------------------------------------------------ native plumbing
     def _apply(self, fn, *a, **k):
         self.__dict__["_weights_dirty"] = True
+        self.__dict__["_shard_dirty"] = True
         return super()._apply(fn, *a, **k)
 
     def refresh_native_weights(self):
         """Call after mutating parameters in place (``load_state_dict`` / ``.to()`` do it for you)."""
         self.__dict__["_weights_dirty"] = True
+        self.__dict__["_shard_dirty"] = True
 
     def __del__(self):
+        try:
+            self._drop_shards()
+        except Exception:
+            pass
         h = self.__dict__.get("_h")
         if h is not None:
             try:
@@ -201,50 +212,61 @@ class DiffusionTransformer(nn.Module):
             operand_dtype=OPERAND_DTYPES[self.operand_dtype], qk_norm=int(self.qk_norm),
             input_concat_dim=self.input_concat_dim * self.patch_size, prepend_cond_dim=self.prepend_cond_dim)
 
-    def _handle(self, device):
+    def _new_handle(self):
+        """A native handle of this model's config and options, with no weights yet."""
         lib = _native.lib()
+        cfg = self.native_config()
+        h = ctypes.c_void_p()
+        _native.check(lib.satb_dit_create(ctypes.byref(cfg), ctypes.byref(h)))
+        options = []
+        if self.conformer:
+            options.append(lambda: lib.satb_dit_set_conformer(h, 1))
+        if self.attention_dtype == "fp8":
+            options.append(lambda: lib.satb_dit_set_attention_fp8(h, 1))
+        if self.ff_spec != (4 * self.embed_dim, 1, 0, 1):
+            options.append(lambda: lib.satb_dit_set_feedforward(h, *self.ff_spec))
+        if self.pos_spec != (1, 0, 0):
+            options.append(lambda: lib.satb_dit_set_positions(h, *self.pos_spec))
+        for set_option in options:
+            rc = set_option()
+            if rc != 0:
+                msg = lib.satb_last_error()
+                lib.satb_dit_destroy(h)
+                raise _native.NativeError(f"satb200 error {rc}: {msg.decode() if msg else '?'}")
+        return h
+
+    def _upload_weights(self, h, device, copy_to=None):
+        """Loads every parameter into handle h and finalizes it, on device's current stream.  copy_to: the device the
+        handle lives on, when it is not the parameters' own (a rank of shard_tokens)."""
+        lib = _native.lib()
+        st = _native.stream_ptr(device)
+        with torch.no_grad():
+            weights = list(self.state_dict().items())
+            if self.transformer.pos_type == "sinusoidal":
+                # a non-persistent buffer, so not in the state dict: handed over as the module holds it (the native
+                # table uses these very values rather than recomputing the powers)
+                weights.append(("transformer.pos_emb.inv_freq", self.transformer.pos_emb.inv_freq))
+            for name, t in weights:
+                if name.endswith("rotary_pos_emb.scale") or t is None:
+                    continue
+                if not t.is_cuda:
+                    raise _native.NativeError(
+                        f"parameter {name} is on {t.device}: move the model to a CUDA device "
+                        "(this package has no CPU path)")
+                src = t.detach().to(torch.float32).contiguous()
+                if copy_to is not None:
+                    src = src.to(copy_to)
+                if self.patch_size > 1 and name in ("preprocess_conv.weight", "postprocess_conv.weight"):
+                    eye = torch.eye(self.patch_size, device=src.device, dtype=src.dtype)
+                    src = torch.kron(src[:, :, 0], eye).unsqueeze(-1).contiguous()
+                _native.check(lib.satb_dit_load_weight(h, name.encode(), _native.ptr(src), src.numel(), st))
+            _native.check(lib.satb_dit_finalize(h, st))
+
+    def _handle(self, device):
         if self.__dict__["_h"] is None:
-            cfg = self.native_config()
-            h = ctypes.c_void_p()
-            _native.check(lib.satb_dit_create(ctypes.byref(cfg), ctypes.byref(h)))
-            options = []
-            if self.conformer:
-                options.append(lambda: lib.satb_dit_set_conformer(h, 1))
-            if self.attention_dtype == "fp8":
-                options.append(lambda: lib.satb_dit_set_attention_fp8(h, 1))
-            if self.ff_spec != (4 * self.embed_dim, 1, 0, 1):
-                options.append(lambda: lib.satb_dit_set_feedforward(h, *self.ff_spec))
-            if self.pos_spec != (1, 0, 0):
-                options.append(lambda: lib.satb_dit_set_positions(h, *self.pos_spec))
-            for set_option in options:
-                rc = set_option()
-                if rc != 0:
-                    msg = lib.satb_last_error()
-                    lib.satb_dit_destroy(h)
-                    raise _native.NativeError(f"satb200 error {rc}: {msg.decode() if msg else '?'}")
-            self.__dict__["_h"] = h
+            self.__dict__["_h"] = self._new_handle()
         if self.__dict__["_weights_dirty"]:
-            st = _native.stream_ptr(device)
-            with torch.no_grad():
-                weights = list(self.state_dict().items())
-                if self.transformer.pos_type == "sinusoidal":
-                    # a non-persistent buffer, so not in the state dict: handed over as the module holds it (the native
-                    # table uses these very values rather than recomputing the powers)
-                    weights.append(("transformer.pos_emb.inv_freq", self.transformer.pos_emb.inv_freq))
-                for name, t in weights:
-                    if name.endswith("rotary_pos_emb.scale") or t is None:
-                        continue
-                    if not t.is_cuda:
-                        raise _native.NativeError(
-                            f"parameter {name} is on {t.device}: move the model to a CUDA device "
-                            "(this package has no CPU path)")
-                    src = t.detach().to(torch.float32).contiguous()
-                    if self.patch_size > 1 and name in ("preprocess_conv.weight", "postprocess_conv.weight"):
-                        eye = torch.eye(self.patch_size, device=src.device, dtype=src.dtype)
-                        src = torch.kron(src[:, :, 0], eye).unsqueeze(-1).contiguous()
-                    _native.check(lib.satb_dit_load_weight(self.__dict__["_h"], name.encode(), _native.ptr(src),
-                                                           src.numel(), st))
-                _native.check(lib.satb_dit_finalize(self.__dict__["_h"], st))
+            self._upload_weights(self.__dict__["_h"], device)
             self.__dict__["_weights_dirty"] = False
             self.__dict__["_cond_key"] = None
             self.__dict__["_graph"] = None
@@ -258,7 +280,14 @@ class DiffusionTransformer(nn.Module):
         key = (self._tkey(cross), self._tkey(neg), self._tkey(glob), bool(use_cfg), B, self._tkey(prepend))
         if key == self.__dict__["_cond_key"]:
             return
+        self._prepare_native(h, cross, neg, glob, use_cfg, device, B, prepend)
+        self.__dict__["_cond_key"] = key
+        self.__dict__["_keepalive"] = (cross, neg, glob, prepend)   # keep the keyed storage alive
+
+    def _prepare_native(self, h, cross, neg, glob, use_cfg, device, B, prepend, copy_to=None):
         f32 = lambda t: None if t is None else t.detach().to(torch.float32).contiguous()
+        if copy_to is not None:
+            f32 = lambda t: None if t is None else t.detach().to(device=copy_to, dtype=torch.float32).contiguous()
         c, n, g, pc = f32(cross), f32(neg), f32(glob), f32(prepend)
         for name, tt in (("cross_attn_cond", c), ("negative_cross_attn_cond", n), ("global_embed", g),
                          ("prepend_cond", pc)):
@@ -271,8 +300,118 @@ class DiffusionTransformer(nn.Module):
                                                               _native.stream_ptr(device)))
         _native.check(_native.lib().satb_dit_prepare_cond(h, _native.ptr(c), _native.ptr(n), _native.ptr(g), B, Mctx,
                                                           1 if use_cfg else 0, _native.stream_ptr(device)))
-        self.__dict__["_cond_key"] = key
-        self.__dict__["_keepalive"] = (cross, neg, glob, prepend)   # keep the keyed storage alive
+
+    # ------------------------------------------------------------------ token sharding
+    def shard_tokens(self, devices):
+        """Run every later call token-sharded over ``devices`` (context parallel); ``None`` returns to one device.
+
+        Rank r runs on ``devices[r]``; a device may repeat (several ranks on one GPU run the same sharded schedule, which
+        is how it is tested on a single GPU).  The parameters stay on the home device ``devices[0]``, where ``forward``
+        takes its inputs and returns its output; each rank gets its own native handle with a copy of the weights,
+        refreshed whenever the parameters change.  ``forward`` splits each item's tokens by the library's plan
+        (``satb_dit_group_plan``: the prepended tokens on rank 0, boundaries on multiples of 128 tokens), runs all ranks
+        with one K/V gather per layer, and concatenates the ranks' outputs on the home device.  Samplers and the VAE run
+        unchanged on the home device.
+
+        Refused with NotImplementedError: conformer blocks and ``use_conv`` feed-forwards (their token convolutions
+        would need the neighbouring ranks' tokens), ``attention_dtype="fp8"`` (its V channel scales span all of an
+        item's tokens) and, at call time, ``return_info``.  ``cuda_graph=True`` is not captured in this mode: each call
+        enqueues every rank's launches eagerly.  Ranks on distinct GPUs need peer-to-peer access between them."""
+        if devices is not None:
+            if self.conformer:
+                raise NotImplementedError("shard_tokens: conformer blocks are not supported (their depthwise convolution "
+                                          "needs the neighbouring ranks' tokens)")
+            if self.ff_spec[2] > 0:
+                raise NotImplementedError("shard_tokens: use_conv feed-forwards are not supported (their token "
+                                          "convolution needs the neighbouring ranks' tokens)")
+            if self.attention_dtype == "fp8":
+                raise NotImplementedError("shard_tokens: attention_dtype='fp8' is not supported (its V channel scales "
+                                          "span all of an item's tokens)")
+            devices = [torch.device(dv) for dv in devices]
+            if not 1 <= len(devices) <= 8:
+                raise ValueError(f"shard_tokens: 1 to 8 devices, got {len(devices)}")
+            for dv in devices:
+                if dv.type != "cuda":
+                    raise _native.NativeError(f"shard_tokens: {dv} is not a CUDA device (this package has no CPU path)")
+            devices = [dv if dv.index is not None else torch.device("cuda", torch.cuda.current_device()) for dv in devices]
+        self._drop_shards()
+        if devices is not None:
+            self.__dict__["_shard"] = dict(devices=devices, handles=None, group=None, streams=None, cond_key=None,
+                                           keepalive=None)
+            self.__dict__["_shard_dirty"] = True
+        return self
+
+    def _drop_shards(self):
+        sh = self.__dict__.get("_shard")
+        self.__dict__["_shard"] = None
+        if sh is None:
+            return
+        lib = _native.lib()
+        if sh["group"] is not None:
+            lib.satb_dit_group_destroy(sh["group"])
+        for h in sh["handles"] or []:
+            lib.satb_dit_destroy(h)
+
+    def _shard_group(self, sh):
+        lib = _native.lib()
+        devs = sh["devices"]
+        if sh["group"] is not None and not self.__dict__["_shard_dirty"]:
+            return sh["group"]
+        if sh["group"] is not None:
+            lib.satb_dit_group_destroy(sh["group"])
+            sh["group"] = None
+        if sh["handles"] is None:
+            sh["handles"] = []
+            for _ in devs:
+                sh["handles"].append(self._new_handle())
+        for h, dv in zip(sh["handles"], devs):
+            with torch.cuda.device(dv):
+                self._upload_weights(h, dv, copy_to=dv)
+        g = ctypes.c_void_p()
+        handles = (ctypes.c_void_p * len(devs))(*[h.value for h in sh["handles"]])
+        ids = (ctypes.c_int * len(devs))(*[dv.index for dv in devs])
+        _native.check(lib.satb_dit_group_create(handles, ids, len(devs), ctypes.byref(g)))
+        sh["group"] = g
+        if sh["streams"] is None:
+            sh["streams"] = [torch.cuda.Stream(device=dv) for dv in devs]
+        sh["cond_key"] = None
+        self.__dict__["_shard_dirty"] = False
+        return g
+
+    def _sharded_forward(self, sh, x, t, cross, neg, glob, prepend, use_cfg, cfg_scale, scale_phi):
+        lib = _native.lib()
+        devs = sh["devices"]
+        home = devs[0]
+        if x.device != home:
+            raise ValueError(f"the token-sharded model's home device is {home}, but x is on {x.device}")
+        g = self._shard_group(sh)
+        B, _, L = x.shape
+        key = (self._tkey(cross), self._tkey(neg), self._tkey(glob), bool(use_cfg), B, self._tkey(prepend))
+        if key != sh["cond_key"]:
+            for h, dv in zip(sh["handles"], devs):
+                with torch.cuda.device(dv):
+                    self._prepare_native(h, cross, neg, glob, use_cfg, dv, B, prepend, copy_to=dv)
+            sh["cond_key"] = key
+            sh["keepalive"] = (cross, neg, glob, prepend)
+        P = 0 if self.global_cond_type == "adaLN" else 1 + (prepend.shape[1] if prepend is not None else 0)
+        tb = _native.group_plan(len(devs), P, L)
+        xin = x.detach().to(torch.float32)
+        tin = t.detach().to(torch.float32).contiguous()
+        xs, ts, outs = [], [], []
+        for r, dv in enumerate(devs):
+            lo, hi = max(tb[r] - P, 0), tb[r + 1] - P          # this rank's latent tokens
+            with torch.cuda.device(dv):
+                xs.append(xin[:, :, lo:hi].to(dv).contiguous())
+                ts.append(tin.to(dv))
+                outs.append(torch.empty(B, self.io_channels * self.patch_size, hi - lo, device=dv, dtype=torch.float32))
+                sh["streams"][r].wait_stream(torch.cuda.current_stream(dv))
+        ptrs = lambda ts_: (ctypes.c_void_p * len(devs))(*[q.data_ptr() for q in ts_])
+        streams = (ctypes.c_void_p * len(devs))(*[s_.cuda_stream for s_ in sh["streams"]])
+        _native.check(lib.satb_dit_group_forward(g, ptrs(xs), ptrs(ts), ptrs(outs), B, L, float(cfg_scale),
+                                                 float(scale_phi), streams))
+        for r, dv in enumerate(devs):
+            torch.cuda.current_stream(dv).wait_stream(sh["streams"][r])
+        return torch.cat([o.to(home) for o in outs], dim=2)
 
     # ------------------------------------------------------------------ forward
     @torch.no_grad()
@@ -282,6 +421,9 @@ class DiffusionTransformer(nn.Module):
                 return_info=False, **kwargs):
         if causal:
             raise AssertionError("Causal mode is not supported for DiffusionTransformer")
+        if return_info and self.__dict__["_shard"] is not None:
+            raise NotImplementedError("return_info is not supported by the token-sharded forward (shard_tokens): "
+                                      "call shard_tokens(None) first")
         if prepend_cond is not None and self.prepend_cond_dim == 0:
             raise ValueError("prepend_cond given to a model built with prepend_cond_dim=0")
         if (input_concat_cond is None) != (self.input_concat_dim == 0):
@@ -348,6 +490,10 @@ class DiffusionTransformer(nn.Module):
                 return (out, {"hidden_states": []}) if return_info else out
             b_, c_, l_ = x.shape
             x = x.reshape(b_, c_, l_ // p, p).transpose(2, 3).reshape(b_, c_ * p, l_ // p)   # channel = c * p + pi
+        sh = self.__dict__["_shard"]
+        if sh is not None:
+            return self._unpatch(self._sharded_forward(sh, x, t, cross_attn_cond, neg, global_embed, prepend_cond,
+                                                       use_cfg, cfg_scale, scale_phi)).to(x.dtype)
         # handles, workspaces and TMA descriptors live on the model's device: make it current for the native calls
         # (generate_diffusion_cond(device='cuda:1') with current device 0 must work)
         with torch.cuda.device(x.device):

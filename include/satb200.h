@@ -139,6 +139,34 @@ int satb_dit_forward(SatbDit* h, const float* x, const float* t, float* out, int
 int satb_dit_forward_debug(SatbDit* h, const float* x, const float* t, float* out, float* hidden, int B, int L,
                            float cfg_scale, float scale_phi, void* stream);
 
+/* ---- Token-sharded (context-parallel) DiT forward: one process drives `world` ranks (1 .. 8), each a finalized handle
+ * with a full copy of the weights on its device; several ranks may share one device.  Rank r holds tokens
+ * token_begin[r] .. token_begin[r + 1] - 1 of every item (positions after the prepend concat, N = n_prepend + L), the
+ * n_prepend prepended tokens (the global-conditioning token and any prepend-conditioning tokens) on rank 0.  Once per
+ * layer each rank gathers every rank's self-attention k / v into one full-sequence buffer and attends its own queries
+ * against all of them; everything else runs per token on the rank's own rows. */
+typedef struct SatbDitGroup SatbDitGroup;
+/* The split, in token_begin[world + 1]: boundaries on multiples of 128 tokens when N >= 128 * world, as even as possible
+ * otherwise; rank 0 holds at least the prepended tokens; no rank is empty.  world > N is refused.  Host only. */
+int satb_dit_group_plan(int world, int n_prepend, int L, int* token_begin);
+/* handles[world]: finalized handles of one model (identical configs and options, checked), one per rank, each its own;
+ * devices[world]: their device ids.  Conformer blocks, use_conv feed-forwards and FP8 self-attention are refused with
+ * -5.  Ranks on distinct devices need peer access between them (refused with a message when missing); it is enabled
+ * for this process.  Each handle keeps its own conditioning: call satb_dit_set_prepend_cond / satb_dit_prepare_cond on
+ * every handle, with the same conditioning, before satb_dit_group_forward.  The handles outlive the group, which must
+ * be destroyed explicitly. */
+int satb_dit_group_create(SatbDit* const* handles, const int* devices, int world, SatbDitGroup** out);
+void satb_dit_group_destroy(SatbDitGroup* g);
+/* One denoiser call over the ranks: x[r] [B, C, L_r] and out[r] [B, io_channels, L_r], rank r's latent tokens (L_r =
+ * token_begin[r + 1] - token_begin[r], less n_prepend on rank 0), and t[r] [B], all on rank r's device; streams[r] is
+ * rank r's stream.  Enqueues only (ranks are ordered with events); the caller's current device is restored. */
+int satb_dit_group_forward(SatbDitGroup* g, const float* const* x, const float* const* t, float* const* out, int B,
+                           int L, float cfg_scale, float scale_phi, void* const* streams);
+/* The group forward's K/V gather on its own (tests and timing): kv [R, N, 2 D] 16-bit = the columns D .. 3 D - 1 of
+ * every rank's qkv[s] [R, n_s, 3 D], rank s's rows at tokens token_begin[s] .. token_begin[s + 1] - 1 of each item
+ * (N = token_begin[world], token_begin[0] = 0).  qkv[s] may be a peer device's pointer. */
+int satb_kv_gather(const void* const* qkv, const int* token_begin, int world, void* kv, int R, int D, void* stream);
+
 /* Per-kernel-class CUDA-event timing used by bench.py's roofline line: enable, run forwards,
  * then read ms[8]/count[8] (0 ff_in GEMM, 1 ff_out GEMM, 2 qkv GEMM, 3 self-attention core,
  * 4 attention out GEMM, 5 cross-attention, 6 LayerNorm, 7 conformer branch (conformer models only)). */
