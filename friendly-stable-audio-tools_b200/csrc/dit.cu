@@ -113,6 +113,9 @@ struct SatbDit {
   AttnFp8Maps attn8_maps;
   int rope_len = 0;
   int res_R = 0, res_L = 0, res_P = -1;
+  // bumped whenever weights, conditioning or workspaces may have moved or changed (satb_dit_finalize,
+  // satb_dit_set_prepend_cond, satb_dit_prepare_cond, reserve_rows): a group's captured graph compares it at launch
+  unsigned long long gen = 0;
   // optional per-category CUDA-event timing (bench.py roofline)
   bool prof_on = false;
   struct ProfRec { int cat; cudaEvent_t a, b; };
@@ -649,6 +652,7 @@ int satb_dit_finalize(SatbDit* d, void* stream_v) {
   SATB_PROPAGATE(rc);
   d->tmaps.maps.clear();
   d->finalized = true;
+  ++d->gen;
   return 0;
 }
 
@@ -739,6 +743,7 @@ static int reserve_rows(SatbDit* d, int R, int n, int tab_len) {
   if (d->rotary) SATB_PROPAGATE(ensure_rope(d, tab_len));
   if (d->pos_type != 0) SATB_PROPAGATE(ensure_pos(d, tab_len));
   d->tmaps.maps.clear();
+  ++d->gen;
   return 0;
 }
 
@@ -780,6 +785,7 @@ extern "C" {
 int satb_dit_set_prepend_cond(SatbDit* d, const float* prepend, int B, int n_tokens, void* stream_v) {
   SATB_REQUIRE(d && d->finalized, "weights not finalized");
   cudaStream_t st = static_cast<cudaStream_t>(stream_v);
+  ++d->gen;
   if (!prepend || n_tokens <= 0) {
     d->Pp = 0;
     d->P = d->adaln ? 0 : 1;
@@ -809,6 +815,7 @@ int satb_dit_prepare_cond(SatbDit* d, const float* cross, const float* neg_cross
   SATB_REQUIRE(B >= 1, "bad batch");
   cudaStream_t st = static_cast<cudaStream_t>(stream_v);
   const int D = d->D;
+  ++d->gen;
   d->B = B;
   d->cfg_on = use_cfg != 0;
   d->has_cross = cross != nullptr && d->ct > 0;
@@ -1269,13 +1276,40 @@ int satb_dit_group_plan(int world, int n_prepend, int L, int* token_begin) {
 
 }  // extern "C"
 
+// The whole-tensor arguments of satb_dit_group_graph_forward, on the home device (rank 0's)
+struct GraphKey {
+  const float *x = nullptr, *t = nullptr;
+  float* out = nullptr;
+  int B = 0, L = 0;
+  float cfg_scale = 0.f, scale_phi = 0.f;
+  bool operator==(const GraphKey& o) const {
+    return x == o.x && t == o.t && out == o.out && B == o.B && L == o.L && cfg_scale == o.cfg_scale &&
+           scale_phi == o.scale_phi;
+  }
+};
+
 struct SatbDitGroup {
   int world = 0;
   std::vector<SatbDit*> h;
   std::vector<int> dev;
   std::vector<DevBuf> kv;                    // per rank, on its device: [R, N, 2D] 16-bit
-  std::vector<cudaEvent_t> ev_qkv, ev_read;  // per rank: its QKV GEMM done / its gather done (the last enqueued)
+  // Per rank, recorded by eager calls only: its QKV GEMM done / its gather done (the last enqueued) / its last work
+  // of the call done.  A captured graph records its own pair (gev_*): an event last recorded inside a capture cannot
+  // be waited on outside it.
+  std::vector<cudaEvent_t> ev_qkv, ev_read, ev_done;
+  std::vector<cudaEvent_t> gev_qkv, gev_read, gev_join;
   int res_R = 0, res_L = 0, res_P = -1;
+  // satb_dit_group_graph_forward: the instantiated graph, what it was captured for, and the fixed per-rank slices of
+  // x, t and out it reads and writes (on each rank's device)
+  cudaGraphExec_t exec = nullptr;
+  GraphKey key;
+  std::vector<unsigned long long> gens;      // every handle's gen at capture
+  unsigned long long graph_launches = 0;     // kernel launches in the graph
+  long long captures = 0, replays = 0;
+  std::vector<DevBuf> gx, gt, gout;
+  cudaEvent_t ev_fork = nullptr;             // home device: the capture's fork
+  cudaEvent_t ev_graph = nullptr;            // home device: recorded after each graph launch (and before a warm-up)
+  cudaStream_t cap = nullptr;                // home device: the capture stream
 };
 
 // The option a group forward cannot run on this handle, or null.  Token convolutions (conformer blocks, use_conv
@@ -1298,14 +1332,29 @@ static bool same_model(const SatbDit* a, const SatbDit* b) {
          a->attn_fp8 == b->attn_fp8;
 }
 
+static void group_drop_graph(SatbDitGroup* g) {
+  if (g->exec) cudaGraphExecDestroy(g->exec);   // a launch still in flight completes; the memory is freed after it
+  g->exec = nullptr;
+  g->key = GraphKey();
+  g->gens.clear();
+}
+
 static void group_release(SatbDitGroup* g) {
   int cur = 0;
   cudaGetDevice(&cur);
+  group_drop_graph(g);
   for (int r = 0; r < g->world; ++r) {
     cudaSetDevice(g->dev[r]);
-    if (r < static_cast<int>(g->kv.size())) g->kv[r].release();
-    if (r < static_cast<int>(g->ev_qkv.size()) && g->ev_qkv[r]) cudaEventDestroy(g->ev_qkv[r]);
-    if (r < static_cast<int>(g->ev_read.size()) && g->ev_read[r]) cudaEventDestroy(g->ev_read[r]);
+    for (std::vector<DevBuf>* b : {&g->kv, &g->gx, &g->gt, &g->gout})
+      if (r < static_cast<int>(b->size())) (*b)[r].release();
+    for (std::vector<cudaEvent_t>* e : {&g->ev_qkv, &g->ev_read, &g->ev_done, &g->gev_qkv, &g->gev_read, &g->gev_join})
+      if (r < static_cast<int>(e->size()) && (*e)[r]) cudaEventDestroy((*e)[r]);
+  }
+  if (g->world > 0) {
+    cudaSetDevice(g->dev[0]);
+    if (g->ev_fork) cudaEventDestroy(g->ev_fork);
+    if (g->ev_graph) cudaEventDestroy(g->ev_graph);
+    if (g->cap) cudaStreamDestroy(g->cap);
   }
   cudaSetDevice(cur);
 }
@@ -1323,10 +1372,16 @@ struct DeviceRestore {
 //        layer l (ev_read).  The first layer of a call waits likewise for the last gathers of the previous call.
 // Within a rank, its own stream orders everything else (its kv buffer is rewritten only after its own attention of the
 // previous layer, on the same stream).
+// in_graph: the stages are being captured.  The same pairs are recorded on the graph's own events (they become graph
+// edges), and the first layer's WAR waits are skipped: the previous call's gathers were recorded outside the capture,
+// and a graph launch runs only after everything before it on its stream (satb_dit_group_graph_forward).
 template <bool BF16, bool FP8>
 static int group_forward_impl(SatbDitGroup* g, const float* const* x, const float* const* t, float* const* out, int B,
-                              int L, float cfg_scale, float scale_phi, cudaStream_t const* st, const int* tb) {
+                              int L, float cfg_scale, float scale_phi, cudaStream_t const* st, const int* tb,
+                              bool in_graph) {
   const int W = g->world, P = g->h[0]->P, N = L + P;
+  const std::vector<cudaEvent_t>& ev_qkv = in_graph ? g->gev_qkv : g->ev_qkv;
+  const std::vector<cudaEvent_t>& ev_read = in_graph ? g->gev_read : g->ev_read;
   const int R = g->h[0]->cfg_on ? 2 * B : B;
   std::vector<DitFwd<BF16, FP8>> f;
   f.reserve(W);
@@ -1344,15 +1399,16 @@ static int group_forward_impl(SatbDitGroup* g, const float* const* x, const floa
   for (int i = 0; i < g->h[0]->depth; ++i) {
     for (int r = 0; r < W; ++r) {
       SATB_CHECK_CUDA(cudaSetDevice(g->dev[r]));
-      for (int s = 0; s < W; ++s) SATB_CHECK_CUDA(cudaStreamWaitEvent(st[r], g->ev_read[s], 0));   // WAR
+      if (!(in_graph && i == 0))
+        for (int s = 0; s < W; ++s) SATB_CHECK_CUDA(cudaStreamWaitEvent(st[r], ev_read[s], 0));   // WAR
       SATB_PROPAGATE(f[r].self_qkv(i));
-      SATB_CHECK_CUDA(cudaEventRecord(g->ev_qkv[r], st[r]));
+      SATB_CHECK_CUDA(cudaEventRecord(ev_qkv[r], st[r]));
     }
     for (int r = 0; r < W; ++r) {
       SATB_CHECK_CUDA(cudaSetDevice(g->dev[r]));
-      for (int s = 0; s < W; ++s) SATB_CHECK_CUDA(cudaStreamWaitEvent(st[r], g->ev_qkv[s], 0));    // RAW
+      for (int s = 0; s < W; ++s) SATB_CHECK_CUDA(cudaStreamWaitEvent(st[r], ev_qkv[s], 0));    // RAW
       SATB_PROPAGATE(launch_kv_gather(qkv.data(), tb, W, g->kv[r].p, R, D, st[r]));
-      SATB_CHECK_CUDA(cudaEventRecord(g->ev_read[r], st[r]));
+      SATB_CHECK_CUDA(cudaEventRecord(ev_read[r], st[r]));
       SATB_PROPAGATE(f[r].self_attn(i, g->kv[r].as<uint16_t>(), N));
       SATB_PROPAGATE(f[r].block_rest(i));
     }
@@ -1417,18 +1473,26 @@ int satb_dit_group_create(SatbDit* const* handles, const int* devices, int world
   g->h.assign(handles, handles + world);
   g->dev.assign(devices, devices + world);
   g->kv.resize(world);
-  g->ev_qkv.assign(world, nullptr);
-  g->ev_read.assign(world, nullptr);
-  for (int r = 0; r < world; ++r) {
-    cudaError_t e = cudaSetDevice(devices[r]);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&g->ev_qkv[r], cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&g->ev_read[r], cudaEventDisableTiming);
-    if (e != cudaSuccess) {
-      group_release(g);
-      delete g;
-      set_last_error(std::string("cudaEventCreate failed: ") + cudaGetErrorString(e));
-      return -2;
-    }
+  g->gx.resize(world);
+  g->gt.resize(world);
+  g->gout.resize(world);
+  for (std::vector<cudaEvent_t>* ev : {&g->ev_qkv, &g->ev_read, &g->ev_done, &g->gev_qkv, &g->gev_read, &g->gev_join})
+    ev->assign(world, nullptr);
+  cudaError_t e = cudaSuccess;
+  for (int r = 0; r < world && e == cudaSuccess; ++r) {
+    e = cudaSetDevice(devices[r]);
+    for (std::vector<cudaEvent_t>* ev : {&g->ev_qkv, &g->ev_read, &g->ev_done, &g->gev_qkv, &g->gev_read, &g->gev_join})
+      if (e == cudaSuccess) e = cudaEventCreateWithFlags(&(*ev)[r], cudaEventDisableTiming);
+  }
+  if (e == cudaSuccess) e = cudaSetDevice(devices[0]);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&g->ev_fork, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&g->ev_graph, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&g->cap, cudaStreamNonBlocking);
+  if (e != cudaSuccess) {
+    group_release(g);
+    delete g;
+    set_last_error(std::string("satb_dit_group_create: ") + cudaGetErrorString(e));
+    return -2;
   }
   *out = g;
   return 0;
@@ -1440,27 +1504,30 @@ void satb_dit_group_destroy(SatbDitGroup* g) {
   delete g;
 }
 
-int satb_dit_group_forward(SatbDitGroup* g, const float* const* x, const float* const* t, float* const* out, int B,
-                           int L, float cfg_scale, float scale_phi, void* const* streams) {
-  SATB_REQUIRE(g && x && t && out && streams, "null argument");
+}  // extern "C"
+
+// Checks one call's arguments against every rank's conditioning and fills the token split tb.
+static int group_check(SatbDitGroup* g, int B, int L, int* tb) {
   const int W = g->world;
   SatbDit* d0 = g->h[0];
   for (int r = 0; r < W; ++r) {
     const SatbDit* d = g->h[r];
     SATB_REQUIRE(d->finalized, "weights not finalized");
-    SATB_REQUIRE(x[r] && t[r] && out[r], "null argument");
     SATB_REQUIRE(B == d->B, "batch size differs from satb_dit_prepare_cond");
     SATB_REQUIRE(d->cfg_on == d0->cfg_on && d->P == d0->P && d->Rc == d0->Rc && d->Mctx == d0->Mctx &&
                      d->has_global == d0->has_global,
                  "every rank needs the same conditioning (satb_dit_set_prepend_cond / satb_dit_prepare_cond)");
   }
   SATB_REQUIRE(L >= 1, "bad shape");
-  int tb[kKvGatherMaxRanks + 1];
-  SATB_PROPAGATE(satb_dit_group_plan(W, d0->P, L, tb));
+  return satb_dit_group_plan(W, d0->P, L, tb);
+}
+
+// Grows every rank's workspace and kv buffer to the call's shape when they do not fit (synchronous when it allocates).
+static int group_reserve(SatbDitGroup* g, int B, int L, const int* tb) {
+  SatbDit* d0 = g->h[0];
   const int N = L + d0->P, R = d0->cfg_on ? 2 * B : B;
-  DeviceRestore restore;
   const bool fresh = R <= g->res_R && L == g->res_L && d0->P == g->res_P;
-  for (int r = 0; r < W; ++r) {
+  for (int r = 0; r < g->world; ++r) {
     SatbDit* d = g->h[r];
     // res_R 0: no single-device forward has reserved since; and the table check of needs_reserve (a reload of the
     // weights marks the position table stale)
@@ -1473,11 +1540,212 @@ int satb_dit_group_forward(SatbDitGroup* g, const float* const* x, const float* 
   g->res_R = std::max(g->res_R, R);
   g->res_L = L;
   g->res_P = d0->P;
+  return 0;
+}
+
+// The whole tensors of satb_dit_group_graph_forward: each rank's slice is copied into (x, t) and out of (out) the
+// group's fixed per-rank buffers on that rank's stream, over peer access between devices.
+struct GroupIo {
+  const float *x, *t;
+  float* out;
+};
+
+// Rank r's latent tokens lo .. lo + n - 1 of every item (rank 0 holds the prepended ones besides).
+static void rank_latents(const int* tb, int P, int r, int* lo, int* n) {
+  *lo = std::max(tb[r] - P, 0);
+  *n = tb[r + 1] - P - *lo;
+}
+
+// One group forward on the ranks' streams: every rank stream first waits for the last graph launch (ev_graph), then
+// the optional input slices, the stages, and the optional output slices.  Eager calls record each rank's ev_done last.
+static int group_run(SatbDitGroup* g, const float* const* x, const float* const* t, float* const* out, int B, int L,
+                     float cfg_scale, float scale_phi, cudaStream_t const* st, const int* tb, bool in_graph,
+                     const GroupIo* io) {
+  const int W = g->world;
+  SatbDit* d0 = g->h[0];
+  const int P = d0->P, Cin = d0->Cin, C = d0->C;
+  for (int r = 0; r < W; ++r) {
+    SATB_CHECK_CUDA(cudaSetDevice(g->dev[r]));
+    if (!in_graph) SATB_CHECK_CUDA(cudaStreamWaitEvent(st[r], g->ev_graph, 0));
+    if (!io) continue;
+    int lo, n;
+    rank_latents(tb, P, r, &lo, &n);
+    if (n > 0)
+      SATB_CHECK_CUDA(cudaMemcpy2DAsync(g->gx[r].p, static_cast<size_t>(n) * 4, io->x + lo, static_cast<size_t>(L) * 4,
+                                        static_cast<size_t>(n) * 4, static_cast<size_t>(B) * Cin, cudaMemcpyDefault,
+                                        st[r]));
+    SATB_CHECK_CUDA(cudaMemcpyAsync(g->gt[r].p, io->t, static_cast<size_t>(B) * 4, cudaMemcpyDefault, st[r]));
+  }
+  int rc;
+  if (d0->fp8)
+    rc = group_forward_impl<false, true>(g, x, t, out, B, L, cfg_scale, scale_phi, st, tb, in_graph);
+  else if (d0->bf16)
+    rc = group_forward_impl<true, false>(g, x, t, out, B, L, cfg_scale, scale_phi, st, tb, in_graph);
+  else
+    rc = group_forward_impl<false, false>(g, x, t, out, B, L, cfg_scale, scale_phi, st, tb, in_graph);
+  SATB_PROPAGATE(rc);
+  for (int r = 0; r < W; ++r) {
+    SATB_CHECK_CUDA(cudaSetDevice(g->dev[r]));
+    int lo, n;
+    rank_latents(tb, P, r, &lo, &n);
+    if (io && n > 0)
+      SATB_CHECK_CUDA(cudaMemcpy2DAsync(io->out + lo, static_cast<size_t>(L) * 4, g->gout[r].p,
+                                        static_cast<size_t>(n) * 4, static_cast<size_t>(n) * 4,
+                                        static_cast<size_t>(B) * C, cudaMemcpyDefault, st[r]));
+    if (!in_graph) SATB_CHECK_CUDA(cudaEventRecord(g->ev_done[r], st[r]));
+  }
+  return 0;
+}
+
+// Enqueues the group forward on g->cap while it captures, ending the capture on every path.  The rank streams fork
+// from g->cap and join it again, so the graph holds every rank's nodes on its own device.
+static int group_capture(SatbDitGroup* g, const float* const* x, const float* const* t, float* const* out, int B,
+                         int L, float cfg_scale, float scale_phi, cudaStream_t const* st, const int* tb,
+                         const GroupIo& io, cudaGraph_t* graph, unsigned long long* launches) {
+  SATB_CHECK_CUDA(cudaSetDevice(g->dev[0]));
+  SATB_CHECK_CUDA(cudaStreamBeginCapture(g->cap, cudaStreamCaptureModeThreadLocal));
+  const unsigned long long n0 = g_launch_count;
+  int rc = 0;
+  cudaError_t e = cudaEventRecord(g->ev_fork, g->cap);
+  for (int r = 0; r < g->world && e == cudaSuccess; ++r) {
+    e = cudaSetDevice(g->dev[r]);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(st[r], g->ev_fork, 0);
+  }
+  if (e == cudaSuccess) {
+    rc = group_run(g, x, t, out, B, L, cfg_scale, scale_phi, st, tb, true, &io);
+    for (int r = 0; r < g->world && rc == 0 && e == cudaSuccess; ++r) {
+      e = cudaSetDevice(g->dev[r]);
+      if (e == cudaSuccess) e = cudaEventRecord(g->gev_join[r], st[r]);
+      if (e == cudaSuccess) e = cudaSetDevice(g->dev[0]);
+      if (e == cudaSuccess) e = cudaStreamWaitEvent(g->cap, g->gev_join[r], 0);
+    }
+  }
+  *launches = g_launch_count - n0;
+  const std::string inner = rc != 0 ? satb_last_error() : "";
+  cudaSetDevice(g->dev[0]);
+  const cudaError_t e_end = cudaStreamEndCapture(g->cap, graph);   // also ends an invalidated capture
+  if (rc != 0 || e != cudaSuccess || e_end != cudaSuccess) {
+    if (e_end == cudaSuccess && *graph) cudaGraphDestroy(*graph);
+    *graph = nullptr;
+    cudaGetLastError();
+    if (rc != 0) {
+      set_last_error("capturing the group forward: " + inner);
+      return rc;
+    }
+    set_last_error(std::string("capturing the group forward: ") + cudaGetErrorString(e != cudaSuccess ? e : e_end));
+    return -3;
+  }
+  return 0;
+}
+
+extern "C" {
+
+int satb_dit_group_forward(SatbDitGroup* g, const float* const* x, const float* const* t, float* const* out, int B,
+                           int L, float cfg_scale, float scale_phi, void* const* streams) {
+  SATB_REQUIRE(g && x && t && out && streams, "null argument");
+  const int W = g->world;
+  for (int r = 0; r < W; ++r) SATB_REQUIRE(x[r] && t[r] && out[r], "null argument");
+  int tb[kKvGatherMaxRanks + 1];
+  SATB_PROPAGATE(group_check(g, B, L, tb));
+  DeviceRestore restore;
+  SATB_PROPAGATE(group_reserve(g, B, L, tb));
   cudaStream_t st[kKvGatherMaxRanks];
   for (int r = 0; r < W; ++r) st[r] = static_cast<cudaStream_t>(streams[r]);
-  if (d0->fp8) return group_forward_impl<false, true>(g, x, t, out, B, L, cfg_scale, scale_phi, st, tb);
-  return d0->bf16 ? group_forward_impl<true, false>(g, x, t, out, B, L, cfg_scale, scale_phi, st, tb)
-                  : group_forward_impl<false, false>(g, x, t, out, B, L, cfg_scale, scale_phi, st, tb);
+  return group_run(g, x, t, out, B, L, cfg_scale, scale_phi, st, tb, false, nullptr);
+}
+
+// Ordering against eager calls, which may run on distinct devices and alternate with graph launches:
+//   * before each launch, home_stream waits for every rank's ev_done, the end of its last eager call (its output
+//     stage, after which that rank touches no buffer of the call), so the graph never overwrites a workspace, a qkv
+//     or a kv buffer an eager call still reads;
+//   * after each launch, ev_graph is recorded on home_stream, and every eager call makes each rank stream wait for
+//     it before its first launch (group_run), so an eager call never overwrites what the graph still reads.
+// The graph's own cross-rank hazards are the eager path's event pairs, captured as edges; successive launches on one
+// stream run one after the other, which stands for the first layer's WAR waits.  With virtual ranks everything is on
+// one device, so these waits are ordinary same-device waits there; between devices they are the same events.
+int satb_dit_group_graph_forward(SatbDitGroup* g, const float* x, const float* t, float* out, int B, int L,
+                                 float cfg_scale, float scale_phi, void* const* rank_streams, void* home_stream) {
+  SATB_REQUIRE(g && x && t && out && rank_streams, "null argument");
+  const int W = g->world;
+  for (int r = 0; r < W; ++r)
+    SATB_REQUIRE(rank_streams[r], "rank streams must be created streams (the legacy default stream cannot be captured)");
+  for (int r = 0; r < W; ++r)
+    SATB_REQUIRE(!g->h[r]->prof_on, "satb_dit_group_graph_forward: profiling (satb_dit_profile) is on for a rank; "
+                                    "its event timing cannot be captured");
+  int tb[kKvGatherMaxRanks + 1];
+  SATB_PROPAGATE(group_check(g, B, L, tb));
+  DeviceRestore restore;
+  cudaStream_t st[kKvGatherMaxRanks];
+  for (int r = 0; r < W; ++r) st[r] = static_cast<cudaStream_t>(rank_streams[r]);
+  cudaStream_t home = static_cast<cudaStream_t>(home_stream);
+  GraphKey key;
+  key.x = x; key.t = t; key.out = out; key.B = B; key.L = L; key.cfg_scale = cfg_scale; key.scale_phi = scale_phi;
+  bool stale = !g->exec || !(key == g->key) || static_cast<int>(g->gens.size()) != W;
+  for (int r = 0; r < W && !stale; ++r) stale = g->gens[r] != g->h[r]->gen;
+  if (stale) {
+    group_drop_graph(g);
+    SatbDit* d0 = g->h[0];
+    const GroupIo io{x, t, out};
+    const float* xs[kKvGatherMaxRanks];
+    const float* ts[kKvGatherMaxRanks];
+    float* os[kKvGatherMaxRanks];
+    for (int r = 0; r < W; ++r) {   // the fixed per-rank slices (at least 256 bytes: a rank may hold no latent token)
+      int lo, n;
+      rank_latents(tb, d0->P, r, &lo, &n);
+      SATB_CHECK_CUDA(cudaSetDevice(g->dev[r]));
+      SATB_PROPAGATE(g->gx[r].ensure(std::max<size_t>(static_cast<size_t>(B) * d0->Cin * n * 4, 256)));
+      SATB_PROPAGATE(g->gt[r].ensure(std::max<size_t>(static_cast<size_t>(B) * 4, 256)));
+      SATB_PROPAGATE(g->gout[r].ensure(std::max<size_t>(static_cast<size_t>(B) * d0->C * n * 4, 256)));
+      xs[r] = g->gx[r].as<float>();
+      ts[r] = g->gt[r].as<float>();
+      os[r] = g->gout[r].as<float>();
+    }
+    // warm-up: one eager call at this shape, so that nothing allocates, makes a tensor map or sets a function
+    // attribute during the capture.  The rank streams start after home_stream's work so far (the caller's inputs).
+    SATB_PROPAGATE(group_reserve(g, B, L, tb));
+    SATB_CHECK_CUDA(cudaSetDevice(g->dev[0]));
+    SATB_CHECK_CUDA(cudaEventRecord(g->ev_graph, home));
+    SATB_PROPAGATE(group_run(g, xs, ts, os, B, L, cfg_scale, scale_phi, st, tb, false, &io));
+    cudaGraph_t graph = nullptr;
+    unsigned long long launches = 0;
+    SATB_PROPAGATE(group_capture(g, xs, ts, os, B, L, cfg_scale, scale_phi, st, tb, io, &graph, &launches));
+    SATB_CHECK_CUDA(cudaSetDevice(g->dev[0]));
+    const cudaError_t e = cudaGraphInstantiate(&g->exec, graph, 0);
+    cudaGraphDestroy(graph);
+    if (e != cudaSuccess) {
+      g->exec = nullptr;
+      cudaGetLastError();
+      set_last_error(std::string("instantiating the group forward's graph: ") + cudaGetErrorString(e));
+      return -3;
+    }
+    g->key = key;
+    g->gens.resize(W);
+    for (int r = 0; r < W; ++r) g->gens[r] = g->h[r]->gen;
+    g->graph_launches = launches;
+    ++g->captures;
+  }
+  SATB_CHECK_CUDA(cudaSetDevice(g->dev[0]));
+  for (int r = 0; r < W; ++r) SATB_CHECK_CUDA(cudaStreamWaitEvent(home, g->ev_done[r], 0));
+  SATB_CHECK_CUDA(cudaGraphLaunch(g->exec, home));
+  SATB_CHECK_CUDA(cudaEventRecord(g->ev_graph, home));
+  g_launch_count += g->graph_launches;
+  ++g->replays;
+  return 0;
+}
+
+int satb_dit_group_graph_reset(SatbDitGroup* g) {
+  SATB_REQUIRE(g, "null argument");
+  group_drop_graph(g);
+  return 0;
+}
+
+int satb_dit_group_graph_stats(const SatbDitGroup* g, long long* captures, long long* replays,
+                               unsigned long long* launches) {
+  SATB_REQUIRE(g && captures && replays && launches, "null argument");
+  *captures = g->captures;
+  *replays = g->replays;
+  *launches = g->exec ? g->graph_launches : 0;
+  return 0;
 }
 
 }  // extern "C"

@@ -125,6 +125,9 @@ SIGNATURES = {
     "satb_dit_group_create": (_I, [_VP, _VP, _I, ctypes.POINTER(_VP)]),
     "satb_dit_group_destroy": (None, [_VP]),
     "satb_dit_group_forward": (_I, [_VP, _VP, _VP, _VP, _I, _I, _F, _F, _VP]),
+    "satb_dit_group_graph_forward": (_I, [_VP, _VP, _VP, _VP, _I, _I, _F, _F, _VP, _VP]),
+    "satb_dit_group_graph_reset": (_I, [_VP]),
+    "satb_dit_group_graph_stats": (_I, [_VP, ctypes.POINTER(_LL), ctypes.POINTER(_LL), ctypes.POINTER(ctypes.c_ulonglong)]),
     "satb_kv_gather": (_I, [_VP, _VP, _I, _VP, _I, _I, _VP]),
     "satb_dit_profile": (_I, [_VP, _I]),
     "satb_dit_profile_read": (_I, [_VP, _VP, _VP]),

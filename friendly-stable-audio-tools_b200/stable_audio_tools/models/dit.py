@@ -22,7 +22,8 @@ and parameter names, ``forward`` signature and CFG semantics); the arithmetic ru
   the library pads project_in's K to a multiple of 8 and project_out's N to a multiple of 32 with zero weights;
 * ``shard_tokens(devices)`` splits every call's tokens over several ranks (``satb_dit_group_*``): each rank holds a full
   copy of the weights and a contiguous range of every item's tokens, and gathers every rank's self-attention K / V once
-  per layer, so one prompt can use several GPUs.
+  per layer, so one prompt can use several GPUs; with ``cuda_graph`` the whole sharded call is replayed from one
+  multi-device CUDA graph the library captures and owns (``satb_dit_group_graph_forward``).
 
 There is no eager / CPU fallback: tensors must live on a CUDA device.
 """
@@ -167,6 +168,8 @@ class DiffusionTransformer(nn.Module):
         # cuda_graph = True: one denoiser call = ONE CUDA-graph launch (the ~280 kernel launches of a forward are
         # captured once per (shape, guidance, conditioning) and replayed).  The returned tensor is then a static
         # buffer that the NEXT call overwrites - fine for the samplers, which consume it at once; off by default.
+        # A token-sharded model (shard_tokens) replays every rank's launches, the K/V gathers and the copies of the
+        # ranks' slices in and out from one multi-device graph the library captures and invalidates itself.
         self.cuda_graph = False
         # nn.Module.load_state_dict on a PARENT (ConditionedDiffusionModelWrapper, DiTWrapper, copy_state_dict(model, sd))
         # recurses through _load_from_state_dict and never calls a child's load_state_dict override; the post hook
@@ -178,12 +181,14 @@ class DiffusionTransformer(nn.Module):
     def _apply(self, fn, *a, **k):
         self.__dict__["_weights_dirty"] = True
         self.__dict__["_shard_dirty"] = True
+        self._drop_shard_graph()
         return super()._apply(fn, *a, **k)
 
     def refresh_native_weights(self):
         """Call after mutating parameters in place (``load_state_dict`` / ``.to()`` do it for you)."""
         self.__dict__["_weights_dirty"] = True
         self.__dict__["_shard_dirty"] = True
+        self._drop_shard_graph()
 
     def __del__(self):
         try:
@@ -315,8 +320,14 @@ class DiffusionTransformer(nn.Module):
 
         Refused with NotImplementedError: conformer blocks and ``use_conv`` feed-forwards (their token convolutions
         would need the neighbouring ranks' tokens), ``attention_dtype="fp8"`` (its V channel scales span all of an
-        item's tokens) and, at call time, ``return_info``.  ``cuda_graph=True`` is not captured in this mode: each call
-        enqueues every rank's launches eagerly.  Ranks on distinct GPUs need peer-to-peer access between them."""
+        item's tokens) and, at call time, ``return_info``.  Ranks on distinct GPUs need peer-to-peer access between them.
+
+        With ``cuda_graph`` off, each call enqueues every rank's launches eagerly.  With it on (the multistep SDE samplers
+        and the v-diffusion ``sample`` switch it on), each call is one launch of a multi-device CUDA graph
+        (``satb_dit_group_graph_forward``): it copies the ranks' slices of the input in, runs the sharded forward and
+        copies the slices of the output back, and returns a static buffer on the home device that the next call
+        overwrites.  The library captures it on the first call and again whenever the shape, the guidance scalars, the
+        conditioning, the weights or a workspace change, and orders it against eager sharded calls itself."""
         if devices is not None:
             if self.conformer:
                 raise NotImplementedError("shard_tokens: conformer blocks are not supported (their depthwise convolution "
@@ -337,7 +348,7 @@ class DiffusionTransformer(nn.Module):
         self._drop_shards()
         if devices is not None:
             self.__dict__["_shard"] = dict(devices=devices, handles=None, group=None, streams=None, cond_key=None,
-                                           keepalive=None)
+                                           keepalive=None, graph_io=None)
             self.__dict__["_shard_dirty"] = True
         return self
 
@@ -352,6 +363,26 @@ class DiffusionTransformer(nn.Module):
         for h in sh["handles"] or []:
             lib.satb_dit_destroy(h)
 
+    def _drop_shard_graph(self):
+        """Drops the sharded model's captured graph and its static buffers; the next graph call captures again."""
+        sh = self.__dict__.get("_shard")
+        if sh is None:
+            return
+        if sh["group"] is not None:
+            _native.check(_native.lib().satb_dit_group_graph_reset(sh["group"]))
+        sh["graph_io"] = None
+
+    def shard_graph_stats(self):
+        """(captures, replays, kernel launches of the current graph) of the sharded model's group, or None when the
+        model is not sharded or its group does not exist yet."""
+        sh = self.__dict__.get("_shard")
+        if sh is None or sh["group"] is None:
+            return None
+        c, r, n = ctypes.c_longlong(), ctypes.c_longlong(), ctypes.c_ulonglong()
+        _native.check(_native.lib().satb_dit_group_graph_stats(sh["group"], ctypes.byref(c), ctypes.byref(r),
+                                                               ctypes.byref(n)))
+        return c.value, r.value, n.value
+
     def _shard_group(self, sh):
         lib = _native.lib()
         devs = sh["devices"]
@@ -360,6 +391,7 @@ class DiffusionTransformer(nn.Module):
         if sh["group"] is not None:
             lib.satb_dit_group_destroy(sh["group"])
             sh["group"] = None
+            sh["graph_io"] = None
         if sh["handles"] is None:
             sh["handles"] = []
             for _ in devs:
@@ -378,14 +410,14 @@ class DiffusionTransformer(nn.Module):
         self.__dict__["_shard_dirty"] = False
         return g
 
-    def _sharded_forward(self, sh, x, t, cross, neg, glob, prepend, use_cfg, cfg_scale, scale_phi):
-        lib = _native.lib()
+    def _sharded_prepare(self, sh, x, cross, neg, glob, prepend, use_cfg):
+        """The group, with every rank handle's conditioning prepared for this call."""
         devs = sh["devices"]
         home = devs[0]
         if x.device != home:
             raise ValueError(f"the token-sharded model's home device is {home}, but x is on {x.device}")
         g = self._shard_group(sh)
-        B, _, L = x.shape
+        B = x.shape[0]
         key = (self._tkey(cross), self._tkey(neg), self._tkey(glob), bool(use_cfg), B, self._tkey(prepend))
         if key != sh["cond_key"]:
             for h, dv in zip(sh["handles"], devs):
@@ -393,6 +425,14 @@ class DiffusionTransformer(nn.Module):
                     self._prepare_native(h, cross, neg, glob, use_cfg, dv, B, prepend, copy_to=dv)
             sh["cond_key"] = key
             sh["keepalive"] = (cross, neg, glob, prepend)
+        return g
+
+    def _sharded_forward(self, sh, x, t, cross, neg, glob, prepend, use_cfg, cfg_scale, scale_phi):
+        lib = _native.lib()
+        devs = sh["devices"]
+        home = devs[0]
+        g = self._sharded_prepare(sh, x, cross, neg, glob, prepend, use_cfg)
+        B, _, L = x.shape
         P = 0 if self.global_cond_type == "adaLN" else 1 + (prepend.shape[1] if prepend is not None else 0)
         tb = _native.group_plan(len(devs), P, L)
         xin = x.detach().to(torch.float32)
@@ -412,6 +452,37 @@ class DiffusionTransformer(nn.Module):
         for r, dv in enumerate(devs):
             torch.cuda.current_stream(dv).wait_stream(sh["streams"][r])
         return torch.cat([o.to(home) for o in outs], dim=2)
+
+    def _sharded_graph_forward(self, sh, x, t, cross, neg, glob, prepend, use_cfg, cfg_scale, scale_phi):
+        """The sharded call as one launch of the group's multi-device CUDA graph (satb_dit_group_graph_forward).  The
+        library captures it, with one eager warm-up call in front, whenever the key (static buffers, shape, guidance)
+        or any rank handle's weights, conditioning or workspaces changed, and orders it against eager sharded calls.
+        x, t and the output are static home-device buffers per (B, C, L); the returned tensor is overwritten by the
+        next call."""
+        devs = sh["devices"]
+        home = devs[0]
+        g = self._sharded_prepare(sh, x, cross, neg, glob, prepend, use_cfg)
+        B, C, L = x.shape
+        io = sh["graph_io"]
+        if io is None or io["key"] != (B, C, L):
+            io = dict(key=(B, C, L), x=torch.empty(B, C, L, device=home, dtype=torch.float32),
+                      t=torch.empty(B, device=home, dtype=torch.float32),
+                      out=torch.empty(B, self.io_channels * self.patch_size, L, device=home, dtype=torch.float32))
+            sh["graph_io"] = io
+        io["x"].copy_(x)
+        io["t"].copy_(t)
+        cur = torch.cuda.current_stream(home)
+        others = {dv for dv in devs if dv != home}
+        for dv in others:                     # the ranks' conditioning was prepared on their devices' current streams
+            cur.wait_stream(torch.cuda.current_stream(dv))
+        streams = (ctypes.c_void_p * len(devs))(*[s_.cuda_stream for s_ in sh["streams"]])
+        with torch.cuda.device(home):
+            _native.check(_native.lib().satb_dit_group_graph_forward(
+                g, _native.ptr(io["x"]), _native.ptr(io["t"]), _native.ptr(io["out"]), B, L, float(cfg_scale),
+                float(scale_phi), streams, ctypes.c_void_p(cur.cuda_stream)))
+        for dv in others:                     # later work there (new conditioning) must not overtake the graph
+            torch.cuda.current_stream(dv).wait_stream(cur)
+        return io["out"]
 
     # ------------------------------------------------------------------ forward
     @torch.no_grad()
@@ -492,8 +563,11 @@ class DiffusionTransformer(nn.Module):
             x = x.reshape(b_, c_, l_ // p, p).transpose(2, 3).reshape(b_, c_ * p, l_ // p)   # channel = c * p + pi
         sh = self.__dict__["_shard"]
         if sh is not None:
-            return self._unpatch(self._sharded_forward(sh, x, t, cross_attn_cond, neg, global_embed, prepend_cond,
-                                                       use_cfg, cfg_scale, scale_phi)).to(x.dtype)
+            run = self._sharded_forward
+            if self.cuda_graph and not torch.cuda.is_current_stream_capturing():
+                run = self._sharded_graph_forward
+            return self._unpatch(run(sh, x, t, cross_attn_cond, neg, global_embed, prepend_cond, use_cfg, cfg_scale,
+                                     scale_phi)).to(x.dtype)
         # handles, workspaces and TMA descriptors live on the model's device: make it current for the native calls
         # (generate_diffusion_cond(device='cuda:1') with current device 0 must work)
         with torch.cuda.device(x.device):

@@ -162,6 +162,23 @@ void satb_dit_group_destroy(SatbDitGroup* g);
  * rank r's stream.  Enqueues only (ranks are ordered with events); the caller's current device is restored. */
 int satb_dit_group_forward(SatbDitGroup* g, const float* const* x, const float* const* t, float* const* out, int B,
                            int L, float cfg_scale, float scale_phi, void* const* streams);
+/* The same call replayed from one CUDA graph whose nodes live on every rank's device: one cudaGraphLaunch on
+ * home_stream.  x [B, C, L], t [B] and out [B, io_channels, L] are whole tensors on rank 0's device, at addresses the
+ * caller keeps fixed; rank_streams[r] (created streams, on rank r's device) are used while capturing.  The graph copies
+ * each rank's slice of x and t in, runs the group forward and copies each rank's slice of out back.  The first call,
+ * and every call after the key (x, t, out, B, L, cfg_scale, scale_phi) changed or after any handle's weights,
+ * conditioning or workspaces may have moved (satb_dit_finalize, satb_dit_set_prepend_cond, satb_dit_prepare_cond, a
+ * workspace reserve), runs one eager group forward at the shape and then captures and instantiates the graph.  Graph
+ * launches and satb_dit_group_forward calls may alternate: the library orders them with events.  Refused while
+ * profiling is on; a failed capture or instantiation returns the CUDA error with its message.  Each launch adds the
+ * kernel launches it replays to satb_launch_count. */
+int satb_dit_group_graph_forward(SatbDitGroup* g, const float* x, const float* t, float* out, int B, int L,
+                                 float cfg_scale, float scale_phi, void* const* rank_streams, void* home_stream);
+/* Drops the group's graph (satb_dit_group_destroy does too); the next graph call captures again. */
+int satb_dit_group_graph_reset(SatbDitGroup* g);
+/* Graphs captured and launched so far, and the kernel launches of the current graph (0: none). */
+int satb_dit_group_graph_stats(const SatbDitGroup* g, long long* captures, long long* replays,
+                               unsigned long long* launches);
 /* The group forward's K/V gather on its own (tests and timing): kv [R, N, 2 D] 16-bit = the columns D .. 3 D - 1 of
  * every rank's qkv[s] [R, n_s, 3 D], rank s's rows at tokens token_begin[s] .. token_begin[s + 1] - 1 of each item
  * (N = token_begin[world], token_begin[0] = 0).  qkv[s] may be a peer device's pointer. */
