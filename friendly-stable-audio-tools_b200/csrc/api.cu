@@ -86,7 +86,8 @@ int satb_dit_post_probe(const float* y, int ldy, float* out, int B, int C, int L
   SATB_REQUIRE(y && out, "null argument");
   SATB_REQUIRE(B >= 1 && B <= kMaxGridYZ && C >= 1 && L >= 1 && P >= 0, "dit post probe: need 1 <= B <= 65535, C, L >= 1 and P >= 0");
   SATB_REQUIRE(N_seq >= P && N_seq - P >= L, "dit post probe: need N_seq >= P + L");
-  return launch_dit_post(y, ldy, out, B, C, L, N_seq, P, cfg != 0, cfg_scale, scale_phi, static_cast<cudaStream_t>(stream));
+  return launch_dit_post(y, y + static_cast<size_t>(B) * N_seq * ldy, ldy, out, B, C, L, N_seq, P, cfg != 0, cfg_scale,
+                         scale_phi, static_cast<cudaStream_t>(stream));
 }
 
 int satb_cast_rows_probe(const float* src, void* dst16, const int* perm, int rows, int cols, long long src_ld,

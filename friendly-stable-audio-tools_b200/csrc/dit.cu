@@ -111,6 +111,7 @@ struct SatbDit {
   DevBuf ws_a8, ws_ascale;   // FP8 mode: e4m3 LayerNorm rows [M, D] and their scales [M]
   DevBuf ws_attn8;            // FP8 self-attention operands (attn_fp8_bufs), with their tensor maps for res_R rows
   AttnFp8Maps attn8_maps;
+  int attn8_R = 0;            // the rows ws_attn8 is carved for and attn8_maps were made for (the last reserve_rows)
   int rope_len = 0;
   int res_R = 0, res_L = 0, res_P = -1;
   // bumped whenever weights, conditioning or workspaces may have moved or changed (satb_dit_finalize,
@@ -739,6 +740,7 @@ static int reserve_rows(SatbDit* d, int R, int n, int tab_len) {
     SATB_CHECK_CUDA(cudaMemset(d->ws_attn8.p, 0, attn_fp8_workspace_bytes(R, d->H, N_seq, N_seq)));
     SATB_PROPAGATE(make_attention_fp8_maps(&d->attn8_maps, attn_fp8_bufs(d->ws_attn8.p, R, d->H, N_seq, N_seq), R, d->H,
                                            N_seq, N_seq));
+    d->attn8_R = R;
   }
   if (d->rotary) SATB_PROPAGATE(ensure_rope(d, tab_len));
   if (d->pos_type != 0) SATB_PROPAGATE(ensure_pos(d, tab_len));
@@ -897,9 +899,13 @@ enum { PROF_FF_IN = 0, PROF_FF_OUT, PROF_QKV, PROF_ATTN_SELF, PROF_ATTN_OUT, PRO
 // which are the prepended ones (global-conditioning and prepend-conditioning tokens).  The tokens are positions
 // pos0 .. pos0 + n - 1 of the rotary and positional tables, which hold tab_len positions.  The single-device forward is
 // the one shard that holds every token: P = d->P, n = tab_len = L + P, pos0 = 0.  A rank of a group forward holds a
-// contiguous range of every item's tokens, with the prepended ones on rank 0 only.
+// contiguous range of every item's tokens, with the prepended ones on rank 0 only.  half: -1 runs every row of the
+// conditioning (2 B under CFG); 0 / 1 runs only the conditional / unconditional half of a CFG call (R = B rows, a rank
+// of the CFG-split group forward), with conditioning rows half * B .. half * B + B - 1: their cross-attention K / V,
+// prepend tokens (zeros on the unconditional half) and adaLN rows, exactly as the batched CFG forward uses them.
 struct FwdShape {
   int B, R, L, P, n, pos0, tab_len;
+  int half = -1;
 };
 
 // One forward as its stages: input (timestep embedding, project_in, prepended rows), then per block self_qkv, self_attn
@@ -914,6 +920,7 @@ struct DitFwd {
   FwdShape s;
   cudaStream_t st;
   int D, C, H, M, Mc;   // Mc: rows running cross-attention (a prefix of the row space)
+  int Rc, kv_row0;      // the Rc rows running cross-attention read conditioning K / V rows kv_row0 .. kv_row0 + Rc - 1
   int64_t ssg_ld;
   SmallWs sw;
   float* h;
@@ -928,7 +935,11 @@ struct DitFwd {
   DitFwd(SatbDit* d_, const FwdShape& s_, cudaStream_t st_) : d(d_), s(s_), st(st_) {
     D = d->D; C = d->C; H = d->H;
     M = s.R * s.n;
-    Mc = d->Rc * s.n;
+    // the conditional half holds the cross-attention rows of the batched CFG forward that fall in its B rows; the
+    // unconditional half has some only with a negative prompt (Rc = 2 B)
+    Rc = s.half < 0 ? d->Rc : s.half == 0 ? std::min(d->Rc, s.B) : (d->Rc == 2 * s.B ? s.B : 0);
+    kv_row0 = s.half == 1 ? s.B : 0;
+    Mc = Rc * s.n;
     ssg_ld = static_cast<int64_t>(d->depth) * 6 * D;
     sw = small_ws(d, 2 * d->B);
     h = d->ws_h.as<float>();
@@ -978,8 +989,8 @@ struct DitFwd {
       SATB_PROPAGATE((linear<EpiStore32, 256, BF16>(d->tmaps, ain, Kin, M, Kin, d->w_in16, D, EpiStore32::Params{h, D, nullptr}, st)));
     if (d->P > 0) {
       if (s.P > 0)
-        SATB_PROPAGATE(launch_write_prepend(sw.tok, d->Pp > 0 ? d->ws_prep.as<float>() : nullptr, pos_tab, h, s.R, B,
-                                            s.n, D, d->Pp, st));
+        SATB_PROPAGATE(launch_write_prepend(sw.tok, d->Pp > 0 && s.half != 1 ? d->ws_prep.as<float>() : nullptr,
+                                            pos_tab, h, s.R, B, s.n, D, d->Pp, st));
     } else {
       // adaLN: all layers' scale/shift/gate in one skinny GEMM (transformer.py:648-651,667)
       SATB_PROPAGATE(launch_skinny_linear(sw.tok, d->w_ssg, nullptr, nullptr, sw.ssg, B, D, d->depth * 6 * D, 0, st));
@@ -1000,7 +1011,7 @@ struct DitFwd {
     const void* w = FP8 ? static_cast<const void*>(W.w8_qkv) : static_cast<const void*>(W.w_qkv);
     const Fp8Scales sc{a_scale, W.s_qkv};
     // FP8 self-attention: q and k leave the epilogue as e4m3 with their scales, v in 16 bits as always
-    const AttnFp8Bufs b8 = d->attn_fp8 ? attn_fp8_bufs(d->ws_attn8.p, d->res_R, H, s.n, s.n) : AttnFp8Bufs{};
+    const AttnFp8Bufs b8 = d->attn_fp8 ? attn_fp8_bufs(d->ws_attn8.p, d->attn8_R, H, s.n, s.n) : AttnFp8Bufs{};
     const QkE4m3Out o8{b8.q8, b8.k8, b8.sq, b8.sk, H, attn_fp8_pad(s.n)};
     if (d->qk_norm) {
       typedef EpiHeadNorm16<BF16> E;   // q, k heads L2-normalised, then rotary
@@ -1033,8 +1044,8 @@ struct DitFwd {
     {
       ProfScope ps(d, PROF_ATTN_SELF, st);
       const int64_t qs = static_cast<int64_t>(s.n) * 3 * D;
-      if (d->attn_fp8) {   // e4m3 operands in the workspace carved for res_R rows; the maps were made for them
-        const AttnFp8Bufs b8 = attn_fp8_bufs(d->ws_attn8.p, d->res_R, H, s.n, s.n);
+      if (d->attn_fp8) {   // e4m3 operands in the workspace carved for attn8_R rows; the maps were made for them
+        const AttnFp8Bufs b8 = attn_fp8_bufs(d->ws_attn8.p, d->attn8_R, H, s.n, s.n);
         SATB_PROPAGATE(launch_attention_fp8_vt(qkv + 2 * D, 3 * D, qs, b8, s.R, H, s.n, BF16, st));
         SATB_PROPAGATE(launch_attention_fp8(d->attn8_maps, b8, att, D, static_cast<int64_t>(s.n) * D, s.R, H, s.n,
                                             s.n, BF16, st));
@@ -1086,16 +1097,17 @@ struct DitFwd {
         typename E::Params ep{q16, D, nullptr, 0};
         SATB_PROPAGATE((linear_auto<E, BF16, FP8>(d->tmaps, a_in, D, Mc, D, wq, D, ep, st, sc)));
       }
-      const uint16_t* kv = d->ws_kv.as<uint16_t>() + static_cast<size_t>(i) * d->Rc * d->Mctx * 2 * d->ce;
+      const uint16_t* kv = d->ws_kv.as<uint16_t>() +
+                           (static_cast<size_t>(i) * d->Rc + kv_row0) * d->Mctx * 2 * d->ce;
       const int64_t kvs = static_cast<int64_t>(d->Mctx) * 2 * d->ce;
       const CUtensorMap *tq = nullptr, *tkv = nullptr;   // k and v are column ranges of one buffer: one map
       if (d->dh == 64) {
-        SATB_PROPAGATE(d->tmaps.get_a(q16, D, n, d->Rc, D, static_cast<int64_t>(n) * D, &tq));
-        SATB_PROPAGATE(d->tmaps.get_a(kv, 2 * d->ce, d->Mctx, d->Rc, 2 * d->ce, kvs, &tkv));
+        SATB_PROPAGATE(d->tmaps.get_a(q16, D, n, Rc, D, static_cast<int64_t>(n) * D, &tq));
+        SATB_PROPAGATE(d->tmaps.get_a(kv, 2 * d->ce, d->Mctx, Rc, 2 * d->ce, kvs, &tkv));
       }
       SATB_PROPAGATE(launch_attention_tc(q16, kv, kv, att, D, 2 * d->ce, 2 * d->ce, D, static_cast<int64_t>(n) * D,
                                          kvs, kvs, static_cast<int64_t>(n) * D, D, 2 * d->ce, 2 * d->ce, 0, 0,
-                                         d->ce, d->Rc, H, Hkv, n, d->Mctx, d->dh, BF16, st, tq, tkv, tkv));
+                                         d->ce, Rc, H, Hkv, n, d->Mctx, d->dh, BF16, st, tq, tkv, tkv));
       EpiResidual::Params ep{h, D, nullptr, nullptr, n, 0, 1};
       SATB_PROPAGATE((linear_auto<EpiResidual, BF16>(d->tmaps, att, D, Mc, D, W.w_co, D, ep, st)));
     }
@@ -1152,16 +1164,25 @@ struct DitFwd {
     return 0;
   }
 
-  int output(float* out, float cfg_scale, float scale_phi, float* hidden_out) {
+  // project_out (with the 1x1 post-conv folded) reads a 16-bit copy of h; its N is C_p (zero weight rows past C)
+  int project_out(float* hidden_out) {
     if (hidden_out)
       SATB_CHECK_CUDA(cudaMemcpyAsync(hidden_out, h, static_cast<size_t>(M) * D * 4, cudaMemcpyDeviceToDevice, st));
-    // project_out (with the 1x1 post-conv folded) reads a 16-bit copy of h; its N is C_p (zero weight rows past C), and
-    // dit_post reads the C real channels of each y row
     const int Cp = d->C_p;
     SATB_PROPAGATE(launch_cast_rows(h, a16, nullptr, M, D, D, D, BF16, st));
     SATB_PROPAGATE((linear<EpiStore32, 64, BF16>(d->tmaps, a16, D, M, D, d->w_out16, Cp, EpiStore32::Params{y, Cp, nullptr}, st)));
-    SATB_PROPAGATE(launch_dit_post(y, Cp, out, s.B, C, s.L, s.n, s.P, d->cfg_on ? 1 : 0, cfg_scale, scale_phi, st));
     return 0;
+  }
+
+  // dit_post: the C real channels of each y row of the first B rows -> out, combined with the unconditional rows yu
+  // (same shape and row pitch) under CFG; yu null: no CFG
+  int combine(float* out, const float* yu, float cfg_scale, float scale_phi) {
+    return launch_dit_post(y, yu, d->C_p, out, s.B, C, s.L, s.n, s.P, yu ? 1 : 0, cfg_scale, scale_phi, st);
+  }
+
+  int output(float* out, float cfg_scale, float scale_phi, float* hidden_out) {
+    SATB_PROPAGATE(project_out(hidden_out));
+    return combine(out, d->cfg_on ? y + static_cast<size_t>(s.B) * s.n * d->C_p : nullptr, cfg_scale, scale_phi);
   }
 };
 
@@ -1289,16 +1310,21 @@ struct GraphKey {
 };
 
 struct SatbDitGroup {
-  int world = 0;
+  int world = 0;                             // ranks of one row (the token split)
+  // satb_dit_group_create_cfg: two rows of `world` ranks, row 0 (ranks 0 .. world - 1) running the conditional half
+  // of each CFG call and row 1 (ranks world .. 2 world - 1) the unconditional half; a call without CFG runs row 0 only
+  bool cfg = false;
+  int ranks = 0;                             // handles: world, or 2 world for a CFG group
   std::vector<SatbDit*> h;
   std::vector<int> dev;
   std::vector<DevBuf> kv;                    // per rank, on its device: [R, N, 2D] 16-bit
   // Per rank, recorded by eager calls only: its QKV GEMM done / its gather done (the last enqueued) / its last work
-  // of the call done.  A captured graph records its own pair (gev_*): an event last recorded inside a capture cannot
-  // be waited on outside it.
-  std::vector<cudaEvent_t> ev_qkv, ev_read, ev_done;
-  std::vector<cudaEvent_t> gev_qkv, gev_read, gev_join;
-  int res_R = 0, res_L = 0, res_P = -1;
+  // of the call done / (CFG group, row 0) its combine done.  A captured graph records its own events (gev_*): an event
+  // last recorded inside a capture cannot be waited on outside it.  ev_y / gev_y (CFG group, row 1): its project_out
+  // done.
+  std::vector<cudaEvent_t> ev_qkv, ev_read, ev_done, ev_y, ev_comb;
+  std::vector<cudaEvent_t> gev_qkv, gev_read, gev_join, gev_y;
+  std::vector<int> res_R, res_L, res_P;      // per rank: the shape its workspace was last reserved for
   // satb_dit_group_graph_forward: the instantiated graph, what it was captured for, and the fixed per-rank slices of
   // x, t and out it reads and writes (on each rank's device)
   cudaGraphExec_t exec = nullptr;
@@ -1311,6 +1337,12 @@ struct SatbDitGroup {
   cudaEvent_t ev_graph = nullptr;            // home device: recorded after each graph launch (and before a warm-up)
   cudaStream_t cap = nullptr;                // home device: the capture stream
 };
+
+// Every per-rank event vector of a group.
+static std::vector<std::vector<cudaEvent_t>*> group_events(SatbDitGroup* g) {
+  return {&g->ev_qkv, &g->ev_read, &g->ev_done, &g->ev_y, &g->ev_comb, &g->gev_qkv, &g->gev_read, &g->gev_join,
+          &g->gev_y};
+}
 
 // The option a group forward cannot run on this handle, or null.  Token convolutions (conformer blocks, use_conv
 // feed-forwards) need the neighbouring ranks' tokens (halos); FP8 self-attention's v channel scales span all of an
@@ -1343,14 +1375,14 @@ static void group_release(SatbDitGroup* g) {
   int cur = 0;
   cudaGetDevice(&cur);
   group_drop_graph(g);
-  for (int r = 0; r < g->world; ++r) {
+  for (int r = 0; r < g->ranks; ++r) {
     cudaSetDevice(g->dev[r]);
     for (std::vector<DevBuf>* b : {&g->kv, &g->gx, &g->gt, &g->gout})
       if (r < static_cast<int>(b->size())) (*b)[r].release();
-    for (std::vector<cudaEvent_t>* e : {&g->ev_qkv, &g->ev_read, &g->ev_done, &g->gev_qkv, &g->gev_read, &g->gev_join})
+    for (std::vector<cudaEvent_t>* e : group_events(g))
       if (r < static_cast<int>(e->size()) && (*e)[r]) cudaEventDestroy((*e)[r]);
   }
-  if (g->world > 0) {
+  if (g->ranks > 0) {
     cudaSetDevice(g->dev[0]);
     if (g->ev_fork) cudaEventDestroy(g->ev_fork);
     if (g->ev_graph) cudaEventDestroy(g->ev_graph);
@@ -1372,62 +1404,89 @@ struct DeviceRestore {
 //        layer l (ev_read).  The first layer of a call waits likewise for the last gathers of the previous call.
 // Within a rank, its own stream orders everything else (its kv buffer is rewritten only after its own attention of the
 // previous layer, on the same stream).
+// split (a CFG call on a CFG group): both rows run, each on its half of the rows, and the pairs above hold within a
+// row (the ranks of a row gather only each other's K / V).  After the last block, row-0 rank j combines its y with
+// row-1 rank j's y (same tokens), read through a peer pointer, and two more pairs order that:
+//   RAW: row-0 rank j's combine waits for row-1 rank j's project_out (ev_y).
+//   WAR: row-1 rank j's project_out of the next call waits for row-0 rank j's combine of this call (ev_comb).
 // in_graph: the stages are being captured.  The same pairs are recorded on the graph's own events (they become graph
-// edges), and the first layer's WAR waits are skipped: the previous call's gathers were recorded outside the capture,
-// and a graph launch runs only after everything before it on its stream (satb_dit_group_graph_forward).
+// edges), and the waits on the previous call (the first layer's WAR, the combine's WAR) are skipped: the previous
+// call was recorded outside the capture, and a graph launch runs only after everything before it on its stream
+// (satb_dit_group_graph_forward).
 template <bool BF16, bool FP8>
 static int group_forward_impl(SatbDitGroup* g, const float* const* x, const float* const* t, float* const* out, int B,
                               int L, float cfg_scale, float scale_phi, cudaStream_t const* st, const int* tb,
-                              bool in_graph) {
-  const int W = g->world, P = g->h[0]->P, N = L + P;
+                              bool split, bool in_graph) {
+  const int W = g->world, NR = split ? 2 * W : W, P = g->h[0]->P, N = L + P;
   const std::vector<cudaEvent_t>& ev_qkv = in_graph ? g->gev_qkv : g->ev_qkv;
   const std::vector<cudaEvent_t>& ev_read = in_graph ? g->gev_read : g->ev_read;
-  const int R = g->h[0]->cfg_on ? 2 * B : B;
+  const std::vector<cudaEvent_t>& ev_y = in_graph ? g->gev_y : g->ev_y;
+  const int R = split ? B : g->h[0]->cfg_on ? 2 * B : B;
   std::vector<DitFwd<BF16, FP8>> f;
-  f.reserve(W);
-  std::vector<const void*> qkv(W);
-  for (int r = 0; r < W; ++r) {
-    const int p = r == 0 ? P : 0, n = tb[r + 1] - tb[r];
-    f.emplace_back(g->h[r], FwdShape{B, R, n - p, p, n, tb[r], N}, st[r]);
+  f.reserve(NR);
+  std::vector<const void*> qkv(NR);
+  for (int r = 0; r < NR; ++r) {
+    const int j = r % W, p = j == 0 ? P : 0, n = tb[j + 1] - tb[j];
+    FwdShape s{B, R, n - p, p, n, tb[j], N};
+    s.half = split ? r / W : -1;
+    f.emplace_back(g->h[r], s, st[r]);
     qkv[r] = g->h[r]->ws_qkv.p;
   }
-  for (int r = 0; r < W; ++r) {
+  for (int r = 0; r < NR; ++r) {
     SATB_CHECK_CUDA(cudaSetDevice(g->dev[r]));
     SATB_PROPAGATE(f[r].input(x[r], t[r]));
   }
   const int D = g->h[0]->D;
   for (int i = 0; i < g->h[0]->depth; ++i) {
-    for (int r = 0; r < W; ++r) {
+    for (int r = 0; r < NR; ++r) {
+      const int row0 = r / W * W;   // the first rank of r's row
       SATB_CHECK_CUDA(cudaSetDevice(g->dev[r]));
       if (!(in_graph && i == 0))
-        for (int s = 0; s < W; ++s) SATB_CHECK_CUDA(cudaStreamWaitEvent(st[r], ev_read[s], 0));   // WAR
+        for (int s = row0; s < row0 + W; ++s) SATB_CHECK_CUDA(cudaStreamWaitEvent(st[r], ev_read[s], 0));   // WAR
       SATB_PROPAGATE(f[r].self_qkv(i));
       SATB_CHECK_CUDA(cudaEventRecord(ev_qkv[r], st[r]));
     }
-    for (int r = 0; r < W; ++r) {
+    for (int r = 0; r < NR; ++r) {
+      const int row0 = r / W * W;
       SATB_CHECK_CUDA(cudaSetDevice(g->dev[r]));
-      for (int s = 0; s < W; ++s) SATB_CHECK_CUDA(cudaStreamWaitEvent(st[r], ev_qkv[s], 0));    // RAW
-      SATB_PROPAGATE(launch_kv_gather(qkv.data(), tb, W, g->kv[r].p, R, D, st[r]));
+      for (int s = row0; s < row0 + W; ++s) SATB_CHECK_CUDA(cudaStreamWaitEvent(st[r], ev_qkv[s], 0));    // RAW
+      SATB_PROPAGATE(launch_kv_gather(qkv.data() + row0, tb, W, g->kv[r].p, R, D, st[r]));
       SATB_CHECK_CUDA(cudaEventRecord(ev_read[r], st[r]));
       SATB_PROPAGATE(f[r].self_attn(i, g->kv[r].as<uint16_t>(), N));
       SATB_PROPAGATE(f[r].block_rest(i));
     }
   }
-  for (int r = 0; r < W; ++r) {
+  if (!split) {
+    for (int r = 0; r < W; ++r) {
+      SATB_CHECK_CUDA(cudaSetDevice(g->dev[r]));
+      SATB_PROPAGATE(f[r].output(out[r], cfg_scale, scale_phi, nullptr));
+    }
+    return 0;
+  }
+  for (int r = W; r < NR; ++r) {   // the unconditional half: project_out only
     SATB_CHECK_CUDA(cudaSetDevice(g->dev[r]));
-    SATB_PROPAGATE(f[r].output(out[r], cfg_scale, scale_phi, nullptr));
+    if (!in_graph) SATB_CHECK_CUDA(cudaStreamWaitEvent(st[r], g->ev_comb[r - W], 0));   // WAR
+    SATB_PROPAGATE(f[r].project_out(nullptr));
+    SATB_CHECK_CUDA(cudaEventRecord(ev_y[r], st[r]));
+  }
+  for (int r = 0; r < W; ++r) {    // the conditional half: project_out, then the combine
+    SATB_CHECK_CUDA(cudaSetDevice(g->dev[r]));
+    SATB_PROPAGATE(f[r].project_out(nullptr));
+    SATB_CHECK_CUDA(cudaStreamWaitEvent(st[r], ev_y[W + r], 0));                          // RAW
+    SATB_PROPAGATE(f[r].combine(out[r], g->h[W + r]->ws_y.as<float>(), cfg_scale, scale_phi));
+    if (!in_graph) SATB_CHECK_CUDA(cudaEventRecord(g->ev_comb[r], st[r]));
   }
   return 0;
 }
 
-extern "C" {
-
-int satb_dit_group_create(SatbDit* const* handles, const int* devices, int world, SatbDitGroup** out) {
-  SATB_REQUIRE(handles && devices && out, "null argument");
-  SATB_REQUIRE(world >= 1 && world <= kKvGatherMaxRanks, "world must be 1 .. 8");
-  for (int r = 0; r < world; ++r) {
+// Checks the handles of one group (satb_dit_group_create: one row; satb_dit_group_create_cfg: two rows) and makes it.
+// refuse_halo: refuse the options whose token convolutions or V scales span the token split (-5).
+static int group_create(SatbDit* const* handles, const int* devices, int world, bool cfg, bool refuse_halo,
+                        SatbDitGroup** out) {
+  const int ranks = cfg ? 2 * world : world;
+  for (int r = 0; r < ranks; ++r) {
     SATB_REQUIRE(handles[r], "null handle");
-    const char* why = group_refusal(handles[r]);
+    const char* why = refuse_halo ? group_refusal(handles[r]) : nullptr;
     if (why) {
       set_last_error(why);
       return -5;
@@ -1439,14 +1498,15 @@ int satb_dit_group_create(SatbDit* const* handles, const int* devices, int world
     for (int s = 0; s < r; ++s)
       SATB_REQUIRE(handles[s] != handles[r], "every rank needs its own handle (its own workspace)");
   }
-  for (int r = 0; r < world; ++r) SATB_REQUIRE(handles[r]->finalized, "weights not finalized");
+  for (int r = 0; r < ranks; ++r) SATB_REQUIRE(handles[r]->finalized, "weights not finalized");
   DeviceRestore restore;
   int n_dev = 0;
   SATB_CHECK_CUDA(cudaGetDeviceCount(&n_dev));
-  for (int r = 0; r < world; ++r) SATB_REQUIRE(devices[r] >= 0 && devices[r] < n_dev, "no such device");
-  // every rank reads every other rank's qkv: peer access between each pair of distinct devices
-  for (int r = 0; r < world; ++r)
-    for (int s = 0; s < world; ++s) {
+  for (int r = 0; r < ranks; ++r) SATB_REQUIRE(devices[r] >= 0 && devices[r] < n_dev, "no such device");
+  // every rank reads every other rank's qkv: peer access between each pair of distinct devices (in a CFG group also
+  // between the rows: the combine reads the other half's y, the graph copies x and t from rank 0's device)
+  for (int r = 0; r < ranks; ++r)
+    for (int s = 0; s < ranks; ++s) {
       if (devices[r] == devices[s]) continue;
       int ok = 0;
       SATB_CHECK_CUDA(cudaDeviceCanAccessPeer(&ok, devices[r], devices[s]));
@@ -1456,9 +1516,9 @@ int satb_dit_group_create(SatbDit* const* handles, const int* devices, int world
         return -1;
       }
     }
-  for (int r = 0; r < world; ++r) {
+  for (int r = 0; r < ranks; ++r) {
     SATB_CHECK_CUDA(cudaSetDevice(devices[r]));
-    for (int s = 0; s < world; ++s) {
+    for (int s = 0; s < ranks; ++s) {
       if (devices[r] == devices[s]) continue;
       const cudaError_t e = cudaDeviceEnablePeerAccess(devices[s], 0);   // this process's context only
       if (e == cudaErrorPeerAccessAlreadyEnabled) {
@@ -1470,18 +1530,22 @@ int satb_dit_group_create(SatbDit* const* handles, const int* devices, int world
   }
   SatbDitGroup* g = new SatbDitGroup();
   g->world = world;
-  g->h.assign(handles, handles + world);
-  g->dev.assign(devices, devices + world);
-  g->kv.resize(world);
-  g->gx.resize(world);
-  g->gt.resize(world);
-  g->gout.resize(world);
-  for (std::vector<cudaEvent_t>* ev : {&g->ev_qkv, &g->ev_read, &g->ev_done, &g->gev_qkv, &g->gev_read, &g->gev_join})
-    ev->assign(world, nullptr);
+  g->cfg = cfg;
+  g->ranks = ranks;
+  g->h.assign(handles, handles + ranks);
+  g->dev.assign(devices, devices + ranks);
+  g->kv.resize(ranks);
+  g->gx.resize(ranks);
+  g->gt.resize(ranks);
+  g->gout.resize(ranks);
+  g->res_R.assign(ranks, 0);
+  g->res_L.assign(ranks, 0);
+  g->res_P.assign(ranks, -1);
+  for (std::vector<cudaEvent_t>* ev : group_events(g)) ev->assign(ranks, nullptr);
   cudaError_t e = cudaSuccess;
-  for (int r = 0; r < world && e == cudaSuccess; ++r) {
+  for (int r = 0; r < ranks && e == cudaSuccess; ++r) {
     e = cudaSetDevice(devices[r]);
-    for (std::vector<cudaEvent_t>* ev : {&g->ev_qkv, &g->ev_read, &g->ev_done, &g->gev_qkv, &g->gev_read, &g->gev_join})
+    for (std::vector<cudaEvent_t>* ev : group_events(g))
       if (e == cudaSuccess) e = cudaEventCreateWithFlags(&(*ev)[r], cudaEventDisableTiming);
   }
   if (e == cudaSuccess) e = cudaSetDevice(devices[0]);
@@ -1491,11 +1555,27 @@ int satb_dit_group_create(SatbDit* const* handles, const int* devices, int world
   if (e != cudaSuccess) {
     group_release(g);
     delete g;
-    set_last_error(std::string("satb_dit_group_create: ") + cudaGetErrorString(e));
+    set_last_error(std::string(cfg ? "satb_dit_group_create_cfg: " : "satb_dit_group_create: ") +
+                   cudaGetErrorString(e));
     return -2;
   }
   *out = g;
   return 0;
+}
+
+extern "C" {
+
+int satb_dit_group_create(SatbDit* const* handles, const int* devices, int world, SatbDitGroup** out) {
+  SATB_REQUIRE(handles && devices && out, "null argument");
+  SATB_REQUIRE(world >= 1 && world <= kKvGatherMaxRanks, "world must be 1 .. 8");
+  return group_create(handles, devices, world, false, true, out);
+}
+
+int satb_dit_group_create_cfg(SatbDit* const* handles, const int* devices, int world, SatbDitGroup** out) {
+  SATB_REQUIRE(handles && devices && out, "null argument");
+  SATB_REQUIRE(world >= 1 && world <= kKvGatherMaxRanks, "world must be 1 .. 8");
+  // a row of one rank holds every token: its token convolutions and FP8 V scales see the whole item
+  return group_create(handles, devices, world, true, world > 1, out);
 }
 
 void satb_dit_group_destroy(SatbDitGroup* g) {
@@ -1506,11 +1586,13 @@ void satb_dit_group_destroy(SatbDitGroup* g) {
 
 }  // extern "C"
 
-// Checks one call's arguments against every rank's conditioning and fills the token split tb.
-static int group_check(SatbDitGroup* g, int B, int L, int* tb) {
+// Checks one call's arguments against the conditioning of every rank it runs and fills the token split tb.  split: a
+// CFG call on a CFG group (both rows run); otherwise only row 0 runs.
+static int group_check(SatbDitGroup* g, int B, int L, int* tb, bool* split) {
   const int W = g->world;
   SatbDit* d0 = g->h[0];
-  for (int r = 0; r < W; ++r) {
+  *split = g->cfg && d0->cfg_on;
+  for (int r = 0; r < (*split ? 2 * W : W); ++r) {
     const SatbDit* d = g->h[r];
     SATB_REQUIRE(d->finalized, "weights not finalized");
     SATB_REQUIRE(B == d->B, "batch size differs from satb_dit_prepare_cond");
@@ -1522,24 +1604,28 @@ static int group_check(SatbDitGroup* g, int B, int L, int* tb) {
   return satb_dit_group_plan(W, d0->P, L, tb);
 }
 
-// Grows every rank's workspace and kv buffer to the call's shape when they do not fit (synchronous when it allocates).
-static int group_reserve(SatbDitGroup* g, int B, int L, const int* tb) {
+// Grows the workspace and kv buffer of every rank the call runs to its shape when they do not fit (synchronous when
+// it allocates).  A rank of a split call runs B rows (its half), else R = 2 B under CFG.
+static int group_reserve(SatbDitGroup* g, int B, int L, const int* tb, bool split) {
   SatbDit* d0 = g->h[0];
-  const int N = L + d0->P, R = d0->cfg_on ? 2 * B : B;
-  const bool fresh = R <= g->res_R && L == g->res_L && d0->P == g->res_P;
-  for (int r = 0; r < g->world; ++r) {
+  const int N = L + d0->P, R = !split && d0->cfg_on ? 2 * B : B;
+  for (int r = 0; r < (split ? 2 * g->world : g->world); ++r) {
     SatbDit* d = g->h[r];
+    const int j = r % g->world;
+    // (the FP8 attention operands are carved for the rows of the last reserve, which may be fewer than res_R)
+    const bool fresh = R <= g->res_R[r] && L == g->res_L[r] && d0->P == g->res_P[r] && (!d->attn_fp8 || R <= d->attn8_R);
     // res_R 0: no single-device forward has reserved since; and the table check of needs_reserve (a reload of the
     // weights marks the position table stale)
-    if (fresh && d->res_R == 0 && !(d->pos_type != 0 && d->pos_len != N)) continue;
-    SATB_CHECK_CUDA(cudaSetDevice(g->dev[r]));
-    SATB_PROPAGATE(reserve_rows(d, R, tb[r + 1] - tb[r], N));
-    SATB_PROPAGATE(g->kv[r].ensure(static_cast<size_t>(R) * N * 2 * d->D * 2));
-    d->res_R = 0;   // the workspace no longer has the single-device forward's shape: its next call reserves again
+    if (!(fresh && d->res_R == 0 && !(d->pos_type != 0 && d->pos_len != N))) {
+      SATB_CHECK_CUDA(cudaSetDevice(g->dev[r]));
+      SATB_PROPAGATE(reserve_rows(d, R, tb[j + 1] - tb[j], N));
+      SATB_PROPAGATE(g->kv[r].ensure(static_cast<size_t>(R) * N * 2 * d->D * 2));
+      d->res_R = 0;   // the workspace no longer has the single-device forward's shape: its next call reserves again
+    }
+    g->res_R[r] = std::max(g->res_R[r], R);
+    g->res_L[r] = L;
+    g->res_P[r] = d0->P;
   }
-  g->res_R = std::max(g->res_R, R);
-  g->res_L = L;
-  g->res_P = d0->P;
   return 0;
 }
 
@@ -1556,20 +1642,21 @@ static void rank_latents(const int* tb, int P, int r, int* lo, int* n) {
   *n = tb[r + 1] - P - *lo;
 }
 
-// One group forward on the ranks' streams: every rank stream first waits for the last graph launch (ev_graph), then
-// the optional input slices, the stages, and the optional output slices.  Eager calls record each rank's ev_done last.
+// One group forward on the streams of the ranks it runs (both rows of a split call, else row 0): every rank stream
+// first waits for the last graph launch (ev_graph), then the optional input slices, the stages, and the optional
+// output slices (row 0's).  Eager calls record each rank's ev_done last.
 static int group_run(SatbDitGroup* g, const float* const* x, const float* const* t, float* const* out, int B, int L,
-                     float cfg_scale, float scale_phi, cudaStream_t const* st, const int* tb, bool in_graph,
+                     float cfg_scale, float scale_phi, cudaStream_t const* st, const int* tb, bool split, bool in_graph,
                      const GroupIo* io) {
-  const int W = g->world;
+  const int W = g->world, NR = split ? 2 * W : W;
   SatbDit* d0 = g->h[0];
   const int P = d0->P, Cin = d0->Cin, C = d0->C;
-  for (int r = 0; r < W; ++r) {
+  for (int r = 0; r < NR; ++r) {
     SATB_CHECK_CUDA(cudaSetDevice(g->dev[r]));
     if (!in_graph) SATB_CHECK_CUDA(cudaStreamWaitEvent(st[r], g->ev_graph, 0));
     if (!io) continue;
     int lo, n;
-    rank_latents(tb, P, r, &lo, &n);
+    rank_latents(tb, P, r % W, &lo, &n);
     if (n > 0)
       SATB_CHECK_CUDA(cudaMemcpy2DAsync(g->gx[r].p, static_cast<size_t>(n) * 4, io->x + lo, static_cast<size_t>(L) * 4,
                                         static_cast<size_t>(n) * 4, static_cast<size_t>(B) * Cin, cudaMemcpyDefault,
@@ -1578,17 +1665,17 @@ static int group_run(SatbDitGroup* g, const float* const* x, const float* const*
   }
   int rc;
   if (d0->fp8)
-    rc = group_forward_impl<false, true>(g, x, t, out, B, L, cfg_scale, scale_phi, st, tb, in_graph);
+    rc = group_forward_impl<false, true>(g, x, t, out, B, L, cfg_scale, scale_phi, st, tb, split, in_graph);
   else if (d0->bf16)
-    rc = group_forward_impl<true, false>(g, x, t, out, B, L, cfg_scale, scale_phi, st, tb, in_graph);
+    rc = group_forward_impl<true, false>(g, x, t, out, B, L, cfg_scale, scale_phi, st, tb, split, in_graph);
   else
-    rc = group_forward_impl<false, false>(g, x, t, out, B, L, cfg_scale, scale_phi, st, tb, in_graph);
+    rc = group_forward_impl<false, false>(g, x, t, out, B, L, cfg_scale, scale_phi, st, tb, split, in_graph);
   SATB_PROPAGATE(rc);
-  for (int r = 0; r < W; ++r) {
+  for (int r = 0; r < NR; ++r) {
     SATB_CHECK_CUDA(cudaSetDevice(g->dev[r]));
     int lo, n;
-    rank_latents(tb, P, r, &lo, &n);
-    if (io && n > 0)
+    rank_latents(tb, P, r % W, &lo, &n);
+    if (io && n > 0 && r < W)
       SATB_CHECK_CUDA(cudaMemcpy2DAsync(io->out + lo, static_cast<size_t>(L) * 4, g->gout[r].p,
                                         static_cast<size_t>(n) * 4, static_cast<size_t>(n) * 4,
                                         static_cast<size_t>(B) * C, cudaMemcpyDefault, st[r]));
@@ -1600,20 +1687,21 @@ static int group_run(SatbDitGroup* g, const float* const* x, const float* const*
 // Enqueues the group forward on g->cap while it captures, ending the capture on every path.  The rank streams fork
 // from g->cap and join it again, so the graph holds every rank's nodes on its own device.
 static int group_capture(SatbDitGroup* g, const float* const* x, const float* const* t, float* const* out, int B,
-                         int L, float cfg_scale, float scale_phi, cudaStream_t const* st, const int* tb,
+                         int L, float cfg_scale, float scale_phi, cudaStream_t const* st, const int* tb, bool split,
                          const GroupIo& io, cudaGraph_t* graph, unsigned long long* launches) {
+  const int NR = split ? 2 * g->world : g->world;
   SATB_CHECK_CUDA(cudaSetDevice(g->dev[0]));
   SATB_CHECK_CUDA(cudaStreamBeginCapture(g->cap, cudaStreamCaptureModeThreadLocal));
   const unsigned long long n0 = g_launch_count;
   int rc = 0;
   cudaError_t e = cudaEventRecord(g->ev_fork, g->cap);
-  for (int r = 0; r < g->world && e == cudaSuccess; ++r) {
+  for (int r = 0; r < NR && e == cudaSuccess; ++r) {
     e = cudaSetDevice(g->dev[r]);
     if (e == cudaSuccess) e = cudaStreamWaitEvent(st[r], g->ev_fork, 0);
   }
   if (e == cudaSuccess) {
-    rc = group_run(g, x, t, out, B, L, cfg_scale, scale_phi, st, tb, true, &io);
-    for (int r = 0; r < g->world && rc == 0 && e == cudaSuccess; ++r) {
+    rc = group_run(g, x, t, out, B, L, cfg_scale, scale_phi, st, tb, split, true, &io);
+    for (int r = 0; r < NR && rc == 0 && e == cudaSuccess; ++r) {
       e = cudaSetDevice(g->dev[r]);
       if (e == cudaSuccess) e = cudaEventRecord(g->gev_join[r], st[r]);
       if (e == cudaSuccess) e = cudaSetDevice(g->dev[0]);
@@ -1643,15 +1731,16 @@ extern "C" {
 int satb_dit_group_forward(SatbDitGroup* g, const float* const* x, const float* const* t, float* const* out, int B,
                            int L, float cfg_scale, float scale_phi, void* const* streams) {
   SATB_REQUIRE(g && x && t && out && streams, "null argument");
-  const int W = g->world;
-  for (int r = 0; r < W; ++r) SATB_REQUIRE(x[r] && t[r] && out[r], "null argument");
   int tb[kKvGatherMaxRanks + 1];
-  SATB_PROPAGATE(group_check(g, B, L, tb));
+  bool split = false;
+  SATB_PROPAGATE(group_check(g, B, L, tb, &split));
+  const int W = g->world, NR = split ? 2 * W : W;
+  for (int r = 0; r < NR; ++r) SATB_REQUIRE(x[r] && t[r] && (r >= W || out[r]), "null argument");
   DeviceRestore restore;
-  SATB_PROPAGATE(group_reserve(g, B, L, tb));
-  cudaStream_t st[kKvGatherMaxRanks];
-  for (int r = 0; r < W; ++r) st[r] = static_cast<cudaStream_t>(streams[r]);
-  return group_run(g, x, t, out, B, L, cfg_scale, scale_phi, st, tb, false, nullptr);
+  SATB_PROPAGATE(group_reserve(g, B, L, tb, split));
+  cudaStream_t st[2 * kKvGatherMaxRanks];
+  for (int r = 0; r < NR; ++r) st[r] = static_cast<cudaStream_t>(streams[r]);
+  return group_run(g, x, t, out, B, L, cfg_scale, scale_phi, st, tb, split, false, nullptr);
 }
 
 // Ordering against eager calls, which may run on distinct devices and alternate with graph launches:
@@ -1661,54 +1750,58 @@ int satb_dit_group_forward(SatbDitGroup* g, const float* const* x, const float* 
 //   * after each launch, ev_graph is recorded on home_stream, and every eager call makes each rank stream wait for
 //     it before its first launch (group_run), so an eager call never overwrites what the graph still reads.
 // The graph's own cross-rank hazards are the eager path's event pairs, captured as edges; successive launches on one
-// stream run one after the other, which stands for the first layer's WAR waits.  With virtual ranks everything is on
-// one device, so these waits are ordinary same-device waits there; between devices they are the same events.
+// stream run one after the other, which stands for the first layer's WAR waits (and, in a CFG group, the combine's).
+// With virtual ranks everything is on one device, so these waits are ordinary same-device waits there; between devices
+// they are the same events.  In a CFG group both rows count as ranks here.
 int satb_dit_group_graph_forward(SatbDitGroup* g, const float* x, const float* t, float* out, int B, int L,
                                  float cfg_scale, float scale_phi, void* const* rank_streams, void* home_stream) {
   SATB_REQUIRE(g && x && t && out && rank_streams, "null argument");
-  const int W = g->world;
-  for (int r = 0; r < W; ++r)
+  const int W = g->world, NH = g->ranks;
+  for (int r = 0; r < NH; ++r)
     SATB_REQUIRE(rank_streams[r], "rank streams must be created streams (the legacy default stream cannot be captured)");
-  for (int r = 0; r < W; ++r)
+  for (int r = 0; r < NH; ++r)
     SATB_REQUIRE(!g->h[r]->prof_on, "satb_dit_group_graph_forward: profiling (satb_dit_profile) is on for a rank; "
                                     "its event timing cannot be captured");
   int tb[kKvGatherMaxRanks + 1];
-  SATB_PROPAGATE(group_check(g, B, L, tb));
+  bool split = false;
+  SATB_PROPAGATE(group_check(g, B, L, tb, &split));
+  const int NR = split ? 2 * W : W;
   DeviceRestore restore;
-  cudaStream_t st[kKvGatherMaxRanks];
-  for (int r = 0; r < W; ++r) st[r] = static_cast<cudaStream_t>(rank_streams[r]);
+  cudaStream_t st[2 * kKvGatherMaxRanks];
+  for (int r = 0; r < NH; ++r) st[r] = static_cast<cudaStream_t>(rank_streams[r]);
   cudaStream_t home = static_cast<cudaStream_t>(home_stream);
   GraphKey key;
   key.x = x; key.t = t; key.out = out; key.B = B; key.L = L; key.cfg_scale = cfg_scale; key.scale_phi = scale_phi;
-  bool stale = !g->exec || !(key == g->key) || static_cast<int>(g->gens.size()) != W;
-  for (int r = 0; r < W && !stale; ++r) stale = g->gens[r] != g->h[r]->gen;
+  bool stale = !g->exec || !(key == g->key) || static_cast<int>(g->gens.size()) != NH;
+  for (int r = 0; r < NH && !stale; ++r) stale = g->gens[r] != g->h[r]->gen;
   if (stale) {
     group_drop_graph(g);
     SatbDit* d0 = g->h[0];
     const GroupIo io{x, t, out};
-    const float* xs[kKvGatherMaxRanks];
-    const float* ts[kKvGatherMaxRanks];
-    float* os[kKvGatherMaxRanks];
-    for (int r = 0; r < W; ++r) {   // the fixed per-rank slices (at least 256 bytes: a rank may hold no latent token)
+    const float* xs[2 * kKvGatherMaxRanks];
+    const float* ts[2 * kKvGatherMaxRanks];
+    float* os[2 * kKvGatherMaxRanks] = {};
+    for (int r = 0; r < NR; ++r) {   // the fixed per-rank slices (at least 256 bytes: a rank may hold no latent token)
       int lo, n;
-      rank_latents(tb, d0->P, r, &lo, &n);
+      rank_latents(tb, d0->P, r % W, &lo, &n);
       SATB_CHECK_CUDA(cudaSetDevice(g->dev[r]));
       SATB_PROPAGATE(g->gx[r].ensure(std::max<size_t>(static_cast<size_t>(B) * d0->Cin * n * 4, 256)));
       SATB_PROPAGATE(g->gt[r].ensure(std::max<size_t>(static_cast<size_t>(B) * 4, 256)));
-      SATB_PROPAGATE(g->gout[r].ensure(std::max<size_t>(static_cast<size_t>(B) * d0->C * n * 4, 256)));
       xs[r] = g->gx[r].as<float>();
       ts[r] = g->gt[r].as<float>();
+      if (r >= W) continue;          // only row 0 writes output
+      SATB_PROPAGATE(g->gout[r].ensure(std::max<size_t>(static_cast<size_t>(B) * d0->C * n * 4, 256)));
       os[r] = g->gout[r].as<float>();
     }
     // warm-up: one eager call at this shape, so that nothing allocates, makes a tensor map or sets a function
     // attribute during the capture.  The rank streams start after home_stream's work so far (the caller's inputs).
-    SATB_PROPAGATE(group_reserve(g, B, L, tb));
+    SATB_PROPAGATE(group_reserve(g, B, L, tb, split));
     SATB_CHECK_CUDA(cudaSetDevice(g->dev[0]));
     SATB_CHECK_CUDA(cudaEventRecord(g->ev_graph, home));
-    SATB_PROPAGATE(group_run(g, xs, ts, os, B, L, cfg_scale, scale_phi, st, tb, false, &io));
+    SATB_PROPAGATE(group_run(g, xs, ts, os, B, L, cfg_scale, scale_phi, st, tb, split, false, &io));
     cudaGraph_t graph = nullptr;
     unsigned long long launches = 0;
-    SATB_PROPAGATE(group_capture(g, xs, ts, os, B, L, cfg_scale, scale_phi, st, tb, io, &graph, &launches));
+    SATB_PROPAGATE(group_capture(g, xs, ts, os, B, L, cfg_scale, scale_phi, st, tb, split, io, &graph, &launches));
     SATB_CHECK_CUDA(cudaSetDevice(g->dev[0]));
     const cudaError_t e = cudaGraphInstantiate(&g->exec, graph, 0);
     cudaGraphDestroy(graph);
@@ -1719,13 +1812,13 @@ int satb_dit_group_graph_forward(SatbDitGroup* g, const float* x, const float* t
       return -3;
     }
     g->key = key;
-    g->gens.resize(W);
-    for (int r = 0; r < W; ++r) g->gens[r] = g->h[r]->gen;
+    g->gens.resize(NH);
+    for (int r = 0; r < NH; ++r) g->gens[r] = g->h[r]->gen;
     g->graph_launches = launches;
     ++g->captures;
   }
   SATB_CHECK_CUDA(cudaSetDevice(g->dev[0]));
-  for (int r = 0; r < W; ++r) SATB_CHECK_CUDA(cudaStreamWaitEvent(home, g->ev_done[r], 0));
+  for (int r = 0; r < NH; ++r) SATB_CHECK_CUDA(cudaStreamWaitEvent(home, g->ev_done[r], 0));
   SATB_CHECK_CUDA(cudaGraphLaunch(g->exec, home));
   SATB_CHECK_CUDA(cudaEventRecord(g->ev_graph, home));
   g_launch_count += g->graph_launches;

@@ -409,11 +409,12 @@ __global__ void gate_sigmoid_kernel(float* __restrict__ ssg, int depth, int D) {
 // ------------------------------------------------------------------ DiT post
 // models/dit.py:219 (drop prepend), :338-347 (CFG combine, std rescale over channels).
 // y rows are token-major [R*N_seq, ldy] (ldy >= C: project_out's N padded up to its store width; only the C real
-// channels are read); one thread per (b, l).  C = 1 with scale_phi != 0 gives NaN, as torch.std (unbiased) of one
+// channels are read); one thread per (b, l).  yu: the unconditional rows [B*N_seq, ldy] of the CFG combine (read only
+// when cfg): y + B*N_seq*ldy when both halves are in y, or the unconditional half's own y (a peer pointer allowed).  C = 1 with scale_phi != 0 gives NaN, as torch.std (unbiased) of one
 // channel does in the reference.
-__global__ void __launch_bounds__(128) dit_post_kernel(const float* __restrict__ y, int ldy, float* __restrict__ out,
-                                                       int B, int C, int L, int N_seq, int P, int cfg, float cfg_scale,
-                                                       float scale_phi) {
+__global__ void __launch_bounds__(128) dit_post_kernel(const float* __restrict__ y, const float* __restrict__ yu_rows,
+                                                       int ldy, float* __restrict__ out, int B, int C, int L, int N_seq,
+                                                       int P, int cfg, float cfg_scale, float scale_phi) {
   const int l = blockIdx.x * blockDim.x + threadIdx.x;
   const int b = blockIdx.y;
   if (l >= L) return;
@@ -423,7 +424,7 @@ __global__ void __launch_bounds__(128) dit_post_kernel(const float* __restrict__
     for (int c = 0; c < C; ++c) o[static_cast<size_t>(c) * L] = yc[c];
     return;
   }
-  const float* yu = y + (static_cast<size_t>(B + b) * N_seq + P + l) * ldy;
+  const float* yu = yu_rows + (static_cast<size_t>(b) * N_seq + P + l) * ldy;
   if (scale_phi == 0.f) {
     for (int c = 0; c < C; ++c) {
       const float cv = yc[c], uv = yu[c];
@@ -689,11 +690,12 @@ int launch_gate_sigmoid(float* ssg, int rows, int depth, int D, cudaStream_t str
   return 0;
 }
 
-int launch_dit_post(const float* y, int ldy, float* out, int B, int C, int L, int N_seq, int P, int cfg,
+int launch_dit_post(const float* y, const float* yu, int ldy, float* out, int B, int C, int L, int N_seq, int P, int cfg,
                     float cfg_scale, float scale_phi, cudaStream_t stream) {
   SATB_REQUIRE(ldy >= C, "dit_post: the row pitch must cover the channels");
+  SATB_REQUIRE(!cfg || yu, "dit_post: the CFG combine needs the unconditional rows");
   dim3 grid(ceil_div(L, 128), B);
-  dit_post_kernel<<<grid, 128, 0, stream>>>(y, ldy, out, B, C, L, N_seq, P, cfg, cfg_scale, scale_phi);
+  dit_post_kernel<<<grid, 128, 0, stream>>>(y, yu, ldy, out, B, C, L, N_seq, P, cfg, cfg_scale, scale_phi);
   count_launch();
   SATB_CHECK_CUDA(cudaGetLastError());
   return 0;

@@ -84,8 +84,10 @@ int launch_write_prepend(const float* tok, const float* pre, const float* pos, f
                          int Pp, cudaStream_t stream);
 // in place: x = sigmoid(1 - x) on column ranges [c0, c0+D) and [c1, c1+D) of every 6D-wide layer block
 int launch_gate_sigmoid(float* ssg, int rows, int depth, int D, cudaStream_t stream);
-// y[R*N_seq, ldy] fp32 (its first C columns) -> out[B, C, L] with CFG combine / rescale (models/dit.py:338-347)
-int launch_dit_post(const float* y, int ldy, float* out, int B, int C, int L, int N_seq, int P, int cfg,
+// y[B*N_seq, ldy] fp32 (its first C columns) -> out[B, C, L] with CFG combine / rescale (models/dit.py:338-347);
+// cfg: yu[B*N_seq, ldy] holds the unconditional rows (y + B*N_seq*ldy in the batched CFG forward, or the other
+// half's y in the CFG-split group forward)
+int launch_dit_post(const float* y, const float* yu, int ldy, float* out, int B, int C, int L, int N_seq, int P, int cfg,
                     float cfg_scale, float scale_phi, cudaStream_t stream);
 // generic fp32 -> 16-bit cast with row gather: dst[r, :] = src[perm ? perm[r] : r, :] * row_scale
 int launch_cast_rows(const float* src, void* dst, const int* perm, int rows, int cols, int64_t src_ld, int64_t dst_ld,

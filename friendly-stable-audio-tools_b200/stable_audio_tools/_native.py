@@ -123,6 +123,7 @@ SIGNATURES = {
     "satb_dit_forward_debug": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _F, _F, _VP]),
     "satb_dit_group_plan": (_I, [_I, _I, _I, _VP]),
     "satb_dit_group_create": (_I, [_VP, _VP, _I, ctypes.POINTER(_VP)]),
+    "satb_dit_group_create_cfg": (_I, [_VP, _VP, _I, ctypes.POINTER(_VP)]),
     "satb_dit_group_destroy": (None, [_VP]),
     "satb_dit_group_forward": (_I, [_VP, _VP, _VP, _VP, _I, _I, _F, _F, _VP]),
     "satb_dit_group_graph_forward": (_I, [_VP, _VP, _VP, _VP, _I, _I, _F, _F, _VP, _VP]),

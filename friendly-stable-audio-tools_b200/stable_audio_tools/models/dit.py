@@ -23,7 +23,10 @@ and parameter names, ``forward`` signature and CFG semantics); the arithmetic ru
 * ``shard_tokens(devices)`` splits every call's tokens over several ranks (``satb_dit_group_*``): each rank holds a full
   copy of the weights and a contiguous range of every item's tokens, and gathers every rank's self-attention K / V once
   per layer, so one prompt can use several GPUs; with ``cuda_graph`` the whole sharded call is replayed from one
-  multi-device CUDA graph the library captures and owns (``satb_dit_group_graph_forward``).
+  multi-device CUDA graph the library captures and owns (``satb_dit_group_graph_forward``);
+* ``shard_tokens([[...], [...]])`` also splits every CFG call by guidance half (``satb_dit_group_create_cfg``): row 0
+  runs the conditional rows and row 1 the unconditional ones, each token-sharded over its own devices, and the halves
+  meet once per call, in the combine.
 
 There is no eager / CPU fallback: tensors must live on a CUDA device.
 """
@@ -322,24 +325,54 @@ class DiffusionTransformer(nn.Module):
         would need the neighbouring ranks' tokens), ``attention_dtype="fp8"`` (its V channel scales span all of an
         item's tokens) and, at call time, ``return_info``.  Ranks on distinct GPUs need peer-to-peer access between them.
 
+        Two rows, ``[[a, b], [c, d]]``, split each classifier-free-guidance call by half as well (CFG split): row 0 runs
+        the conditional rows and row 1 the unconditional rows, each token-sharded over its own devices by the same plan,
+        and row 0 combines the two halves' outputs, the only exchange between the rows.  The rows have equal lengths of
+        1 to 8 devices; the home device is ``devices[0][0]``.  A call without CFG (``cfg_scale == 1``, or neither
+        cross-attention nor prepend conditioning) runs on row 0 only, as ``shard_tokens(row 0)`` would.  The refusals
+        above apply only when a row has more than one device: ``[[a], [b]]`` runs every model option.
+
         With ``cuda_graph`` off, each call enqueues every rank's launches eagerly.  With it on (the multistep SDE samplers
         and the v-diffusion ``sample`` switch it on), each call is one launch of a multi-device CUDA graph
         (``satb_dit_group_graph_forward``): it copies the ranks' slices of the input in, runs the sharded forward and
         copies the slices of the output back, and returns a static buffer on the home device that the next call
         overwrites.  The library captures it on the first call and again whenever the shape, the guidance scalars, the
         conditioning, the weights or a workspace change, and orders it against eager sharded calls itself."""
+        cfg_split = False
         if devices is not None:
-            if self.conformer:
-                raise NotImplementedError("shard_tokens: conformer blocks are not supported (their depthwise convolution "
-                                          "needs the neighbouring ranks' tokens)")
-            if self.ff_spec[2] > 0:
-                raise NotImplementedError("shard_tokens: use_conv feed-forwards are not supported (their token "
-                                          "convolution needs the neighbouring ranks' tokens)")
-            if self.attention_dtype == "fp8":
-                raise NotImplementedError("shard_tokens: attention_dtype='fp8' is not supported (its V channel scales "
-                                          "span all of an item's tokens)")
+            devices = list(devices)
+            nested = [isinstance(dv, (list, tuple)) for dv in devices]
+            if any(nested):
+                if not all(nested):
+                    raise ValueError("shard_tokens: give a flat list of devices or two rows of devices, not a mix")
+                if len(devices) != 2:
+                    raise ValueError(f"shard_tokens: a CFG split takes two rows of devices (conditional, unconditional), "
+                                     f"got {len(devices)}")
+                rows = [list(row) for row in devices]
+                if any(isinstance(dv, (list, tuple)) for row in rows for dv in row):
+                    raise ValueError("shard_tokens: each row is a list of devices (no deeper nesting)")
+                if len(rows[0]) != len(rows[1]):
+                    raise ValueError(f"shard_tokens: the two rows need the same length, got {len(rows[0])} and "
+                                     f"{len(rows[1])}")
+                if not 1 <= len(rows[0]) <= 8:
+                    raise ValueError(f"shard_tokens: 1 to 8 devices per row, got {len(rows[0])}")
+                cfg_split = True
+                world = len(rows[0])
+                devices = rows[0] + rows[1]
+            else:
+                world = len(devices)
+            if world > 1 or not cfg_split:      # a CFG row of one device holds every token
+                if self.conformer:
+                    raise NotImplementedError("shard_tokens: conformer blocks are not supported (their depthwise "
+                                              "convolution needs the neighbouring ranks' tokens)")
+                if self.ff_spec[2] > 0:
+                    raise NotImplementedError("shard_tokens: use_conv feed-forwards are not supported (their token "
+                                              "convolution needs the neighbouring ranks' tokens)")
+                if self.attention_dtype == "fp8":
+                    raise NotImplementedError("shard_tokens: attention_dtype='fp8' is not supported (its V channel "
+                                              "scales span all of an item's tokens)")
             devices = [torch.device(dv) for dv in devices]
-            if not 1 <= len(devices) <= 8:
+            if not 1 <= world <= 8:
                 raise ValueError(f"shard_tokens: 1 to 8 devices, got {len(devices)}")
             for dv in devices:
                 if dv.type != "cuda":
@@ -347,8 +380,8 @@ class DiffusionTransformer(nn.Module):
             devices = [dv if dv.index is not None else torch.device("cuda", torch.cuda.current_device()) for dv in devices]
         self._drop_shards()
         if devices is not None:
-            self.__dict__["_shard"] = dict(devices=devices, handles=None, group=None, streams=None, cond_key=None,
-                                           keepalive=None, graph_io=None)
+            self.__dict__["_shard"] = dict(devices=devices, world=world, cfg_split=cfg_split, handles=None, group=None,
+                                           streams=None, cond_key=None, keepalive=None, graph_io=None)
             self.__dict__["_shard_dirty"] = True
         return self
 
@@ -402,7 +435,8 @@ class DiffusionTransformer(nn.Module):
         g = ctypes.c_void_p()
         handles = (ctypes.c_void_p * len(devs))(*[h.value for h in sh["handles"]])
         ids = (ctypes.c_int * len(devs))(*[dv.index for dv in devs])
-        _native.check(lib.satb_dit_group_create(handles, ids, len(devs), ctypes.byref(g)))
+        create = lib.satb_dit_group_create_cfg if sh["cfg_split"] else lib.satb_dit_group_create
+        _native.check(create(handles, ids, sh["world"], ctypes.byref(g)))
         sh["group"] = g
         if sh["streams"] is None:
             sh["streams"] = [torch.cuda.Stream(device=dv) for dv in devs]
@@ -434,22 +468,27 @@ class DiffusionTransformer(nn.Module):
         g = self._sharded_prepare(sh, x, cross, neg, glob, prepend, use_cfg)
         B, _, L = x.shape
         P = 0 if self.global_cond_type == "adaLN" else 1 + (prepend.shape[1] if prepend is not None else 0)
-        tb = _native.group_plan(len(devs), P, L)
+        W = sh["world"]
+        tb = _native.group_plan(W, P, L)
+        # the ranks this call runs: both rows of a CFG split under CFG, else row 0; row 0 writes the output
+        run = devs if sh["cfg_split"] and use_cfg else devs[:W]
         xin = x.detach().to(torch.float32)
         tin = t.detach().to(torch.float32).contiguous()
         xs, ts, outs = [], [], []
-        for r, dv in enumerate(devs):
-            lo, hi = max(tb[r] - P, 0), tb[r + 1] - P          # this rank's latent tokens
+        for r, dv in enumerate(run):
+            lo, hi = max(tb[r % W] - P, 0), tb[r % W + 1] - P  # this rank's latent tokens
             with torch.cuda.device(dv):
                 xs.append(xin[:, :, lo:hi].to(dv).contiguous())
                 ts.append(tin.to(dv))
-                outs.append(torch.empty(B, self.io_channels * self.patch_size, hi - lo, device=dv, dtype=torch.float32))
+                if r < W:
+                    outs.append(torch.empty(B, self.io_channels * self.patch_size, hi - lo, device=dv,
+                                            dtype=torch.float32))
                 sh["streams"][r].wait_stream(torch.cuda.current_stream(dv))
         ptrs = lambda ts_: (ctypes.c_void_p * len(devs))(*[q.data_ptr() for q in ts_])
         streams = (ctypes.c_void_p * len(devs))(*[s_.cuda_stream for s_ in sh["streams"]])
         _native.check(lib.satb_dit_group_forward(g, ptrs(xs), ptrs(ts), ptrs(outs), B, L, float(cfg_scale),
                                                  float(scale_phi), streams))
-        for r, dv in enumerate(devs):
+        for r, dv in enumerate(run):
             torch.cuda.current_stream(dv).wait_stream(sh["streams"][r])
         return torch.cat([o.to(home) for o in outs], dim=2)
 

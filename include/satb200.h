@@ -156,15 +156,30 @@ int satb_dit_group_plan(int world, int n_prepend, int L, int* token_begin);
  * every handle, with the same conditioning, before satb_dit_group_forward.  The handles outlive the group, which must
  * be destroyed explicitly. */
 int satb_dit_group_create(SatbDit* const* handles, const int* devices, int world, SatbDitGroup** out);
+/* The CFG-split group: two rows of `world` ranks (1 .. 8 each), handles[2 world] and devices[2 world] holding row 0's
+ * ranks, then row 1's.  A CFG call (the handles' conditioning prepared with use_cfg) runs its conditional rows on row
+ * 0 and its unconditional rows on row 1, each row token-sharded over its own ranks by satb_dit_group_plan(world, ...),
+ * so the two halves exchange nothing until the combine: row-0 rank j reads row-1 rank j's project_out output (same
+ * tokens) through a peer pointer and writes the guided output; row 1 writes none.  Every rank keeps the conditioning
+ * of the batched CFG forward and uses the rows of its half (cross-attention K / V, prepend tokens, adaLN rows), so each
+ * half computes what the batched forward computes for those rows.  A call without CFG runs row 0 only, as the group of
+ * satb_dit_group_create(row 0's handles) would.  Conformer blocks, use_conv feed-forwards and FP8 self-attention are
+ * refused with -5 only when world > 1 (a row of one rank holds every token).  Peer access is needed, and enabled,
+ * between every pair of distinct devices.  The group takes the same forward, graph, reset, stats and destroy calls as
+ * a satb_dit_group_create group; its graph is captured again when any of the 2 world handles changes. */
+int satb_dit_group_create_cfg(SatbDit* const* handles, const int* devices, int world, SatbDitGroup** out);
 void satb_dit_group_destroy(SatbDitGroup* g);
 /* One denoiser call over the ranks: x[r] [B, C, L_r] and out[r] [B, io_channels, L_r], rank r's latent tokens (L_r =
  * token_begin[r + 1] - token_begin[r], less n_prepend on rank 0), and t[r] [B], all on rank r's device; streams[r] is
- * rank r's stream.  Enqueues only (ranks are ordered with events); the caller's current device is restored. */
+ * rank r's stream.  Enqueues only (ranks are ordered with events); the caller's current device is restored.  On a
+ * satb_dit_group_create_cfg group, x, t and streams hold 2 world entries (row 0's ranks, then row 1's; row 1's x and t
+ * are read by CFG calls only and may be null otherwise) and out holds world entries, row 0's. */
 int satb_dit_group_forward(SatbDitGroup* g, const float* const* x, const float* const* t, float* const* out, int B,
                            int L, float cfg_scale, float scale_phi, void* const* streams);
 /* The same call replayed from one CUDA graph whose nodes live on every rank's device: one cudaGraphLaunch on
  * home_stream.  x [B, C, L], t [B] and out [B, io_channels, L] are whole tensors on rank 0's device, at addresses the
- * caller keeps fixed; rank_streams[r] (created streams, on rank r's device) are used while capturing.  The graph copies
+ * caller keeps fixed; rank_streams[r] (created streams, on rank r's device; 2 world of them for a CFG group) are used
+ * while capturing.  The graph copies
  * each rank's slice of x and t in, runs the group forward and copies each rank's slice of out back.  The first call,
  * and every call after the key (x, t, out, B, L, cfg_scale, scale_phi) changed or after any handle's weights,
  * conditioning or workspaces may have moved (satb_dit_finalize, satb_dit_set_prepend_cond, satb_dit_prepare_cond, a
