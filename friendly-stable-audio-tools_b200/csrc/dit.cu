@@ -47,6 +47,9 @@ struct LayerW {
   // FP8 mode: e4m3 copies of to_qkv, cross_attn.to_q and ff.0 (in place of their 16-bit ones) and their row scales
   uint8_t *w8_qkv = nullptr, *w8_q = nullptr, *w8_ff1 = nullptr;
   float *s_qkv = nullptr, *s_q = nullptr, *s_ff1 = nullptr;
+  // FP8 FF-out option (satb_dit_set_ff_out_fp8): the e4m3 copy of ff.2 (in place of w_ff2) and its row scales
+  uint8_t* w8_ff2 = nullptr;
+  float* s_ff2 = nullptr;
   // conformer branch (satb_dit_set_conformer): in_norm, glu.proj folded with pointwise_conv (16-bit, SwiGLU row
   // interleave, bias interleaved alike), depthwise_conv [D][17] fp32, mid_norm, pointwise_conv_2 (16-bit)
   float *cf_in_g = nullptr, *cf_in_b = nullptr, *cf_b1 = nullptr, *cf_dw = nullptr, *cf_mid_g = nullptr,
@@ -74,6 +77,7 @@ struct SatbDit {
   bool bf16, fp8, adaln, qk_norm = false;   // fp8: e4m3 operands for the QKV, cross q and FF-in GEMMs (fp16 elsewhere)
   bool conformer = false;     // every block runs the conformer branch (satb_dit_set_conformer)
   bool attn_fp8 = false;      // self-attention with e4m3 q, k, v and P (satb_dit_set_attention_fp8)
+  bool ff_out_fp8 = false;    // FF-out on e4m3 operands, 1 x 128 block scales for the activations (satb_dit_set_ff_out_fp8)
   int* cf_perm = nullptr;     // SwiGLU row interleave of the folded [2D, D] conformer GLU weight
   // feed-forward (satb_dit_set_feedforward; default: SwiGLU Linear, inner 4D, biased).  ffi above is ff_inner padded up
   // to a multiple of 64.  ff_k: kernel size of the token convolutions, 0 = Linear (with ff_glu, FF-out only).  ff_bias:
@@ -259,6 +263,10 @@ static int load_ff_weight(SatbDit* d, LayerW& L, const std::string& name, const 
     if (!L.w8_ff1) rc = d->alloc(&L.w8_ff1, static_cast<size_t>(rows) * in_p);
     if (rc == 0 && !L.s_ff1) rc = d->alloc(&L.s_ff1, rows);
     if (rc == 0) rc = launch_quant_rows_fp8(tmp, L.w8_ff1, L.s_ff1, G == 2 ? d->ff_perm : nullptr, rows, in_p, st);
+  } else if (rc == 0 && what == W_OUT && d->ff_out_fp8) {   // e4m3 rows; the zero pad columns leave the scales alone
+    if (!L.w8_ff2) rc = d->alloc(&L.w8_ff2, static_cast<size_t>(rows) * in_p);
+    if (rc == 0 && !L.s_ff2) rc = d->alloc(&L.s_ff2, rows);
+    if (rc == 0) rc = launch_quant_rows_fp8(tmp, L.w8_ff2, L.s_ff2, nullptr, rows, in_p, st);
   } else if (rc == 0) {
     if (!*w16) rc = d->alloc(w16, static_cast<size_t>(rows) * in_p);
     if (rc == 0) rc = launch_cast_rows(tmp, *w16, G == 2 ? d->ff_perm : nullptr, rows, in_p, in_p, in_p, d->bf16, st);
@@ -400,6 +408,23 @@ int satb_dit_set_attention_fp8(SatbDit* d, int enable) {
   return 0;
 }
 
+// FP8 FF-out (DESIGN.md sections 3-5): call before the first satb_dit_load_weight, after satb_dit_set_feedforward.
+int satb_dit_set_ff_out_fp8(SatbDit* d, int enable) {
+  SATB_REQUIRE(d, "null handle");
+  SATB_REQUIRE(enable == 0 || enable == 1, "enable must be 0 or 1");
+  SATB_REQUIRE(d->loaded.empty(), "satb_dit_set_ff_out_fp8 must be called before the first weight is loaded (it decides "
+                                  "how ff.ff.2.weight is stored)");
+  if (enable) {
+    SATB_REQUIRE(d->fp8, "the FP8 FF-out option needs operand_dtype 2 (fp8)");
+    SATB_REQUIRE(d->ff_k == 0, "the FP8 FF-out option is not supported with use_conv feed-forwards (FF-out is a token "
+                               "convolution there)");
+    SATB_REQUIRE(d->ffi % 128 == 0, ("the FP8 FF-out option needs a feed-forward inner width that is a multiple of 128 "
+                                     "(padded to 64 it is " + std::to_string(d->ffi) + ")").c_str());
+  }
+  d->ff_out_fp8 = enable != 0;
+  return 0;
+}
+
 void satb_dit_destroy(SatbDit* d) {
   if (!d) return;
   for (void* p : d->owned) cudaFree(p);
@@ -509,7 +534,8 @@ int satb_dit_load_weight(SatbDit* d, const char* name_c, const float* src, long 
       if (!L.b_ff1) SATB_PROPAGATE(d->alloc(&L.b_ff1, 2 * d->ffi));
       return launch_gather_f32(src, L.b_ff1, d->ff_perm, 2 * d->ffi, st);
     }
-    if (k == "ff.ff.2.weight") return cast16(&L.w_ff2, D, d->ffi, nullptr);
+    if (k == "ff.ff.2.weight")
+      return d->ff_out_fp8 ? quant8(&L.w8_ff2, &L.s_ff2, D, d->ffi, nullptr) : cast16(&L.w_ff2, D, d->ffi, nullptr);
     if (k == "ff.ff.2.bias") return copy_f32(&L.b_ff2, D);
     if (k == "to_scale_shift_gate.1.weight") {
       SATB_REQUIRE(numel == 6LL * D * D, ("bad size for " + name).c_str());
@@ -584,7 +610,7 @@ int satb_dit_finalize(SatbDit* d, void* stream_v) {
       need(in8 ? L.w8_ff1 != nullptr : L.w_ff1 != nullptr, d->ff_glu ? "0.proj.weight" : "0.1.weight");
       if (d->ff_glu) need(L.b_ff1 != nullptr, "0.proj.bias");
       else if (d->ff_bias) need(L.b_ff1 != nullptr, "0.1.bias");
-      need(L.w_ff2 != nullptr, "2.weight");
+      need(d->ff_out_fp8 ? L.w8_ff2 != nullptr : L.w_ff2 != nullptr, "2.weight");
       if (d->ff_bias) need(L.b_ff2 != nullptr, "2.bias");
       if (!miss.empty()) {
         set_last_error("feed-forward weights missing in layer " + std::to_string(i) + ": " + miss);
@@ -598,6 +624,9 @@ int satb_dit_finalize(SatbDit* d, void* stream_v) {
     return -1;
   }
   if (d->pos_type == 2) SATB_REQUIRE(d->pos_emb, "absolute positional embedding missing: transformer.pos_emb.emb.weight");
+  // satb_dit_set_feedforward may follow satb_dit_set_ff_out_fp8
+  SATB_REQUIRE(!d->ff_out_fp8 || (d->ff_k == 0 && d->ffi % 128 == 0),
+               "the FP8 FF-out option needs a Linear feed-forward whose inner width is a multiple of 128");
   SATB_REQUIRE(d->ts_w && d->te0_w && d->te0_b && d->te2_w && d->te2_b, "timestep embedding weights missing");
   SATB_REQUIRE(d->pin_w && d->pout_w && d->pre_w && d->post_w, "project_in/out or pre/post conv weights missing");
   if (d->rotary) SATB_REQUIRE(d->inv_freq, "rotary inv_freq missing");
@@ -608,7 +637,8 @@ int satb_dit_finalize(SatbDit* d, void* stream_v) {
     const LayerW& L = d->layers[i];
     const bool ff_in8 = d->fp8 && !d->ff_conv_in();   // a token-convolution FF-in keeps 16-bit weights in every mode
     SATB_REQUIRE(L.pre_g && L.ff_g && (d->fp8 ? L.w8_qkv != nullptr : L.w_qkv != nullptr) &&
-                     (ff_in8 ? L.w8_ff1 != nullptr : L.w_ff1 != nullptr) && L.w_o && L.w_ff2,
+                     (ff_in8 ? L.w8_ff1 != nullptr : L.w_ff1 != nullptr) && L.w_o &&
+                     (d->ff_out_fp8 ? L.w8_ff2 != nullptr : L.w_ff2 != nullptr),
                  "transformer layer weights missing");
     if (d->ct > 0)
       SATB_REQUIRE(L.ca_g && (d->fp8 ? L.w8_q != nullptr : L.w_q != nullptr) && L.w_kv && L.w_co,
@@ -726,7 +756,8 @@ static int reserve_rows(SatbDit* d, int R, int n, int tab_len) {
   SATB_PROPAGATE(d->ws_qkv.ensure(M * 3 * D * 2));
   SATB_PROPAGATE(d->ws_attn.ensure(M * D * 2));
   SATB_PROPAGATE(d->ws_q16.ensure(M * D * 2));
-  // the FF intermediate [M, ffi], and the conformer branch's two [M, D] intermediates
+  // the FF intermediate [M, ffi] (FP8 FF-out: e4m3 [M, ffi], then its scales [M, ffi / 128], in fewer bytes), and the
+  // conformer branch's two [M, D] intermediates
   SATB_PROPAGATE(d->ws_ff.ensure(M * std::max(d->ffi, d->conformer ? 2 * D : 0) * 2));
   SATB_PROPAGATE(d->ws_ain.ensure(M * d->Cin_p * 2));
   SATB_PROPAGATE(d->ws_y.ensure(M * d->C_p * 4));
@@ -929,6 +960,7 @@ struct DitFwd {
   float* a_scale;
   const void* a_in;
   uint16_t *qkv, *att, *q16, *ff, *ain;
+  BlockE4m3Out ff8;     // FP8 FF-out: the e4m3 FF intermediate and its block scales, in ws_ff in place of ff
   float* y;
   const float *cos_tab, *sin_tab, *pos_tab;
 
@@ -951,6 +983,8 @@ struct DitFwd {
     att = d->ws_attn.as<uint16_t>();
     q16 = d->ws_q16.as<uint16_t>();
     ff = d->ws_ff.as<uint16_t>();
+    uint8_t* ff_bytes = d->ws_ff.as<uint8_t>();
+    ff8 = BlockE4m3Out{ff_bytes, reinterpret_cast<float*>(ff_bytes + static_cast<size_t>(M) * d->ffi), d->ffi};
     ain = d->ws_ain.as<uint16_t>();
     y = d->ws_y.as<float>();
     // rotary off (satb_dit_set_positions): null tables, which the QKV epilogues take as no rotation
@@ -1140,7 +1174,15 @@ struct DitFwd {
     {
       ProfScope ps(d, PROF_FF_IN, st);
       const void* w = FP8 ? static_cast<const void*>(W.w8_ff1) : static_cast<const void*>(W.w_ff1);
-      if (d->ff_glu) {
+      if (FP8 && d->ff_out_fp8) {   // the FF intermediate leaves the epilogue as e4m3 blocks (ff8) for FF-out
+        const Fp8Scales sc{a_scale, W.s_ff1};
+        if (d->ff_glu)
+          SATB_PROPAGATE((linear<EpiSwigluE4m3, 256, false, true>(d->tmaps, a_in, D, M, D, w, 2 * d->ffi,
+                                                                   EpiSwigluE4m3::Params{ff8, W.b_ff1}, st, 1, sc)));
+        else
+          SATB_PROPAGATE((linear_auto<EpiSiluE4m3, false, true>(d->tmaps, a_in, D, M, D, w, d->ffi,
+                                                                 EpiSiluE4m3::Params{ff8, W.b_ff1}, st, sc)));
+      } else if (d->ff_glu) {
         typedef EpiSwiglu<BF16> E;
         typename E::Params ep{ff, d->ffi, W.b_ff1};
         SATB_PROPAGATE((linear<E, 256, BF16, FP8>(d->tmaps, a_in, D, M, D, w, 2 * d->ffi, ep, st, 1,
@@ -1157,7 +1199,10 @@ struct DitFwd {
     }
     ProfScope ps(d, PROF_FF_OUT, st);
     EpiResidual::Params ep{h, D, W.b_ff2, ssg_l ? ssg_l + 5 * D : nullptr, n, static_cast<int>(ssg_ld), s.B};
-    if (d->ff_k == 0)
+    if (FP8 && d->ff_out_fp8)
+      SATB_PROPAGATE((linear<BlockScaledA<EpiResidual>, 128, false, true>(d->tmaps, ff8.q, d->ffi, M, d->ffi, W.w8_ff2, D,
+                                                                         ep, st, 1, Fp8Scales{ff8.scale, W.s_ff2})));
+    else if (d->ff_k == 0)
       SATB_PROPAGATE((linear_auto<EpiResidual, BF16>(d->tmaps, ff, d->ffi, M, d->ffi, W.w_ff2, D, ep, st)));
     else
       SATB_PROPAGATE((token_conv<EpiResidual, BF16>(d->tmaps, ff, n, s.R, n, d->ffi, W.w_ff2, D, d->ff_k, ep, st)));
@@ -1361,7 +1406,7 @@ static bool same_model(const SatbDit* a, const SatbDit* b) {
   return std::memcmp(&a->cfg, &b->cfg, sizeof(SatbDitConfig)) == 0 && a->ff_inner == b->ff_inner &&
          a->ff_glu == b->ff_glu && a->ff_bias == b->ff_bias && a->ff_k == b->ff_k && a->rotary == b->rotary &&
          a->pos_type == b->pos_type && a->abs_max_len == b->abs_max_len && a->conformer == b->conformer &&
-         a->attn_fp8 == b->attn_fp8;
+         a->attn_fp8 == b->attn_fp8 && a->ff_out_fp8 == b->ff_out_fp8;
 }
 
 static void group_drop_graph(SatbDitGroup* g) {
@@ -2043,6 +2088,45 @@ int satb_gemm_probe_qk8(const void* a, const void* w, const float* a_scale, cons
     return p->bf16 ? norm(std::true_type{}) : norm(std::false_type{});
   set_last_error("gemm probe qk8: no such instance (epi " + std::to_string(p->epi) + ", BN " + std::to_string(bn) +
                  "); the forward's are qkv_rope_e4m3 BN 256 and head_norm_e4m3 BN 256 (FP8 operands: BN 128)");
+  return -1;
+}
+
+// The GEMMs of the FP8 FF-out option as the forward launches them: FF-in with an e4m3 block epilogue (EpiSwigluE4m3
+// BN 256, EpiSiluE4m3 BN 128 / 256) and FF-out on block-scaled A (BlockScaledA<EpiResidual> BN 128).
+int satb_gemm_probe_ff8(const void* a8, const void* w8, const float* a_scale, const float* w_scale, int M, int N, int K,
+                        const SatbGemmProbe* p, void* ff8, float* ff_scale, void* stream) {
+  SATB_REQUIRE(a8 && w8 && a_scale && w_scale && p, "null argument");
+  SATB_REQUIRE(M >= 1 && N >= 32 && K >= 128 && K % 128 == 0, "gemm probe ff8: need M >= 1, N >= 32 and K % 128 == 0");
+  SATB_REQUIRE(aligned16(a8) && aligned16(w8) && aligned16(w_scale), "gemm probe ff8: operands must be 16-byte aligned");
+  SATB_REQUIRE(p->bf16 == 0, "gemm probe ff8: the FP8 instances are fp16-mode instances (bf16 must be 0)");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const Fp8Scales sc{a_scale, w_scale};
+  const int bn = p->bn;
+  if (p->epi == SATB_EPI_SWIGLU_E4M3 || p->epi == SATB_EPI_SILU_E4M3) {
+    const bool glu = p->epi == SATB_EPI_SWIGLU_E4M3;
+    const int cols = glu ? N / 2 : N;
+    SATB_REQUIRE(ff8 && ff_scale && aligned16(ff8) && aligned16(ff_scale) && aligned16(p->bias),
+                 "gemm probe ff8: ff8, ff_scale (and bias) must be 16-byte aligned device pointers");
+    SATB_REQUIRE(p->ld >= cols && p->ld % 128 == 0, "gemm probe ff8: ld must cover the output row and be a multiple of 128");
+    const BlockE4m3Out o{static_cast<uint8_t*>(ff8), ff_scale, p->ld};
+    if (glu && bn == 256)
+      return probe_run<EpiSwigluE4m3, 256, false, true>(a8, w8, M, N, K, EpiSwigluE4m3::Params{o, p->bias}, p->b_static,
+                                                        st, sc);
+    if (!glu && bn == 128)
+      return probe_run<EpiSiluE4m3, 128, false, true>(a8, w8, M, N, K, EpiSiluE4m3::Params{o, p->bias}, p->b_static, st, sc);
+    if (!glu && bn == 256)
+      return probe_run<EpiSiluE4m3, 256, false, true>(a8, w8, M, N, K, EpiSiluE4m3::Params{o, p->bias}, p->b_static, st, sc);
+  } else if (p->epi == SATB_EPI_RESIDUAL_A8 && bn == 128) {
+    SatbGemmProbe q = *p;
+    q.epi = SATB_EPI_RESIDUAL;   // the residual epilogue's output checks
+    SATB_PROPAGATE(probe_check_outputs(q, N));
+    SATB_REQUIRE(!p->gate || (p->rows_per_item >= 1 && p->n_items >= 1 && p->gate_ld % 4 == 0),
+                 "gemm probe: the gate needs rows_per_item, n_items >= 1 and gate_ld % 4 == 0");
+    const EpiResidual::Params ep{p->h, p->ld, p->bias, p->gate, p->rows_per_item, p->gate_ld, p->n_items};
+    return probe_run<BlockScaledA<EpiResidual>, 128, false, true>(a8, w8, M, N, K, ep, p->b_static, st, sc);
+  }
+  set_last_error("gemm probe ff8: no such instance (epi " + std::to_string(p->epi) + ", BN " + std::to_string(bn) +
+                 "); the forward's are swiglu_e4m3 BN 256, silu_e4m3 BN 128 / 256 and residual_a8 BN 128");
   return -1;
 }
 

@@ -161,12 +161,29 @@ struct Fp8Scales {
 };
 constexpr int kBlockKFp8 = 128;   // 128 x 8-bit = 128 B
 
+// Block-scaled A (the FP8 FF-out option): an FP8 instance whose epilogue type is BlockScaledA<Epi> reads A with one
+// power-of-two scale per (row, k-block of 128), sc.a [rows of A, K / 128], instead of one per row.  Each k-block's four
+// e4m3 MMAs go into a temporary accumulator, which is retired (wgmma.wait_group 0) and promoted into the accumulator,
+// acc += tmp * a_scale[row, kb] (exact: the scale is a power of two); w_scale[col] is applied once before the epilogue.
+// The flag rides on the epilogue type so that the existing instances keep their template arguments.  BN 128 only: the
+// two accumulators take 64 + 64 registers.
+template <class Epi>
+struct BlockScaledA : Epi {
+  static constexpr bool kBlockScaledA = true;
+};
+template <class Epi, class = void>
+struct EpiBlockScaledA : std::false_type {};
+template <class Epi>
+struct EpiBlockScaledA<Epi, std::void_t<decltype(Epi::kBlockScaledA)>> : std::bool_constant<Epi::kBlockScaledA> {};
+
 template <class Epi, int BN, bool BF16, bool FP8 = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmA2, const GemmShape s, const typename Epi::Params ep,
                   const Fp8Scales sc) {
   static_assert(!(FP8 && BF16), "the FP8 mode keeps fp16 as its 16-bit type");
+  constexpr bool kBlockA = EpiBlockScaledA<Epi>::value;
+  static_assert(!kBlockA || (FP8 && BN == 128), "block-scaled A: FP8 operands, BN 128");
   constexpr int kKElems = FP8 ? kBlockKFp8 : kBlockK;   // elements of one k-block
   using Cfg = GemmCfg<BN, kStagedCols<Epi>, Epi::kStageBytes>;
   extern __shared__ uint8_t smem_raw[];
@@ -274,6 +291,61 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       const int batch = rem / m_tiles;
       const int m0 = (rem - batch * m_tiles) * kBlockM;
       const int n0 = nt * BN;
+      if constexpr (kBlockA) {
+        // block-scaled mainloop (BlockScaledA): rows r0, r0 + 8 of the fragment; the next k-block's scales are
+        // requested while this one's MMAs run
+        const int r0 = m0 + 64 * cw + 16 * (warp & 3) + (lane >> 2);
+        const bool ok0 = r0 < s.L, ok1 = r0 + 8 < s.L;
+        const float* sa0 = sc.a + (static_cast<size_t>(batch) * s.L + (ok0 ? r0 : 0)) * num_kb;
+        const float* sa1 = sc.a + (static_cast<size_t>(batch) * s.L + (ok1 ? r0 + 8 : 0)) * num_kb;
+        float s0 = ok0 ? __ldg(sa0) : 0.f, s1 = ok1 ? __ldg(sa1) : 0.f;
+        float tmp[BN / 2];
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&full_bar[stage], phase);
+          const uint32_t a_addr = smem_u32(smem + stage * Cfg::kStage) + cw * 64 * kBlockK * 2;
+          const uint32_t b_addr = smem_u32(smem + stage * Cfg::kStage) + Cfg::kStageA;
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < kBlockK / kWgmmaK; ++k)
+            wgmma_ss_e4m3<BN>(tmp, make_desc_kmajor_sw128(a_addr + k * kWgmmaK * 2),
+                              make_desc_kmajor_sw128(b_addr + k * kWgmmaK * 2), k != 0 ? 1u : 0u);
+          wgmma_commit();
+          float s0_next = 0.f, s1_next = 0.f;
+          if (kb + 1 < num_kb) {
+            if (ok0) s0_next = __ldg(sa0 + kb + 1);
+            if (ok1) s1_next = __ldg(sa1 + kb + 1);
+          }
+          wgmma_wait<0>(tmp);
+          if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[stage]);
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            acc[4 * j] = fmaf(tmp[4 * j], s0, acc[4 * j]);
+            acc[4 * j + 1] = fmaf(tmp[4 * j + 1], s0, acc[4 * j + 1]);
+            acc[4 * j + 2] = fmaf(tmp[4 * j + 2], s1, acc[4 * j + 2]);
+            acc[4 * j + 3] = fmaf(tmp[4 * j + 3], s1, acc[4 * j + 3]);
+          }
+          s0 = s0_next;
+          s1 = s1_next;
+          if (++stage == Cfg::kStages) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+        const int fc = 2 * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int col = n0 + 8 * j + fc;
+          const float2 sw = col < s.N ? __ldg(reinterpret_cast<const float2*>(sc.w + col)) : make_float2(0.f, 0.f);
+          acc[4 * j] *= sw.x;
+          acc[4 * j + 1] *= sw.y;
+          acc[4 * j + 2] *= sw.x;
+          acc[4 * j + 3] *= sw.y;
+        }
+        Epi::template apply_fragment<BN>(ep, acc, s.L, s.N, r0, n0, batch, lane);
+        continue;
+      }
       // mainloop: one wgmma group per k-block; the smem slot of k-block kb - 1 is released once group kb is issued
       // and group kb - 1 has retired
       int prev = -1;
@@ -918,6 +990,134 @@ struct EpiSwiglu {
           store16_group_pair(static_cast<uint16_t*>(p.out) + static_cast<size_t>(batch * L + l) * p.ld,
                              (col0 >> 1) + 8 * jp, w[0], w[1], lane, l < L);
         }
+      }
+    }
+  }
+};
+
+// The FF intermediate of the FP8 FF-out option in e4m3 with one power-of-two scale per (row, 128-column block): q [rows,
+// ld] e4m3, scale [rows, ld / 128] fp32, by the rule of fp8_row_exp applied to the block's fp32 amax.  One block is one
+// k-block of the FF-out GEMM that reads it (BlockScaledA).
+struct BlockE4m3Out {
+  uint8_t* q;
+  float* scale;
+  int ld;   // a multiple of 128
+};
+
+// Quantises and stores one fragment row's 128-column block starting at column c0: v[2 g], v[2 g + 1] hold columns
+// c0 + 8 g + fc, + 1 (g < 16, fc = 2 (lane & 3)), so the quad's four lanes hold the whole block and its amax takes two
+// shfl_xor.  Per four groups g0 .. g0 + 3, two exchanges inside the quad (as in store16_group_pair, then between lanes
+// q and q ^ 2) leave lane q with all 8 bytes of group g0 + q, so the quad stores one whole 32-byte sector.  Every lane
+// of the warp must take part; `ok` gates the stores.
+__device__ __forceinline__ void store_e4m3_block(const BlockE4m3Out& o, int row, int c0, const float (&v)[32], int lane,
+                                                 bool ok) {
+  float amax = 0.f;
+#pragma unroll
+  for (int i = 0; i < 32; ++i) amax = fmaxf(amax, fabsf(v[i]));
+  amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
+  amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
+  const int e = fp8_row_exp(amax);
+  const float inv = pow2f(-e);
+  const bool odd = lane & 1, hi = lane & 2;
+  uint8_t* dst = o.q + static_cast<size_t>(row) * o.ld + c0 + 8 * (lane & 3);
+#pragma unroll
+  for (int g0 = 0; g0 < 16; g0 += 4) {
+    uint32_t w[4];   // this lane's byte pair of groups g0 .. g0 + 3
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int g = g0 + i;
+      w[i] = __nv_cvt_float2_to_fp8x2(make_float2(v[2 * g] * inv, v[2 * g + 1] * inv), __NV_SATFINITE, __NV_E4M3);
+    }
+    // after the first exchange, lane q holds 4 bytes: of group g0 + (q & 1) in u01, of g0 + 2 + (q & 1) in u23, bytes
+    // 0-3 for q < 2 and 4-7 for q >= 2
+    const uint32_t got01 = __shfl_xor_sync(0xffffffffu, odd ? w[0] : w[1], 1);
+    const uint32_t got23 = __shfl_xor_sync(0xffffffffu, odd ? w[2] : w[3], 1);
+    const uint32_t u01 = odd ? got01 | (w[1] << 16) : w[0] | (got01 << 16);
+    const uint32_t u23 = odd ? got23 | (w[3] << 16) : w[2] | (got23 << 16);
+    const uint32_t got = __shfl_xor_sync(0xffffffffu, hi ? u01 : u23, 2);
+    if (ok) *reinterpret_cast<uint2*>(dst + 8 * g0) = hi ? make_uint2(got, u23) : make_uint2(u01, got);
+  }
+  if (ok && (lane & 3) == 0) o.scale[static_cast<size_t>(row) * (o.ld / 128) + c0 / 128] = pow2f(e);
+}
+
+// EpiSwiglu with the output stored as e4m3 blocks (BlockE4m3Out) instead of 16 bits: the same fp32 values, quantised.
+// BN 256: a tile's 128 output columns are one block.  N a multiple of 256.
+struct EpiSwigluE4m3 {
+  static constexpr int kCols = 256;
+  static constexpr int kStageBytes = 0;
+  static constexpr bool kFragment = true;
+  struct Params {
+    BlockE4m3Out o;     // ld: inner dim (N / 2)
+    const float* bias;  // interleaved like the weight rows; may be null
+  };
+  template <int BN>
+  __device__ static __forceinline__ void apply_fragment(const Params& p, const float (&acc)[BN / 2], int L, int N,
+                                                        int row0, int n0, int batch, int lane) {
+    static_assert(BN == 256, "one tile = one 128-column output block");
+    const int fc = 2 * (lane & 3);
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      const int l = row0 + 8 * rr;
+      float v[32];
+#pragma unroll
+      for (int g = 0; g < 4; ++g) {
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {   // value columns c, c + 1 and gate columns c + 32, c + 33 of group g
+          const int c = n0 + 64 * g + 8 * jj + fc;
+          const int av = 4 * (8 * g + jj) + 2 * rr, ag = av + 16;
+          float a0 = acc[av], a1 = acc[av + 1], g0 = acc[ag], g1 = acc[ag + 1];
+          if (p.bias) {
+            const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + c));
+            const float2 bg = __ldg(reinterpret_cast<const float2*>(p.bias + c + 32));
+            a0 += bv.x;
+            a1 += bv.y;
+            g0 += bg.x;
+            g1 += bg.y;
+          }
+          v[2 * (4 * g + jj)] = a0 * silu_f(g0);
+          v[2 * (4 * g + jj) + 1] = a1 * silu_f(g1);
+        }
+      }
+      store_e4m3_block(p.o, batch * L + l, n0 >> 1, v, lane, l < L);
+    }
+  }
+};
+
+// The plain-SiLU FF-in (EpiStore16 with act 1) with the output stored as e4m3 blocks (BlockE4m3Out): silu(acc + bias).
+// N a multiple of 128.
+struct EpiSiluE4m3 {
+  static constexpr int kCols = 128;
+  static constexpr int kStageBytes = 0;
+  static constexpr bool kFragment = true;
+  struct Params {
+    BlockE4m3Out o;     // ld: N
+    const float* bias;  // may be null
+  };
+  template <int BN>
+  __device__ static __forceinline__ void apply_fragment(const Params& p, const float (&acc)[BN / 2], int L, int N,
+                                                        int row0, int n0, int batch, int lane) {
+    const int fc = 2 * (lane & 3);
+#pragma unroll
+    for (int blk = 0; blk < BN / 128; ++blk) {
+      const int c0 = n0 + 128 * blk;
+      if (c0 >= N) break;
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int l = row0 + 8 * rr;
+        float v[32];
+#pragma unroll
+        for (int g = 0; g < 16; ++g) {
+          const int a = 4 * (16 * blk + g) + 2 * rr;
+          float x0 = acc[a], x1 = acc[a + 1];
+          if (p.bias) {
+            const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + c0 + 8 * g + fc));
+            x0 += b.x;
+            x1 += b.y;
+          }
+          v[2 * g] = silu_f(x0);
+          v[2 * g + 1] = silu_f(x1);
+        }
+        store_e4m3_block(p.o, batch * L + l, c0, v, lane, l < L);
       }
     }
   }

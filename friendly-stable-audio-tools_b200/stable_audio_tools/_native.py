@@ -64,6 +64,8 @@ EPI_RESIDUAL_LN = 6   # retired (the LayerNorm-fold residual epilogue): refused,
 EPI_STORE32_POS = 7   # store32 plus a [seq_len, N] position-table row (project_in with a positional embedding)
 # satb_gemm_probe_qk8 only: the e4m3 QKV epilogues of FP8 self-attention
 EPI_QKV_ROPE_E4M3, EPI_HEAD_NORM_E4M3 = 8, 9
+# satb_gemm_probe_ff8 only: the GEMMs of the FP8 FF-out option
+EPI_SWIGLU_E4M3, EPI_SILU_E4M3, EPI_RESIDUAL_A8 = 13, 14, 15
 # satb_t5_gemm_probe only: the T5 encoder's FF-in epilogues
 EPI_RELU16, EPI_GEGLU16 = 10, 11
 # satb_roberta_linear_probe only: the RoBERTa encoder's FF-in epilogue
@@ -114,6 +116,7 @@ SIGNATURES = {
     "satb_dit_set_feedforward": (_I, [_VP, _I, _I, _I, _I]),
     "satb_dit_set_positions": (_I, [_VP, _I, _I, _I]),
     "satb_dit_set_attention_fp8": (_I, [_VP, _I]),
+    "satb_dit_set_ff_out_fp8": (_I, [_VP, _I]),
     "satb_dit_load_weight": (_I, [_VP, ctypes.c_char_p, _VP, _LL, _VP]),
     "satb_dit_finalize": (_I, [_VP, _VP]),
     "satb_dit_reserve": (_I, [_VP, _I, _I]),
@@ -157,6 +160,7 @@ SIGNATURES = {
     "satb_attention_fp8_vt": (_I, [_VP] * 3 + [_I, _I, _I, _I, _VP]),
     "satb_gemm_probe_qk8": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, ctypes.POINTER(SatbGemmProbe), ctypes.POINTER(SatbQkE4m3),
                                  _VP]),
+    "satb_gemm_probe_ff8": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, ctypes.POINTER(SatbGemmProbe), _VP, _VP, _VP]),
     "satb_attention_fp8_core": (_I, [_VP] * 7 + [_I, _I, _I, _I, _I, _VP]),
     "satb_conformer_dwconv": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _VP]),
     "satb_oobleck_create": (_I, [ctypes.POINTER(SatbOobleckConfig), ctypes.POINTER(_VP)]),

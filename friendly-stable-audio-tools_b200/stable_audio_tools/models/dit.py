@@ -16,6 +16,8 @@ and parameter names, ``forward`` signature and CFG semantics); the arithmetic ru
 * ``ff_kwargs`` (any ``mult``, ``no_bias``, ``glu=False``, ``use_conv`` with an odd ``conv_kernel_size``) select the
   native feed-forward variant (``satb_dit_set_feedforward``); its token convolutions run as k-tap GEMMs over each
   item, with 16-bit operands in every ``operand_dtype``;
+* ``ff_out_dtype="fp8"`` (with ``operand_dtype="fp8"``) runs every block's FF-out GEMM on e4m3 operands, its
+  activations with one scale per (token, 128 inner columns) written by FF-in's epilogue (``satb_dit_set_ff_out_fp8``);
 * ``rotary_pos_emb=False``, ``use_sinusoidal_emb`` and ``use_abs_pos_emb`` select the native positional options
   (``satb_dit_set_positions``); the embedding is added to every row, prepended ones included, in project_in's epilogue;
 * any ``io_channels`` and ``input_concat_dim`` (an inpainting DiT's latent + 1 mask channel, PQMF sub-bands, raw audio):
@@ -50,6 +52,12 @@ OPERAND_DTYPES = {"fp16": 0, "bf16": 1, "fp8": 2}
 # q, k, v and probabilities with power-of-two scales (satb_dit_set_attention_fp8), head dim 64 only, with any
 # operand_dtype; cross-attention stays 16-bit.  A precision choice with its own tolerance (DESIGN.md section 5).
 ATTENTION_DTYPES = (None, "fp8")
+# ff_out_dtype: None (default) keeps the feed-forward output GEMM (ff.ff.2) at fp16 operands in the "fp8" operand mode.
+# "fp8" (operand_dtype="fp8" only; satb_dit_set_ff_out_fp8): its activations are e4m3 with one power-of-two scale per
+# (token, 128 inner columns), written by FF-in's epilogue, and its weight e4m3 with one scale per output row.  Linear
+# feed-forwards whose inner width (padded to 64) is a multiple of 128.  A precision choice with its own tolerance
+# (DESIGN.md section 5).
+FF_OUT_DTYPES = (None, "fp8")
 
 
 class DiffusionTransformer(nn.Module):
@@ -69,6 +77,7 @@ class DiffusionTransformer(nn.Module):
                  global_cond_type: str = "prepend",
                  operand_dtype: str = "fp16",
                  attention_dtype=None,
+                 ff_out_dtype=None,
                  **kwargs):
         super().__init__()
         if transformer_type != "continuous_transformer":
@@ -105,6 +114,10 @@ class DiffusionTransformer(nn.Module):
             raise ValueError(f"attention_dtype must be None or 'fp8', got {attention_dtype!r}")
         if attention_dtype == "fp8" and embed_dim // num_heads != 64:
             raise NotImplementedError(f"attention_dtype='fp8' needs head dim 64 (got {embed_dim // num_heads})")
+        if ff_out_dtype not in FF_OUT_DTYPES:
+            raise ValueError(f"ff_out_dtype must be None or 'fp8', got {ff_out_dtype!r}")
+        if ff_out_dtype == "fp8" and operand_dtype != "fp8":
+            raise ValueError(f"ff_out_dtype='fp8' extends operand_dtype='fp8' (got operand_dtype={operand_dtype!r})")
         self.patch_size = patch_size
         self.cond_token_dim = cond_token_dim
         self.input_concat_dim = input_concat_dim
@@ -120,6 +133,7 @@ class DiffusionTransformer(nn.Module):
         self.global_cond_type = global_cond_type
         self.operand_dtype = operand_dtype
         self.attention_dtype = attention_dtype
+        self.ff_out_dtype = ff_out_dtype
         self.qk_norm = bool(kwargs.get("attn_kwargs", {}).get("qk_norm", False))
         # conformer=True (ContinuousTransformer kwarg): every block adds the conformer branch (satb_dit_set_conformer)
         self.conformer = bool(kwargs.get("conformer", False))
@@ -153,6 +167,15 @@ class DiffusionTransformer(nn.Module):
         # to satb_dit_set_feedforward only when it differs from the default SwiGLU (mult 4, biased, Linear)
         ff = self.transformer.layers[0].ff if depth > 0 else None
         self.ff_spec = ff.native_spec() if ff is not None else (4 * embed_dim, 1, 0, 1)
+        if ff_out_dtype == "fp8":
+            inner, _, conv_k, _ = self.ff_spec
+            if conv_k > 0:
+                raise NotImplementedError("ff_out_dtype='fp8' is not supported with use_conv feed-forwards (their FF-out "
+                                          "is a token convolution)")
+            padded = -(-inner // 64) * 64     # the native inner width (zero-padded to a multiple of 64)
+            if padded % 128 != 0:
+                raise NotImplementedError(f"ff_out_dtype='fp8' needs a feed-forward inner width that is a multiple of "
+                                          f"128, the FP8 GEMM's k-block (got {inner}, padded to {padded})")
         # positions (ContinuousTransformer kwargs): the satb_dit_set_positions arguments (rotary, pos_type, abs_max_len),
         # handed over only when they differ from the default (rotary, no embedding)
         tr = self.transformer
@@ -233,6 +256,8 @@ class DiffusionTransformer(nn.Module):
             options.append(lambda: lib.satb_dit_set_attention_fp8(h, 1))
         if self.ff_spec != (4 * self.embed_dim, 1, 0, 1):
             options.append(lambda: lib.satb_dit_set_feedforward(h, *self.ff_spec))
+        if self.ff_out_dtype == "fp8":                # after the feed-forward variant, whose inner width it checks
+            options.append(lambda: lib.satb_dit_set_ff_out_fp8(h, 1))
         if self.pos_spec != (1, 0, 0):
             options.append(lambda: lib.satb_dit_set_positions(h, *self.pos_spec))
         for set_option in options:

@@ -114,6 +114,15 @@ int satb_dit_set_positions(SatbDit* h, int rotary, int pos_type, int abs_max_len
  * Head dim 64 only; works with every operand_dtype.  Call before satb_dit_finalize; a later call, another head dim
  * with enable 1, and an enable other than 0 or 1 are refused.  Default 0. */
 int satb_dit_set_attention_fp8(SatbDit* h, int enable);
+/* FP8 FF-out (DiffusionTransformer ff_out_dtype "fp8"; DESIGN.md sections 3-5): enable 1 runs every block's FF-out GEMM
+ * on e4m3 operands.  FF-in's epilogue then stores the SwiGLU (or plain SiLU) output as e4m3 with one power-of-two scale
+ * per (row, 128 columns) instead of 16 bits, and ff.ff.2.weight is kept only as an e4m3 copy with one scale per row;
+ * each 128-wide k-block's partial product is scaled by its activation block scale before it is accumulated.  Needs
+ * operand_dtype 2 (fp8), a Linear feed-forward (no conv_kernel_size) and an inner width that, padded to a multiple of 64,
+ * is a multiple of 128.  Call after satb_dit_set_feedforward and before the first satb_dit_load_weight (the option
+ * decides how ff.ff.2.weight is stored), so before satb_dit_finalize; a later call, a null handle, an enable other than
+ * 0 or 1, and enable 1 on any other model are refused before any CUDA call.  Default 0. */
+int satb_dit_set_ff_out_fp8(SatbDit* h, int enable);
 /* One state-dict entry (key relative to DiffusionTransformer, e.g.
  * "transformer.layers.0.self_attn.to_qkv.weight"); src: device fp32, contiguous.
  * Replaces nn.Module.load_state_dict for this module (models/pretrained.py:24). */
@@ -240,6 +249,10 @@ int satb_linear_f32out(const void* a16, const void* w16, float* c, int M, int N,
 /* e4m3 QKV epilogues of FP8 self-attention (satb_gemm_probe_qk8 only; the other probes refuse them): */
 #define SATB_EPI_QKV_ROPE_E4M3 8   /* qkv_rope at head dim 64 (nf 16), q / k columns stored e4m3 (SatbQkE4m3), v 16-bit */
 #define SATB_EPI_HEAD_NORM_E4M3 9  /* head_norm16 with norm_cols = 128 heads, q / k stored e4m3 (SatbQkE4m3), v 16-bit */
+/* The GEMMs of the FP8 FF-out option (satb_gemm_probe_ff8 only; the other probes refuse them): */
+#define SATB_EPI_SWIGLU_E4M3 13    /* swiglu, the N / 2 outputs stored as e4m3 blocks of 128 columns with their scales */
+#define SATB_EPI_SILU_E4M3 14      /* silu(acc (+ bias)), stored as e4m3 blocks of 128 columns with their scales */
+#define SATB_EPI_RESIDUAL_A8 15    /* residual, A e4m3 with one scale per (row, 128-wide k-block) */
 typedef struct SatbGemmProbe {
   int epi, bn, bf16, b_static;      /* b_static 1: weight prefetch before the dependency wait, as the forward runs */
   void* out;                        /* store32 (fp32), store16, head_norm16, qkv_rope, swiglu (16-bit) */
@@ -382,6 +395,17 @@ int satb_attention_fp8_core(const void* q8, const void* k8, const float* sq, con
                             const float* sv, void* o16, int B, int H, int Nq, int Nk, int bf16, void* stream);
 int satb_gemm_probe_qk8(const void* a, const void* w, const float* a_scale, const float* w_scale, int M, int N, int K,
                         const SatbGemmProbe* p, const SatbQkE4m3* o, void* stream);
+/* Test entry point of the FP8 FF-out option (satb_dit_set_ff_out_fp8), through the instances the DiT forward launches;
+ * a8 [M, K] and w8 [N, K] e4m3, w_scale [N], K a multiple of 128, bf16 0.
+ *   SATB_EPI_SWIGLU_E4M3 (bn 256) and SATB_EPI_SILU_E4M3 (bn 128 / 256): FF-in, a_scale [M] (one per row).  The epilogue's
+ *     fp32 outputs (N / 2 SwiGLU columns or N SiLU columns, bias as in swiglu / store16) are stored as ff8 [M, ld] e4m3
+ *     and ff_scale [M, ld / 128]: for every row and 128-column block, scale = 2^e with e the smallest integer (>= -126)
+ *     with max |y| <= 448 * 2^e (1 for an all-zero block), ff8 = e4m3_rn(y / scale).  ld a multiple of 128.
+ *   SATB_EPI_RESIDUAL_A8 (bn 128): FF-out, a_scale [M, K / 128] (the scale of a8[m, k] is a_scale[m, k / 128]);
+ *     C[m, n] = w_scale[n] sum_kb a_scale[m, kb] sum_{k in kb} a8[m, k] w8[n, k] goes through the residual epilogue (h, ld,
+ *     bias, gate).  ff8 and ff_scale are ignored. */
+int satb_gemm_probe_ff8(const void* a8, const void* w8, const float* a_scale, const float* w_scale, int M, int N, int K,
+                        const SatbGemmProbe* p, void* ff8, float* ff_scale, void* stream);
 
 /* Test entry point: the kernel of the conformer branch, out = silu(LayerNorm(depthwise_conv(g))) per item
  * (transformer.py:583-586): g, out [items * n_seq, D] 16-bit (fp16/bf16 bits), 16-byte aligned; the convolution runs
