@@ -103,6 +103,13 @@ constexpr int kKvGatherMaxRanks = 8;
 int launch_kv_gather(const void* const* qkv, const int* token_begin, int world, void* kv, int R, int D,
                      cudaStream_t stream);
 
+// ---- time_gather.cu (time-sharded Oobleck decode / encode)
+// out [rows, T] fp32: positions begin[q] .. begin[q + 1] - 1 of every row from rank q's src[q] [rows, src_len[q]],
+// starting at its position src_off[q] (begin[0] = 0, begin[world] = T).  src[q] may live on another device (a peer
+// pointer).
+int launch_time_gather(const float* const* src, const int* src_len, const int* src_off, const int* begin, int world,
+                       float* out, int rows, int T, cudaStream_t stream);
+
 // ---- conformer.cu
 // out16 = silu(LayerNorm(depthwise_conv17(g16))) per item of n_seq rows (zero padding at each item's ends, eps 1e-5):
 // g16, out16 [items * n_seq, D] 16-bit; w fp32 [D][17]; gamma, beta [D] (beta may be null).  D <= kConformerMaxDim.

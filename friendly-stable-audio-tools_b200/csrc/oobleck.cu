@@ -19,6 +19,7 @@
 // (use_nearest_upsample=True) is a 3-tap GEMM over the low-rate input with N = s*Cout (run_conv_gemm kind 3).
 #include <algorithm>
 #include <cmath>
+#include <cstring>
 #include <tuple>
 #include <type_traits>
 #include <map>
@@ -29,6 +30,7 @@
 #include "common.cuh"
 #include "conv_halo.cuh"
 #include "kernels.h"
+#include "linear.cuh"
 
 namespace satb {
 
@@ -1012,6 +1014,295 @@ int satb_oobleck_weights(SatbOobleck* h, const char* prefix, void* dst, long lon
                                     cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));
   }
   return 0;
+}
+
+}  // extern "C"
+
+// ---- Time-sharded decode / encode: one process drives `world` ranks, each a finalized handle with a full copy of the
+// weights on its device (several ranks may share a device).  Rank r computes latents begin[r] .. begin[r + 1] - 1 of
+// every item (their samples for the encoder) by running the ordinary single-device decode / encode on an extended
+// slice: its range plus a recompute margin of m latents on each interior side, clipped to the item.  Every kept output
+// position then reads the same inputs through the same arithmetic as on one device:
+//   * each convolution's output at a position is its k-block x tap accumulation of its own input rows, in the same
+//     order for every row of a tile; the tile a row falls in decides nothing (no split-K, no per-tile fast path: the
+//     lean epilogue runs the same arithmetic on ragged chunks, and its choice against the general one is per launch);
+//   * the route of each layer (fused ResidualUnit, halo-tile final conv, implicit GEMM and its N tile, CUDA-core input
+//     conv) depends on the channels, taps, dilation and operand mode only, which are the same on every rank;
+//   * an extended slice starts at a whole latent, so at every level of the decoder (encoder) its first position is a
+//     multiple of that level's cumulative stride: the transposed convs' phases and the strided convs' taps line up.
+// Only the positions within the margin of a slice's interior ends see zeros in place of a neighbour's data, and the
+// margin is the receptive field in latents, so none of them is kept.  Recomputing the margin needs no change to any
+// convolution kernel or tensor-map route, where a per-layer halo exchange would need one per layer and route.
+
+namespace {
+
+int64_t floor_div(int64_t a, int64_t b) { return a >= 0 ? a / b : -((-a + b - 1) / b); }
+
+// The receptive field of one latent (decoder: the latents any output sample of latent 0 reads; encoder: the latents
+// whose samples latent 0 reads, in whole latents) on either side, from the layer list: k7 input conv, per block the
+// up / down conv and three k7 ResidualUnits at dilations 1, 3, 9 (3 + 9 + 27 positions each way), the final conv (k7
+// decoder, k3 encoder).  The interval of positions a layer's outputs [lo, hi] read is walked back from the output.
+int receptive_margin(const SatbOobleckConfig& c, bool nearest) {
+  const int n = c.n_stages;
+  int64_t ratio = 1;
+  for (int i = 0; i < n; ++i) ratio *= c.strides[i];
+  constexpr int kResUnits = 3 * (1 + 3 + 9);
+  if (c.is_decoder) {
+    int64_t lo = -3, hi = ratio - 1 + 3;                     // the final conv k7 over the samples of latent 0
+    for (int b = n; b >= 1; --b) {
+      const int s = c.strides[n - b];
+      lo -= kResUnits;
+      hi += kResUnits;
+      if (nearest) {                                         // output s m + ph reads m - 1 .. m + 1
+        lo = floor_div(lo, s) - 1;
+        hi = floor_div(hi, s) + 1;
+      } else {                                               // output o reads l - 1, l with l = floor((o + pad) / s)
+        const int p = (s + 1) / 2;
+        lo = floor_div(lo + p, s) - 1;
+        hi = floor_div(hi + p, s);
+      }
+    }
+    lo -= 3;                                                 // the input conv k7
+    hi += 3;
+    return static_cast<int>(std::max(-lo, hi));
+  }
+  int64_t lo = -1, hi = 1;                                   // the final conv k3 around latent 0
+  for (int b = n; b >= 1; --b) {
+    const int s = c.strides[b - 1], p = (s + 1) / 2;         // output o reads o s - p .. o s - p + 2 s - 1
+    lo = lo * s - p - kResUnits;
+    hi = hi * s - p + 2 * s - 1 + kResUnits;
+  }
+  lo -= 3;                                                   // the input conv k7
+  hi += 3;
+  return static_cast<int>(std::max(floor_div(-lo + ratio - 1, ratio), floor_div(hi - (ratio - 1) + ratio - 1, ratio)));
+}
+
+}  // namespace
+
+extern "C" int satb_oobleck_group_plan(int world, int L, const SatbOobleckConfig* cfg, int nearest_upsample,
+                                       int* begin, int* ext, int* margin) {
+  SATB_REQUIRE(cfg && begin && ext && margin, "null argument");
+  SATB_REQUIRE(world >= 1 && world <= kKvGatherMaxRanks, "world must be 1 .. 8");
+  SATB_REQUIRE(L >= 1, "need L >= 1");
+  SATB_REQUIRE(cfg->n_stages >= 1 && cfg->n_stages <= SATB_MAX_STAGES, "bad number of stages");
+  for (int i = 0; i < cfg->n_stages; ++i) SATB_REQUIRE(cfg->strides[i] >= 2, "strides must be >= 2");
+  SATB_REQUIRE(nearest_upsample == 0 || (nearest_upsample == 1 && cfg->is_decoder),
+               "nearest_upsample must be 0, or 1 for a decoder");
+  if (world > L) {
+    set_last_error("world " + std::to_string(world) + " exceeds the " + std::to_string(L) +
+                   " latents of an item: every rank needs at least one latent");
+    return -1;
+  }
+  const int m = receptive_margin(*cfg, nearest_upsample != 0);
+  for (int r = 0; r <= world; ++r) begin[r] = static_cast<int>(static_cast<int64_t>(r) * L / world);
+  for (int r = 0; r < world; ++r) {
+    const int n = begin[r + 1] - begin[r];
+    if (world > 1 && n < m) {
+      set_last_error("rank " + std::to_string(r) + " would hold " + std::to_string(n) + " of the " + std::to_string(L) +
+                     " latents, fewer than the recompute margin of " + std::to_string(m) +
+                     " latents each rank recomputes on each interior side: use fewer ranks or a longer clip");
+      return -1;
+    }
+    ext[2 * r] = std::max(begin[r] - m, 0);
+    ext[2 * r + 1] = std::min(begin[r + 1] + m, L);
+  }
+  *margin = m;
+  return 0;
+}
+
+struct SatbOobleckGroup {
+  int world = 0;
+  std::vector<SatbOobleck*> h;
+  std::vector<int> dev;
+  std::vector<cudaStream_t> st;        // per rank, on its device (the library's own)
+  std::vector<cudaEvent_t> ev_done;    // per rank: its decode / encode of the last call done
+  std::vector<DevBuf> in, out;         // per rank, on its device: the extended slice's input and output
+  cudaEvent_t ev_in = nullptr;         // home device: the caller's stream reached the call (its input is ready)
+  cudaEvent_t ev_gathered = nullptr;   // home device: the last call's gather done
+};
+
+namespace {
+
+void group_release(SatbOobleckGroup* g) {
+  int cur = 0;
+  cudaGetDevice(&cur);
+  if (g->ev_gathered) cudaEventSynchronize(g->ev_gathered);   // the last gather may still read the ranks' outputs
+  for (int r = 0; r < g->world; ++r) {
+    cudaSetDevice(g->dev[r]);
+    if (r < static_cast<int>(g->st.size()) && g->st[r]) cudaStreamSynchronize(g->st[r]);
+    if (r < static_cast<int>(g->in.size())) g->in[r].release();
+    if (r < static_cast<int>(g->out.size())) g->out[r].release();
+    if (r < static_cast<int>(g->ev_done.size()) && g->ev_done[r]) cudaEventDestroy(g->ev_done[r]);
+    if (r < static_cast<int>(g->st.size()) && g->st[r]) cudaStreamDestroy(g->st[r]);
+  }
+  if (g->world > 0) {
+    cudaSetDevice(g->dev[0]);
+    if (g->ev_in) cudaEventDestroy(g->ev_in);
+    if (g->ev_gathered) cudaEventDestroy(g->ev_gathered);
+  }
+  cudaSetDevice(cur);
+}
+
+struct CurrentDeviceRestore {
+  int cur = 0;
+  CurrentDeviceRestore() { cudaGetDevice(&cur); }
+  ~CurrentDeviceRestore() { cudaSetDevice(cur); }
+};
+
+// One sharded call.  Ordered with events only:
+//   RAW: each rank's input copy waits for the caller's stream (ev_in); the gather waits for every rank (ev_done).
+//   WAR: each rank's work waits for the previous call's gather (ev_gathered), which reads the rank's output buffer.
+// The input slices are 2-D copies on the rank streams (the copy engines move a strided slice over the peer link without
+// taking SMs from the rank's decode, as the DiT group graph's copies do); the gather is a kernel on the home device.
+int group_run(SatbOobleckGroup* g, bool dec, const float* in, float* out, int B, int L, cudaStream_t home) {
+  SatbOobleck* h0 = g->h[0];
+  const SatbOobleckConfig& c = h0->cfg;
+  const int W = g->world;
+  int begin[kKvGatherMaxRanks + 1], ext[2 * kKvGatherMaxRanks], m = 0;
+  SATB_PROPAGATE(satb_oobleck_group_plan(W, L, &c, h0->nearest ? 1 : 0, begin, ext, &m));
+  int64_t ratio = 1;
+  for (int i = 0; i < c.n_stages; ++i) ratio *= c.strides[i];
+  // per latent: positions of the input and the output; and their channels
+  const int64_t in_rate = dec ? 1 : ratio, out_rate = dec ? ratio : 1;
+  const int in_ch = dec ? c.latent_dim : c.in_channels, out_ch = dec ? c.in_channels : c.latent_dim;
+  SATB_REQUIRE(static_cast<int64_t>(L) * ratio < (int64_t(1) << 31), "sequence too long");
+  CurrentDeviceRestore restore;
+  for (int r = 0; r < W; ++r) {   // workspaces at the extended shape; growing one waits for the gather that reads it
+    const int64_t n = ext[2 * r + 1] - ext[2 * r];
+    const size_t need_in = static_cast<size_t>(B) * in_ch * n * in_rate * 4;
+    const size_t need_out = static_cast<size_t>(B) * out_ch * n * out_rate * 4;
+    if (need_in > g->in[r].bytes || need_out > g->out[r].bytes) {
+      SATB_CHECK_CUDA(cudaEventSynchronize(g->ev_gathered));
+      SATB_CHECK_CUDA(cudaSetDevice(g->dev[r]));
+      SATB_PROPAGATE(g->in[r].ensure(need_in));
+      SATB_PROPAGATE(g->out[r].ensure(need_out));
+    }
+  }
+  SATB_CHECK_CUDA(cudaSetDevice(g->dev[0]));
+  SATB_CHECK_CUDA(cudaEventRecord(g->ev_in, home));
+  for (int r = 0; r < W; ++r) {
+    const int64_t e0 = ext[2 * r], n = ext[2 * r + 1] - e0;
+    SATB_CHECK_CUDA(cudaSetDevice(g->dev[r]));
+    SATB_CHECK_CUDA(cudaStreamWaitEvent(g->st[r], g->ev_in, 0));         // RAW: the input
+    SATB_CHECK_CUDA(cudaStreamWaitEvent(g->st[r], g->ev_gathered, 0));   // WAR: the previous gather read out[r]
+    SATB_CHECK_CUDA(cudaMemcpy2DAsync(g->in[r].p, static_cast<size_t>(n * in_rate) * 4, in + e0 * in_rate,
+                                      static_cast<size_t>(L * in_rate) * 4, static_cast<size_t>(n * in_rate) * 4,
+                                      static_cast<size_t>(B) * in_ch, cudaMemcpyDefault, g->st[r]));
+    if (dec)
+      SATB_PROPAGATE(satb_oobleck_decode(g->h[r], g->in[r].as<float>(), g->out[r].as<float>(), B, static_cast<int>(n),
+                                         g->st[r]));
+    else
+      SATB_PROPAGATE(satb_oobleck_encode(g->h[r], g->in[r].as<float>(), g->out[r].as<float>(), B, n * ratio, g->st[r]));
+    SATB_CHECK_CUDA(cudaEventRecord(g->ev_done[r], g->st[r]));
+  }
+  SATB_CHECK_CUDA(cudaSetDevice(g->dev[0]));
+  const float* src[kKvGatherMaxRanks];
+  int src_len[kKvGatherMaxRanks], src_off[kKvGatherMaxRanks], ob[kKvGatherMaxRanks + 1];
+  for (int r = 0; r < W; ++r) {
+    SATB_CHECK_CUDA(cudaStreamWaitEvent(home, g->ev_done[r], 0));         // RAW: rank r's output
+    src[r] = g->out[r].as<float>();
+    src_len[r] = static_cast<int>((ext[2 * r + 1] - ext[2 * r]) * out_rate);
+    src_off[r] = static_cast<int>((begin[r] - ext[2 * r]) * out_rate);
+    ob[r] = static_cast<int>(begin[r] * out_rate);
+  }
+  ob[W] = static_cast<int>(L * out_rate);
+  SATB_PROPAGATE(launch_time_gather(src, src_len, src_off, ob, W, out, B * out_ch, ob[W], home));
+  SATB_CHECK_CUDA(cudaEventRecord(g->ev_gathered, home));
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int satb_oobleck_group_create(SatbOobleck* const* handles, const int* devices, int world, SatbOobleckGroup** out) {
+  SATB_REQUIRE(handles && devices && out, "null argument");
+  SATB_REQUIRE(world >= 1 && world <= kKvGatherMaxRanks, "world must be 1 .. 8");
+  for (int r = 0; r < world; ++r) {
+    SATB_REQUIRE(handles[r], "null handle");
+    const SatbOobleck* a = handles[0];
+    const SatbOobleck* b = handles[r];
+    if (std::memcmp(&a->cfg, &b->cfg, sizeof(SatbOobleckConfig)) != 0 || a->act != b->act || a->nearest != b->nearest) {
+      set_last_error("rank " + std::to_string(r) + "'s handle has another config or block option than rank 0's");
+      return -1;
+    }
+    for (int s = 0; s < r; ++s)
+      SATB_REQUIRE(handles[s] != handles[r], "every rank needs its own handle (its own workspace)");
+  }
+  for (int r = 0; r < world; ++r) SATB_REQUIRE(handles[r]->finalized, "weights not finalized");
+  CurrentDeviceRestore restore;
+  int n_dev = 0;
+  SATB_CHECK_CUDA(cudaGetDeviceCount(&n_dev));
+  for (int r = 0; r < world; ++r) SATB_REQUIRE(devices[r] >= 0 && devices[r] < n_dev, "no such device");
+  // the home device reads every rank's output, and every rank copies its input slice from the home device
+  for (int r = 1; r < world; ++r) {
+    if (devices[r] == devices[0]) continue;
+    for (const auto& pr : {std::make_pair(devices[0], devices[r]), std::make_pair(devices[r], devices[0])}) {
+      int ok = 0;
+      SATB_CHECK_CUDA(cudaDeviceCanAccessPeer(&ok, pr.first, pr.second));
+      if (!ok) {
+        set_last_error("device " + std::to_string(pr.first) + " cannot access device " + std::to_string(pr.second) +
+                       " peer to peer: the time-sharded decode gathers every rank's output over peer links");
+        return -1;
+      }
+      SATB_CHECK_CUDA(cudaSetDevice(pr.first));
+      const cudaError_t e = cudaDeviceEnablePeerAccess(pr.second, 0);   // this process's context only
+      if (e == cudaErrorPeerAccessAlreadyEnabled) {
+        cudaGetLastError();
+      } else {
+        SATB_CHECK_CUDA(e);
+      }
+    }
+  }
+  SatbOobleckGroup* g = new SatbOobleckGroup();
+  g->world = world;
+  g->h.assign(handles, handles + world);
+  g->dev.assign(devices, devices + world);
+  g->st.assign(world, nullptr);
+  g->ev_done.assign(world, nullptr);
+  g->in.resize(world);
+  g->out.resize(world);
+  cudaError_t e = cudaSuccess;
+  for (int r = 0; r < world && e == cudaSuccess; ++r) {
+    e = cudaSetDevice(devices[r]);
+    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&g->st[r], cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&g->ev_done[r], cudaEventDisableTiming);
+  }
+  if (e == cudaSuccess) e = cudaSetDevice(devices[0]);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&g->ev_in, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&g->ev_gathered, cudaEventDisableTiming);
+  if (e != cudaSuccess) {
+    group_release(g);
+    delete g;
+    set_last_error(std::string("satb_oobleck_group_create: ") + cudaGetErrorString(e));
+    return -2;
+  }
+  *out = g;
+  return 0;
+}
+
+void satb_oobleck_group_destroy(SatbOobleckGroup* g) {
+  if (!g) return;
+  group_release(g);
+  delete g;
+}
+
+int satb_oobleck_group_decode(SatbOobleckGroup* g, const float* z, float* audio, int B, int L, void* stream) {
+  SATB_REQUIRE(g && z && audio && B >= 1 && L >= 1, "bad argument");
+  for (int r = 0; r < g->world; ++r) SATB_REQUIRE(g->h[r]->finalized, "oobleck: weights not finalized");
+  SATB_REQUIRE(g->h[0]->cfg.is_decoder, "oobleck group: the handles are encoders");
+  return group_run(g, true, z, audio, B, L, static_cast<cudaStream_t>(stream));
+}
+
+int satb_oobleck_group_encode(SatbOobleckGroup* g, const float* audio, float* latents, int B, long long T, void* stream) {
+  SATB_REQUIRE(g && audio && latents && B >= 1 && T >= 1, "bad argument");
+  for (int r = 0; r < g->world; ++r) SATB_REQUIRE(g->h[r]->finalized, "oobleck: weights not finalized");
+  SATB_REQUIRE(!g->h[0]->cfg.is_decoder, "oobleck group: the handles are decoders");
+  int64_t ratio = 1;
+  for (int i = 0; i < g->h[0]->cfg.n_stages; ++i) ratio *= g->h[0]->cfg.strides[i];
+  SATB_REQUIRE(T % ratio == 0, "encoder: audio length must be a multiple of the downsampling ratio");
+  SATB_REQUIRE(T / ratio < (int64_t(1) << 31), "encoder: sequence too long");
+  return group_run(g, false, audio, latents, B, static_cast<int>(T / ratio), static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -170,6 +170,11 @@ SIGNATURES = {
     "satb_oobleck_finalize": (_I, [_VP, _VP]),
     "satb_oobleck_decode": (_I, [_VP, _VP, _VP, _I, _I, _VP]),
     "satb_oobleck_encode": (_I, [_VP, _VP, _VP, _I, _LL, _VP]),
+    "satb_oobleck_group_plan": (_I, [_I, _I, ctypes.POINTER(SatbOobleckConfig), _I, _VP, _VP, _VP]),
+    "satb_oobleck_group_create": (_I, [_VP, _VP, _I, ctypes.POINTER(_VP)]),
+    "satb_oobleck_group_destroy": (None, [_VP]),
+    "satb_oobleck_group_decode": (_I, [_VP, _VP, _VP, _I, _I, _VP]),
+    "satb_oobleck_group_encode": (_I, [_VP, _VP, _VP, _I, _LL, _VP]),
     "satb_oobleck_probe": (_I, [_VP, ctypes.POINTER(SatbOobleckProbe), _VP]),
     "satb_oobleck_weights": (_I, [_VP, ctypes.c_char_p, _VP, ctypes.POINTER(_LL), _VP]),
     "satb_pqmf_create": (_I, [_I, _I, ctypes.POINTER(_VP)]),
@@ -248,6 +253,15 @@ def group_plan(world, n_prepend, L):
     tb = (ctypes.c_int * (world + 1))()
     check(lib().satb_dit_group_plan(int(world), int(n_prepend), int(L), tb))
     return list(tb)
+
+
+def oobleck_group_plan(world, L, cfg, nearest_upsample=False):
+    """The split of a time-sharded Oobleck decode / encode (satb_oobleck_group_plan) for a handle of SatbOobleckConfig
+    cfg: (begin[world + 1], [(lo, hi)] * world extended latent ranges, margin in latents).  Host only."""
+    begin, ext, m = (ctypes.c_int * (world + 1))(), (ctypes.c_int * (2 * world))(), ctypes.c_int()
+    check(lib().satb_oobleck_group_plan(int(world), int(L), ctypes.byref(cfg), int(bool(nearest_upsample)), begin, ext,
+                                        ctypes.byref(m)))
+    return list(begin), [(ext[2 * r], ext[2 * r + 1]) for r in range(world)], m.value
 
 
 def launch_count():

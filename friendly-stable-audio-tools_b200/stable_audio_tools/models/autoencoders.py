@@ -16,8 +16,10 @@ inner blocks are parameter containers.  ``antialias_activation=True`` is refused
 ``alias_free_torch``, which this package does not ship.  The chunking / cross-fade orchestration is host-side tensor
 slicing on the device, exactly as in the reference.  A nested ``pqmf`` pretransform (``PQMFPretransform``) runs around
 the encoder and decoder where the reference runs it; the encoder then reads, and the decoder writes, io_channels x
-num_bands sub-bands.  Other nested pretransform kinds are refused.
+num_bands sub-bands.  Other nested pretransform kinds are refused.  ``AudioAutoencoder.shard_time(devices)`` runs the
+unchunked encode / decode time-sharded over several ranks (``satb_oobleck_group_*``), bit-identical to one device.
 """
+import contextlib
 import ctypes
 import math
 import typing as tp
@@ -136,6 +138,23 @@ def check_oobleck_io_channels(c, what):
                                   "output must be 1 or 2 channels, or a multiple of 8 up to 128")
 
 
+def check_time_shard_devices(devices):
+    """shard_time's argument, checked as shard_tokens checks a flat list: None, or 1 to 8 CUDA devices (a device may
+    repeat); returns the torch.device list, a device without an index taking the current one."""
+    if devices is None:
+        return None
+    devices = list(devices)
+    if any(isinstance(dv, (list, tuple)) for dv in devices):
+        raise ValueError("shard_time: give a flat list of devices (there is no row layout for the VAE)")
+    if not 1 <= len(devices) <= 8:
+        raise ValueError(f"shard_time: 1 to 8 devices, got {len(devices)}")
+    devices = [torch.device(dv) for dv in devices]
+    for dv in devices:
+        if dv.type != "cuda":
+            raise _native.NativeError(f"shard_time: {dv} is not a CUDA device (this package has no CPU path)")
+    return [dv if dv.index is not None else torch.device("cuda", torch.cuda.current_device()) for dv in devices]
+
+
 class _NativeOobleck(nn.Module):
     """Shared native-handle plumbing of OobleckEncoder / OobleckDecoder."""
 
@@ -145,6 +164,8 @@ class _NativeOobleck(nn.Module):
                      use_snake=True, use_nearest_upsample=False):
         self.__dict__["_h"] = None
         self.__dict__["_dirty"] = True
+        self.__dict__["_shard"] = None           # shard_time state: devices, rank handles, group
+        self.__dict__["_shard_dirty"] = True
         self.__dict__["_ncfg"] = dict(audio_channels=audio_channels, channels=channels, latent_dim=latent_dim,
                                       c_mults=list(c_mults), strides=list(strides), final_tanh=bool(final_tanh),
                                       operand_dtype=operand_dtype, use_snake=bool(use_snake),
@@ -154,12 +175,18 @@ class _NativeOobleck(nn.Module):
 
     def _apply(self, fn, *a, **k):
         self.__dict__["_dirty"] = True
+        self.__dict__["_shard_dirty"] = True
         return super()._apply(fn, *a, **k)
 
     def refresh_native_weights(self):
         self.__dict__["_dirty"] = True
+        self.__dict__["_shard_dirty"] = True
 
     def __del__(self):
+        try:
+            self._drop_shards()
+        except Exception:
+            pass
         h = self.__dict__.get("_h")
         if h is not None:
             try:
@@ -167,41 +194,120 @@ class _NativeOobleck(nn.Module):
             except Exception:
                 pass
 
-    def _handle(self, device):
-        lib = _native.lib()
+    def native_config(self):
+        """The SatbOobleckConfig this module creates its native handles with."""
         nc = self.__dict__["_ncfg"]
+        cfg = _native.SatbOobleckConfig()
+        cfg.in_channels, cfg.channels, cfg.latent_dim = nc["audio_channels"], nc["channels"], nc["latent_dim"]
+        cfg.n_stages = len(nc["c_mults"])
+        for i, (m, s) in enumerate(zip(nc["c_mults"], nc["strides"])):
+            cfg.c_mults[i], cfg.strides[i] = m, s
+        cfg.final_tanh = int(nc["final_tanh"])
+        cfg.is_decoder = int(self._is_decoder)
+        # "fp16" (default) | "bf16" | "fp16x3": split-operand mode, every conv product as (hi, hi) + (lo, hi) + (hi, lo)
+        # with x_lo = fp16(x - x_hi): ~fp32 accuracy (the reference runs these convolutions in strict fp32,
+        # inference/generation.py:165-166) at ~3x the tensor-core work
+        if nc["operand_dtype"] not in ("fp16", "bf16", "fp16x3"):
+            raise ValueError(f"operand_dtype must be fp16, bf16 or fp16x3, got {nc['operand_dtype']}")
+        cfg.operand_dtype = {"fp16": 0, "bf16": 1, "fp16x3": 2}[nc["operand_dtype"]]
+        return cfg
+
+    def _new_handle(self):
+        nc = self.__dict__["_ncfg"]
+        cfg = self.native_config()
+        h = ctypes.c_void_p()
+        act = _native.OOB_ACT_SNAKE if nc["use_snake"] else _native.OOB_ACT_ELU
+        _native.check(_native.lib().satb_oobleck_create_variant(ctypes.byref(cfg), act, int(nc["use_nearest_upsample"]),
+                                                                ctypes.byref(h)))
+        return h
+
+    def _upload_weights(self, h, device, copy_to=None):
+        """Loads every parameter into handle h and finalizes it, on device's current stream.  copy_to: the device the
+        handle lives on, when it is not the parameters' own (a rank of shard_time)."""
+        lib = _native.lib()
+        st = _native.stream_ptr(device)
+        with torch.no_grad():
+            for name, t in self.state_dict().items():
+                if not t.is_cuda:
+                    raise _native.NativeError(f"parameter {name} is on {t.device}: move the model to a CUDA device "
+                                              "(this package has no CPU path)")
+                src = t.detach().to(torch.float32).contiguous()
+                if copy_to is not None:
+                    src = src.to(copy_to)
+                _native.check(lib.satb_oobleck_load_weight(h, name.encode(), _native.ptr(src), src.numel(), st))
+            _native.check(lib.satb_oobleck_finalize(h, st))
+
+    def _handle(self, device):
         if self.__dict__["_h"] is None:
-            cfg = _native.SatbOobleckConfig()
-            cfg.in_channels, cfg.channels, cfg.latent_dim = nc["audio_channels"], nc["channels"], nc["latent_dim"]
-            cfg.n_stages = len(nc["c_mults"])
-            for i, (m, s) in enumerate(zip(nc["c_mults"], nc["strides"])):
-                cfg.c_mults[i], cfg.strides[i] = m, s
-            cfg.final_tanh = int(nc["final_tanh"])
-            cfg.is_decoder = int(self._is_decoder)
-            # "fp16" (default) | "bf16" | "fp16x3": split-operand mode, every conv product as (hi, hi) + (lo, hi) + (hi, lo)
-            # with x_lo = fp16(x - x_hi): ~fp32 accuracy (the reference runs these convolutions in strict fp32,
-            # inference/generation.py:165-166) at ~3x the tensor-core work
-            if nc["operand_dtype"] not in ("fp16", "bf16", "fp16x3"):
-                raise ValueError(f"operand_dtype must be fp16, bf16 or fp16x3, got {nc['operand_dtype']}")
-            cfg.operand_dtype = {"fp16": 0, "bf16": 1, "fp16x3": 2}[nc["operand_dtype"]]
-            h = ctypes.c_void_p()
-            act = _native.OOB_ACT_SNAKE if nc["use_snake"] else _native.OOB_ACT_ELU
-            _native.check(lib.satb_oobleck_create_variant(ctypes.byref(cfg), act, int(nc["use_nearest_upsample"]),
-                                                          ctypes.byref(h)))
-            self.__dict__["_h"] = h
+            self.__dict__["_h"] = self._new_handle()
         if self.__dict__["_dirty"]:
-            st = _native.stream_ptr(device)
-            with torch.no_grad():
-                for name, t in self.state_dict().items():
-                    if not t.is_cuda:
-                        raise _native.NativeError(f"parameter {name} is on {t.device}: move the model to a CUDA device "
-                                                  "(this package has no CPU path)")
-                    src = t.detach().to(torch.float32).contiguous()
-                    _native.check(lib.satb_oobleck_load_weight(self.__dict__["_h"], name.encode(), _native.ptr(src),
-                                                               src.numel(), st))
-                _native.check(lib.satb_oobleck_finalize(self.__dict__["_h"], st))
+            self._upload_weights(self.__dict__["_h"], device)
             self.__dict__["_dirty"] = False
         return self.__dict__["_h"]
+
+    # ------------------------------------------------------------------ time sharding
+    def shard_time(self, devices):
+        """Run every later call time-sharded over ``devices`` (see ``AudioAutoencoder.shard_time``); ``None`` returns to
+        one device."""
+        devices = check_time_shard_devices(devices)
+        self._drop_shards()
+        if devices is not None:
+            self.__dict__["_shard"] = dict(devices=devices, handles=None, group=None)
+            self.__dict__["_shard_dirty"] = True
+        return self
+
+    def _drop_shards(self):
+        sh = self.__dict__.get("_shard")
+        self.__dict__["_shard"] = None
+        if sh is None:
+            return
+        lib = _native.lib()
+        if sh["group"] is not None:
+            lib.satb_oobleck_group_destroy(sh["group"])
+        for h in sh["handles"] or []:
+            lib.satb_oobleck_destroy(h)
+
+    def _shard_group(self, sh):
+        """The group, with every rank handle holding the current weights."""
+        devs = sh["devices"]
+        if sh["handles"] is None:
+            sh["handles"] = [self._new_handle() for _ in devs]
+        if self.__dict__["_shard_dirty"]:
+            for h, dv in zip(sh["handles"], devs):
+                with torch.cuda.device(dv):
+                    self._upload_weights(h, dv, copy_to=dv)   # finalize synchronizes: the weights are in place
+            self.__dict__["_shard_dirty"] = False
+        if sh["group"] is None:
+            g = ctypes.c_void_p()
+            handles = (ctypes.c_void_p * len(devs))(*[h.value for h in sh["handles"]])
+            ids = (ctypes.c_int * len(devs))(*[dv.index for dv in devs])
+            _native.check(_native.lib().satb_oobleck_group_create(handles, ids, len(devs), ctypes.byref(g)))
+            sh["group"] = g
+        return sh["group"]
+
+    def _run(self, x, out_len, single, group):
+        """x [B, C, T] -> fp32 [B, out channels, out_len] by the single-device entry point, or by the group one when the
+        module is time-sharded (and not paused by a chunked path of AudioAutoencoder)."""
+        sh = self.__dict__["_shard"]
+        lib = _native.lib()
+        xin = x.detach().to(torch.float32).contiguous()
+        B, _, T = xin.shape
+        n = ctypes.c_longlong(T) if not self._is_decoder else T
+        if sh is None or self.__dict__.get("_paused"):
+            with torch.cuda.device(x.device):        # the native handle / workspaces live on the model's device
+                h = self._handle(x.device)
+                out = torch.empty(B, self.out_width, out_len, device=x.device, dtype=torch.float32)
+                _native.check(getattr(lib, single)(h, _native.ptr(xin), _native.ptr(out), B, n,
+                                                   _native.stream_ptr(x.device)))
+            return out
+        home = sh["devices"][0]
+        if x.device != home:
+            raise ValueError(f"the time-sharded model's home device is {home}, but the input is on {x.device}")
+        g = self._shard_group(sh)
+        with torch.cuda.device(home):
+            out = torch.empty(B, self.out_width, out_len, device=home, dtype=torch.float32)
+            _native.check(getattr(lib, group)(g, _native.ptr(xin), _native.ptr(out), B, n, _native.stream_ptr(home)))
+        return out
 
 
 class OobleckEncoder(_NativeOobleck):
@@ -225,19 +331,14 @@ class OobleckEncoder(_NativeOobleck):
         self.layers = nn.Sequential(*layers)
         self.downsampling_ratio = int(math.prod(strides))
         self.latent_dim = latent_dim
+        self.out_width = latent_dim
 
     @torch.no_grad()
     def forward(self, x):
         """audio [B, in_channels, T] -> pre-bottleneck [B, latent_dim, T / prod(strides)]"""
         if not x.is_cuda:
             raise _native.NativeError("OobleckEncoder.forward needs CUDA tensors (no CPU fallback)")
-        with torch.cuda.device(x.device):            # the native handle / workspaces live on the model's device
-            h = self._handle(x.device)
-            xin = x.detach().to(torch.float32).contiguous()
-            B, C, T = xin.shape
-            out = torch.empty(B, self.latent_dim, T // self.downsampling_ratio, device=x.device, dtype=torch.float32)
-            _native.check(_native.lib().satb_oobleck_encode(h, _native.ptr(xin), _native.ptr(out), B,
-                                                            ctypes.c_longlong(T), _native.stream_ptr(x.device)))
+        out = self._run(x, x.shape[-1] // self.downsampling_ratio, "satb_oobleck_encode", "satb_oobleck_group_encode")
         return out.to(x.dtype)
 
 
@@ -267,19 +368,14 @@ class OobleckDecoder(_NativeOobleck):
         self.layers = nn.Sequential(*layers)
         self.upsampling_ratio = int(math.prod(strides))
         self.out_channels = out_channels
+        self.out_width = out_channels
 
     @torch.no_grad()
     def forward(self, z):
         """latents [B, latent_dim, L] -> audio [B, out_channels, L * prod(strides)]"""
         if not z.is_cuda:
             raise _native.NativeError("OobleckDecoder.forward needs CUDA tensors (no CPU fallback)")
-        with torch.cuda.device(z.device):            # the native handle / workspaces live on the model's device
-            h = self._handle(z.device)
-            zin = z.detach().to(torch.float32).contiguous()
-            B, C, L = zin.shape
-            out = torch.empty(B, self.out_channels, L * self.upsampling_ratio, device=z.device, dtype=torch.float32)
-            _native.check(_native.lib().satb_oobleck_decode(h, _native.ptr(zin), _native.ptr(out), B, L,
-                                                            _native.stream_ptr(z.device)))
+        out = self._run(z, z.shape[-1] * self.upsampling_ratio, "satb_oobleck_decode", "satb_oobleck_group_decode")
         return out.to(z.dtype)
 
 
@@ -340,6 +436,42 @@ class AudioAutoencoder(nn.Module):
             decoded = torch.tanh(decoded)
         return decoded
 
+    # -- time sharding -------------------------------------------------------------------
+    def shard_time(self, devices):
+        """Run every later unchunked ``encode`` / ``decode`` (``encode_audio`` / ``decode_audio`` with
+        ``chunked=False``) time-sharded over ``devices``; ``None`` returns to one device.
+
+        Rank r runs on ``devices[r]``; a device may repeat (several ranks on one GPU run the same schedule, which is how
+        it is tested on a single GPU).  The parameters stay on the home device ``devices[0]``, where the calls take their
+        inputs and return their outputs; each rank gets its own native Oobleck handle with a copy of the weights,
+        refreshed whenever the parameters change.  Each item's latents are split evenly over the ranks
+        (``satb_oobleck_group_plan``); every rank decodes (encodes) its range plus a recompute margin of the decoder's
+        (encoder's) receptive field on each interior side, and the home device gathers the ranks' own ranges.  The
+        result is bit-identical to the single-device call.  A rank range shorter than the margin, or more ranks than
+        latents, is refused at call time.  Ranks on distinct GPUs need peer-to-peer access with the home device.
+
+        The chunked paths and ``reconstruct_audio(chunked=True)`` run on the home device: their chunks are already the
+        split.  A PQMF pretransform runs on the home device around the sharded Oobleck.  Sharding the DiT of a
+        diffusion model (``shard_tokens``) leaves its pretransform on one device; call this on it to shard the VAE too."""
+        devices = check_time_shard_devices(devices)
+        for m in (self.encoder, self.decoder):
+            if isinstance(m, _NativeOobleck):
+                m.shard_time(devices)
+        return self
+
+    @contextlib.contextmanager
+    def _on_home_device(self):
+        """The chunked paths run their chunks unsharded."""
+        mods = [m for m in (self.encoder, self.decoder) if isinstance(m, _NativeOobleck)]
+        prev = [m.__dict__.get("_paused") for m in mods]
+        for m in mods:
+            m.__dict__["_paused"] = True
+        try:
+            yield
+        finally:
+            for m, p in zip(mods, prev):
+                m.__dict__["_paused"] = p
+
     # -- chunked paths (reference :410-645) ----------------------------------------------
     @staticmethod
     def _chunk_starts(total, chunk, hop, extra=0):
@@ -362,7 +494,8 @@ class AudioAutoencoder(nn.Module):
         return out
 
     def _run_chunks(self, chunks, fn, max_batch_size):
-        outs = [fn(chunks[i:i + max_batch_size]) for i in range(0, chunks.shape[0], max_batch_size)]
+        with self._on_home_device():
+            outs = [fn(chunks[i:i + max_batch_size]) for i in range(0, chunks.shape[0], max_batch_size)]
         return torch.cat(outs, dim=0)
 
     def encode_audio(self, audio, chunked=False, chunk_size=128, overlap=4, max_batch_size=1, **kwargs):

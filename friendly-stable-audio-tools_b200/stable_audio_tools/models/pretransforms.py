@@ -60,6 +60,12 @@ class AutoencoderPretransform(Pretransform):
     def load_state_dict(self, state_dict, strict=True):
         self.model.load_state_dict(state_dict, strict=strict)
 
+    def shard_time(self, devices):
+        """The autoencoder's ``shard_time``: time-shard its unchunked encode / decode over ``devices`` (None: one
+        device)."""
+        self.model.shard_time(devices)
+        return self
+
 
 # ---------------------------------------------------------------------------------------------------- PQMF
 def check_pqmf_bands(num_bands):

@@ -440,6 +440,35 @@ int satb_oobleck_decode(SatbOobleck* h, const float* z, float* audio, int B, int
  * (the deterministic mean|scale tensor; the VAE sampling stays in PyTorch, bottleneck.py:46-62). */
 int satb_oobleck_encode(SatbOobleck* h, const float* audio, float* latents, int B, long long T, void* stream);
 
+/* ---- Time-sharded Oobleck decode / encode: one process drives `world` ranks (1 .. 8), each a finalized handle with a
+ * full copy of the weights on its device; several ranks may share one device.  Rank r runs the ordinary decode (encode)
+ * of latents ext[2r] .. ext[2r + 1] - 1 (their samples for the encoder): its own range begin[r] .. begin[r + 1] - 1 plus
+ * a recompute margin on each interior side, clipped to the item.  The home device (rank 0's) then gathers every rank's
+ * own range, read through peer pointers, into the whole output.  The margin covers the receptive field, and no
+ * convolution route depends on where a position falls in a tile, so the result is bit-identical to the single-device
+ * call. */
+typedef struct SatbOobleckGroup SatbOobleckGroup;
+/* The split of an item of L latents for a handle of config cfg (is_decoder picks the decoder or the encoder) and
+ * nearest_upsample (as satb_oobleck_create_variant): begin[world + 1] (an even split, begin[0] = 0, begin[world] = L),
+ * ext[2 world] (rank r's extended range [ext[2r], ext[2r + 1]) in latents) and *margin, the receptive field of one latent
+ * in latents on either side, derived from the layer list.  world > L is refused, and so is, for world > 1, a rank range
+ * shorter than the margin.  Host only. */
+int satb_oobleck_group_plan(int world, int L, const SatbOobleckConfig* cfg, int nearest_upsample, int* begin, int* ext,
+                            int* margin);
+/* handles[world]: finalized handles of one model (same config and block options, checked), one per rank, each its own;
+ * devices[world]: their device ids, devices[0] the home device.  Ranks on a device other than the home device need peer
+ * access in both directions with it (refused with a message when missing); it is enabled for this process.  The group
+ * owns one stream per rank; the handles outlive the group, which must be destroyed explicitly. */
+int satb_oobleck_group_create(SatbOobleck* const* handles, const int* devices, int world, SatbOobleckGroup** out);
+void satb_oobleck_group_destroy(SatbOobleckGroup* g);
+/* As satb_oobleck_decode / satb_oobleck_encode over the ranks: z, audio (and audio, latents) are whole tensors on the
+ * home device, stream a stream there.  Each rank copies its extended input slice from the home device on its own
+ * stream after the work already on `stream`, then decodes (encodes); the gather kernel runs on `stream` after every
+ * rank, and each rank's next call waits for it.  Enqueues only; the caller's current device is restored.  The per-rank
+ * slices are allocated at their extended shapes and grow when needed (after the last gather). */
+int satb_oobleck_group_decode(SatbOobleckGroup* g, const float* z, float* audio, int B, int L, void* stream);
+int satb_oobleck_group_encode(SatbOobleckGroup* g, const float* audio, float* latents, int B, long long T, void* stream);
+
 /* Test entry points (no product path calls them).
  * satb_oobleck_probe runs ONE step of a finalized handle's decode or encode on caller-owned device buffers, through
  * the same host function (and so the same kernel instances, route, next Snake and raw-stream choice) as the product
