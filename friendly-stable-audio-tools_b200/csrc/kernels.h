@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+struct SatbSamplerStep;   // include/satb200.h
+
 namespace satb {
 
 // ---- attention_tc.cu (tensor-core flash attention; head_dim 32, 64, 96 or 128)
@@ -62,6 +64,9 @@ int launch_quant_rows_fp8(const float* src, void* dst, float* row_scale, const i
 int launch_sampler_update(const float* x, const float* v, const float* d1, const float* d2, const float* nz, float* den,
                           float* x_next, float* x_in, long long n, float c_skip, float c_out, float A, float B, float C,
                           float D, float S, float c_in_next, cudaStream_t stream);
+// One model call's sampler arithmetic of the fixed-step samplers, inpainting blend included (see sampler.cu and
+// SatbSamplerStep in include/satb200.h).
+int launch_sampler_step(const ::SatbSamplerStep& p, cudaStream_t stream);
 // One v-diffusion DDIM step in the reference's fp32 operation order (see elementwise.cu).
 int launch_vdiffusion_update(const float* x, const float* v, const float* nz, float* x_next, float* pred, long long n,
                              float alpha, float sigma, float alpha_next, float adj_sigma, float ddim_sigma,

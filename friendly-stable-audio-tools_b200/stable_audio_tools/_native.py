@@ -83,6 +83,18 @@ class SatbGemmProbe(ctypes.Structure):
                 + [("cos_tab", _VP), ("sin_tab", _VP), ("norm_cols", _I), ("pos_tab", _VP)])
 
 
+SATB_SAMPLER_STEP_BUFS = 4
+
+
+# satb_sampler_step: the parameter block of include/satb200.h
+class SatbSamplerStep(ctypes.Structure):
+    _fields_ = ([("x", _VP), ("y", _VP), ("buf", _VP * SATB_SAMPLER_STEP_BUFS)]
+                + [(n, _VP) for n in ("noise", "mask", "init", "renoise", "den", "d", "x_next", "x_in_next")]
+                + [("n", _LL), ("L", _I)]
+                + [(n, _F) for n in ("c_skip", "c_out", "inv_sigma", "a", "b", "g")] + [("c", _F * SATB_SAMPLER_STEP_BUFS)]
+                + [(n, _F) for n in ("s", "c_in_next", "blend_sigma", "blend_thr")])
+
+
 # satb_attention_probe (tests only): the parameter block of include/satb200.h
 class SatbAttentionProbe(ctypes.Structure):
     _fields_ = ([(n, _I) for n in ("B", "H", "Hkv", "Nq", "Nk", "head_dim", "bf16")]
@@ -138,6 +150,7 @@ SIGNATURES = {
     "satb_snake_beta": (_I, [_VP, _VP, _VP, _VP, _I, _I, _LL, _I, _VP]),
     "satb_sampler_update": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _LL] + [_F] * 8 + [_VP]),
     "satb_vdiffusion_update": (_I, [_VP, _VP, _VP, _VP, _VP, _LL] + [_F] * 5 + [_VP]),
+    "satb_sampler_step": (_I, [ctypes.POINTER(SatbSamplerStep), _VP]),
     "satb_layernorm": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _VP]),
     "satb_layernorm_fp8": (_I, [_VP, _VP, _VP, _VP, _VP, _LL, _I, _I, _VP, _VP, _I, _I, _VP]),
     "satb_linear_f32out": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _VP]),

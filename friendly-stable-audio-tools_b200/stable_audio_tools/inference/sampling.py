@@ -15,6 +15,8 @@ k-diffusion's Brownian-tree noise (torchsde) is replaced by one ``randn_like`` d
 step, which has the same distribution over the disjoint sigma intervals; pass
 ``noise_sampler=`` to inject an explicit sequence.
 """
+import contextlib
+import ctypes
 import math
 
 import torch
@@ -64,15 +66,211 @@ def _noise_fn(x, noise_sampler):
     return lambda sigma, sigma_next: torch.randn_like(x)
 
 
+# ---- the native step path: one satb_sampler_step launch per model call (include/satb200.h gives the algebra)
+def _fusable(x):
+    """The native step path's condition on the sampler state: CUDA fp32 in whole 16-byte vectors."""
+    return x.is_cuda and x.dtype == torch.float32 and x.numel() % 4 == 0
+
+
+def _graph_dit(model):
+    """The native DiT behind a model callable (a DiffusionTransformer, or a DiTWrapper holding one as ``.model``),
+    which can run each call as one CUDA-graph replay; None for any other callable."""
+    dit = None
+    for cand in (model, getattr(model, "model", None)):
+        if cand is not None and hasattr(cand, "cuda_graph") and hasattr(cand, "_graph_forward"):
+            dit = cand
+    return dit
+
+
+@contextlib.contextmanager
+def _graph_replay(dit):
+    """Switch the DiT's ``cuda_graph`` on for a sampling loop and restore it after.  A graph call returns a static buffer
+    that the next call overwrites, so inside the loop no raw model output may be kept across two calls."""
+    if dit is None:
+        yield
+        return
+    prev, dit.cuda_graph = dit.cuda_graph, True
+    try:
+        yield
+    finally:
+        dit.cuda_graph = prev
+
+
+def _launch_step(p):
+    """satb_sampler_step on the parameter dict built by ``_step`` (the CPU tests substitute a torch restatement)."""
+    from .. import _native
+    s = _native.SatbSamplerStep()
+    for k in ("x", "y", "noise", "mask", "init", "renoise", "den", "d", "x_next", "x_in_next"):
+        setattr(s, k, _native.ptr(p[k]))
+    for j, (c, t) in enumerate(zip(p["c"], p["buf"])):
+        s.buf[j], s.c[j] = _native.ptr(t), c
+    for k in ("n", "L", "c_skip", "c_out", "inv_sigma", "a", "b", "g", "s", "c_in_next", "blend_sigma", "blend_thr"):
+        setattr(s, k, p[k])
+    _native.check(_native.lib().satb_sampler_step(ctypes.byref(s), _native.stream_ptr(p["x"].device)))
+
+
+def _step(x, y, c_skip=0.0, c_out=1.0, inv_sigma=0.0, a=0.0, b=0.0, g=0.0, bufs=(), noise=None, s=0.0, blend=None,
+          den=False, d=False, x_next=True, c_in_next=None):
+    """One launch: den = c_out y + c_skip x, the optional inpainting blend of x (in place), d = (x - den) inv_sigma,
+    x_next = a x + b den + g d + sum c buf + s noise and x_in_next = x_next c_in_next.  ``bufs`` holds (c, tensor)
+    pairs, ``blend`` is (inpainting callback, step index, re-noise, sigma).  The default c_out = 1, c_skip = 0 takes y
+    as den.  Returns fresh (den, d, x_next, x_in_next) tensors, None for those not asked for."""
+    if len(bufs) > 4:
+        raise ValueError("satb_sampler_step reads at most 4 stored tensors")
+    new = lambda want: torch.empty_like(x) if want else None
+    p = dict(x=x, y=y, buf=[t for _, t in bufs] + [None] * (4 - len(bufs)),
+             c=[float(c) for c, _ in bufs] + [0.0] * (4 - len(bufs)),
+             noise=None if noise is None else noise.to(x.dtype).contiguous(), mask=None, init=None, renoise=None,
+             den=new(den), d=new(d), x_next=new(x_next), x_in_next=new(c_in_next is not None), n=x.numel(),
+             L=x.shape[-1], c_skip=c_skip, c_out=c_out, inv_sigma=inv_sigma, a=a, b=b, g=g, s=s,
+             c_in_next=c_in_next or 0.0, blend_sigma=0.0, blend_thr=0.0)
+    if blend is not None:
+        inpaint, i, renoise, sigma = blend
+        p.update(mask=inpaint.mask, init=inpaint.init_data, renoise=renoise, blend_sigma=sigma,
+                 blend_thr=(i + 1) / inpaint.steps)
+    _launch_step(p)
+    return p["den"], p["d"], p["x_next"], p["x_in_next"]
+
+
+class _NativeSteps:
+    """The fixed-step k-samplers over a ``VDenoiser`` on the native step path: the inner model is called on
+    x * c_in(sigma) produced by the previous launch, and each call is followed by ONE ``satb_sampler_step`` launch
+    that makes the VDenoiser combine, the update and the next model input.  A step's first call keeps the callback
+    semantics of the torch samplers: the inpainting callback of ``sample_k`` alone is folded into that launch (its
+    re-noise drawn with the same ``torch.randn_like`` call); any other callback gets fresh x / denoised tensors from a
+    denoised-only launch first and may change x in place before the update launch reads it.  Every kept tensor (the
+    state before a two-stage step, derivatives, denoised estimates) is a fresh launch output, never the model's own
+    output buffer, so a graph-replayed DiT may overwrite that at its next call."""
+
+    def __init__(self, model, x, sigmas, extra_args, callback):
+        self.model, self.sigmas, self.extra = model, sigmas, extra_args or {}
+        self.sig = [float(v) for v in sigmas]          # host copies: no device sync inside the loop
+        self.ones = x.new_ones([x.shape[0]])
+        self.inpaint = callback if isinstance(callback, InpaintingCallback) and callback.foldable(x) else None
+        self.callback = None if self.inpaint is not None else callback
+        self.dit = _graph_dit(model.inner_model)
+
+    def scalings(self, sigma):
+        """(c_skip, c_out, c_in) of the VDenoiser at sigma, in float64."""
+        return tuple(float(c) for c in self.model.get_scalings(torch.tensor(float(sigma), dtype=torch.float64)))
+
+    def c_in_after(self, i, sigma):
+        """c_in of the model call that follows step i's last launch (None after the last step)."""
+        return self.scalings(sigma)[2] if i + 2 < len(self.sig) else None
+
+    def call(self, x_in, sigma):
+        """The inner model on an already scaled input; sigma is a schedule entry or a float, as the torch samplers
+        pass it to the VDenoiser (so t is the same fp32 value)."""
+        t = self.model.sigma_to_t(sigma * self.ones)
+        return self.model.inner_model(x_in, t, **self.extra).to(x_in.dtype).contiguous()
+
+    def after_call(self, x, v, i, noise=None, **upd):
+        """The launch(es) after the model call at the start of step i, whose output is v; ``noise`` is a callable drawn
+        after the callback's own draws, as the torch samplers draw it."""
+        c_skip, c_out, _ = self.scalings(self.sig[i])
+        if self.callback is not None:
+            den = _step(x, v, c_skip, c_out, den=True, x_next=False)[0]
+            self.callback({"x": x, "i": i, "sigma": self.sigmas[i], "sigma_hat": self.sigmas[i], "denoised": den})
+            out = _step(x, den, noise=noise() if noise else None, **dict(upd, den=False))
+            return (den,) + out[1:]
+        blend = None
+        if self.inpaint is not None:
+            blend = (self.inpaint, i, torch.randn_like(self.inpaint.init_data), self.sig[i])
+        return _step(x, v, c_skip, c_out, noise=noise() if noise else None, blend=blend, **upd)
+
+    def first(self, x, i, x_in, noise=None, **upd):
+        return self.after_call(x, self.call(x_in, self.sigmas[i]), i, noise, **upd)
+
+    def second(self, x, sigma, x_in, noise=None, **upd):
+        """The launch after a step's second model call at sigma (no callback there)."""
+        v = self.call(x_in, sigma)
+        c_skip, c_out, _ = self.scalings(sigma)
+        return _step(x, v, c_skip, c_out, noise=noise() if noise else None, **upd)
+
+    def run(self, sampler, x, *args):
+        with _graph_replay(self.dit):
+            x = x.contiguous()
+            return sampler(x, x * self.scalings(self.sig[0])[2], *args)
+
+    def heun(self, x, x_in):
+        sig = self.sig
+        for i in range(len(sig) - 1):
+            dt = sig[i + 1] - sig[i]
+            if sig[i + 1] == 0:
+                x = self.first(x, i, x_in, inv_sigma=1.0 / sig[i], a=1.0, g=dt)[2]
+            else:
+                _, d, x_2, x_in_2 = self.first(x, i, x_in, inv_sigma=1.0 / sig[i], a=1.0, g=dt, d=True,
+                                               c_in_next=self.scalings(sig[i + 1])[2])
+                _, _, x, x_in = self.second(x_2, self.sigmas[i + 1], x_in_2, inv_sigma=1.0 / sig[i + 1], g=0.5 * dt,
+                                            bufs=((1.0, x), (0.5 * dt, d)), c_in_next=self.c_in_after(i, sig[i + 1]))
+        return x
+
+    def dpm_2(self, x, x_in):
+        sig = self.sig
+        for i in range(len(sig) - 1):
+            if sig[i + 1] == 0:
+                x = self.first(x, i, x_in, inv_sigma=1.0 / sig[i], a=1.0, g=sig[i + 1] - sig[i])[2]
+            else:
+                sigma_mid = math.exp(0.5 * (math.log(sig[i]) + math.log(sig[i + 1])))
+                _, _, x_2, x_in_2 = self.first(x, i, x_in, inv_sigma=1.0 / sig[i], a=1.0, g=sigma_mid - sig[i],
+                                               c_in_next=self.scalings(sigma_mid)[2])
+                _, _, x, x_in = self.second(x_2, sigma_mid, x_in_2, inv_sigma=1.0 / sigma_mid, g=sig[i + 1] - sig[i],
+                                            bufs=((1.0, x),), c_in_next=self.c_in_after(i, sig[i + 1]))
+        return x
+
+    def lms(self, x, x_in, order):
+        sig, ds = self.sig, []                         # ds: the derivatives of the previous steps, oldest first
+        for i in range(len(sig) - 1):
+            cur = min(i + 1, order)
+            coef = [_lms_coeff(cur, sig, i, j) for j in range(cur)]
+            _, d, x, x_in = self.first(x, i, x_in, inv_sigma=1.0 / sig[i], a=1.0, g=coef[0],
+                                       bufs=tuple((coef[j], ds[-j]) for j in range(1, cur)), d=i + 2 < len(sig),
+                                       c_in_next=self.c_in_after(i, sig[i + 1]))
+            ds = (ds + [d])[-(order - 1):] if order > 1 else []
+        return x
+
+    def dpmpp_2s_ancestral(self, x, x_in, eta, s_noise, noise):
+        sig = self.sig
+        for i in range(len(sig) - 1):
+            sigma_down, sigma_up = get_ancestral_step(sig[i], sig[i + 1], eta)
+            nz, s = None, 0.0
+            if sig[i + 1] > 0 and sigma_up > 0:
+                nz, s = (lambda i=i: noise(self.sigmas[i], self.sigmas[i + 1])), s_noise * sigma_up
+            if sigma_down == 0:
+                x, x_in = self.first(x, i, x_in, nz, s=s, inv_sigma=1.0 / sig[i], a=1.0, g=sigma_down - sig[i],
+                                     c_in_next=self.c_in_after(i, sig[i + 1]))[2:]
+            else:
+                t, t_next = -math.log(sig[i]), -math.log(sigma_down)
+                h = t_next - t
+                s_mid = t + 0.5 * h
+                sigma_mid = math.exp(-s_mid)
+                _, _, x_2, x_in_2 = self.first(x, i, x_in, a=sigma_mid / math.exp(-t), b=-math.expm1(-0.5 * h),
+                                               c_in_next=self.scalings(sigma_mid)[2])
+                x, x_in = self.second(x_2, sigma_mid, x_in_2, nz, s=s, b=-math.expm1(-h),
+                                      bufs=((math.exp(-t_next) / math.exp(-t), x),),
+                                      c_in_next=self.c_in_after(i, sig[i + 1]))[2:]
+        return x
+
+
+def _native_steps(model, x, sigmas, extra_args, callback):
+    """A ``_NativeSteps`` when the native step path applies to (model, x), else None (CPU tensors, other dtypes and
+    wrappers other than ``VDenoiser`` keep the torch samplers)."""
+    if isinstance(model, VDenoiser) and _fusable(x):
+        return _NativeSteps(model, x, sigmas, extra_args, callback)
+    return None
+
+
 class MultistepSdeStepper:
     """DPM-Solver++(2M) SDE / DPM-Solver++(3M) SDE as a state machine with one model call per ``step()``.
 
     Every update of both samplers is linear in the tensors involved,
         x_next = A x + B den + C den_1 + D den_2 + S noise,
     with scalars that depend only on the sigma schedule (``coeffs``).  On CUDA, with the standard ``VDenoiser``
-    wrapper and no callback, the denoiser scalings, this update and the scaling of the next model input run
-    as ONE kernel (``satb_sampler_update``) instead of ~20 elementwise launches; otherwise the same algebra is
-    evaluated with torch ops (CPU tensors in the tests, callbacks that need ``denoised`` before the update).
+    wrapper, the denoiser scalings, this update and the scaling of the next model input run as ONE kernel instead
+    of ~20 elementwise launches: ``satb_sampler_update`` without a callback, ``satb_sampler_step`` with the inpainting
+    blend folded in for ``sample_k``'s inpainting callback, and a denoised-only launch, the callback, then the update
+    launch for any other callback (``_NativeSteps.after_call``).  Otherwise the same algebra is evaluated with torch
+    ops (CPU tensors, other dtypes and wrappers).
     """
 
     def __init__(self, model, x, sigmas, order=3, extra_args=None, callback=None, eta=1.0, s_noise=1.0,
@@ -86,16 +284,14 @@ class MultistepSdeStepper:
         self.i = 0
         self.den_1 = self.den_2 = None
         self.h_1 = self.h_2 = None
-        self.fused = (isinstance(model, VDenoiser) and callback is None and x.is_cuda and x.dtype == torch.float32
-                      and x.numel() % 4 == 0)
+        self.fused = isinstance(model, VDenoiser) and _fusable(x)
         # the native DiT (directly, or as DiTWrapper.model) can run a call as one CUDA-graph launch; its output is then a
         # static buffer, which is safe here because the fused update consumes v before the next model call
-        self.graph_dit = None
-        if self.fused:
-            inner = getattr(model, "inner_model", None)
-            for cand in (inner, getattr(inner, "model", None)):
-                if cand is not None and hasattr(cand, "cuda_graph") and hasattr(cand, "_graph_forward"):
-                    self.graph_dit = cand
+        self.graph_dit = _graph_dit(model.inner_model) if self.fused else None
+        self.native = None
+        if self.fused and callback is not None:
+            self.x = x.contiguous()
+            self.native = _NativeSteps(model, x, sigmas, self.extra_args, callback)
         self.x_in = None                               # x * c_in(sigma_i), produced by the previous fused update
 
     def coeffs(self, i):
@@ -145,15 +341,22 @@ class MultistepSdeStepper:
                 self.x_in = x * c_in
             t = self.model.sigma_to_t(self.sigmas[i]) * self.ones
             v = self.model.inner_model(self.x_in, t, **self.extra_args)
-            v = v.to(torch.float32).contiguous()
+            v = v.to(x.dtype).contiguous()
             c_in_next = 1.0 / math.sqrt(sig[i + 1] ** 2 + self.model.sigma_data ** 2)
-            den, x_next, x_in_next = torch.empty_like(x), torch.empty_like(x), torch.empty_like(x)
-            xc = x.contiguous()
-            _native.check(_native.lib().satb_sampler_update(
-                _native.ptr(xc), _native.ptr(v), _native.ptr(self.den_1 if C != 0.0 else None),
-                _native.ptr(self.den_2 if D != 0.0 else None), _native.ptr(nz.contiguous() if nz is not None else None),
-                _native.ptr(den), _native.ptr(x_next), _native.ptr(x_in_next), x.numel(), c_skip, c_out, A, B, C, D, S,
-                c_in_next, _native.stream_ptr(x.device)))
+            if self.native is not None:
+                bufs = tuple((c, t) for c, t in ((C, self.den_1), (D, self.den_2)) if c != 0.0)
+                den, _, x_next, x_in_next = self.native.after_call(x, v, i, a=A, b=B, bufs=bufs, s=S,
+                                                                   noise=(lambda: nz) if nz is not None else None,
+                                                                   den=True, c_in_next=c_in_next)
+            else:
+                den, x_next, x_in_next = torch.empty_like(x), torch.empty_like(x), torch.empty_like(x)
+                xc = x.contiguous()
+                _native.check(_native.lib().satb_sampler_update(
+                    _native.ptr(xc), _native.ptr(v), _native.ptr(self.den_1 if C != 0.0 else None),
+                    _native.ptr(self.den_2 if D != 0.0 else None),
+                    _native.ptr(nz.contiguous() if nz is not None else None), _native.ptr(den), _native.ptr(x_next),
+                    _native.ptr(x_in_next), x.numel(), c_skip, c_out, A, B, C, D, S, c_in_next,
+                    _native.stream_ptr(x.device)))
             self.x_in = x_in_next
         else:
             den = self.model(x, self.sigmas[i] * self.ones, **self.extra_args)
@@ -173,15 +376,9 @@ class MultistepSdeStepper:
         return x_next
 
     def run(self):
-        prev = None
-        if self.graph_dit is not None:
-            prev, self.graph_dit.cuda_graph = self.graph_dit.cuda_graph, True
-        try:
+        with _graph_replay(self.graph_dit):
             for _ in range(len(self.sig) - 1):
                 self.step()
-        finally:
-            if self.graph_dit is not None:
-                self.graph_dit.cuda_graph = prev
         return self.x
 
 
@@ -207,6 +404,9 @@ def _to_d(x, sigma, denoised):
 @torch.no_grad()
 def sample_heun(model, x, sigmas, extra_args=None, callback=None, disable=None, **_):
     """Karras et al. 2022, Algorithm 1 without churn: Euler step + trapezoidal correction."""
+    native = _native_steps(model, x, sigmas, extra_args, callback)
+    if native is not None:
+        return native.run(native.heun, x)
     extra_args = extra_args or {}
     ones = x.new_ones([x.shape[0]])
     sig = [float(v) for v in sigmas]
@@ -228,6 +428,9 @@ def sample_heun(model, x, sigmas, extra_args=None, callback=None, disable=None, 
 @torch.no_grad()
 def sample_dpm_2(model, x, sigmas, extra_args=None, callback=None, disable=None, **_):
     """Second-order sampler with the midpoint taken in log-sigma (Karras et al. 2022, Algorithm 2 without churn)."""
+    native = _native_steps(model, x, sigmas, extra_args, callback)
+    if native is not None:
+        return native.run(native.dpm_2, x)
     extra_args = extra_args or {}
     ones = x.new_ones([x.shape[0]])
     sig = [float(v) for v in sigmas]
@@ -261,6 +464,9 @@ def _lms_coeff(order, t, i, j):
 @torch.no_grad()
 def sample_lms(model, x, sigmas, extra_args=None, callback=None, disable=None, order=4, **_):
     """Linear multistep (Adams-Bashforth in sigma) of order <= 4 over the derivative history."""
+    native = _native_steps(model, x, sigmas, extra_args, callback)
+    if native is not None and 1 <= order <= 4:
+        return native.run(native.lms, x, order)
     extra_args = extra_args or {}
     ones = x.new_ones([x.shape[0]])
     sig = [float(v) for v in sigmas]
@@ -291,6 +497,9 @@ def sample_dpmpp_2s_ancestral(model, x, sigmas, extra_args=None, callback=None, 
                               noise_sampler=None):
     """DPM-Solver++(2S) with ancestral noise (Lu et al. 2022, data-prediction, single-step second order)."""
     noise = _noise_fn(x, noise_sampler)
+    native = _native_steps(model, x, sigmas, extra_args, callback)
+    if native is not None:
+        return native.run(native.dpmpp_2s_ancestral, x, eta, s_noise, noise)
     extra_args = extra_args or {}
     ones = x.new_ones([x.shape[0]])
     sig = [float(v) for v in sigmas]
@@ -435,7 +644,15 @@ def sample_dpm_fast(model, x, sigma_min, sigma_max, n, extra_args=None, callback
     """DPM-Solver with a fixed budget of n model evaluations between sigma_max and sigma_min."""
     if sigma_min <= 0 or sigma_max <= 0:
         raise ValueError("sigma_min and sigma_max must not be 0")
-    return _DPMSolver(model, extra_args, callback).fast(x, -math.log(sigma_max), -math.log(sigma_min), n)
+    with _graph_replay(_dpm_solver_dit(model, x)):
+        return _DPMSolver(model, extra_args, callback).fast(x, -math.log(sigma_max), -math.log(sigma_min), n)
+
+
+def _dpm_solver_dit(model, x):
+    """The DPM-Solver samplers keep their torch arithmetic (the adaptive one needs the error norm on the host every
+    step) and only replay the DiT from its graph, under the native step path's condition.  Safe: every eps they keep
+    is computed from the VDenoiser's output, a fresh tensor, never the graph's output buffer itself."""
+    return _graph_dit(model.inner_model) if isinstance(model, VDenoiser) and _fusable(x) else None
 
 
 @torch.no_grad()
@@ -444,8 +661,9 @@ def sample_dpm_adaptive(model, x, sigma_min, sigma_max, extra_args=None, callbac
     """DPM-Solver-12/23 with adaptive step size (PID controller on the embedded error estimate)."""
     if sigma_min <= 0 or sigma_max <= 0:
         raise ValueError("sigma_min and sigma_max must not be 0")
-    return _DPMSolver(model, extra_args, callback).adaptive(x, -math.log(sigma_max), -math.log(sigma_min), order, rtol,
-                                                            atol, h_init, pcoeff, icoeff, dcoeff, accept_safety)
+    with _graph_replay(_dpm_solver_dit(model, x)):
+        return _DPMSolver(model, extra_args, callback).adaptive(x, -math.log(sigma_max), -math.log(sigma_min), order,
+                                                                rtol, atol, h_init, pcoeff, icoeff, dcoeff, accept_safety)
 
 
 # sampler_type -> (function, takes a sigma schedule?)  (reference inference/sampling.py:211-228)
@@ -459,6 +677,30 @@ SAMPLERS = {
 def get_bmask(i, steps, mask):
     """Shrinking hard mask for soft-mask inpainting (reference generation.py:277-281)."""
     return torch.where(mask <= (i + 1) / steps, 1, 0)
+
+
+class InpaintingCallback:
+    """The k-diffusion callback of soft-mask inpainting (reference inference/sampling.py:187-198): after each step's first
+    model call it re-noises init_data to that step's sigma and pastes it into x, in place, where the shrinking hard
+    mask keeps the input.  A class rather than a closure so that the native step path recognises it and folds the
+    blend into its update launch (``foldable``)."""
+
+    def __init__(self, init_data, mask, steps):
+        self.init_data, self.mask, self.steps = init_data, mask, steps
+
+    def __call__(self, args):
+        i, xx, sigma = args["i"], args["x"], args["sigma"]
+        noised = self.init_data + torch.randn_like(self.init_data) * sigma
+        bm = get_bmask(i, self.steps, self.mask)
+        xx[:, :, :] = (noised * bm + xx * (1 - bm))[:, :, :]
+
+    def foldable(self, x):
+        """Whether satb_sampler_step can apply the blend to the state x: a [L] fp32 mask over its last dim and an
+        init_data of its own shape and dtype, contiguous and on its device."""
+        m, d = self.mask, self.init_data
+        return (m.dim() == 1 and m.shape[0] == x.shape[-1] and m.dtype == torch.float32 and m.device == x.device
+                and m.is_contiguous() and d.shape == x.shape and d.dtype == x.dtype and d.device == x.device
+                and d.is_contiguous())
 
 
 def sample_k(model_fn, noise, init_data=None, mask=None, steps=100, sampler_type="dpmpp-2m-sde", sigma_min=0.5,
@@ -477,13 +719,7 @@ def sample_k(model_fn, noise, init_data=None, mask=None, steps=100, sampler_type
     elif exists(mask) and exists(init_data):
         bmask = get_bmask(0, steps, mask)                       # inpainting
         x = (init_data + noise) * bmask + noise * (1 - bmask)
-
-        def inpainting_callback(args):
-            i, xx, sigma = args["i"], args["x"], args["sigma"]
-            noised = init_data + torch.randn_like(init_data) * sigma
-            bm = get_bmask(i, steps, mask)
-            xx[:, :, :] = (noised * bm + xx * (1 - bm))[:, :, :]
-
+        inpainting_callback = InpaintingCallback(init_data, mask, steps)
         if callback is None:
             wrapped_callback = inpainting_callback
         else:
@@ -542,15 +778,7 @@ def sample(model, x, steps, eta, verbose: bool = True, noise_sampler=None, **ext
     noise = noise_sampler if noise_sampler is not None else (lambda i: torch.randn_like(x))
     ones = x.new_ones([x.shape[0]])
     fused = x.is_cuda and x.dtype == torch.float32
-    graph_dit = None
-    if fused:
-        for cand in (model, getattr(model, "model", None)):
-            if cand is not None and hasattr(cand, "cuda_graph") and hasattr(cand, "_graph_forward"):
-                graph_dit = cand
-    prev = None
-    if graph_dit is not None:
-        prev, graph_dit.cuda_graph = graph_dit.cuda_graph, True
-    try:
+    with _graph_replay(_graph_dit(model) if fused else None):
         pred = None
         for i, (t_i, a, s, a_next, adj, ddim) in enumerate(sched):
             v = model(x, ones * t_i, **extra_args).float()
@@ -574,18 +802,30 @@ def sample(model, x, steps, eta, verbose: bool = True, noise_sampler=None, **ext
                     x = pred * a_next + eps * adj
                     if nz is not None:
                         x += nz * ddim
-    finally:
-        if graph_dit is not None:
-            graph_dit.cuda_graph = prev
     return pred
 
 
 @torch.no_grad()
 def sample_discrete_euler(model, x, steps, sigma_max=1, callback=None, **extra_args):
     """Rectified-flow sampling (reference inference/sampling.py:29-60): the network predicts the velocity and
-    the state is integrated from t = sigma_max down to 0 on a uniform grid, x += (t_next - t) * v(x, t)."""
+    the state is integrated from t = sigma_max down to 0 on a uniform grid, x += (t_next - t) * v(x, t).
+
+    CUDA fp32 state (``_fusable``): the update is one ``satb_sampler_step`` launch per call, and a native DiT (a
+    DiTWrapper or a DiffusionTransformer) runs each call as one CUDA-graph replay; a callback gets x and a fresh
+    denoised = x - t v from a launch of its own, before the update launch reads x."""
     ts = torch.linspace(sigma_max, 0, steps + 1)
     ones = x.new_ones([x.shape[0]])
+    if _fusable(x):
+        with _graph_replay(_graph_dit(model)):
+            x = x.contiguous()
+            for i in range(steps):
+                t_curr, t_next = float(ts[i]), float(ts[i + 1])
+                v = model(x, t_curr * ones, **extra_args).to(x.dtype).contiguous()
+                if callback is not None:
+                    den = _step(x, v, c_skip=1.0, c_out=-t_curr, den=True, x_next=False)[0]
+                    callback({"x": x, "i": i, "t": t_curr, "denoised": den})
+                x = _step(x, v, a=1.0, b=t_next - t_curr)[2]
+        return x
     for i in range(steps):
         t_curr, t_next = float(ts[i]), float(ts[i + 1])
         v = model(x, t_curr * ones, **extra_args)

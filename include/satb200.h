@@ -339,6 +339,38 @@ int satb_sampler_update(const float* x, const float* v, const float* den_1, cons
  * All tensors fp32 with n >= 1 elements; outputs must not overlap the inputs. */
 int satb_vdiffusion_update(const float* x, const float* v, const float* noise, float* x_next, float* pred, long long n,
                            float alpha, float sigma, float alpha_next, float adj_sigma, float ddim_sigma, void* stream);
+/* One model call's worth of sampler arithmetic for every fixed-step sampler of inference/sampling.py (Euler for
+ * rectified flow, Heun, DPM-2, linear multistep, DPM-Solver++(2S) ancestral, and the multistep SDE samplers with a
+ * callback or inpainting) in a single pass over the latents.  Each of them is linear in x (the state the model was
+ * called at), y (the model output), a few stored tensors and the noise, so one kernel serves all of them with
+ * host-computed scalars:
+ *   den    = c_out y + c_skip x                                     (VDenoiser.forward; c_out = 1, c_skip = 0 passes a
+ *                                                                    den computed earlier through as y)
+ *   x      = mask[l] <= blend_thr ? init + renoise * blend_sigma : x (the inpainting callback, written back into x;
+ *                                                                    only when mask is given; l = index % L)
+ *   d      = (x - den) * inv_sigma                                  (the Karras ODE derivative)
+ *   x_next = a x + b den + g d + sum_k c[k] buf[k] + s noise;  x_in_next = x_next * c_in_next.
+ * den, d, x_next and x_in_next are written when non-NULL (at least one must be); buf[k] is read when non-NULL, noise
+ * when non-NULL.  All tensors fp32, n elements (n % 4 == 0), 16-byte aligned, no output overlapping an input; mask
+ * is [L] fp32 and the blend rounds init + renoise * blend_sigma like the fp32 torch expression. */
+#define SATB_SAMPLER_STEP_BUFS 4
+typedef struct SatbSamplerStep {
+  float* x;                                   /* read; written back only with a mask */
+  const float* y;
+  const float* buf[SATB_SAMPLER_STEP_BUFS];
+  const float* noise;
+  const float* mask;                          /* [L] */
+  const float* init;
+  const float* renoise;
+  float* den;
+  float* d;
+  float* x_next;
+  float* x_in_next;
+  long long n;
+  int L;
+  float c_skip, c_out, inv_sigma, a, b, g, c[SATB_SAMPLER_STEP_BUFS], s, c_in_next, blend_sigma, blend_thr;
+} SatbSamplerStep;
+int satb_sampler_step(const SatbSamplerStep* p, void* stream);
 /* softmax(q k^T / sqrt(64)) v (transformer.py:496-536): q [B, Nq, H*64], k/v [B, Nk, Hkv*64],
  * out [B, Nq, H*64]; 16-bit, contiguous. */
 int satb_attention(const void* q16, const void* k16, const void* v16, void* o16, int B, int H, int Hkv, int Nq, int Nk,
