@@ -2,14 +2,8 @@
 //   O = softmax(Q K^T / sqrt(D)) V      (reference models/transformer.py:496-536)
 //
 // Head dim 64 (every shipped model) runs attn_wgmma_kernel, described at the kernel below.  The other head dims run
-// attn_kernel<D>:
-// One CTA of four warps per 64 query rows of one (batch item, head); each warp owns 16 query rows.  Keys are
-// processed in tiles of 64, double-buffered in shared memory by cp.async (rows past the end are zero-filled, their
-// scores masked).  Per tile and warp: S = Q K^T with mma.sync m16n8k16 (Q fragments stay in registers for the whole
-// row block, K fragments by ldmatrix), online softmax in fp32 on the S fragments (exp2, row max / sum reduced over the
-// four lanes of a row), then O += P V with P repacked from the S fragments into 16-bit A fragments and V fragments
-// by ldmatrix.trans.  The normalised output goes through shared memory so that it leaves as 16-byte row segments.
-// The kernel is a template on D: D / 16 k-slices of Q K^T, D / 8 output fragments, 64 x D tiles.
+// attn_kernel<D>: one CTA of four warps per 64 query rows of one (batch item, head), the mma.sync flash-attention core
+// of mma_tile.cuh (mma_attention) with the 1 / sqrt(D) scale in log2 units; head h reads kv head h / group.
 #include "common.cuh"
 #include "gemm.cuh"
 #include "kernels.h"
@@ -22,14 +16,6 @@ namespace satb {
 
 namespace {
 
-constexpr int kQ = 64;          // query rows per CTA
-constexpr int kK = 64;          // keys per tile
-constexpr int kAttnThreads = 128;
-template <int D>
-constexpr int tile_elems() { return 64 * D; }                    // one 64 x D 16-bit tile: 4, 8, 12 or 16 KB
-template <int D>
-constexpr int attn_smem() { return (1 + 2 * 2) * tile_elems<D>() * 2; }   // Q, two K and two V buffers: 20 .. 80 KB
-
 struct AttnArgs {
   const uint16_t *q, *k, *v;
   uint16_t* o;
@@ -40,153 +26,17 @@ struct AttnArgs {
 };
 
 template <int D, bool BF16>
-__global__ void __launch_bounds__(kAttnThreads) attn_kernel(const AttnArgs p) {
-  constexpr int kTileElems = tile_elems<D>();
-  constexpr int kChunks = D / 8;   // 16-byte chunks per tile row
+__global__ void __launch_bounds__(kMmaAttnThreads) attn_kernel(const AttnArgs p) {
   extern __shared__ __align__(128) uint16_t smem_attn[];
-  uint16_t* sQ = smem_attn;
-  uint16_t* sK = sQ + kTileElems;        // [2][64 x D]
-  uint16_t* sV = sK + 2 * kTileElems;    // [2][64 x D]
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * kQ, h = blockIdx.y, b = blockIdx.z;
+  // the item's rows and the head's columns come from the arguments alone: worked out while the previous kernel drains
+  const int h = blockIdx.y, b = blockIdx.z;
   const int hk = h / p.group;
-  const uint16_t* qb = p.q + b * p.q_bs;
-  const uint16_t* kbase = p.k + b * p.k_bs;
-  const uint16_t* vbase = p.v + b * p.v_bs;
+  const uint16_t *q = p.q + b * p.q_bs, *k = p.k + b * p.k_bs, *v = p.v + b * p.v_bs;
   const int qc = p.q_col + h * D, kc = p.k_col + hk * D, vc = p.v_col + hk * D;
-  const int n_tiles = (p.Nk + kK - 1) / kK;
-
   pdl_launch_dependents();
   pdl_wait();   // q / k / v are written by the previous kernels
-  load_tile<D>(sQ, qb, p.ldq, q0, p.Nq, qc);
-  load_tile<D>(sK, kbase, p.ldk, 0, p.Nk, kc);
-  load_tile<D>(sV, vbase, p.ldv, 0, p.Nk, vc);
-  cp_async_commit();
-
-  uint32_t qf[D / 16][4];   // Q fragments of this warp's 16 rows, D / 16 16-wide slices of the head dim
-  float o[D / 8][4];        // O: 16 rows x D columns as D / 8 8-column fragments
-  float m[2] = {-1e30f, -1e30f}, l[2] = {0.f, 0.f};   // rows lane / 4 and lane / 4 + 8 (scaled log2 units)
-#pragma unroll
-  for (int j = 0; j < D / 8; ++j) o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f;
-
-  for (int t = 0; t < n_tiles; ++t) {
-    const int buf = t & 1;
-    if (t + 1 < n_tiles) {   // next tile into the other buffer (freed by the barrier at the end of tile t - 1)
-      load_tile<D>(sK + (buf ^ 1) * kTileElems, kbase, p.ldk, (t + 1) * kK, p.Nk, kc);
-      load_tile<D>(sV + (buf ^ 1) * kTileElems, vbase, p.ldv, (t + 1) * kK, p.Nk, vc);
-      cp_async_commit();
-      cp_async_wait<1>();
-    } else {
-      cp_async_wait<0>();
-    }
-    __syncthreads();
-    if (t == 0) {
-      const uint32_t sq = smem_u32(sQ);
-#pragma unroll
-      for (int kk = 0; kk < D / 16; ++kk) {
-        const int r = warp * 16 + (lane & 7) + 8 * ((lane >> 3) & 1), c = 2 * kk + (lane >> 4);
-        ldsm_x4(sq + swz<D>(r, c) * 2, qf[kk][0], qf[kk][1], qf[kk][2], qf[kk][3]);
-      }
-    }
-    // S = Q K^T: 16 rows x 64 keys
-    float s[8][4];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
-    const uint32_t sk = smem_u32(sK + buf * kTileElems);
-#pragma unroll
-    for (int kk = 0; kk < D / 16; ++kk) {
-#pragma unroll
-      for (int nb = 0; nb < 4; ++nb) {   // keys 16 nb .. 16 nb + 15
-        const int r = 16 * nb + (lane & 7) + 8 * (lane >> 4), c = 2 * kk + ((lane >> 3) & 1);
-        uint32_t b0, b1, b2, b3;
-        ldsm_x4(sk + swz<D>(r, c) * 2, b0, b1, b2, b3);
-        mma16816<BF16>(s[2 * nb], qf[kk], b0, b1);
-        mma16816<BF16>(s[2 * nb + 1], qf[kk], b2, b3);
-      }
-    }
-    // online softmax
-    const int key0 = t * kK + 2 * (lane & 3);
-    float mx[2] = {m[0], m[1]};
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const bool ok = key0 + 8 * j + (e & 1) < p.Nk;
-        s[j][e] = ok ? s[j][e] * p.scale_log2 : -INFINITY;
-        mx[e >> 1] = fmaxf(mx[e >> 1], s[j][e]);
-      }
-    }
-    float alpha[2];
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 1));
-      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 2));
-      alpha[i] = exp2f(m[i] - mx[i]);
-      m[i] = mx[i];
-      l[i] *= alpha[i];
-    }
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        s[j][e] = exp2f(s[j][e] - m[e >> 1]);
-        l[e >> 1] += s[j][e];
-        if (j < D / 8) o[j][e] *= alpha[e >> 1];
-      }
-    }
-#pragma unroll
-    for (int j = 8; j < D / 8; ++j) {   // head dims 96, 128: the O fragments past the eighth
-#pragma unroll
-      for (int e = 0; e < 4; ++e) o[j][e] *= alpha[e >> 1];
-    }
-    // O += P V
-    const uint32_t sv = smem_u32(sV + buf * kTileElems);
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {   // keys 16 kk .. 16 kk + 15
-      uint32_t a[4];
-      a[0] = Op16<BF16>::pack(s[2 * kk][0], s[2 * kk][1]);
-      a[1] = Op16<BF16>::pack(s[2 * kk][2], s[2 * kk][3]);
-      a[2] = Op16<BF16>::pack(s[2 * kk + 1][0], s[2 * kk + 1][1]);
-      a[3] = Op16<BF16>::pack(s[2 * kk + 1][2], s[2 * kk + 1][3]);
-#pragma unroll
-      for (int db = 0; db < D / 16; ++db) {   // head-dim columns 16 db .. 16 db + 15
-        const int r = 16 * kk + (lane & 7) + 8 * ((lane >> 3) & 1), c = 2 * db + (lane >> 4);
-        uint32_t b0, b1, b2, b3;
-        ldsm_x4_t(sv + swz<D>(r, c) * 2, b0, b1, b2, b3);
-        mma16816<BF16>(o[2 * db], a, b0, b1);
-        mma16816<BF16>(o[2 * db + 1], a, b2, b3);
-      }
-    }
-    __syncthreads();   // this buffer may be refilled
-  }
-
-  // normalise; stage the warp's 16 rows in its own rows of the Q tile, then 16-byte stores
-  float inv[2];
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    l[i] += __shfl_xor_sync(0xffffffffu, l[i], 1);
-    l[i] += __shfl_xor_sync(0xffffffffu, l[i], 2);
-    inv[i] = 1.f / l[i];
-  }
-  const int rr = warp * 16 + (lane >> 2);
-#pragma unroll
-  for (int j = 0; j < D / 8; ++j) {
-    const int col = 8 * j + 2 * (lane & 3);
-    *reinterpret_cast<uint32_t*>(sQ + swz<D>(rr, col >> 3) + (col & 7)) = Op16<BF16>::pack(o[j][0] * inv[0], o[j][1] * inv[0]);
-    *reinterpret_cast<uint32_t*>(sQ + swz<D>(rr + 8, col >> 3) + (col & 7)) =
-        Op16<BF16>::pack(o[j][2] * inv[1], o[j][3] * inv[1]);
-  }
-  __syncwarp();
-  uint16_t* ob = p.o + b * p.o_bs + h * D;
-#pragma unroll
-  for (int i = 0; i < 16 * kChunks / 32; ++i) {
-    const int idx = lane + 32 * i;
-    const int r = warp * 16 + chunk_row<kChunks>(idx), c = chunk_col<kChunks>(idx);
-    if (q0 + r < p.Nq)
-      *reinterpret_cast<uint4*>(ob + static_cast<int64_t>(q0 + r) * p.ldo + c * 8) =
-          *reinterpret_cast<const uint4*>(sQ + swz<D>(r, c));
-  }
+  mma_attention<D, BF16>(smem_attn, q, p.ldq, qc, k, p.ldk, kc, v, p.ldv, vc, p.o + b * p.o_bs, p.ldo, h * D,
+                         blockIdx.x * 64, p.Nq, p.Nk, ScaleScore{p.scale_log2});
 }
 
 // ------------------------------------------------------------------------------------------------ head dim 64, wgmma
@@ -537,19 +387,21 @@ int launch_attention_tc(const void* q, const void* k, const void* v, void* o, in
     SATB_CHECK_CUDA(cudaGetLastError());
     return 0;
   }
-  const dim3 grid(ceil_div(Nq, kQ), H, batch);
+  const dim3 grid(ceil_div(Nq, 64), H, batch);
   SATB_REQUIRE(grid.y <= 65535 && grid.z <= 65535, "attention grid too large");
-  auto go = [&](auto kern, int smem, PerDeviceOnce& once) -> int {
-    if (once.first()) SATB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    SATB_CHECK_CUDA(launch_pdl(kern, grid, dim3(kAttnThreads), smem, stream, a));
-    return 0;
-  };
-  static PerDeviceOnce once[4][2];   // [head_dim / 32 - 1][bf16]
-  PerDeviceOnce& on = once[head_dim / 32 - 1][bf16 ? 1 : 0];
   switch (head_dim) {
-    case 32: SATB_PROPAGATE(bf16 ? go(attn_kernel<32, true>, attn_smem<32>(), on) : go(attn_kernel<32, false>, attn_smem<32>(), on)); break;
-    case 96: SATB_PROPAGATE(bf16 ? go(attn_kernel<96, true>, attn_smem<96>(), on) : go(attn_kernel<96, false>, attn_smem<96>(), on)); break;
-    default: SATB_PROPAGATE(bf16 ? go(attn_kernel<128, true>, attn_smem<128>(), on) : go(attn_kernel<128, false>, attn_smem<128>(), on)); break;
+    case 32:
+      SATB_PROPAGATE((bf16 ? launch_mma_attention<attn_kernel<32, true>, 32>(grid, stream, a)
+                          : launch_mma_attention<attn_kernel<32, false>, 32>(grid, stream, a)));
+      break;
+    case 96:
+      SATB_PROPAGATE((bf16 ? launch_mma_attention<attn_kernel<96, true>, 96>(grid, stream, a)
+                          : launch_mma_attention<attn_kernel<96, false>, 96>(grid, stream, a)));
+      break;
+    default:
+      SATB_PROPAGATE((bf16 ? launch_mma_attention<attn_kernel<128, true>, 128>(grid, stream, a)
+                          : launch_mma_attention<attn_kernel<128, false>, 128>(grid, stream, a)));
+      break;
   }
   count_launch();
   SATB_CHECK_CUDA(cudaGetLastError());

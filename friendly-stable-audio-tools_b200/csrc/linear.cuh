@@ -5,6 +5,7 @@
 #include <map>
 #include <string>
 #include <tuple>
+#include <vector>
 
 #include "common.cuh"
 #include "gemm.cuh"
@@ -37,6 +38,14 @@ struct DevBuf {
     return static_cast<T*>(p);
   }
 };
+
+// v into buf (grown as needed, at least 256 bytes), ordered on st: the per-item offsets and lengths the encoders'
+// attention kernels read.
+inline int dev_int_upload(DevBuf& buf, const std::vector<int>& v, cudaStream_t st) {
+  SATB_PROPAGATE(buf.ensure(v.size() * sizeof(int) < 256 ? 256 : v.size() * sizeof(int)));
+  SATB_CHECK_CUDA(cudaMemcpyAsync(buf.p, v.data(), v.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  return 0;
+}
 
 // Tensor maps by (pointer, shape, strides, box rows, element bytes): one buffer may be read as 16-bit and as e4m3 rows.
 struct TmapCache {

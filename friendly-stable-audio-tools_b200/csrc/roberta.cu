@@ -170,159 +170,25 @@ __global__ void __launch_bounds__(kRbThreads) rb_layernorm_kernel(const float* x
 }
 
 // ---- attention core: O = softmax(Q K^T / 8 + key mask) V per (item, head), RobertaSelfAttention at head dim 64.
-// mma.sync, as t5.cu's t5_attn_kernel: one CTA of four warps per (64-query tile, head, item); keys in 64-key tiles
-// double-buffered by cp.async; S = Q K^T in m16n8k16 fragments; online softmax in fp32 with exp2; P rounded to the
-// 16-bit operand type into O += P V.  Every one of the item's L query rows is computed and stored; only keys
-// [0, len) take part.  len >= 1 (the host refuses empty prompts), so every row has a key.
-constexpr int kRbAttnSmem = 5 * 64 * kRbHeadDim * 2;   // Q, two K and two V tiles
-
+// One CTA of four warps per (64-query tile, head, item) runs mma_tile.cuh's mma.sync core (mma_attention), scale 1/8
+// in log2 units.  Every one of the item's L query rows is computed and stored; only keys [0, len) take part.  len >= 1
+// (the host refuses empty prompts), so every row has a key.
+// qkv [B L, 3 H 64]: q of head h at column 64 h, k at 64 (H + h), v at 64 (2 H + h); o [B L, H 64]; lens [B]
 template <bool BF16>
-__global__ void __launch_bounds__(kRbThreads) rb_attn_kernel(const uint16_t* qkv, uint16_t* o, const int* lens, int L,
-                                                              int H) {
+__global__ void __launch_bounds__(kMmaAttnThreads) rb_attn_kernel(const uint16_t* qkv, uint16_t* o, const int* lens,
+                                                                   int L, int H) {
   constexpr int D = kRbHeadDim;
-  constexpr int kTileElems = 64 * D;
-  constexpr int kChunks = D / 8;
   extern __shared__ __align__(128) uint16_t smem_rb[];
-  uint16_t* sQ = smem_rb;
-  uint16_t* sK = sQ + kTileElems;
-  uint16_t* sV = sK + 2 * kTileElems;
-
   pdl_launch_dependents();
   pdl_wait();   // qkv is written by the previous kernel
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * 64, h = blockIdx.y, b = blockIdx.z;
+  const int h = blockIdx.y, b = blockIdx.z;
   const int n = lens[b];
   const int inner = H * D;
   const int64_t ld = 3LL * inner;
   const uint16_t* base = qkv + static_cast<int64_t>(b) * L * ld;
-  const int qc = h * D, kc = inner + h * D, vc = 2 * inner + h * D;
-  const int n_tiles = (n + 63) / 64;
-
-  load_tile<D, kRbThreads>(sQ, base, ld, q0, L, qc);
-  load_tile<D, kRbThreads>(sK, base, ld, 0, n, kc);
-  load_tile<D, kRbThreads>(sV, base, ld, 0, n, vc);
-  cp_async_commit();
-
-  uint32_t qf[D / 16][4];
-  float acc[D / 8][4];
-  float m[2] = {-1e30f, -1e30f}, l[2] = {0.f, 0.f};
-#pragma unroll
-  for (int j = 0; j < D / 8; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
-  constexpr float kScaleLog2e = 0.125f * 1.4426950408889634f;   // 1 / sqrt(64), in log2 units
-
-  for (int t = 0; t < n_tiles; ++t) {
-    const int buf = t & 1;
-    if (t + 1 < n_tiles) {
-      load_tile<D, kRbThreads>(sK + (buf ^ 1) * kTileElems, base, ld, (t + 1) * 64, n, kc);
-      load_tile<D, kRbThreads>(sV + (buf ^ 1) * kTileElems, base, ld, (t + 1) * 64, n, vc);
-      cp_async_commit();
-      cp_async_wait<1>();
-    } else {
-      cp_async_wait<0>();
-    }
-    __syncthreads();
-    if (t == 0) {
-      const uint32_t sq = smem_u32(sQ);
-#pragma unroll
-      for (int kk = 0; kk < D / 16; ++kk) {
-        const int r = warp * 16 + (lane & 7) + 8 * ((lane >> 3) & 1), c = 2 * kk + (lane >> 4);
-        ldsm_x4(sq + swz<D>(r, c) * 2, qf[kk][0], qf[kk][1], qf[kk][2], qf[kk][3]);
-      }
-    }
-    float s[8][4];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
-    const uint32_t sk = smem_u32(sK + buf * kTileElems);
-#pragma unroll
-    for (int kk = 0; kk < D / 16; ++kk) {
-#pragma unroll
-      for (int nb = 0; nb < 4; ++nb) {
-        const int r = 16 * nb + (lane & 7) + 8 * (lane >> 4), c = 2 * kk + ((lane >> 3) & 1);
-        uint32_t b0, b1, b2, b3;
-        ldsm_x4(sk + swz<D>(r, c) * 2, b0, b1, b2, b3);
-        mma16816<BF16>(s[2 * nb], qf[kk], b0, b1);
-        mma16816<BF16>(s[2 * nb + 1], qf[kk], b2, b3);
-      }
-    }
-    const int key0 = t * 64 + 2 * (lane & 3);
-    float mx[2] = {m[0], m[1]};
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int key = key0 + 8 * j + (e & 1);
-        s[j][e] = key < n ? s[j][e] * kScaleLog2e : -INFINITY;
-        mx[e >> 1] = fmaxf(mx[e >> 1], s[j][e]);
-      }
-    }
-    float alpha[2];
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 1));
-      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 2));
-      alpha[i] = exp2f(m[i] - mx[i]);
-      m[i] = mx[i];
-      l[i] *= alpha[i];
-    }
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        s[j][e] = exp2f(s[j][e] - m[e >> 1]);
-        l[e >> 1] += s[j][e];
-      }
-    }
-#pragma unroll
-    for (int j = 0; j < D / 8; ++j) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) acc[j][e] *= alpha[e >> 1];
-    }
-    const uint32_t sv = smem_u32(sV + buf * kTileElems);
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      uint32_t a[4];
-      a[0] = Op16<BF16>::pack(s[2 * kk][0], s[2 * kk][1]);
-      a[1] = Op16<BF16>::pack(s[2 * kk][2], s[2 * kk][3]);
-      a[2] = Op16<BF16>::pack(s[2 * kk + 1][0], s[2 * kk + 1][1]);
-      a[3] = Op16<BF16>::pack(s[2 * kk + 1][2], s[2 * kk + 1][3]);
-#pragma unroll
-      for (int db = 0; db < D / 16; ++db) {
-        const int r = 16 * kk + (lane & 7) + 8 * ((lane >> 3) & 1), c = 2 * db + (lane >> 4);
-        uint32_t b0, b1, b2, b3;
-        ldsm_x4_t(sv + swz<D>(r, c) * 2, b0, b1, b2, b3);
-        mma16816<BF16>(acc[2 * db], a, b0, b1);
-        mma16816<BF16>(acc[2 * db + 1], a, b2, b3);
-      }
-    }
-    __syncthreads();
-  }
-
-  float inv[2];
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    l[i] += __shfl_xor_sync(0xffffffffu, l[i], 1);
-    l[i] += __shfl_xor_sync(0xffffffffu, l[i], 2);
-    inv[i] = 1.f / l[i];
-  }
-  const int rr = warp * 16 + (lane >> 2);
-#pragma unroll
-  for (int j = 0; j < D / 8; ++j) {
-    const int col = 8 * j + 2 * (lane & 3);
-    *reinterpret_cast<uint32_t*>(sQ + swz<D>(rr, col >> 3) + (col & 7)) =
-        Op16<BF16>::pack(acc[j][0] * inv[0], acc[j][1] * inv[0]);
-    *reinterpret_cast<uint32_t*>(sQ + swz<D>(rr + 8, col >> 3) + (col & 7)) =
-        Op16<BF16>::pack(acc[j][2] * inv[1], acc[j][3] * inv[1]);
-  }
-  __syncwarp();
-  uint16_t* ob = o + static_cast<int64_t>(b) * L * inner + h * D;
-#pragma unroll
-  for (int i = 0; i < 16 * kChunks / 32; ++i) {
-    const int idx = lane + 32 * i;
-    const int r = warp * 16 + chunk_row<kChunks>(idx), c = chunk_col<kChunks>(idx);
-    if (q0 + r < L)
-      *reinterpret_cast<uint4*>(ob + static_cast<int64_t>(q0 + r) * inner + c * 8) =
-          *reinterpret_cast<const uint4*>(sQ + swz<D>(r, c));
-  }
+  mma_attention<D, BF16>(smem_rb, base, ld, h * D, base, ld, inner + h * D, base, ld, 2 * inner + h * D,
+                         o + static_cast<int64_t>(b) * L * inner, inner, h * D, blockIdx.x * 64, L, n,
+                         ScaleScore{0.125f * 1.4426950408889634f});
 }
 
 }  // namespace
@@ -356,8 +222,8 @@ static int launch_rb_attention(const void* qkv, const int* lens_dev, int B, int 
   SATB_REQUIRE(grid.y <= 65535 && grid.z <= 65535, "RoBERTa attention grid too large");
   const uint16_t* q = static_cast<const uint16_t*>(qkv);
   uint16_t* out = static_cast<uint16_t*>(o);
-  if (bf16) SATB_CHECK_CUDA(launch_pdl(rb_attn_kernel<true>, grid, dim3(kRbThreads), kRbAttnSmem, st, q, out, lens_dev, L, H));
-  else SATB_CHECK_CUDA(launch_pdl(rb_attn_kernel<false>, grid, dim3(kRbThreads), kRbAttnSmem, st, q, out, lens_dev, L, H));
+  SATB_PROPAGATE((bf16 ? launch_mma_attention<rb_attn_kernel<true>, kRbHeadDim>(grid, st, q, out, lens_dev, L, H)
+                       : launch_mma_attention<rb_attn_kernel<false>, kRbHeadDim>(grid, st, q, out, lens_dev, L, H)));
   count_launch();
   return 0;
 }
@@ -471,12 +337,6 @@ static int rb_lengths(const int* lengths, int B, int L, std::vector<int>* v) {
   v->assign(lengths, lengths + B);
   for (int b = 0; b < B; ++b)
     SATB_REQUIRE(lengths[b] >= 1 && lengths[b] <= L, "RoBERTa: every length must lie in [1, L]");
-  return 0;
-}
-
-static int rb_upload(DevBuf& buf, const std::vector<int>& v, cudaStream_t st) {
-  SATB_PROPAGATE(buf.ensure(v.size() * sizeof(int) < 256 ? 256 : v.size() * sizeof(int)));
-  SATB_CHECK_CUDA(cudaMemcpyAsync(buf.p, v.data(), v.size() * sizeof(int), cudaMemcpyHostToDevice, st));
   return 0;
 }
 
@@ -624,7 +484,7 @@ int satb_roberta_encode(SatbRoberta* t, const long long* ids, const int* lengths
   cudaStream_t st = static_cast<cudaStream_t>(stream_v);
   std::vector<int> lens;
   SATB_PROPAGATE(rb_lengths(lengths, B, L, &lens));
-  SATB_PROPAGATE(rb_upload(t->ws_len, lens, st));
+  SATB_PROPAGATE(dev_int_upload(t->ws_len, lens, st));
   SATB_PROPAGATE(rb_reserve(t, B * L));
   return t->bf16 ? rb_encode_impl<true>(t, ids, B, L, out, st) : rb_encode_impl<false>(t, ids, B, L, out, st);
 }
@@ -661,7 +521,7 @@ int satb_roberta_attention_probe(const void* qkv16, const int* lengths, int B, i
   SATB_PROPAGATE(rb_lengths(lengths, B, L, &lens));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   DevBuf d_len;
-  int rc = rb_upload(d_len, lens, st);
+  int rc = dev_int_upload(d_len, lens, st);
   if (rc == 0) rc = launch_rb_attention(qkv16, d_len.as<int>(), B, L, H, bf16 != 0, o16, st);
   const cudaError_t e = cudaStreamSynchronize(st);
   d_len.release();

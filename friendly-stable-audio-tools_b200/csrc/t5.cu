@@ -151,179 +151,44 @@ __global__ void __launch_bounds__(kNormThreads) t5_scatter_kernel(const float* s
 
 // ---- attention core: O = softmax(Q K^T + bias[h, j - i]) V per (item, head), T5Attention.forward
 // (modeling_t5.py:253-340) on packed rows, with no 1 / sqrt(d) scale (T5 folds it into the q weights' initialisation).
-// mma.sync, the structure of attention_tc.cu attn_kernel<D>: one CTA of four warps per (64-query tile, head, item);
-// keys of the item only, in 64-key tiles double-buffered by cp.async; S = Q K^T in m16n8k16 fragments, plus the bias
-// row from shared memory; online softmax in fp32 with exp2; P rounded to the 16-bit operand type into O += P V.
-// mma.sync rather than wgmma: a prompt holds at most 512 keys and usually 10 - 40, so the CTA tile is 64 queries
-// (a wgmma consumer warpgroup would want 128 and leave most rows empty), and there is no key stream long enough
-// for a producer / consumer ring to hide anything.  The bias row of the head (kT5BiasSpan fp32) sits in shared memory;
-// rows past the item's length are computed on zero queries and never stored.
-struct T5AttnArgs {
-  const uint16_t* qkv;   // [M, ld]: q of head h at column h D, k at inner + h D, v at 2 inner + h D
-  int64_t ld;
-  uint16_t* o;           // [M, ldo], head h at column h D
-  int64_t ldo;
-  const int* off;        // [B + 1]
-  const float* bias;     // [H, kT5BiasSpan]
-  int inner;
-};
-constexpr int kT5AttnThreads = 128;
-template <int D>
-constexpr int t5_attn_smem() { return 5 * 64 * D * 2; }   // Q, two K and two V tiles
+// One CTA of four warps per (64-query tile, head, item) runs mma_tile.cuh's mma.sync core (mma_attention) over the
+// keys of the item only, with the bias row of the head (kT5BiasSpan fp32) staged in shared memory.  mma.sync rather
+// than wgmma: a prompt holds at most 512 keys and usually 10 - 40, so the CTA tile is 64 queries (a wgmma consumer
+// warpgroup would want 128 and leave most rows empty), and there is no key stream long enough for a producer /
+// consumer ring to hide anything.  Rows past the item's length are computed on zero queries and never stored.
 
+// (s + bias of relative position key - query) in log2 units, from the head's bias row in shared memory.  Query rows
+// past the item use the last row's entries: in range, and never stored.
+struct T5BiasScore {
+  const float* sbias;   // [kT5BiasSpan]
+  int last;             // the item's last row
+  __device__ __forceinline__ float operator()(float s, int query, int key) const {
+    return (s + sbias[key - min(query, last) + kT5MaxLen - 1]) * 1.4426950408889634f;
+  }
+};
+
+// qkv [M, 3 inner]: q of head h at column h D, k at inner + h D, v at 2 inner + h D; o [M, inner]; off [B + 1];
+// bias [H, kT5BiasSpan]
 template <int D, bool BF16>
-__global__ void __launch_bounds__(kT5AttnThreads) t5_attn_kernel(const T5AttnArgs p) {
-  constexpr int kTileElems = 64 * D;
-  constexpr int kChunks = D / 8;
+__global__ void __launch_bounds__(kMmaAttnThreads) t5_attn_kernel(const uint16_t* qkv, uint16_t* o, const int* off,
+                                                                   const float* bias, int inner) {
   extern __shared__ __align__(128) uint16_t smem_t5[];
   __shared__ float sbias[kT5BiasSpan];
-  uint16_t* sQ = smem_t5;
-  uint16_t* sK = sQ + kTileElems;
-  uint16_t* sV = sK + 2 * kTileElems;
-
   pdl_launch_dependents();
   pdl_wait();   // qkv is written by the previous kernel
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * 64, h = blockIdx.y, b = blockIdx.z;
-  const int start = p.off[b], n = p.off[b + 1] - start;
+  const int start = off[b], n = off[b + 1] - start;
   if (q0 >= n) return;
-  const uint16_t* base = p.qkv + static_cast<int64_t>(start) * p.ld;
-  const int qc = h * D, kc = p.inner + h * D, vc = 2 * p.inner + h * D;
-  const int n_tiles = (n + 63) / 64;
-
-  load_tile<D, kT5AttnThreads>(sQ, base, p.ld, q0, n, qc);
-  load_tile<D, kT5AttnThreads>(sK, base, p.ld, 0, n, kc);
-  load_tile<D, kT5AttnThreads>(sV, base, p.ld, 0, n, vc);
-  cp_async_commit();
-  {   // bias entries of relative positions j - i, i in [q0, min(q0 + 63, n - 1)], j in [0, n)
-    const float* brow = p.bias + static_cast<size_t>(h) * kT5BiasSpan;
+  {   // bias entries of relative positions j - i, i in [q0, min(q0 + 63, n - 1)], j in [0, n), by cp.async: they join
+      // mma_attention's first copy group, so their fetch overlaps that of the first Q / K / V tiles
+    const float* brow = bias + static_cast<size_t>(h) * kT5BiasSpan;
     const int lo = kT5MaxLen - 1 - min(q0 + 63, n - 1), hi = kT5MaxLen - 1 + n - 1;
-    for (int i = lo + threadIdx.x; i <= hi; i += kT5AttnThreads) sbias[i] = __ldg(brow + i);
+    for (int i = lo + threadIdx.x; i <= hi; i += kMmaAttnThreads) cp_async4(smem_u32(sbias + i), brow + i);
   }
-
-  uint32_t qf[D / 16][4];
-  float o[D / 8][4];
-  float m[2] = {-1e30f, -1e30f}, l[2] = {0.f, 0.f};
-#pragma unroll
-  for (int j = 0; j < D / 8; ++j) o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f;
-  // this thread's query rows (rows past the item use the last row's bias entries: in range, and never stored)
-  const int qi0 = min(q0 + warp * 16 + (lane >> 2), n - 1), qi1 = min(q0 + warp * 16 + (lane >> 2) + 8, n - 1);
-  constexpr float kLog2e = 1.4426950408889634f;
-
-  for (int t = 0; t < n_tiles; ++t) {
-    const int buf = t & 1;
-    if (t + 1 < n_tiles) {
-      load_tile<D, kT5AttnThreads>(sK + (buf ^ 1) * kTileElems, base, p.ld, (t + 1) * 64, n, kc);
-      load_tile<D, kT5AttnThreads>(sV + (buf ^ 1) * kTileElems, base, p.ld, (t + 1) * 64, n, vc);
-      cp_async_commit();
-      cp_async_wait<1>();
-    } else {
-      cp_async_wait<0>();
-    }
-    __syncthreads();
-    if (t == 0) {
-      const uint32_t sq = smem_u32(sQ);
-#pragma unroll
-      for (int kk = 0; kk < D / 16; ++kk) {
-        const int r = warp * 16 + (lane & 7) + 8 * ((lane >> 3) & 1), c = 2 * kk + (lane >> 4);
-        ldsm_x4(sq + swz<D>(r, c) * 2, qf[kk][0], qf[kk][1], qf[kk][2], qf[kk][3]);
-      }
-    }
-    float s[8][4];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
-    const uint32_t sk = smem_u32(sK + buf * kTileElems);
-#pragma unroll
-    for (int kk = 0; kk < D / 16; ++kk) {
-#pragma unroll
-      for (int nb = 0; nb < 4; ++nb) {
-        const int r = 16 * nb + (lane & 7) + 8 * (lane >> 4), c = 2 * kk + ((lane >> 3) & 1);
-        uint32_t b0, b1, b2, b3;
-        ldsm_x4(sk + swz<D>(r, c) * 2, b0, b1, b2, b3);
-        mma16816<BF16>(s[2 * nb], qf[kk], b0, b1);
-        mma16816<BF16>(s[2 * nb + 1], qf[kk], b2, b3);
-      }
-    }
-    // + bias, mask, online softmax (log2 units)
-    const int key0 = t * 64 + 2 * (lane & 3);
-    float mx[2] = {m[0], m[1]};
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int key = key0 + 8 * j + (e & 1);
-        const int qi = e >> 1 ? qi1 : qi0;
-        s[j][e] = key < n ? (s[j][e] + sbias[key - qi + kT5MaxLen - 1]) * kLog2e : -INFINITY;
-        mx[e >> 1] = fmaxf(mx[e >> 1], s[j][e]);
-      }
-    }
-    float alpha[2];
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 1));
-      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 2));
-      alpha[i] = exp2f(m[i] - mx[i]);
-      m[i] = mx[i];
-      l[i] *= alpha[i];
-    }
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        s[j][e] = exp2f(s[j][e] - m[e >> 1]);
-        l[e >> 1] += s[j][e];
-      }
-    }
-#pragma unroll
-    for (int j = 0; j < D / 8; ++j) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) o[j][e] *= alpha[e >> 1];
-    }
-    const uint32_t sv = smem_u32(sV + buf * kTileElems);
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      uint32_t a[4];
-      a[0] = Op16<BF16>::pack(s[2 * kk][0], s[2 * kk][1]);
-      a[1] = Op16<BF16>::pack(s[2 * kk][2], s[2 * kk][3]);
-      a[2] = Op16<BF16>::pack(s[2 * kk + 1][0], s[2 * kk + 1][1]);
-      a[3] = Op16<BF16>::pack(s[2 * kk + 1][2], s[2 * kk + 1][3]);
-#pragma unroll
-      for (int db = 0; db < D / 16; ++db) {
-        const int r = 16 * kk + (lane & 7) + 8 * ((lane >> 3) & 1), c = 2 * db + (lane >> 4);
-        uint32_t b0, b1, b2, b3;
-        ldsm_x4_t(sv + swz<D>(r, c) * 2, b0, b1, b2, b3);
-        mma16816<BF16>(o[2 * db], a, b0, b1);
-        mma16816<BF16>(o[2 * db + 1], a, b2, b3);
-      }
-    }
-    __syncthreads();
-  }
-
-  float inv[2];
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    l[i] += __shfl_xor_sync(0xffffffffu, l[i], 1);
-    l[i] += __shfl_xor_sync(0xffffffffu, l[i], 2);
-    inv[i] = 1.f / l[i];
-  }
-  const int rr = warp * 16 + (lane >> 2);
-#pragma unroll
-  for (int j = 0; j < D / 8; ++j) {
-    const int col = 8 * j + 2 * (lane & 3);
-    *reinterpret_cast<uint32_t*>(sQ + swz<D>(rr, col >> 3) + (col & 7)) = Op16<BF16>::pack(o[j][0] * inv[0], o[j][1] * inv[0]);
-    *reinterpret_cast<uint32_t*>(sQ + swz<D>(rr + 8, col >> 3) + (col & 7)) =
-        Op16<BF16>::pack(o[j][2] * inv[1], o[j][3] * inv[1]);
-  }
-  __syncwarp();
-  uint16_t* ob = p.o + static_cast<int64_t>(start) * p.ldo + h * D;
-#pragma unroll
-  for (int i = 0; i < 16 * kChunks / 32; ++i) {
-    const int idx = lane + 32 * i;
-    const int r = warp * 16 + chunk_row<kChunks>(idx), c = chunk_col<kChunks>(idx);
-    if (q0 + r < n)
-      *reinterpret_cast<uint4*>(ob + static_cast<int64_t>(q0 + r) * p.ldo + c * 8) =
-          *reinterpret_cast<const uint4*>(sQ + swz<D>(r, c));
-  }
+  const int64_t ld = 3LL * inner;
+  const uint16_t* base = qkv + start * ld;
+  mma_attention<D, BF16>(smem_t5, base, ld, h * D, base, ld, inner + h * D, base, ld, 2 * inner + h * D,
+                         o + static_cast<int64_t>(start) * inner, inner, h * D, q0, n, n, T5BiasScore{sbias, n - 1});
 }
 
 }  // namespace
@@ -346,25 +211,17 @@ static int launch_t5_attention(const void* qkv, const float* bias, const int* of
                                int dk, bool bf16, void* o, cudaStream_t st) {
   SATB_REQUIRE(dk == 64 || dk == 128, "T5 attention: d_kv must be 64 or 128");
   if (B <= 0 || max_len <= 0) return 0;
-  T5AttnArgs a;
-  a.qkv = static_cast<const uint16_t*>(qkv);
-  a.ld = 3LL * H * dk;
-  a.o = static_cast<uint16_t*>(o);
-  a.ldo = static_cast<int64_t>(H) * dk;
-  a.off = off_dev;
-  a.bias = bias;
-  a.inner = H * dk;
   const dim3 grid(ceil_div(max_len, 64), H, B);
   SATB_REQUIRE(grid.y <= 65535 && grid.z <= 65535, "T5 attention grid too large");
-  auto go = [&](auto kern, int smem, PerDeviceOnce& once) -> int {
-    if (once.first()) SATB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    SATB_CHECK_CUDA(launch_pdl(kern, grid, dim3(kT5AttnThreads), smem, st, a));
-    return 0;
-  };
-  static PerDeviceOnce once[2][2];
-  PerDeviceOnce& on = once[dk == 128][bf16];
-  if (dk == 64) SATB_PROPAGATE(bf16 ? go(t5_attn_kernel<64, true>, t5_attn_smem<64>(), on) : go(t5_attn_kernel<64, false>, t5_attn_smem<64>(), on));
-  else SATB_PROPAGATE(bf16 ? go(t5_attn_kernel<128, true>, t5_attn_smem<128>(), on) : go(t5_attn_kernel<128, false>, t5_attn_smem<128>(), on));
+  const uint16_t* q = static_cast<const uint16_t*>(qkv);
+  uint16_t* out = static_cast<uint16_t*>(o);
+  const int inner = H * dk;
+  if (dk == 64)
+    SATB_PROPAGATE((bf16 ? launch_mma_attention<t5_attn_kernel<64, true>, 64>(grid, st, q, out, off_dev, bias, inner)
+                         : launch_mma_attention<t5_attn_kernel<64, false>, 64>(grid, st, q, out, off_dev, bias, inner)));
+  else
+    SATB_PROPAGATE((bf16 ? launch_mma_attention<t5_attn_kernel<128, true>, 128>(grid, st, q, out, off_dev, bias, inner)
+                         : launch_mma_attention<t5_attn_kernel<128, false>, 128>(grid, st, q, out, off_dev, bias, inner)));
   count_launch();
   return 0;
 }
@@ -490,12 +347,6 @@ static int t5_encode_impl(SatbT5* t, const long long* ids, int B, int L, int M, 
   SATB_CHECK_CUDA(launch_pdl(t5_scatter_kernel, dim3(B * L), dim3(kNormThreads), 0, st, static_cast<const float*>(y),
                              off, L, n_out, out));
   count_launch();
-  return 0;
-}
-
-static int dev_int_upload(DevBuf& buf, const std::vector<int>& v, cudaStream_t st) {
-  SATB_PROPAGATE(buf.ensure(v.size() * sizeof(int) < 256 ? 256 : v.size() * sizeof(int)));
-  SATB_CHECK_CUDA(cudaMemcpyAsync(buf.p, v.data(), v.size() * sizeof(int), cudaMemcpyHostToDevice, st));
   return 0;
 }
 
